@@ -441,7 +441,9 @@ void b200_keccak256(const uint8_t* data, size_t len, uint8_t out[32]);
  * mismatches in *mismatches (0 expected). */
 int b200_selftest_field(b200_ctx* ctx, uint64_t seed, size_t iters, uint64_t* mismatches);
 /* out[i] = a[i] (op) b[i] on the device; field: 0 = Fr, 1 = Fq; op: 0 mul, 1 add, 2 sub,
- * 3 inverse of a.  Host buffers, n x 4 limbs (Montgomery).  For parity tests. */
+ * 3 inverse of a, 4 square of a (the dedicated squarer), 5 a[i] b[i] + a[j] b[j] and
+ * 6 a[i] b[i] - a[j] b[j] with j = n - 1 - i (the fused two-product forms of the curve additions).
+ * Host buffers, n x 4 limbs (Montgomery).  For parity tests. */
 int b200_field_op(b200_ctx* ctx, int field, int op, const uint64_t* a, const uint64_t* b, size_t n,
                   uint64_t* out);
 

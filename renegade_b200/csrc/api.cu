@@ -111,6 +111,7 @@ __global__ void selftest_field_kernel(uint64_t seed, size_t iters, unsigned long
     if (bad) atomicAdd(mismatches, bad);
 }
 
+// ops 5 and 6 pair element i with element n - 1 - i, so one call reaches the fused two-product forms
 template <class C>
 __global__ void field_op_kernel(int op, const fe* a, const fe* b, size_t n, fe* out) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -121,7 +122,10 @@ __global__ void field_op_kernel(int op, const fe* a, const fe* b, size_t n, fe* 
         case 0: r = fe_mul<C>(x, y); break;
         case 1: r = fe_add<C>(x, y); break;
         case 2: r = fe_sub<C>(x, y); break;
-        default: r = fe_inv<C>(x); break;
+        case 3: r = fe_inv<C>(x); break;
+        case 4: r = fe_sqr<C>(x); break;
+        case 5: r = fe_mul_add2<C>(x, y, fe_load(a + (n - 1 - i)), fe_load(b + (n - 1 - i))); break;
+        default: r = fe_mul_sub2<C>(x, y, fe_load(a + (n - 1 - i)), fe_load(b + (n - 1 - i))); break;
     }
     fe_store(out + i, r);
 }
@@ -576,7 +580,7 @@ int b200_selftest_field(b200_ctx* ctx, uint64_t seed, size_t iters, uint64_t* mi
 
 int b200_field_op(b200_ctx* ctx, int field, int op, const uint64_t* a, const uint64_t* b, size_t n, uint64_t* out) {
     B200_TRY
-    if (!ctx || !a || !b || !out || field < 0 || field > 1 || op < 0 || op > 3) return B200_ERR_INVALID;
+    if (!ctx || !a || !b || !out || field < 0 || field > 1 || op < 0 || op > 6) return B200_ERR_INVALID;
     if (n == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
     B200_CUDA(cudaSetDevice(ctx->c.device));

@@ -1,5 +1,5 @@
-"""GPU parity: device field arithmetic (IMAD.WIDE Montgomery multiplier, carry-chain add/sub,
-Fermat inverse) vs the oracle, bit-exact, through the C ABI."""
+"""GPU parity: device field arithmetic (IMAD.WIDE Montgomery multiplier, squarer, fused two-product forms,
+carry-chain add/sub, Fermat inverse) vs the oracle and Python integers, bit-exact, through the C ABI."""
 import numpy as np
 import pytest
 
@@ -31,6 +31,24 @@ def test_field_ops_vs_oracle(ctx, oracle, pyoracle, field):
     got = ctx.field_op(field, 3, a[:64], b[:64])
     exp = np.stack([oracle.fp_unop("orc_fp_inv", field, a[i]) for i in range(64)])
     assert (got == exp).all()
+
+
+@pytest.mark.parametrize("field", [0, 1], ids=["fr", "fq"])
+def test_field_ops_on_edge_operands(ctx, field):
+    """All seven device ops of b200_field_op — product, add, sub, inverse, the dedicated squarer and the fused
+    a*b +- c*d of the curve additions — against Python integers on the edge operands of tests/field_edges.py: the whole
+    residue range (for Fq the operands in [r, q) included), powers of two and their neighbours, limb patterns, and
+    products that land exactly on 1 and p - 1."""
+    import field_edges as fx
+    p = fx.R_FR if field == 0 else fx.Q
+    a, b = fx.pairs(p)
+    assert len(a) > 10000 and any(x >= fx.R_FR for x in a) == (field == 1)
+    da, db = fx.to_array(a), fx.to_array(b)
+    for op in range(7):
+        got = fx.from_array(ctx.field_op(field, op, da, db))
+        exp = fx.expected(op, a, b, p)
+        bad = [i for i in range(len(a)) if got[i] != exp[i]]
+        assert not bad, (op, len(bad), [(hex(a[i]), hex(b[i])) for i in bad[:3]])
 
 
 @pytest.mark.parametrize("n", [1, 15, 16, 17, 4095, 4096, 4097, 3 * 4096 + 5])

@@ -238,6 +238,48 @@ int b200_plonk_verify_link(const uint64_t* comm1, const uint64_t* comm2, unsigne
  * (srs.rs:236-266: e(tau^i G, tau H) == e(tau^(i+1) G, H)). */
 int b200_pairing_check(const uint64_t* g1_points, const uint64_t* g2_points, size_t k, int* is_one);
 
+/* ---- batch verification (device) -------------------------------------------------------------
+ * The flat verifying key b200_plonk_verify takes. */
+typedef struct {
+    unsigned log_n;
+    size_t num_inputs;
+    const uint64_t* k;              /* 5 x 4 */
+    const uint64_t* selector_comms; /* 13 x 8 */
+    const uint64_t* sigma_comms;    /* 5 x 8 */
+} b200_verifying_key;
+/* One proof of a batch: vks[vk] is its key; pub_inputs holds that key's num_inputs values. */
+typedef struct {
+    unsigned vk;
+    const uint64_t* pub_inputs;
+    const b200_proof* proof;
+} b200_batch_proof;
+/* One link proof of a batch: the arguments of b200_plonk_verify_link. */
+typedef struct {
+    const uint64_t* comm1;
+    const uint64_t* comm2;
+    unsigned alignment;
+    size_t offset;
+    size_t size;
+    const b200_link_proof* proof;
+} b200_batch_link;
+/* Verifies n_proofs proofs and n_links link proofs with ONE pairing: every check e(A_i, [tau]_2) == e(B_i, [1]_2) is
+ * weighted by a random rho_i and the sums are checked at once, e(sum rho_i A_i, [tau]_2) == e(sum rho_i B_i, [1]_2)
+ * (two MSMs on the device, one pairing on the host).  The rho_i are Fiat–Shamir outputs over the whole batch:
+ *   d_i   = keccak(0 || proof i's final transcript state), or
+ *           keccak(1 || link i's final transcript state || pi || alignment u32 || offset u64 || size u64), big-endian;
+ *   seed  = keccak("b200 batch verify v1" || d_0 || ... || d_{k-1} || g2_h || g2_tau_h);
+ *   rho_i = keccak(seed || i as u64 big-endian) as a big-endian integer mod r (1 if that is 0).
+ * Items are numbered proofs first, then links.  *all_accepted = 1 exactly when every item would be accepted by
+ * b200_plonk_verify / b200_plonk_verify_link with the same G2 pair.  verdicts (may be NULL): n_proofs + n_links bytes,
+ * verdicts[i] = that single verifier's answer for item i; when the combined check fails the failing items are found
+ * by bisection over subsets (each step one MSM pair and one pairing).  With verdicts NULL the call stops after the
+ * combined check.  An item with an off-curve G1 point is rejected (verdict 0) and left out of the combination.
+ * Errors: B200_ERR_NOT_ON_CURVE for an off-curve G2 point; B200_ERR_INVALID for a vk index out of range, log_n > 28,
+ * a link with alignment > 28 or size == 0, or a NULL pointer.  Zero items are accepted. */
+int b200_plonk_batch_verify(b200_ctx* ctx, const b200_verifying_key* vks, size_t n_vks, const b200_batch_proof* proofs,
+                            size_t n_proofs, const b200_batch_link* links, size_t n_links, const uint64_t g2_h[16],
+                            const uint64_t g2_tau_h[16], int* all_accepted, uint8_t* verdicts);
+
 /* Wall-clock milliseconds of the last proof's phases on this context: round 1, round 2, round 3
  * (coset NTTs + quotient + split), round 3 commitments, round 4, round 5, then two spare slots. */
 int b200_plonk_last_timings(b200_ctx* ctx, float out_ms[8]);

@@ -352,6 +352,23 @@ class VerifyingKey:
         return VerifyingKey(pk.log_n, pk.num_inputs, pk.k, pk.selector_comms, pk.sigma_comms, g2_h, g2_tau_h)
 
 
+class B200VerifyingKey(C.Structure):
+    """b200_verifying_key: the flat verifying key of b200_plonk_verify."""
+    _fields_ = [("log_n", C.c_uint), ("num_inputs", C.c_size_t), ("k", C.c_void_p), ("selector_comms", C.c_void_p),
+                ("sigma_comms", C.c_void_p)]
+
+
+class B200BatchProof(C.Structure):
+    """b200_batch_proof: one proof of a batch (index of its key, public inputs, proof)."""
+    _fields_ = [("vk", C.c_uint), ("pub_inputs", C.c_void_p), ("proof", C.c_void_p)]
+
+
+class B200BatchLink(C.Structure):
+    """b200_batch_link: one link proof of a batch."""
+    _fields_ = [("comm1", C.c_void_p), ("comm2", C.c_void_p), ("alignment", C.c_uint), ("offset", C.c_size_t),
+                ("size", C.c_size_t), ("proof", C.c_void_p)]
+
+
 def _u64(a, shape=None) -> np.ndarray:
     a = np.ascontiguousarray(a, dtype=np.uint64)
     return a.reshape(shape) if shape is not None else a
@@ -395,6 +412,70 @@ class PlonkKzgSnark:
                                                  _ptr(pi) if pi.size else None, C.byref(proof), _ptr(_u64(vk.g2_h)),
                                                  _ptr(_u64(vk.g2_tau_h)), C.byref(ok)))
         return bool(ok.value)
+
+    @staticmethod
+    def batch_verify(ctx: Context, vks, pub_inputs, proofs, links=(), g2=None):
+        """Verifies many proofs and link proofs with ONE pairing on `ctx`'s device (`b200_plonk_batch_verify`).
+
+        vks[i], pub_inputs[i], proofs[i]: the arguments of `verify` for proof i; links: (comm_a, comm_b, B200LinkProof,
+        GroupLayout) tuples, the arguments of `verify_link_proof`.  Every key must carry the same G2 pair (else
+        ValueError); `g2 = (g2_h, g2_tau_h)` supplies it when there are only links.  Returns (all_ok, verdicts) with
+        verdicts[i] the single verifier's answer for item i, proofs first, then links.  A wrong public-input count is
+        a False verdict, as in `verify`."""
+        vks, pub_inputs, proofs, links = list(vks), list(pub_inputs), list(proofs), list(links)
+        if not (len(vks) == len(pub_inputs) == len(proofs)):
+            raise ValueError("one verifying key and one public-input vector per proof")
+        g2_pairs = {(_u64(vk.g2_h).tobytes(), _u64(vk.g2_tau_h).tobytes()) for vk in vks}
+        if g2 is not None:
+            g2_pairs.add((_u64(g2[0]).tobytes(), _u64(g2[1]).tobytes()))
+        if len(g2_pairs) > 1:
+            raise ValueError("the verifying keys of one batch must share the G2 pair (h, beta_h)")
+        n_items = len(proofs) + len(links)
+        if not g2_pairs:
+            if n_items:
+                raise ValueError("links without proofs need g2=(g2_h, g2_tau_h)")
+            return True, []
+        g2_h, g2_tau_h = (np.frombuffer(b, dtype=np.uint64).copy() for b in next(iter(g2_pairs)))
+        keep = []  # the arrays the C structs point into stay alive until the call returns
+        # distinct verifying keys
+        vk_index, c_vks = {}, []
+        for vk in vks:
+            arrs = (_u64(vk.k, (5, 4)), _u64(vk.selector_comms, (13, 8)), _u64(vk.sigma_comms, (5, 8)))
+            key = (vk.log_n, vk.num_inputs) + tuple(a.tobytes() for a in arrs)
+            if key not in vk_index:
+                vk_index[key] = len(c_vks)
+                keep.append(arrs)
+                c_vks.append(B200VerifyingKey(vk.log_n, vk.num_inputs, *(_ptr(a) for a in arrs)))
+        c_proofs, proof_pos = [], []
+        for i, (vk, pi, proof) in enumerate(zip(vks, pub_inputs, proofs)):
+            p = _u64(pi, (-1, 4))
+            if p.shape[0] != vk.num_inputs:
+                continue  # not accepted (the reference's verifier errors on a wrong public-input count)
+            keep.append(p)
+            key = (vk.log_n, vk.num_inputs) + tuple(
+                a.tobytes() for a in (_u64(vk.k, (5, 4)), _u64(vk.selector_comms, (13, 8)), _u64(vk.sigma_comms, (5, 8))))
+            c_proofs.append(B200BatchProof(vk_index[key], _ptr(p) if p.size else None, C.cast(C.pointer(proof), C.c_void_p)))
+            proof_pos.append(i)
+        c_links = []
+        for comm_a, comm_b, lproof, layout in links:
+            a, b = _u64(comm_a), _u64(comm_b)
+            keep.append((a, b))
+            c_links.append(B200BatchLink(_ptr(a), _ptr(b), layout.alignment, layout.offset, layout.size,
+                                         C.cast(C.pointer(lproof), C.c_void_p)))
+        arr_vks = (B200VerifyingKey * max(1, len(c_vks)))(*c_vks)
+        arr_proofs = (B200BatchProof * max(1, len(c_proofs)))(*c_proofs)
+        arr_links = (B200BatchLink * max(1, len(c_links)))(*c_links)
+        n_c = len(c_proofs) + len(c_links)
+        verdicts = (C.c_uint8 * max(1, n_c))()
+        ok = C.c_int(0)
+        _lib.check(ctx._lib.b200_plonk_batch_verify(ctx._h, arr_vks, len(c_vks), arr_proofs, len(c_proofs), arr_links,
+                                                    len(c_links), _ptr(g2_h), _ptr(g2_tau_h), C.byref(ok), verdicts))
+        out = [False] * n_items
+        for j, i in enumerate(proof_pos):
+            out[i] = bool(verdicts[j])
+        for j in range(len(c_links)):
+            out[len(proofs) + j] = bool(verdicts[len(c_proofs) + j])
+        return bool(ok.value) and len(c_proofs) == len(proofs), out
 
     @staticmethod
     def preprocess(ctx: Context, srs: Bases, log_n: int, num_inputs: int, selectors: np.ndarray,

@@ -251,6 +251,25 @@ def verify_singleprover_proof(circuit: type, statement, proof: PlonkProof) -> No
     circuit.verify(statement, proof)
 
 
+def batch_verify_singleprover_proofs(items) -> None:
+    """`verify_singleprover_proof` for many (circuit, statement, proof) triples at once: one batch check with ONE
+    pairing on the `SYSTEM_SRS` context's device (`PlonkKzgSnark.batch_verify`).  Raises VerifierError naming the
+    indices of the proofs that fail."""
+    items = list(items)
+    if not items:
+        return
+    srs = system_srs()
+    vks = [c.verifying_key() for c, _, _ in items]
+    pis = [c.statement_scalars(s) for c, s, _ in items]
+    try:
+        _, verdicts = PlonkKzgSnark.batch_verify(srs.ctx, vks, pis, [p for _, _, p in items])
+    except _lib.B200Error as e:
+        raise VerifierError(f"Plonk({e})") from e
+    bad = [i for i, ok in enumerate(verdicts) if not ok]
+    if bad:
+        raise VerifierError(f"Plonk(WrongProof) at indices {bad}")
+
+
 def singleprover_prove_and_verify(circuit: type, witness, statement, rng=None) -> None:
     proof = circuit.prove(witness, statement, rng)
     try:

@@ -103,6 +103,10 @@ fe host_root_of_unity(unsigned log_n);
 int ntt_device(const Domain* d, fe* data, fe* scratch, int inverse, int coset, unsigned batch,
                size_t stride, cudaStream_t st);
 
+// data[i] <- 1 / data[i] (num == nullptr) or num[i] / data[i], zeros stay zero; enqueue only.  scratch: n elements.
+// Montgomery's trick on two levels, one field inversion per 4096 elements (plonk.cu).
+void batch_inverse_enqueue(const fe* num, fe* data, fe* scratch, size_t n, cudaStream_t st);
+
 // ---- MSM ------------------------------------------------------------------------------------
 struct MsmPlan {
     int c = 0;        // window bits (signed digits in [-2^(c-1), 2^(c-1)])
@@ -162,8 +166,11 @@ struct MsmScratch {
 MsmPlan msm_choose_plan(size_t n, int c_override, size_t mem_budget_bytes);
 int bases_create(const g1_affine* h_points, size_t n, int c_override, int check_on_curve,
                  cudaStream_t st, Bases** out);
+// table_budget_bytes: device memory the precomputed window tables may take (kTablesAuto = half the free memory);
+// 0 = no tables, every window physical (bases used once, e.g. the batch verifier's)
+constexpr size_t kTablesAuto = ~(size_t)0;
 int bases_create_device(const g1_affine* d_points, size_t n, int c_override, cudaStream_t st,
-                        Bases** out);
+                        Bases** out, size_t table_budget_bytes = kTablesAuto);
 // scalars on device (n x 32 B); result: XYZZ sums of the n_phys windows copied to host and
 // combined there (Horner + one inversion).
 int msm_device(const Bases* b, size_t base_off, const fe* d_scalars, size_t n, int montgomery,

@@ -885,14 +885,14 @@ static size_t table_mem_budget() {
 }
 
 int bases_create_device(const g1_affine* d_points, size_t n, int c_override, cudaStream_t st,
-                        Bases** out) {
+                        Bases** out, size_t table_budget_bytes) {
     if (n == 0 || n > ((size_t)1 << kIdxBits)) {
         set_error("bases: n must be in [1, 2^26]");
         return B200_ERR_INVALID;
     }
     Bases* b = new Bases();
     b->n = n;
-    b->plan = msm_choose_plan(n, c_override, table_mem_budget());
+    b->plan = msm_choose_plan(n, c_override, table_budget_bytes == kTablesAuto ? table_mem_budget() : table_budget_bytes);
     cudaError_t e = cudaMalloc(&b->tables, (size_t)b->plan.n_tables * n * sizeof(g1_affine));
     if (e != cudaSuccess) {
         delete b;

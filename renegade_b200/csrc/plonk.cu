@@ -443,7 +443,7 @@ inline unsigned grid_for(size_t n, unsigned bs) { return (unsigned)((n + bs - 1)
 }  // namespace
 
 // data[i] <- 1 / data[i] (num == nullptr) or num[i] / data[i]; enqueue only.  scratch: n elements.
-static void batch_inverse_enqueue(const fe* num, fe* data, fe* scratch, size_t n, cudaStream_t st) {
+void batch_inverse_enqueue(const fe* num, fe* data, fe* scratch, size_t n, cudaStream_t st) {
     if (num) B200_LAUNCH(k_block_inverse<true>, grid_for(n, kInvBlock), kInvThreads, 0, st)(num, data, scratch, n);
     else B200_LAUNCH(k_block_inverse<false>, grid_for(n, kInvBlock), kInvThreads, 0, st)(nullptr, data, scratch, n);
 }

@@ -197,6 +197,28 @@ int b200_plonk_prove(b200_ctx* ctx, const b200_pk* pk, const uint64_t* wires,
                      const uint64_t* pub_inputs, const uint64_t* blinders, b200_proof* proof,
                      uint64_t* link_poly, uint64_t* challenges);
 
+/* One witness of a batch: the arguments of b200_plonk_prove. */
+typedef struct {
+    const uint64_t* wires;      /* 5 x n, host or device pointer */
+    const uint64_t* pub_inputs; /* the key's num_inputs values */
+    const uint64_t* blinders;   /* 17, draw order as b200_plonk_prove */
+    b200_proof* proof;
+    uint64_t* link_poly;        /* may be NULL; (n + 2) x 4 limbs */
+    uint64_t* challenges;       /* may be NULL; beta gamma alpha zeta v u */
+} b200_prove_item;
+/* Proves k witnesses of ONE key together: every kernel launch covers all of them, every commitment round is one batched
+ * MSM over the same SRS bases, and the five host round trips (Fiat–Shamir between rounds) are made once per batch.
+ * Item i's proof, link_poly and challenges are byte-identical to b200_plonk_prove(ctx, pk, items[i].wires, ...).
+ * statuses (may be NULL) receives k codes: B200_OK, or B200_ERR_UNSATISFIED for a witness that does not satisfy the
+ * circuit (its proof is zeroed, its challenges are not written; every other item is still proved).  Returns B200_OK when
+ * every item was proved, B200_ERR_UNSATISFIED when any was not; a CUDA, memory or argument error fails the whole call
+ * (B200_ERR_INVALID for a NULL items pointer with k > 0, or an item with a NULL wires / blinders / proof pointer, or a NULL
+ * pub_inputs for a key with num_inputs > 0).  k = 0 is accepted.
+ * The batch runs in chunks of as many proofs as half the free device memory holds (about 100 MB per proof at n = 2^14,
+ * 400 MB at 2^16; at most 64); the results do not depend on the chunk size.  A batch runs eagerly (no CUDA graphs) in
+ * buffers of its own on the context, kept for the next batch: single proofs keep replaying their graphs. */
+int b200_plonk_prove_batch(b200_ctx* ctx, const b200_pk* pk, const b200_prove_item* items, size_t k, int* statuses);
+
 /* Flat link proof, field order of mpc-plonk `LinkingProof { quotient_commitment, opening_proof }`
  * (crates/relayer-types/types-proofs/src/mocks.rs:28-30). */
 typedef struct {
@@ -308,6 +330,12 @@ b200_ctx* b200_pool_ctx(b200_pool* pool, unsigned worker);
 int b200_pool_submit_prove(b200_pool* pool, const b200_pk* pk, const uint64_t* wires,
                            const uint64_t* pub_inputs, size_t num_inputs, const uint64_t* blinders,
                            b200_proof* proof, uint64_t* link_poly, uint64_t* ticket);
+/* Queue one `b200_plonk_prove_batch(ctx_of_some_worker, pk, items, k, statuses)` as ONE job on one worker.  The items'
+ * pub_inputs and blinders are copied at submit (the items array too); wires, the proof / link_poly / challenges buffers
+ * and statuses (may be NULL) stay owned by the caller until the ticket has been waited for.  The ticket's status is the
+ * call's: B200_ERR_UNSATISFIED when any item was not proved (see statuses). */
+int b200_pool_submit_prove_batch(b200_pool* pool, const b200_pk* pk, const b200_prove_item* items, size_t k, int* statuses,
+                                 uint64_t* ticket);
 /* Queue one `b200_plonk_link(...)` (the reference forks its link proofs the same way:
  * native_proof_manager.rs:726-782). */
 int b200_pool_submit_link(b200_pool* pool, const b200_bases* srs, const uint64_t* a1, size_t len1,

@@ -16,6 +16,7 @@ from __future__ import annotations
 
 import ctypes as C
 from dataclasses import dataclass
+from typing import Any
 
 import numpy as np
 
@@ -508,6 +509,77 @@ class PlonkKzgSnark:
         return (proof, hint, ch) if want_challenges else (proof, hint)
 
 
+    @staticmethod
+    def prove_batch(ctx: Context, pk: ProvingKey, wires_list, pub_inputs_list, blinders_list, link_hints: bool = False,
+                    want_challenges: bool = False):
+        """Proves k witnesses of one key in ONE call (`b200_plonk_prove_batch`): every launch covers all k proofs and every
+        commitment round is one batched MSM.  wires_list[i]: a 5 x n wire table (array) or the address of one in device or
+        pinned host memory (int); pub_inputs_list[i], blinders_list[i]: as for `prove_with_link_hint`.  Returns
+        (proofs, hints, statuses[, challenges]): item i's proof, hint and challenges equal `prove_with_link_hint` of the same
+        arguments; statuses[i] is 0, or -7 (B200_ERR_UNSATISFIED) for a witness that does not satisfy the circuit, whose
+        proof is zeroed and whose hint is None (hints is None without link_hints).  Argument errors raise ValueError before
+        any device work; other failures raise B200Error."""
+        items, keep = _prove_items(pk, wires_list, pub_inputs_list, blinders_list, link_hints, want_challenges)
+        k = len(keep)
+        statuses = (C.c_int * max(1, k))()
+        rc = ctx._lib.b200_plonk_prove_batch(ctx._h, pk._h, items, k, statuses)
+        if rc not in (0, -7):
+            _lib.check(rc)
+        return _batch_results(keep, statuses, link_hints, want_challenges)
+
+
+class B200ProveItem(C.Structure):
+    """b200_prove_item: one witness of a batch."""
+    _fields_ = [("wires", C.c_void_p), ("pub_inputs", C.c_void_p), ("blinders", C.c_void_p), ("proof", C.c_void_p),
+                ("link_poly", C.c_void_p), ("challenges", C.c_void_p)]
+
+
+def _prove_items(pk: ProvingKey, wires_list, pub_inputs_list, blinders_list, link_hints: bool, want_challenges: bool):
+    """Checks a batch's arguments (ValueError) and builds its b200_prove_item array.  Returns (items, keep): keep[i] holds
+    the arrays item i points into, and its outputs (proof, link polynomial, challenges)."""
+    wires_list, pub_inputs_list, blinders_list = list(wires_list), list(pub_inputs_list), list(blinders_list)
+    k = len(wires_list)
+    if len(pub_inputs_list) != k or len(blinders_list) != k:
+        raise ValueError(f"prove_batch: {k} wire tables, {len(pub_inputs_list)} public-input vectors and "
+                         f"{len(blinders_list)} blinder vectors: one of each per witness")
+    n = pk.domain_size
+    items = (B200ProveItem * max(1, k))()
+    keep = []
+    for i, (wires, pub_inputs, blinders) in enumerate(zip(wires_list, pub_inputs_list, blinders_list)):
+        if isinstance(wires, (int, np.integer)):
+            w, w_ptr = None, C.c_void_p(int(wires))
+        else:
+            w = np.ascontiguousarray(wires, dtype=np.uint64)
+            if w.size != 5 * n * 4:
+                raise ValueError(f"prove_batch: wire table {i} has {w.size // 4} elements, the key needs 5 x {n}")
+            w_ptr = _ptr(w)
+        pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64).reshape(-1, 4)
+        if pi.shape[0] != pk.num_inputs:
+            raise ValueError(f"prove_batch: item {i} has {pi.shape[0]} public inputs, the key takes {pk.num_inputs}")
+        bl = np.ascontiguousarray(blinders, dtype=np.uint64)
+        if bl.size != 17 * 4:
+            raise ValueError(f"prove_batch: item {i} has {bl.size // 4} blinders, the prover draws 17")
+        proof = B200Proof()
+        link = np.zeros((n + 2, 4), dtype=np.uint64) if link_hints else None
+        ch = np.zeros((6, 4), dtype=np.uint64) if want_challenges else None
+        items[i] = B200ProveItem(w_ptr, _ptr(pi) if pi.size else None, _ptr(bl), C.cast(C.pointer(proof), C.c_void_p),
+                                 _ptr(link) if link is not None else None, _ptr(ch) if ch is not None else None)
+        keep.append((w, pi, bl, proof, link, ch))
+    return items, keep
+
+
+def _batch_results(keep, statuses, link_hints: bool, want_challenges: bool):
+    proofs = [x[3] for x in keep]
+    st = [int(statuses[i]) for i in range(len(keep))]
+    hints = None
+    if link_hints:
+        hints = [LinkingHint(linking_wire_poly=x[4], linking_wire_comm=np.array(x[3].wires_poly_comms[0], dtype=np.uint64))
+                 if s == 0 else None for x, s in zip(keep, st)]
+    if want_challenges:
+        return proofs, hints, st, [x[5] for x in keep]
+    return proofs, hints, st
+
+
 def keccak256(data: bytes) -> bytes:
     out = (C.c_uint8 * 32)()
     _lib.load().b200_keccak256(data, len(data), out)
@@ -623,6 +695,14 @@ class BundleLink(C.Structure):
                 ("proof", C.c_void_p)]
 
 
+@dataclass
+class _PoolBatch:
+    """What a queued batch job writes into: its items' arrays and outputs, and the statuses."""
+    held: list
+    statuses: Any
+    link_hints: bool
+
+
 class ProverPool:
     """b200_pool: the device-side counterpart of the reference's `NativeProofManager` thread pool
     (crates/workers/proof-manager/src/implementations/native_proof_manager.rs:138-201, `spawn_fifo`
@@ -672,6 +752,18 @@ class ProverPool:
                                                     pi.size // 4, _ptr(bl), C.byref(proof),
                                                     _ptr(link) if link is not None else None, C.byref(ticket)))
         self._keep[ticket.value] = (proof, link, keep, pk)
+        return ticket.value
+
+    def submit_prove_batch(self, pk: "ProvingKey", wires_list, pub_inputs_list, blinders_list, link_hints: bool = False,
+                           keep=None) -> int:
+        """Queue one `b200_plonk_prove_batch` as a single job on one worker; returns the ticket.  Arguments as for
+        `PlonkKzgSnark.prove_batch`; wire tables given by address stay owned by the caller until `wait(ticket)` returns
+        (pass their owners as `keep`).  `wait(ticket)` returns (proofs, hints, statuses) like `prove_batch`."""
+        items, held = _prove_items(pk, wires_list, pub_inputs_list, blinders_list, link_hints, False)
+        statuses = (C.c_int * max(1, len(held)))()
+        ticket = C.c_uint64()
+        _lib.check(self._lib.b200_pool_submit_prove_batch(self._h, pk._h, items, len(held), statuses, C.byref(ticket)))
+        self._keep[ticket.value] = (_PoolBatch(held, statuses, link_hints), None, (items, keep), pk)
         return ticket.value
 
     def submit_link(self, srs: "Bases", hint_a: "LinkingHint", hint_b: "LinkingHint", layout: "GroupLayout") -> int:
@@ -726,6 +818,10 @@ class ProverPool:
         job's own status and message if it failed."""
         rc = self._lib.b200_pool_wait(self._h, ticket)
         proof, link, _, _ = self._keep.pop(ticket, (None, None, None, None))
+        if isinstance(proof, _PoolBatch):  # a batch job: unsatisfied items are reported in its statuses
+            if rc not in (0, -7):
+                _lib.check(rc)
+            return _batch_results(proof.held, proof.statuses, proof.link_hints, False)
         _lib.check(rc)
         return (proof, link) if link is not None else proof
 

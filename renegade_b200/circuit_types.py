@@ -4,6 +4,7 @@ circuits-core/src/lib.rs:112-142, so that callers (and the parity tests) read li
 
     proof          = singleprover_prove(ValidBalanceCreate, witness, statement)
     proof, hint    = singleprover_prove_with_hint(C, witness, statement)
+    proofs         = singleprover_prove_batch(C, [(witness, statement), ...])   # one batch call on the device
     verify_singleprover_proof(C, statement, proof)         # raises VerifierError
     singleprover_prove_and_verify(C, witness, statement)
 
@@ -26,7 +27,7 @@ from __future__ import annotations
 import os
 import threading
 from dataclasses import dataclass
-from typing import Any, Dict, Optional, Tuple
+from typing import Any, Dict, List, Optional, Tuple
 
 import numpy as np
 
@@ -195,6 +196,50 @@ class SingleProverCircuit:
 
     @classmethod
     def prove_with_link_hint(cls, witness, statement, rng=None) -> Tuple[PlonkProof, ProofLinkingHint]:
+        pk, circ = cls._arithmetize(witness, statement)
+        srs = system_srs()
+        try:
+            if srs.pool is None:
+                return PlonkKzgSnark.prove_with_link_hint(srs.ctx, pk, circ.wires, circ.pub_inputs, draw_blinders(rng))
+            wires = np.ascontiguousarray(circ.wires, dtype=np.uint64)
+            tk = srs.pool.submit_prove(pk, wires.ctypes.data, circ.pub_inputs, draw_blinders(rng), with_link_poly=True,
+                                       keep=wires)
+            proof, link = srs.pool.wait(tk)
+            return proof, LinkingHint(linking_wire_poly=link,
+                                      linking_wire_comm=np.array(proof.wires_poly_comms[0], dtype=np.uint64))
+        except _lib.B200Error as e:  # WrongQuotientPolyDegree et al.
+            raise ProverError("Plonk", e) from e
+
+    @classmethod
+    def prove_batch_with_link_hint(cls, instances, rng=None) -> List[Tuple[PlonkProof, ProofLinkingHint]]:
+        """Many (witness, statement) pairs of this circuit: each is synthesised on the host, then ONE batch call
+        (`PlonkKzgSnark.prove_batch`, or one pool job when the SRS has a pool) proves them all.  Raises ProverError naming
+        the indices whose witness does not satisfy the circuit."""
+        instances = list(instances)
+        if not instances:
+            return []
+        arith = [cls._arithmetize(w, s) for w, s in instances]
+        pk = arith[0][0]
+        wires = [np.ascontiguousarray(c.wires, dtype=np.uint64) for _, c in arith]
+        pis = [c.pub_inputs for _, c in arith]
+        blinders = [draw_blinders(rng) for _ in arith]
+        srs = system_srs()
+        try:
+            if srs.pool is None:
+                proofs, hints, statuses = PlonkKzgSnark.prove_batch(srs.ctx, pk, wires, pis, blinders, link_hints=True)
+            else:
+                tk = srs.pool.submit_prove_batch(pk, wires, pis, blinders, link_hints=True)
+                proofs, hints, statuses = srs.pool.wait(tk)
+        except _lib.B200Error as e:
+            raise ProverError("Plonk", e) from e
+        bad = [i for i, st in enumerate(statuses) if st != 0]
+        if bad:
+            raise ProverError("Plonk", f"WrongQuotientPolyDegree at indices {bad}")
+        return list(zip(proofs, hints))
+
+    @classmethod
+    def _arithmetize(cls, witness, statement):
+        """The proving key and the witness's arithmetized tables (synthesis on the host), shape-checked against the key."""
         pk = cls.proving_key()
         keyed = _CIRCUIT_STRUCTURE.get(cls.name(), 0)
         try:
@@ -214,18 +259,7 @@ class SingleProverCircuit:
         if keyed and getattr(circ, "structure_digest", 0) and circ.structure_digest != keyed:
             raise ProverError("Circuit", f"{cls.name()}: the instance's gates / wiring differ from the circuit its key was "
                                          "preprocessed from (synthesis must be witness-independent)")
-        srs = system_srs()
-        try:
-            if srs.pool is None:
-                return PlonkKzgSnark.prove_with_link_hint(srs.ctx, pk, circ.wires, circ.pub_inputs, draw_blinders(rng))
-            wires = np.ascontiguousarray(circ.wires, dtype=np.uint64)
-            tk = srs.pool.submit_prove(pk, wires.ctypes.data, circ.pub_inputs, draw_blinders(rng), with_link_poly=True,
-                                       keep=wires)
-            proof, link = srs.pool.wait(tk)
-            return proof, LinkingHint(linking_wire_poly=link,
-                                      linking_wire_comm=np.array(proof.wires_poly_comms[0], dtype=np.uint64))
-        except _lib.B200Error as e:  # WrongQuotientPolyDegree et al.
-            raise ProverError("Plonk", e) from e
+        return pk, circ
 
     @classmethod
     def verify(cls, statement, proof: PlonkProof) -> None:
@@ -245,6 +279,16 @@ def singleprover_prove(circuit: type, witness, statement, rng=None) -> PlonkProo
 
 def singleprover_prove_with_hint(circuit: type, witness, statement, rng=None) -> Tuple[PlonkProof, ProofLinkingHint]:
     return circuit.prove_with_link_hint(witness, statement, rng)
+
+
+def singleprover_prove_batch(circuit: type, instances, rng=None) -> List[PlonkProof]:
+    """`singleprover_prove` for many (witness, statement) pairs of one circuit in ONE batch call on the device; raises
+    ProverError naming the indices whose witness does not satisfy the circuit."""
+    return [p for p, _ in circuit.prove_batch_with_link_hint(instances, rng)]
+
+
+def singleprover_prove_batch_with_hint(circuit: type, instances, rng=None) -> List[Tuple[PlonkProof, ProofLinkingHint]]:
+    return circuit.prove_batch_with_link_hint(instances, rng)
 
 
 def verify_singleprover_proof(circuit: type, statement, proof: PlonkProof) -> None:

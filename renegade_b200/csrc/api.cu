@@ -192,6 +192,9 @@ int b200_init(int device, b200_ctx** out) {
     ctx->c.heavy_plonk = prio && !(pe && pe[0] == '1');  // B200_STREAM_PRIORITIES=1: accumulation only
     ctx->c.msm.hv_fork = ctx->c.hv_fork;
     ctx->c.msm.hv_join = ctx->c.hv_join;
+    ctx->c.batch.msm.hv_stream = ctx->c.heavy;
+    ctx->c.batch.msm.hv_fork = ctx->c.hv_fork;
+    ctx->c.batch.msm.hv_join = ctx->c.hv_join;
     *out = ctx;
     return B200_OK;
     B200_CATCH

@@ -234,6 +234,13 @@ struct Context {
     int use_graphs = -1;  // 1 / 0: replay prover rounds as CUDA graphs or not; -1: B200_GRAPHS from the environment (default on)
     std::vector<ProofGraphSet*> graph_sets;
     uint64_t graph_clock = 0;
+    // b200_plonk_prove_batch's own workspace, NTT scratch, parameter blocks and MSM scratch: a batch never grows (moves) the
+    // buffers above, which the single prover's captured graphs refer to
+    struct BatchBufs {
+        DevBuf ws, nscr, nscr2, d_params;
+        HostPinned h_small, h_params;
+        MsmScratch msm;
+    } batch;
     ~Context();
 };
 

@@ -117,36 +117,44 @@ __global__ void __launch_bounds__(kInvThreads) k_block_inverse(const fe* __restr
 // `dyn`: a pointer into the context's device copy of ProofParams, so that the kernel ARGUMENTS are the same for every
 // proof of a key and a round can be replayed as a CUDA graph.  dyn == nullptr: the by-value fields are used (link
 // proofs, the stand-alone polynomial entry points).
+// A batch of k proofs of one key runs every launch once over all k: the proof index is a grid index (blockIdx.y, or
+// the first free one), each proof's data sits `*stride` elements after the previous proof's, and its scalars are the
+// next ProofParams of the array (`dstride` = sizeof(ProofParams) in elements).  A single proof is the k = 1 case.
 struct BlindArgs {
     fe b[3];
     int count;
     const fe* dyn;
 };
-// poly += (b0 + b1 X + ...) * (X^n - 1)
-__global__ void k_blind(fe* poly, size_t n, BlindArgs a) {
+// poly += (b0 + b1 X + ...) * (X^n - 1); block p: proof p
+__global__ void k_blind(fe* poly, size_t n, BlindArgs a, size_t pstride, size_t dstride) {
     const int i = threadIdx.x;
     if (i >= a.count) return;
-    const fe b = a.dyn ? fe_load_ro(a.dyn + i) : a.b[i];
+    poly += blockIdx.x * pstride;
+    const fe b = a.dyn ? fe_load_ro(a.dyn + blockIdx.x * dstride + i) : a.b[i];
     fe_store(poly + i, FSUB(fe_load(poly + i), b));
     fe_store(poly + n + i, FADD(fe_load(poly + n + i), b));
 }
 
-// the five wire polynomials in one launch: thread (i, t) adds blinder t of wire i
-__global__ void k_blind_wires(fe* wpoly, size_t stride, size_t n, const fe* __restrict__ dyn /* [NW][2] */) {
+// the five wire polynomials in one launch: thread (i, t) adds blinder t of wire i; block p: proof p
+__global__ void k_blind_wires(fe* wpoly, size_t stride, size_t n, const fe* __restrict__ dyn /* [NW][2] */, size_t dstride) {
     const int i = threadIdx.x >> 1, t = threadIdx.x & 1;
     if (i >= NW) return;
-    fe* poly = wpoly + (size_t)i * stride;
-    const fe b = fe_load_ro(dyn + 2 * i + t);
+    fe* poly = wpoly + ((size_t)blockIdx.x * NW + i) * stride;
+    const fe b = fe_load_ro(dyn + blockIdx.x * dstride + 2 * i + t);
     fe_store(poly + t, FSUB(fe_load(poly + t), b));
     fe_store(poly + n + t, FADD(fe_load(poly + n + t), b));
 }
 
-// per row j: num = prod_i (w_ij + beta k_i w^j + gamma), den = prod_i (w_ij + beta sigma_ij + gamma)
+// per row j: num = prod_i (w_ij + beta k_i w^j + gamma), den = prod_i (w_ij + beta sigma_ij + gamma); blockIdx.y: proof
 __global__ void k_perm_num_den(const fe* __restrict__ wires, const fe* __restrict__ sig_evals,
-                               const fe* __restrict__ dom, KArr k, const fe* __restrict__ beta_gamma, size_t n,
+                               const fe* __restrict__ dom, KArr k, const fe* __restrict__ beta_gamma, size_t dstride, size_t n,
                                fe* __restrict__ num, fe* __restrict__ den) {
     const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= n) return;
+    wires += (size_t)blockIdx.y * NW * n;
+    beta_gamma += blockIdx.y * dstride;
+    num += (size_t)blockIdx.y * n;
+    den += (size_t)blockIdx.y * n;
     const fe beta = fe_load_ro(beta_gamma), gamma = fe_load_ro(beta_gamma + 1);
     const fe bw = FMUL(beta, fe_load_ro(dom + j));
     fe a = fe_one<Fr>(), b = fe_one<Fr>();
@@ -160,12 +168,15 @@ __global__ void k_perm_num_den(const fe* __restrict__ wires, const fe* __restric
     fe_store(den + j, b);
 }
 
-// exclusive multiplicative scan, chunked: data[j] <- prod_{i<j} data[i]
-__global__ void k_scan_mul_local(fe* __restrict__ data, size_t n, fe* __restrict__ totals) {
+// segmented exclusive multiplicative scan, chunked: data[j] <- product of the elements before j in its segment of `seg`.
+// A chunk never straddles two segments: thread t runs chunk t % cps of segment t / cps (cps = chunks per segment), so
+// the chunk totals are again `cps`-long segments, one per proof.
+__global__ void k_scan_mul_local(fe* __restrict__ data, size_t seg, size_t cps, size_t n_chunks, fe* __restrict__ totals) {
     const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const size_t beg = t * CH;
-    if (beg >= n) return;
-    const size_t end = beg + CH < n ? beg + CH : n;
+    if (t >= n_chunks) return;
+    const size_t s = t / cps;
+    const size_t beg = s * seg + (t - s * cps) * CH, seg_end = (s + 1) * seg;
+    const size_t end = beg + CH < seg_end ? beg + CH : seg_end;
     fe run = fe_one<Fr>();
     for (size_t i = beg; i < end; ++i) {
         const fe v = fe_load(data + i);
@@ -174,60 +185,73 @@ __global__ void k_scan_mul_local(fe* __restrict__ data, size_t n, fe* __restrict
     }
     fe_store(totals + t, run);
 }
-__global__ void k_scan_mul_apply(fe* __restrict__ data, size_t n, const fe* __restrict__ offs) {
+__global__ void k_scan_mul_apply(fe* __restrict__ data, size_t seg, size_t total, size_t cps, const fe* __restrict__ offs) {
     const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n || j < CH) return;  // the first chunk's offset is 1
-    fe_store(data + j, FMUL(fe_load(data + j), fe_load_ro(offs + j / CH)));
+    if (j >= total) return;
+    const size_t s = j / seg, jl = j - s * seg;
+    if (jl < CH) return;  // the first chunk's offset is 1
+    fe_store(data + j, FMUL(fe_load(data + j), fe_load_ro(offs + s * cps + jl / CH)));
 }
 
 // ---- Horner suffix scan: S[j] = sum_{i >= j} p[i] z^(i-j) -------------------------------------------
 // S[0] = p(z) (evaluation) and S[1..] are the coefficients of p(X) / (X - z) (synthetic division).
-__global__ void k_horner_local(const fe* __restrict__ p, size_t len, fe z_val, const fe* __restrict__ z_dyn, fe* __restrict__ S,
-                               fe* __restrict__ H) {
+// Batches (blockIdx.y = proof): the strides of HornerStrides below; H holds [proof][chunk].
+__global__ void k_horner_local(const fe* __restrict__ p, size_t pstride, size_t len, fe z_val, const fe* __restrict__ z_dyn,
+                               size_t dstride, fe* __restrict__ S, size_t sstride, fe* __restrict__ H) {
     const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const size_t beg = t * CH;
     if (beg >= len) return;
     const size_t end = beg + CH < len ? beg + CH : len;
-    const fe z = z_dyn ? fe_load_ro(z_dyn) : z_val;
+    const size_t q = blockIdx.y;
+    p += q * pstride;
+    if (S) S += q * sstride;
+    const fe z = z_dyn ? fe_load_ro(z_dyn + q * dstride) : z_val;
     fe run = fe_zero();
     for (size_t i = end; i-- > beg;) {
         run = FADD(FMUL(run, z), fe_load_ro(p + i));
         if (S) fe_store(S + i, run);
     }
-    fe_store(H + t, run);
+    fe_store(H + q * ((len + CH - 1) / CH) + t, run);
 }
-// batched evaluation-only variant: blockIdx.y selects the polynomial
+// batched evaluation-only variant: blockIdx.y selects the polynomial, blockIdx.z the proof
 constexpr int kMaxEval = 10;
 struct EvalArgs {
     const fe* p[kMaxEval];
+    size_t pstride[kMaxEval];  // proof y's polynomial q: p[q] + y * pstride[q]
     fe* H[kMaxEval];
+    size_t hstride;            // proof y's outputs: H[q] + y * hstride
     fe z[kMaxEval];
     uint32_t len[kMaxEval];
-    const fe* dyn;  // z[] of this level in device memory, or null
+    const fe* dyn;   // z[] of this level in device memory, or null
+    size_t dstride;  // proof y's z[]: dyn + y * dstride
 };
 __global__ void k_horner_local_batch(EvalArgs a) {
     const int q = blockIdx.y;
+    const size_t y = blockIdx.z;
     const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const size_t beg = t * CH, len = a.len[q];
     if (beg >= len) return;
     const size_t end = beg + CH < len ? beg + CH : len;
-    const fe z = a.dyn ? fe_load_ro(a.dyn + q) : a.z[q];
-    const fe* p = a.p[q];
+    const fe z = a.dyn ? fe_load_ro(a.dyn + y * a.dstride + q) : a.z[q];
+    const fe* p = a.p[q] + y * a.pstride[q];
     fe run = fe_zero();
     for (size_t i = end; i-- > beg;) run = FADD(FMUL(run, z), fe_load_ro(p + i));
-    fe_store(a.H[q] + t, run);
+    fe_store(a.H[q] + y * a.hstride + t, run);
 }
-// S[j] += z^(chunk_end - j) * T[chunk + 1], one thread per element; zpow[e] = z^e for e = 1..CH
+// S[j] += z^(chunk_end - j) * T[chunk + 1], one thread per element; zpow[e] = z^e for e = 1..CH; blockIdx.y: proof
 struct ZPow {
     fe v[CH + 1];
 };
-__global__ void k_horner_apply(fe* __restrict__ S, size_t len, ZPow zp, const fe* __restrict__ zp_dyn, const fe* __restrict__ T,
-                               size_t n_chunks) {
+__global__ void k_horner_apply(fe* __restrict__ S, size_t sstride, size_t len, ZPow zp, const fe* __restrict__ zp_dyn,
+                               size_t dstride, const fe* __restrict__ T, size_t n_chunks) {
     const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const size_t t = j / CH;
     if (j >= len || t + 1 >= n_chunks) return;  // the last chunk has no carry
+    const size_t q = blockIdx.y;
+    S += q * sstride;
+    T += q * n_chunks;
     const size_t e = (t + 1) * CH - j;
-    const fe ze = zp_dyn ? fe_load_ro(zp_dyn + e) : zp.v[e];
+    const fe ze = zp_dyn ? fe_load_ro(zp_dyn + q * dstride + e) : zp.v[e];
     fe_store(S + j, FADD(fe_load(S + j), FMUL(ze, fe_load_ro(T + t + 1))));
 }
 
@@ -261,11 +285,13 @@ constexpr int kMaxCosets = 8;
 struct CombineArgs {
     fe minv[kMaxCosets * kMaxCosets];  // inverse of the Vandermonde matrix V[j][k] = c_j^k, row-major [k][j]
 };
-// in place: q[j * n + i] holds (n^-1-scaled) coefficient i of u_j(s_j X); afterwards q[k * n + i] = t_k[i]
+// in place: q[j * n + i] holds (n^-1-scaled) coefficient i of u_j(s_j X); afterwards q[k * n + i] = t_k[i];
+// blockIdx.y: proof (NC * n elements each)
 template <int NC>
 __global__ void k_coset_combine(fe* __restrict__ q, size_t n, const fe* __restrict__ cscale_inv, CombineArgs a) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    q += (size_t)blockIdx.y * NC * n;
     fe u[NC];
 #pragma unroll
     for (int j = 0; j < NC; ++j) u[j] = FMUL(fe_load(q + (size_t)j * n + i), fe_load_ro(cscale_inv + (size_t)j * n + i));
@@ -281,29 +307,35 @@ __global__ void k_coset_combine(fe* __restrict__ q, size_t n, const fe* __restri
 struct QuotArgs {
     const fe* sel;   // 13 x m resident coset evaluations
     const fe* sig;   // 5 x m
-    const fe* ext;   // 7 x m: wires 0..4, public-input polynomial, z
+    const fe* ext;   // per proof NW x m: wires 0..4
+    const fe* pi;    // per proof m: public-input polynomial
+    const fe* zext;  // per proof m: z
     const fe* pts;   // m evaluation points s_j * w_n^h
     const fe* l1_inv;  // 1 / (n (x_i - 1))
-    fe* out;
+    fe* out;         // per proof m
     size_t m;        // nc * n
     unsigned log_n;
     KArr k;
     const fe* chal;  // device: beta, gamma, alpha, alpha^2
+    size_t dstride;  // next proof's chal[]
     fe zh_inv[8];    // 1 / (c_j - 1)
 };
 // k_quotient chains ~60 field products; fully unrolled it is ~180 KB of code and starves on the
 // instruction cache ("no instruction" stalls; an out-of-line multiplier was slower still, through
-// stack traffic).  The per-wire loops are therefore kept rolled.
+// stack traffic).  The per-wire loops are therefore kept rolled.  blockIdx.y: proof.
 __global__ void __launch_bounds__(128) k_quotient(QuotArgs a) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.m) return;
-    const size_t m = a.m;
-    const fe beta = fe_load_ro(a.chal), gamma = fe_load_ro(a.chal + 1);
+    const size_t m = a.m, pr = blockIdx.y;
+    const fe* ext = a.ext + pr * NW * m;
+    const fe* zext = a.zext + pr * m;
+    const fe* chal = a.chal + pr * a.dstride;
+    const fe beta = fe_load_ro(chal), gamma = fe_load_ro(chal + 1);
     fe w[NW];
 #pragma unroll
-    for (int j = 0; j < NW; ++j) w[j] = fe_load_ro(a.ext + j * m + i);
+    for (int j = 0; j < NW; ++j) w[j] = fe_load_ro(ext + j * m + i);
     // gate: q_c + pi + sum q_lc w + q_mul0 w0 w1 + q_mul1 w2 w3 + q_ecc w0..w4 + sum q_hash w^5 - q_o w4
-    fe acc = FADD(fe_load_ro(a.sel + 11 * m + i), fe_load_ro(a.ext + 5 * m + i));
+    fe acc = FADD(fe_load_ro(a.sel + 11 * m + i), fe_load_ro(a.pi + pr * m + i));
 #pragma unroll 1
     for (int j = 0; j < 4; ++j) {
         acc = FADD(acc, FMUL(fe_load_ro(a.sel + j * m + i), w[j]));
@@ -316,9 +348,9 @@ __global__ void __launch_bounds__(128) k_quotient(QuotArgs a) {
     acc = FADD(acc, FMUL(fe_load_ro(a.sel + 12 * m + i), FMUL(FMUL(w01, w23), w[4])));
     acc = FSUB(acc, FMUL(fe_load_ro(a.sel + 10 * m + i), w[4]));
     // permutation: alpha * ( z prod(w + beta k x + gamma) - z(wx) prod(w + beta sigma + gamma) )
-    const fe zx = fe_load_ro(a.ext + 6 * m + i);
+    const fe zx = fe_load_ro(zext + i);
     const size_t nmask = ((size_t)1 << a.log_n) - 1;
-    const fe zxw = fe_load_ro(a.ext + 6 * m + ((i & ~nmask) | ((i + 1) & nmask)));  // z(w x): next point of the same coset
+    const fe zxw = fe_load_ro(zext + ((i & ~nmask) | ((i + 1) & nmask)));  // z(w x): next point of the same coset
     const fe bx = FMUL(beta, fe_load_ro(a.pts + i));
     fe p1 = zx, p2 = zxw;
 #pragma unroll 1
@@ -327,17 +359,20 @@ __global__ void __launch_bounds__(128) k_quotient(QuotArgs a) {
         p1 = FMUL(p1, FADD(t, FMUL(a.k.v[j], bx)));
         p2 = FMUL(p2, FADD(t, FMUL(beta, fe_load_ro(a.sig + j * m + i))));
     }
-    acc = FADD(acc, FMUL(fe_load_ro(a.chal + 2), FSUB(p1, p2)));
+    acc = FADD(acc, FMUL(fe_load_ro(chal + 2), FSUB(p1, p2)));
     acc = FMUL(acc, a.zh_inv[i >> a.log_n]);
     // alpha^2 (z - 1) L1(x) / Z_H(x)
-    acc = FADD(acc, FMUL(FMUL(fe_load_ro(a.chal + 3), FSUB(zx, fe_one<Fr>())), fe_load_ro(a.l1_inv + i)));
-    fe_store(a.out + i, acc);
+    acc = FADD(acc, FMUL(FMUL(fe_load_ro(chal + 3), FSUB(zx, fe_one<Fr>())), fe_load_ro(a.l1_inv + i)));
+    fe_store(a.out + pr * m + i, acc);
 }
 
-// flag bit 0: a coefficient above `deg` is non-zero; bit 1: coefficient `deg` is zero
+// flag bit 0: a coefficient above `deg` is non-zero; bit 1: coefficient `deg` is zero; blockIdx.y: proof (its m
+// coefficients and its own flag)
 __global__ void k_check_degree(const fe* __restrict__ q, size_t deg, size_t m, uint32_t* flag) {
     const size_t i = deg + (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m) return;
+    q += (size_t)blockIdx.y * m;
+    flag += blockIdx.y;
     const bool zero = fe_is_zero(fe_load_ro(q + i));
     if (i == deg) {
         if (zero) atomicOr(flag, 2u);
@@ -383,12 +418,15 @@ __global__ void k_fr_vec_op(int op, const fe* __restrict__ a, const fe* __restri
 }
 
 
-// t_i = quot[i(n+2) .. ) - b_{i-1} + b_i X^(n+2)   (the last chunk has n coefficients)
-__global__ void k_split_quotient(const fe* __restrict__ quot, size_t n, size_t stride, const fe* __restrict__ dyn /* b[4] */,
-                                 fe* __restrict__ out) {
+// t_i = quot[i(n+2) .. ) - b_{i-1} + b_i X^(n+2)   (the last chunk has n coefficients); blockIdx.z: proof
+__global__ void k_split_quotient(const fe* __restrict__ quot, size_t qstride, size_t n, size_t stride,
+                                 const fe* __restrict__ dyn /* b[4] */, size_t dstride, fe* __restrict__ out) {
     const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int i = blockIdx.y;
     if (j >= n + 3) return;
+    quot += blockIdx.z * qstride;
+    dyn += blockIdx.z * dstride;
+    out += (size_t)blockIdx.z * NW * stride;
     const size_t len = i < NW - 1 ? n + 2 : n;
     fe v = j < len ? fe_load_ro(quot + (size_t)i * (n + 2) + j) : fe_zero();
     if (j == 0 && i > 0) v = FSUB(v, fe_load_ro(dyn + i - 1));
@@ -400,18 +438,23 @@ __global__ void k_split_quotient(const fe* __restrict__ quot, size_t n, size_t s
 constexpr int kMaxLin = 32;
 struct LinArgs {
     const fe* p[kMaxLin];
+    uint32_t pstride[kMaxLin];  // proof y's term t: p[t] + y * pstride[t] (0: a polynomial of the key)
     uint32_t len[kMaxLin];
     fe s[kMaxLin];
     int count;
     const fe* dyn;  // s[] in device memory, or null
+    size_t dstride; // proof y's s[]: dyn + y * dstride
 };
-__global__ void k_lincomb(LinArgs a, size_t out_len, fe* __restrict__ out) {
+// blockIdx.y: proof (output `ostride` apart)
+__global__ void k_lincomb(LinArgs a, size_t out_len, fe* __restrict__ out, size_t ostride) {
     const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= out_len) return;
+    const size_t y = blockIdx.y;
     fe acc = fe_zero();
     for (int t = 0; t < a.count; ++t)
-        if (j < a.len[t]) acc = FADD(acc, FMUL(a.dyn ? fe_load_ro(a.dyn + t) : a.s[t], fe_load_ro(a.p[t] + j)));
-    fe_store(out + j, acc);
+        if (j < a.len[t])
+            acc = FADD(acc, FMUL(a.dyn ? fe_load_ro(a.dyn + y * a.dstride + t) : a.s[t], fe_load_ro(a.p[t] + y * a.pstride[t] + j)));
+    fe_store(out + y * ostride + j, acc);
 }
 
 // ---- per-proof scalars ------------------------------------------------------------------------------------
@@ -540,57 +583,72 @@ struct HeavyScope {
     }
 };
 
-// exclusive product scan of `data[0..n)` in place; scratch >= n/CH + n/CH^2 + 2*CH + 8 elements
-static void scan_mul_exclusive(fe* data, size_t n, fe* scratch, cudaStream_t st) {
-    if (n <= 1) {
-        // data[0] <- 1 handled by the local kernel as well
-    }
-    const size_t n1 = (n + CH - 1) / CH;
-    B200_LAUNCH(k_scan_mul_local, grid_for(n1, 128), 128, 0, st)(data, n, scratch);
-    if (n1 > 1) {
-        scan_mul_exclusive(scratch, n1, scratch + n1, st);
-        B200_LAUNCH(k_scan_mul_apply, grid_for(n, 256), 256, 0, st)(data, n, scratch);
+// exclusive product scan of k segments of `seg` elements (data[0..k*seg)) in place, each segment on its own;
+// scratch >= k * (seg/CH + seg/CH^2 + 2*CH + 8) elements
+static void scan_mul_exclusive(fe* data, size_t seg, unsigned k, fe* scratch, cudaStream_t st) {
+    const size_t cps = (seg + CH - 1) / CH, n1 = cps * k;
+    B200_LAUNCH(k_scan_mul_local, grid_for(n1, 128), 128, 0, st)(data, seg, cps, n1, scratch);
+    if (cps > 1) {
+        scan_mul_exclusive(scratch, cps, k, scratch + n1, st);
+        B200_LAUNCH(k_scan_mul_apply, grid_for(seg * k, 256), 256, 0, st)(data, seg, seg * k, cps, scratch);
     }
 }
 
+// k Horner scans at once: proof q's polynomial is p + q * p, its suffix sums S + q * s, its p(z) out_total + q * out,
+// its point and powers dyn + q * dyn (elements)
+struct HornerStrides {
+    unsigned k = 1;
+    size_t p = 0, s = 0, out = 0, dyn = 0;
+};
+
 // Horner suffix scan; S may be null (evaluation only).  The value p(z) ends up at out_total (device).
-// scratch >= 2 * (len/CH + len/CH^2 + 2*CH + 8) elements
+// scratch >= k * 2 * (len/CH + len/CH^2 + 2*CH + 8) elements
 // `dyn` (device, or null): the point and its powers per level come from there instead of `z` (see ProofParams).
 static void horner_suffix(const fe* p, size_t len, fe z, fe* S, fe* out_total, fe* scratch, cudaStream_t st,
-                          const OpenParams* dyn = nullptr, int level = 0) {
+                          const OpenParams* dyn = nullptr, HornerStrides b = {}, int level = 0) {
     const size_t n1 = (len + CH - 1) / CH;
-    fe* H = scratch;
-    fe* T = scratch + n1;
-    B200_LAUNCH(k_horner_local, grid_for(n1, 128), 128, 0, st)(p, len, z, dyn ? &dyn->z[level] : nullptr, S, H);
+    fe* H = scratch;           // [proof][n1]
+    fe* T = scratch + b.k * n1;
+    B200_LAUNCH(k_horner_local, dim3(grid_for(n1, 128), b.k), 128, 0, st)(p, b.p, len, z, dyn ? &dyn->z[level] : nullptr, b.dyn,
+                                                                          S, b.s, H);
     if (n1 == 1) {
-        cudaMemcpyAsync(out_total, H, sizeof(fe), cudaMemcpyDeviceToDevice, st);
+        if (b.k == 1) cudaMemcpyAsync(out_total, H, sizeof(fe), cudaMemcpyDeviceToDevice, st);
+        else cudaMemcpy2DAsync(out_total, b.out * sizeof(fe), H, sizeof(fe), sizeof(fe), b.k, cudaMemcpyDeviceToDevice, st);
         return;
     }
     const fe zc = dyn ? z : host_pow(z, CH);
-    horner_suffix(H, n1, zc, S ? T : nullptr, out_total, scratch + 2 * n1, st, dyn, level + 1);
+    HornerStrides next = b;
+    next.p = next.s = n1;
+    horner_suffix(H, n1, zc, S ? T : nullptr, out_total, scratch + 2 * b.k * n1, st, dyn, next, level + 1);
     if (S) {
         ZPow zp{};
         if (!dyn) {
             zp.v[0] = fe_one<Fr>();
             for (int e = 1; e <= CH; ++e) zp.v[e] = FMUL(zp.v[e - 1], z);
         }
-        B200_LAUNCH(k_horner_apply, grid_for(len, 256), 256, 0, st)(S, len, zp, dyn ? dyn->zp[level].v : nullptr, T, n1);
+        B200_LAUNCH(k_horner_apply, dim3(grid_for(len, 256), b.k), 256, 0, st)(S, b.s, len, zp, dyn ? dyn->zp[level].v : nullptr,
+                                                                               b.dyn, T, n1);
     }
 }
 
-// p_q(z_q) for up to kMaxEval polynomials, written to out[q];
-// scratch: count * (max_len/CH + max_len/CH^2 + 2*CH + 16)
-// `dyn_z` (device, or null): [level][kMaxEval] evaluation points, points[q]^(CH^level); `points` is unused then.
+// p_q(z_q) for up to kMaxEval polynomials, written to out[q], for k proofs at once: proof y's polynomial q is
+// polys[q] + y * pstrides[q] (pstrides may be null: one proof), its results go to out + y * ostride;
+// scratch: k * count * (max_len/CH + max_len/CH^2 + 2*CH + 16)
+// `dyn_z` (device, or null): [level][kMaxEval] evaluation points, points[q]^(CH^level), proof y's `dstride` elements
+// after proof 0's; `points` is unused then.
 static void eval_batch(const fe* const* polys, const size_t* lens, const fe* points, int count, fe* out, fe* scratch,
-                       cudaStream_t st, const fe (*dyn_z)[kMaxEval] = nullptr) {
+                       cudaStream_t st, const fe (*dyn_z)[kMaxEval] = nullptr, unsigned k = 1, const size_t* pstrides = nullptr,
+                       size_t ostride = 0, size_t dstride = 0) {
     EvalArgs a;
     size_t cur_len[kMaxEval], max_len = 0;
     for (int q = 0; q < count; ++q) {
         a.p[q] = polys[q];
+        a.pstride[q] = pstrides ? pstrides[q] : 0;
         a.z[q] = dyn_z ? fe_zero() : points[q];
         cur_len[q] = lens[q];
         max_len = lens[q] > max_len ? lens[q] : max_len;
     }
+    a.dstride = dstride;
     // two disjoint regions per polynomial (levels alternate A, B, A, ...): a level reads one and
     // writes the other
     const size_t region_a = max_len / CH + 2, region_b = max_len / CH / CH + CH + 2;
@@ -609,11 +667,13 @@ static void eval_batch(const fe* const* polys, const size_t* lens, const fe* poi
             // levels alternate between the two halves of each polynomial's scratch slice
             a.H[q] = last ? out + q : scratch + (size_t)q * per_poly + (level & 1 ? region_a : 0);
         }
+        a.hstride = last ? ostride : (size_t)count * per_poly;
         a.dyn = dyn_z ? &dyn_z[level][0] : nullptr;
-        B200_LAUNCH(k_horner_local_batch, dim3(grid_for(max_chunks, 64), count), 64, 0, st)(a);
+        B200_LAUNCH(k_horner_local_batch, dim3(grid_for(max_chunks, 64), count, k), 64, 0, st)(a);
         if (last) break;
         for (int q = 0; q < count; ++q) {
             a.p[q] = a.H[q];
+            a.pstride[q] = a.hstride;
             if (!dyn_z) a.z[q] = host_pow(a.z[q], CH);
             cur_len[q] = (cur_len[q] + CH - 1) / CH;
         }
@@ -621,37 +681,45 @@ static void eval_batch(const fe* const* polys, const size_t* lens, const fe* poi
     }
 }
 
+// The prover's device workspace for k proofs: every region holds the k proofs' copies one after the other (proof p's
+// wire polynomials at wpoly + p * NW * S, its quotient at quot + p * m, ...), so that each step is one launch over
+// all k with a uniform stride.  pi_poly sits directly behind the k * NW wire polynomials, and in `ext` the k public-input
+// evaluations directly behind the wires': one batch of (NW + 1) k polynomials for the transforms, k * NW (no public
+// input) for the commitments.  With k = 1 this is the single prover's layout.
 struct Workspace {
-    fe *wires_ev, *wpoly, *pi_poly, *zpoly, *num, *den, *tmp, *scan, *ext, *quot, *split, *lin, *sdiv, *hscr, *escr, *evals;
-    uint32_t* flag;
+    fe *wires_ev, *wpoly, *pi_poly, *zpoly, *num, *den, *tmp, *scan, *ext, *zext, *quot, *split, *lin, *sdiv, *hscr, *escr, *evals;
+    uint32_t* flag;  // one per proof
     size_t S;  // stride of the (n + 3)-coefficient polynomials
 };
-static size_t workspace_elems(size_t n) {
+constexpr size_t kEvalSlots = 32;  // per proof in `evals`: the 2 NW evaluations, then the two opening totals at 16, 17
+static size_t workspace_elems(size_t n, unsigned k) {
     const size_t S = n + 4, m = 8 * n;
-    return NW * n + NW * S + S + S + 3 * n + (2 * (n / CH) + 4 * CH + 64) + 7 * m + m + NW * S + S + 2 * (S + 8) +
-           4 * (S / CH + 4 * CH + 64) + kMaxEval * (S / CH + S / CH / CH + 2 * CH + 16) + 32 + 8;
+    return k * (NW * n + NW * S + S + S + 3 * n + (2 * (n / CH) + 4 * CH + 64) + 7 * m + m + NW * S + S + 2 * (S + 8) +
+                4 * (S / CH + 4 * CH + 64) + kMaxEval * (S / CH + S / CH / CH + 2 * CH + 16) + kEvalSlots) +
+           (k + 7) / 8 + 8;
 }
-static Workspace carve(fe* base, size_t n) {
+static Workspace carve(fe* base, size_t n, unsigned k) {
     Workspace w;
     const size_t S = n + 4, m = 8 * n;
     w.S = S;
     fe* p = base;
-    w.wires_ev = p; p += NW * n;
-    w.wpoly = p; p += NW * S;
-    w.pi_poly = p; p += S;  // directly behind the wire polynomials: one batch of 6 for the coset evaluations
-    w.zpoly = p; p += S;
-    w.num = p; p += n;
-    w.den = p; p += n;
-    w.tmp = p; p += n;
-    w.scan = p; p += 2 * (n / CH) + 4 * CH + 64;  // all levels of the product scan: n / CH * (1 + 1/CH + ...)
-    w.ext = p; p += 7 * m;
-    w.quot = p; p += m;
-    w.split = p; p += NW * S;
-    w.lin = p; p += S;
-    w.sdiv = p; p += 2 * (S + 8);
-    w.hscr = p; p += 4 * (S / CH + 4 * CH + 64);
-    w.escr = p; p += kMaxEval * (S / CH + S / CH / CH + 2 * CH + 16);
-    w.evals = p; p += 32;
+    w.wires_ev = p; p += k * NW * n;
+    w.wpoly = p; p += k * NW * S;
+    w.pi_poly = p; p += k * S;
+    w.zpoly = p; p += k * S;
+    w.num = p; p += k * n;
+    w.den = p; p += k * n;
+    w.tmp = p; p += k * n;
+    w.scan = p; p += k * (2 * (n / CH) + 4 * CH + 64);  // all levels of the product scan: n / CH * (1 + 1/CH + ...)
+    w.ext = p; p += k * (NW + 1) * m;
+    w.zext = p; p += k * m;
+    w.quot = p; p += k * m;
+    w.split = p; p += k * NW * S;
+    w.lin = p; p += k * S;
+    w.sdiv = p; p += k * 2 * (S + 8);
+    w.hscr = p; p += k * 4 * (S / CH + 4 * CH + 64);
+    w.escr = p; p += k * kMaxEval * (S / CH + S / CH / CH + 2 * CH + 16);
+    w.evals = p; p += k * kEvalSlots;
     w.flag = reinterpret_cast<uint32_t*>(p);
     return w;
 }
@@ -659,9 +727,8 @@ static Workspace carve(fe* base, size_t n) {
 // `count` commitments to polynomials `stride` coefficients apart, in one batched MSM
 static int commit_batch(Context* c, const ProvingKey* pk, const fe* d_coeffs, size_t len, size_t stride,
                         unsigned count, g1_affine* out) {
-    int inf[32];
-    if (count > 32) return B200_ERR_INVALID;
-    int rc = msm_device_batch(pk->srs, 0, d_coeffs, len, stride, count, /*montgomery=*/1, &c->msm, c->stream, out, inf);
+    std::vector<int> inf(count);
+    int rc = msm_device_batch(pk->srs, 0, d_coeffs, len, stride, count, /*montgomery=*/1, &c->msm, c->stream, out, inf.data());
     if (rc != B200_OK) return rc;
     for (unsigned i = 0; i < count; ++i)
         if (inf[i]) std::memset(&out[i], 0, sizeof(out[i]));
@@ -901,26 +968,25 @@ static int run_segment(ProofGraphSet* gs, int idx, cudaStream_t st, F&& fn) {
 
 // Enqueue `count` commitments as segment `idx` (after `before`'s launches), leaving the batch pending for commit_collect.
 template <class F>
-static int commit_enqueue(Context* c, const Bases* srs, ProofGraphSet* gs, int idx, const fe* d_coeffs, size_t len, size_t stride,
-                          unsigned count, F&& before) {
+static int commit_enqueue(Context* c, MsmScratch* msm, const Bases* srs, ProofGraphSet* gs, int idx, const fe* d_coeffs, size_t len,
+                          size_t stride, unsigned count, F&& before) {
     cudaStream_t st = c->stream;
     const int r = run_segment(gs, idx, st, [&]() -> int {
         const int r2 = before();
         if (r2 != B200_OK) return r2;
-        return msm_launch_batch(srs, 0, d_coeffs, len, stride, count, /*montgomery=*/1, &c->msm, st);
+        return msm_launch_batch(srs, 0, d_coeffs, len, stride, count, /*montgomery=*/1, msm, st);
     });
     if (r != B200_OK) return r;
     if (gs) {  // what msm_launch_batch leaves behind when it runs outside a capture
-        msm_mark_pending(srs, len, count, &c->msm);
-        B200_CUDA(cudaEventRecord(c->msm.done_ev, st));
+        msm_mark_pending(srs, len, count, msm);
+        B200_CUDA(cudaEventRecord(msm->done_ev, st));
     }
     return B200_OK;
 }
 
-static int commit_collect(Context* c, unsigned count, g1_affine* out) {
-    int inf[32];
-    if (count > 32) return B200_ERR_INVALID;
-    const int rc = msm_finish_batch(&c->msm, out, inf);
+static int commit_collect(MsmScratch* msm, unsigned count, g1_affine* out) {
+    std::vector<int> inf(count);
+    const int rc = msm_finish_batch(msm, out, inf.data());
     if (rc != B200_OK) return rc;
     for (unsigned i = 0; i < count; ++i)
         if (inf[i]) std::memset(&out[i], 0, sizeof(out[i]));
@@ -936,18 +1002,59 @@ static void fill_open_params(OpenParams* o, fe z) {
     }
 }
 
-static int prove(Context* c, const ProvingKey* pk, const fe* h_wires, const fe* h_pub_inputs, const fe* h_blinders,
-                 ProofOut* proof, fe* h_link_poly, fe* h_challenges) {
+// One proof of a prover call: its inputs, its outputs, and its status (B200_OK, or B200_ERR_UNSATISFIED when the witness
+// does not satisfy the circuit).
+struct ProveItem {
+    const fe* wires;
+    const fe* pub_inputs;
+    const fe* blinders;
+    ProofOut* proof;
+    fe* link_poly;
+    fe* challenges;
+    int status;
+};
+
+// The buffers a prover call runs in: the context's own (single proofs; their captured graphs refer to these addresses)
+// or the context's batch set (Context::batch), which batches grow instead.
+struct ProverBufs {
+    DevBuf *ws, *nscr, *nscr2, *d_params;
+    HostPinned *h_small, *h_params;
+    MsmScratch* msm;
+};
+static ProverBufs single_bufs(Context* c) {
+    return {&c->plonk_ws, &c->ntt_scratch, &c->ntt_scratch2, &c->d_params, &c->h_small, &c->h_params, &c->msm};
+}
+static ProverBufs batch_bufs(Context* c) {
+    Context::BatchBufs& b = c->batch;
+    return {&b.ws, &b.nscr, &b.nscr2, &b.d_params, &b.h_small, &b.h_params, &b.msm};
+}
+
+// Commitment epilogue of a batch: from this many commitments in one MSM on, the last step of every window sum (sum_b 2^b
+// T_b) runs on the device (msm_horner_kernel, one warp per window, all windows at once) instead of on the host
+// (msm_finish_batch, serial in the number of commitments).  Measured with tools/prove_batch_bench.py on an H100 80GB HBM3
+// at 700 W (DESIGN §6): even at 5 commitments of 2^12-2^14 points, the device ahead from 10 on (2^13: 0.64 vs 0.71 ms
+// at 10, 2.85 vs 3.86 ms at 64).
+constexpr unsigned kDeviceHornerFrom = 10;
+
+// The five prover rounds for k proofs of one key.  Every launch covers all k proofs (see Workspace and the kernels'
+// batch index); every commitment round is ONE batched MSM over the k proofs' polynomials; the host runs the k
+// Fiat–Shamir transcripts between rounds, so a batch makes the five host round trips once.
+// single: b200_plonk_prove (k = 1 on the context's own buffers, each segment replayed as a CUDA graph from the second
+// proof of a key on); otherwise a batch, eager, on Context::batch.  An unsatisfied item gets B200_ERR_UNSATISFIED in its
+// status and incomplete outputs; the others are proved.  When no item is left after round 3 the call returns
+// B200_ERR_UNSATISFIED.
+static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveItem* items, unsigned k, bool single) {
     const size_t n = pk->n, m = pk->m;
     const unsigned log_n = pk->log_n;
     cudaStream_t st = c->stream;
     int rc;
-    if ((rc = c->plonk_ws.reserve(workspace_elems(n) * sizeof(fe))) != B200_OK) return rc;
-    if ((rc = c->ntt_scratch.reserve((size_t)7 * m * sizeof(fe))) != B200_OK) return rc;
-    if ((rc = c->ntt_scratch2.reserve((size_t)6 * m * sizeof(fe))) != B200_OK) return rc;
-    if ((rc = c->h_small.reserve(4096)) != B200_OK) return rc;
-    if ((rc = c->h_params.reserve(sizeof(ProofParams))) != B200_OK) return rc;
-    if ((rc = c->d_params.reserve(sizeof(ProofParams))) != B200_OK) return rc;
+    const size_t flags_bytes = ((size_t)k * 4 + 63) / 64 * 64;  // h_small: the k degree flags, then k x 2 NW evaluations
+    if ((rc = bf.ws->reserve(workspace_elems(n, k) * sizeof(fe))) != B200_OK) return rc;
+    if ((rc = bf.nscr->reserve((size_t)k * 7 * m * sizeof(fe))) != B200_OK) return rc;
+    if ((rc = bf.nscr2->reserve((size_t)k * 6 * m * sizeof(fe))) != B200_OK) return rc;
+    if ((rc = bf.h_small->reserve(std::max<size_t>(4096, flags_bytes + (size_t)k * 2 * NW * sizeof(fe)))) != B200_OK) return rc;
+    if ((rc = bf.h_params->reserve(k * sizeof(ProofParams))) != B200_OK) return rc;
+    if ((rc = bf.d_params->reserve(k * sizeof(ProofParams))) != B200_OK) return rc;
     if (!c->stream2) {
         int prio_least = 0, prio_greatest = 0;
         cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest);
@@ -955,32 +1062,36 @@ static int prove(Context* c, const ProvingKey* pk, const fe* h_wires, const fe* 
         B200_CUDA(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
         B200_CUDA(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
     }
-    Workspace w = carve(reinterpret_cast<fe*>(c->plonk_ws.p), n);
-    fe* nscr = reinterpret_cast<fe*>(c->ntt_scratch.p);
+    Workspace w = carve(reinterpret_cast<fe*>(bf.ws->p), n, k);
+    fe* nscr = reinterpret_cast<fe*>(bf.nscr->p);
     const size_t S = w.S;
     Domain* dn = nullptr;
     if ((rc = get_domain(c, log_n, &dn)) != B200_OK) return rc;
     const fe one = fe_one<Fr>();
 
     // graphs: only once a proof of this key has run eagerly on this context (every buffer has its final size then)
-    ProofGraphSet* gset = graph_set_for(c, pk->id);
+    ProofGraphSet* gset = single ? graph_set_for(c, pk->id) : nullptr;
     ProofGraphSet* gs = gset && gset->proofs_seen > 0 ? gset : nullptr;
-    c->msm.in_graph = gs != nullptr;
+    bf.msm->in_graph = gs != nullptr;
     struct InGraphReset {
         MsmScratch& s;
         ~InGraphReset() { s.in_graph = false; }
-    } in_graph_reset{c->msm};
-    ProofParams* hp = reinterpret_cast<ProofParams*>(c->h_params.p);  // pinned staging copy
-    ProofParams* dp = reinterpret_cast<ProofParams*>(c->d_params.p);  // what the kernels read
-    // first operation of every segment that follows a host update of *hp
+    } in_graph_reset{*bf.msm};
+    ProofParams* hp = reinterpret_cast<ProofParams*>(bf.h_params->p);  // pinned staging copy, one block per proof
+    ProofParams* dp = reinterpret_cast<ProofParams*>(bf.d_params->p);  // what the kernels read
+    static_assert(sizeof(ProofParams) % sizeof(fe) == 0, "ProofParams is an array of field elements");
+    constexpr size_t D = sizeof(ProofParams) / sizeof(fe);  // elements from one proof's parameters to the next's
+    // first operation of every segment that follows a host update of hp[]
     auto push_params = [&]() -> int {
-        B200_CUDA(cudaMemcpyAsync(dp, hp, sizeof(ProofParams), cudaMemcpyHostToDevice, st));
+        B200_CUDA(cudaMemcpyAsync(dp, hp, k * sizeof(ProofParams), cudaMemcpyHostToDevice, st));
         return B200_OK;
     };
     auto commit_enqueue = [&](int idx, const fe* d_coeffs, size_t len, size_t stride, unsigned count, auto&& before) -> int {
-        return b200::commit_enqueue(c, pk->srs, gs, idx, d_coeffs, len, stride, count, before);
+        if (!single) bf.msm->host_horner = count < kDeviceHornerFrom;
+        return b200::commit_enqueue(c, bf.msm, pk->srs, gs, idx, d_coeffs, len, stride, count, before);
     };
     auto nothing = []() -> int { return B200_OK; };
+    std::vector<g1_affine> comms((size_t)NW * k);  // the commitments of the current round, [proof][i]
 
     using clk = std::chrono::steady_clock;
     auto t_prev = clk::now();
@@ -990,36 +1101,44 @@ static int prove(Context* c, const ProvingKey* pk, const fe* h_wires, const fe* 
         if (phase < 8) c->plonk_ms[phase++] = std::chrono::duration<float, std::milli>(now - t_prev).count();
         t_prev = now;
     };
-    SolidityTranscript tr;
-    tr.append_u32_be(254);  // field size in bits
-    tr.append_u64_be((uint64_t)n);
-    tr.append_u64_be((uint64_t)pk->num_inputs);
-    for (int i = 0; i < NW; ++i) tr.append_field_elem(pk->k.v[i]);
-    for (int s = 0; s < NS; ++s) tr.append_commitment(pk->sel_comms[s]);
-    for (int i = 0; i < NW; ++i) tr.append_commitment(pk->sig_comms[i]);
-    for (size_t i = 0; i < pk->num_inputs; ++i) tr.append_field_elem(h_pub_inputs[i]);
+    std::vector<SolidityTranscript> trs(k);
+    for (unsigned p = 0; p < k; ++p) {
+        items[p].status = B200_OK;
+        SolidityTranscript& tr = trs[p];
+        tr.append_u32_be(254);  // field size in bits
+        tr.append_u64_be((uint64_t)n);
+        tr.append_u64_be((uint64_t)pk->num_inputs);
+        for (int i = 0; i < NW; ++i) tr.append_field_elem(pk->k.v[i]);
+        for (int s = 0; s < NS; ++s) tr.append_commitment(pk->sel_comms[s]);
+        for (int i = 0; i < NW; ++i) tr.append_commitment(pk->sig_comms[i]);
+        for (size_t i = 0; i < pk->num_inputs; ++i) tr.append_field_elem(items[p].pub_inputs[i]);
+    }
 
     // ---- round 1 ------------------------------------------------------------------------------------
     // caller-owned buffers are copied outside the graphs (their addresses change from proof to proof)
-    B200_CUDA(cudaMemcpyAsync(w.wires_ev, h_wires, NW * n * sizeof(fe), cudaMemcpyDefault, st));  // host or device pointer (UVA)
-    B200_CUDA(cudaMemsetAsync(w.wpoly, 0, (NW + 1) * S * sizeof(fe), st));  // wire slots and the public-input slot behind them
+    for (unsigned p = 0; p < k; ++p)  // host or device pointer (UVA)
+        B200_CUDA(cudaMemcpyAsync(w.wires_ev + (size_t)p * NW * n, items[p].wires, NW * n * sizeof(fe), cudaMemcpyDefault, st));
+    B200_CUDA(cudaMemsetAsync(w.wpoly, 0, (NW + 1) * k * S * sizeof(fe), st));  // wire slots and the public-input slots behind them
     if (pk->num_inputs)
-        B200_CUDA(cudaMemcpyAsync(w.pi_poly, h_pub_inputs, pk->num_inputs * sizeof(fe), cudaMemcpyHostToDevice, st));
-    for (int i = 0; i < NW; ++i) {
-        hp->blind_w[i][0] = h_blinders[2 * i];
-        hp->blind_w[i][1] = h_blinders[2 * i + 1];
-    }
+        for (unsigned p = 0; p < k; ++p)
+            B200_CUDA(cudaMemcpyAsync(w.pi_poly + (size_t)p * S, items[p].pub_inputs, pk->num_inputs * sizeof(fe),
+                                      cudaMemcpyHostToDevice, st));
+    for (unsigned p = 0; p < k; ++p)
+        for (int i = 0; i < NW; ++i) {
+            hp[p].blind_w[i][0] = items[p].blinders[2 * i];
+            hp[p].blind_w[i][1] = items[p].blinders[2 * i + 1];
+        }
     rc = run_segment(gs, 0, st, [&]() -> int {
         int r = push_params();
         if (r != B200_OK) return r;
-        B200_CUDA(cudaMemcpy2DAsync(w.wpoly, S * sizeof(fe), w.wires_ev, n * sizeof(fe), n * sizeof(fe), NW,
+        B200_CUDA(cudaMemcpy2DAsync(w.wpoly, S * sizeof(fe), w.wires_ev, n * sizeof(fe), n * sizeof(fe), NW * k,
                                     cudaMemcpyDeviceToDevice, st));
         {
-            // wires and public inputs: evaluations -> coefficients, one batch of 6 (pi_poly sits directly behind wpoly)
+            // wires and public inputs: evaluations -> coefficients, one batch of 6k (pi_poly sits directly behind wpoly)
             HeavyScope hv(c, st);
-            if ((r = ntt_device(dn, w.wpoly, nscr, 1, 0, NW + 1, S, hv.run)) != B200_OK) return r;
+            if ((r = ntt_device(dn, w.wpoly, nscr, 1, 0, (NW + 1) * k, S, hv.run)) != B200_OK) return r;
         }
-        B200_LAUNCH(k_blind_wires, 1, 32, 0, st)(w.wpoly, S, n, &dp->blind_w[0][0]);
+        B200_LAUNCH(k_blind_wires, k, 32, 0, st)(w.wpoly, S, n, &dp->blind_w[0][0], D);
         return B200_OK;
     });
     if (rc != B200_OK) return rc;
@@ -1038,69 +1157,84 @@ static int prove(Context* c, const ProvingKey* pk, const fe* h_wires, const fe* 
         B200_CUDA(cudaEventRecord(c->ev_fork, st));
         B200_CUDA(cudaStreamWaitEvent(s2, c->ev_fork, 0));
         side.pending = true;
-        // 5 wire polynomials (n + 2 coefficients) and the public-input polynomial (n, zero tail) in one batch
+        // 5k wire polynomials (n + 2 coefficients) and the k public-input polynomials (n, zero tail) in one batch
         rc = run_segment(gs, 1, s2, [&]() -> int {
-            return coset_evals(pk, dn, w.wpoly, S, n + 2, NW + 1, w.ext, reinterpret_cast<fe*>(c->ntt_scratch2.p), s2);
+            return coset_evals(pk, dn, w.wpoly, S, n + 2, (NW + 1) * k, w.ext, reinterpret_cast<fe*>(bf.nscr2->p), s2);
         });
         if (rc != B200_OK) return rc;
         B200_CUDA(cudaEventRecord(c->ev_join, s2));
     }
-    if ((rc = commit_enqueue(2, w.wpoly, n + 2, S, NW, nothing)) != B200_OK) return rc;
-    if ((rc = commit_collect(c, NW, proof->wires_poly_comms)) != B200_OK) return rc;
-    if (h_link_poly)  // completes under round 2; the stream is synchronised several times before this call returns
-        B200_CUDA(cudaMemcpyAsync(h_link_poly, w.wpoly, (n + 2) * sizeof(fe), cudaMemcpyDeviceToHost, st));
-    for (int i = 0; i < NW; ++i) tr.append_commitment(proof->wires_poly_comms[i]);
+    if ((rc = commit_enqueue(2, w.wpoly, n + 2, S, NW * k, nothing)) != B200_OK) return rc;
+    if ((rc = commit_collect(bf.msm, NW * k, comms.data())) != B200_OK) return rc;
+    for (unsigned p = 0; p < k; ++p) {
+        ProofOut* proof = items[p].proof;
+        std::memcpy(proof->wires_poly_comms, &comms[(size_t)p * NW], sizeof(proof->wires_poly_comms));
+        if (items[p].link_poly)  // completes under round 2; the stream is synchronised several times before this call returns
+            B200_CUDA(cudaMemcpyAsync(items[p].link_poly, w.wpoly + (size_t)p * NW * S, (n + 2) * sizeof(fe), cudaMemcpyDeviceToHost, st));
+        for (int i = 0; i < NW; ++i) trs[p].append_commitment(proof->wires_poly_comms[i]);
+    }
     mark();  // [0] round 1
 
     // ---- round 2 ------------------------------------------------------------------------------------
-    const fe beta = tr.get_and_append_challenge();
-    const fe gamma = tr.get_and_append_challenge();
-    hp->chal[0] = beta;
-    hp->chal[1] = gamma;
-    for (int i = 0; i < 3; ++i) hp->blind_z[i] = h_blinders[10 + i];
-    rc = commit_enqueue(3, w.zpoly, n + 3, n + 3, 1, [&]() -> int {
+    std::vector<fe> beta(k), gamma(k), alpha(k), zeta(k), zeta_w(k), v(k);
+    for (unsigned p = 0; p < k; ++p) {
+        beta[p] = trs[p].get_and_append_challenge();
+        gamma[p] = trs[p].get_and_append_challenge();
+        hp[p].chal[0] = beta[p];
+        hp[p].chal[1] = gamma[p];
+        for (int i = 0; i < 3; ++i) hp[p].blind_z[i] = items[p].blinders[10 + i];
+    }
+    rc = commit_enqueue(3, w.zpoly, n + 3, S, k, [&]() -> int {
         int r = push_params();
         if (r != B200_OK) return r;
-        B200_LAUNCH(k_perm_num_den, grid_for(n, 128), 128, 0, st)(w.wires_ev, pk->sig_evals, pk->dom, pk->k, &dp->chal[0], n, w.num, w.den);
-        batch_inverse_enqueue(w.num, w.den, w.tmp, n, st);
-        scan_mul_exclusive(w.den, n, w.scan, st);  // z(w^j) = prod_{i<j} ratio_i
-        B200_CUDA(cudaMemsetAsync(w.zpoly, 0, S * sizeof(fe), st));
-        B200_CUDA(cudaMemcpyAsync(w.zpoly, w.den, n * sizeof(fe), cudaMemcpyDeviceToDevice, st));
-        if ((r = ntt_device(dn, w.zpoly, nscr, 1, 0, 1, S, st)) != B200_OK) return r;
+        B200_LAUNCH(k_perm_num_den, dim3(grid_for(n, 128), k), 128, 0, st)(w.wires_ev, pk->sig_evals, pk->dom, pk->k, &dp->chal[0], D, n,
+                                                                           w.num, w.den);
+        batch_inverse_enqueue(w.num, w.den, w.tmp, k * n, st);  // the k proofs' denominators as one vector
+        scan_mul_exclusive(w.den, n, k, w.scan, st);             // z(w^j) = prod_{i<j} ratio_i, per proof
+        B200_CUDA(cudaMemsetAsync(w.zpoly, 0, k * S * sizeof(fe), st));
+        B200_CUDA(cudaMemcpy2DAsync(w.zpoly, S * sizeof(fe), w.den, n * sizeof(fe), n * sizeof(fe), k, cudaMemcpyDeviceToDevice, st));
+        if ((r = ntt_device(dn, w.zpoly, nscr, 1, 0, k, S, st)) != B200_OK) return r;
         BlindArgs b{};
         b.count = 3;
         b.dyn = &dp->blind_z[0];
-        B200_LAUNCH(k_blind, 1, 32, 0, st)(w.zpoly, n, b);
+        B200_LAUNCH(k_blind, k, 32, 0, st)(w.zpoly, n, b, S, D);
         return B200_OK;
     });
     if (rc != B200_OK) return rc;
-    if ((rc = commit_collect(c, 1, &proof->prod_perm_poly_comm)) != B200_OK) return rc;
-    tr.append_commitment(proof->prod_perm_poly_comm);
+    if ((rc = commit_collect(bf.msm, k, comms.data())) != B200_OK) return rc;
+    for (unsigned p = 0; p < k; ++p) {
+        items[p].proof->prod_perm_poly_comm = comms[p];
+        trs[p].append_commitment(comms[p]);
+    }
     mark();  // [1] round 2
 
     // ---- round 3 ------------------------------------------------------------------------------------
-    const fe alpha = tr.get_and_append_challenge();
-    hp->chal[2] = alpha;
-    hp->chal[3] = fe_sqr<Fr>(alpha);
-    for (int i = 0; i < 4; ++i) hp->blind_q[i] = h_blinders[13 + i];
+    for (unsigned p = 0; p < k; ++p) {
+        alpha[p] = trs[p].get_and_append_challenge();
+        hp[p].chal[2] = alpha[p];
+        hp[p].chal[3] = fe_sqr<Fr>(alpha[p]);
+        for (int i = 0; i < 4; ++i) hp[p].blind_q[i] = items[p].blinders[13 + i];
+    }
     B200_CUDA(cudaStreamWaitEvent(st, c->ev_join, 0));  // join: wire / PI coset evaluations are ready
     side.pending = false;
     const size_t deg = NW * (n + 1) + 2;
-    uint32_t* h_flag = reinterpret_cast<uint32_t*>(c->h_small.p);  // pinned; read after the commitments below are in
+    uint32_t* h_flag = reinterpret_cast<uint32_t*>(bf.h_small->p);  // pinned; read after the commitments below are in
     mark();  // [2] round 3 (host part)
     // the last chunk has n coefficients; its tail up to n + 3 is zero, so one batch length serves
-    rc = commit_enqueue(4, w.split, n + 3, S, NW, [&]() -> int {
+    rc = commit_enqueue(4, w.split, n + 3, S, NW * k, [&]() -> int {
         int r = push_params();
         if (r != B200_OK) return r;
         {
             HeavyScope hv(c, st);
-            if ((r = coset_evals(pk, dn, w.zpoly, S, n + 3, 1, w.ext + 6 * m, nscr, hv.run)) != B200_OK) return r;
+            if ((r = coset_evals(pk, dn, w.zpoly, S, n + 3, k, w.zext, nscr, hv.run)) != B200_OK) return r;
         }
         {
             QuotArgs q;
             q.sel = pk->ce_sel;
             q.sig = pk->ce_sig;
             q.ext = w.ext;
+            q.pi = w.ext + (size_t)k * NW * m;  // the public-input evaluations follow all k proofs' wire evaluations
+            q.zext = w.zext;
             q.pts = pk->coset_pts;
             q.l1_inv = pk->l1_inv;
             q.out = w.quot;
@@ -1108,144 +1242,200 @@ static int prove(Context* c, const ProvingKey* pk, const fe* h_wires, const fe* 
             q.log_n = log_n;
             q.k = pk->k;
             q.chal = &dp->chal[0];
+            q.dstride = D;
             for (int i = 0; i < 8; ++i) q.zh_inv[i] = pk->zh_inv[i];
             HeavyScope hv(c, st);
-            B200_LAUNCH(k_quotient, grid_for(m, 128), 128, 0, hv.run)(q);
-            // back to coefficients: nc size-n inverse transforms, then un-scale and un-mix the cosets
-            if ((r = ntt_device(dn, w.quot, nscr, 1, 0, (unsigned)pk->nc, n, hv.run)) != B200_OK) return r;
-            if (pk->nc == 6) B200_LAUNCH(k_coset_combine<6>, grid_for(n, 128), 128, 0, hv.run)(w.quot, n, pk->cscale_inv, pk->comb);
-            else B200_LAUNCH(k_coset_combine<8>, grid_for(n, 128), 128, 0, hv.run)(w.quot, n, pk->cscale_inv, pk->comb);
+            B200_LAUNCH(k_quotient, dim3(grid_for(m, 128), k), 128, 0, hv.run)(q);
+            // back to coefficients: nc size-n inverse transforms per proof, then un-scale and un-mix the cosets
+            if ((r = ntt_device(dn, w.quot, nscr, 1, 0, (unsigned)pk->nc * k, n, hv.run)) != B200_OK) return r;
+            if (pk->nc == 6) B200_LAUNCH(k_coset_combine<6>, dim3(grid_for(n, 128), k), 128, 0, hv.run)(w.quot, n, pk->cscale_inv, pk->comb);
+            else B200_LAUNCH(k_coset_combine<8>, dim3(grid_for(n, 128), k), 128, 0, hv.run)(w.quot, n, pk->cscale_inv, pk->comb);
         }
-        B200_CUDA(cudaMemsetAsync(w.flag, 0, 4, st));
-        B200_LAUNCH(k_check_degree, grid_for(m - deg, 256), 256, 0, st)(w.quot, deg, m, w.flag);
-        B200_CUDA(cudaMemcpyAsync(h_flag, w.flag, 4, cudaMemcpyDeviceToHost, st));
-        B200_LAUNCH(k_split_quotient, dim3(grid_for(n + 3, 256), NW), 256, 0, st)(w.quot, n, S, &dp->blind_q[0], w.split);
+        B200_CUDA(cudaMemsetAsync(w.flag, 0, 4 * k, st));
+        B200_LAUNCH(k_check_degree, dim3(grid_for(m - deg, 256), k), 256, 0, st)(w.quot, deg, m, w.flag);
+        B200_CUDA(cudaMemcpyAsync(h_flag, w.flag, 4 * k, cudaMemcpyDeviceToHost, st));
+        B200_LAUNCH(k_split_quotient, dim3(grid_for(n + 3, 256), NW, k), 256, 0, st)(w.quot, m, n, S, &dp->blind_q[0], D, w.split);
         return B200_OK;
     });
     if (rc != B200_OK) return rc;
-    if ((rc = commit_collect(c, NW, proof->split_quot_poly_comms)) != B200_OK) return rc;
-    if (*h_flag) {  // copied before the commitments' window sums on the same stream
+    if ((rc = commit_collect(bf.msm, NW * k, comms.data())) != B200_OK) return rc;
+    unsigned satisfied = 0;
+    for (unsigned p = 0; p < k; ++p) {  // the flags were copied before the commitments' window sums on the same stream
+        if (h_flag[p]) items[p].status = B200_ERR_UNSATISFIED;
+        else ++satisfied;
+    }
+    if (!satisfied) {
         set_error("WrongQuotientPolyDegree: the witness does not satisfy the circuit");
         return B200_ERR_UNSATISFIED;
     }
-    for (int i = 0; i < NW; ++i) tr.append_commitment(proof->split_quot_poly_comms[i]);
+    for (unsigned p = 0; p < k; ++p) {
+        ProofOut* proof = items[p].proof;
+        std::memcpy(proof->split_quot_poly_comms, &comms[(size_t)p * NW], sizeof(proof->split_quot_poly_comms));
+        for (int i = 0; i < NW; ++i) trs[p].append_commitment(proof->split_quot_poly_comms[i]);
+    }
     mark();  // [3] round 3: quotient and its 5 commitments
 
     // ---- round 4 ------------------------------------------------------------------------------------
-    const fe zeta = tr.get_and_append_challenge();
-    const fe zeta_w = FMUL(zeta, pk->group_gen);
-    fe* h_evals = reinterpret_cast<fe*>(reinterpret_cast<char*>(c->h_small.p) + 64);  // pinned
+    for (unsigned p = 0; p < k; ++p) {
+        zeta[p] = trs[p].get_and_append_challenge();
+        zeta_w[p] = FMUL(zeta[p], pk->group_gen);
+    }
+    fe* h_evals = reinterpret_cast<fe*>(reinterpret_cast<char*>(bf.h_small->p) + flags_bytes);  // pinned, [proof][2 NW]
     {
+        // proof 0's polynomials; proof p's are `pstrides` further (the key's sigmas are shared)
         const fe* polys[kMaxEval];
-        size_t lens[kMaxEval];
-        fe pts[kMaxEval];
-        for (int i = 0; i < NW; ++i) { polys[i] = w.wpoly + (size_t)i * S; lens[i] = n + 2; pts[i] = zeta; }
-        for (int i = 0; i < NW - 1; ++i) { polys[NW + i] = pk->sig_coeffs + (size_t)i * n; lens[NW + i] = n; pts[NW + i] = zeta; }
-        polys[2 * NW - 1] = w.zpoly; lens[2 * NW - 1] = n + 3; pts[2 * NW - 1] = zeta_w;
-        for (int q = 0; q < 2 * NW; ++q) {
-            fe z = pts[q];
-            for (int l = 0; l < kLevels; ++l) {
-                hp->eval_z[l][q] = z;
-                z = host_pow(z, CH);
+        size_t lens[kMaxEval], pstrides[kMaxEval];
+        for (int i = 0; i < NW; ++i) { polys[i] = w.wpoly + (size_t)i * S; lens[i] = n + 2; pstrides[i] = NW * S; }
+        for (int i = 0; i < NW - 1; ++i) { polys[NW + i] = pk->sig_coeffs + (size_t)i * n; lens[NW + i] = n; pstrides[NW + i] = 0; }
+        polys[2 * NW - 1] = w.zpoly; lens[2 * NW - 1] = n + 3; pstrides[2 * NW - 1] = S;
+        for (unsigned p = 0; p < k; ++p)
+            for (int q = 0; q < 2 * NW; ++q) {
+                fe z = q == 2 * NW - 1 ? zeta_w[p] : zeta[p];
+                for (int l = 0; l < kLevels; ++l) {
+                    hp[p].eval_z[l][q] = z;
+                    z = host_pow(z, CH);
+                }
             }
-        }
         rc = run_segment(gs, 5, st, [&]() -> int {
             int r = push_params();
             if (r != B200_OK) return r;
-            eval_batch(polys, lens, pts, 2 * NW, w.evals, w.escr, st, dp->eval_z);
-            B200_CUDA(cudaMemcpyAsync(h_evals, w.evals, 2 * NW * sizeof(fe), cudaMemcpyDeviceToHost, st));
+            eval_batch(polys, lens, nullptr, 2 * NW, w.evals, w.escr, st, dp->eval_z, k, pstrides, kEvalSlots, D);
+            B200_CUDA(cudaMemcpy2DAsync(h_evals, 2 * NW * sizeof(fe), w.evals, kEvalSlots * sizeof(fe), 2 * NW * sizeof(fe), k,
+                                        cudaMemcpyDeviceToHost, st));
             return B200_OK;
         });
         if (rc != B200_OK) return rc;
     }
     B200_CUDA(cudaStreamSynchronize(st));
-    for (int i = 0; i < NW; ++i) proof->wires_evals[i] = h_evals[i];
-    for (int i = 0; i < NW - 1; ++i) proof->wire_sigma_evals[i] = h_evals[NW + i];
-    proof->perm_next_eval = h_evals[2 * NW - 1];
-    for (int i = 0; i < NW; ++i) tr.append_field_elem(proof->wires_evals[i]);
-    for (int i = 0; i < NW - 1; ++i) tr.append_field_elem(proof->wire_sigma_evals[i]);
-    tr.append_field_elem(proof->perm_next_eval);
+    for (unsigned p = 0; p < k; ++p) {
+        ProofOut* proof = items[p].proof;
+        const fe* he = h_evals + (size_t)p * 2 * NW;
+        for (int i = 0; i < NW; ++i) proof->wires_evals[i] = he[i];
+        for (int i = 0; i < NW - 1; ++i) proof->wire_sigma_evals[i] = he[NW + i];
+        proof->perm_next_eval = he[2 * NW - 1];
+        for (int i = 0; i < NW; ++i) trs[p].append_field_elem(proof->wires_evals[i]);
+        for (int i = 0; i < NW - 1; ++i) trs[p].append_field_elem(proof->wire_sigma_evals[i]);
+        trs[p].append_field_elem(proof->perm_next_eval);
+    }
     mark();  // [4] round 4
 
     // ---- round 5 ------------------------------------------------------------------------------------
-    const fe v = tr.get_and_append_challenge();
+    // pointers and lengths (proof 0's, and the stride to proof p's): launch arguments; scalars: ProofParams
     LinArgs la{};
-    {
+    for (unsigned p = 0; p < k; ++p) {
+        v[p] = trs[p].get_and_append_challenge();
+        const ProofOut* proof = items[p].proof;
         const fe* we = proof->wires_evals;
         const fe* se = proof->wire_sigma_evals;
+        const fe al = alpha[p], be = beta[p], ga = gamma[p], ze = zeta[p];
         int t = 0;
-        auto push = [&](const fe* p, size_t len, const fe& s) {  // pointers and lengths: launch arguments; scalars: ProofParams
-            la.p[t] = p;
+        auto push = [&](const fe* ptr, size_t pstride, size_t len, const fe& s) {
+            la.p[t] = ptr;
+            la.pstride[t] = (uint32_t)pstride;
             la.len[t] = (uint32_t)len;
-            hp->lin_s[t] = s;
+            hp[p].lin_s[t] = s;
             ++t;
         };
         auto pow5 = [&](const fe& x) { return FMUL(fe_sqr<Fr>(fe_sqr<Fr>(x)), x); };
         const fe* sel = pk->sel_coeffs;
-        for (int j = 0; j < 4; ++j) push(sel + (size_t)j * n, n, we[j]);
-        push(sel + 4 * n, n, FMUL(we[0], we[1]));
-        push(sel + 5 * n, n, FMUL(we[2], we[3]));
-        for (int j = 0; j < 4; ++j) push(sel + (size_t)(6 + j) * n, n, pow5(we[j]));
-        push(sel + 10 * n, n, fe_neg<Fr>(we[4]));
-        push(sel + 11 * n, n, one);
-        push(sel + 12 * n, n, FMUL(FMUL(FMUL(we[0], we[1]), FMUL(we[2], we[3])), we[4]));
+        for (int j = 0; j < 4; ++j) push(sel + (size_t)j * n, 0, n, we[j]);
+        push(sel + 4 * n, 0, n, FMUL(we[0], we[1]));
+        push(sel + 5 * n, 0, n, FMUL(we[2], we[3]));
+        for (int j = 0; j < 4; ++j) push(sel + (size_t)(6 + j) * n, 0, n, pow5(we[j]));
+        push(sel + 10 * n, 0, n, fe_neg<Fr>(we[4]));
+        push(sel + 11 * n, 0, n, one);
+        push(sel + 12 * n, 0, n, FMUL(FMUL(FMUL(we[0], we[1]), FMUL(we[2], we[3])), we[4]));
         // z(X): alpha prod(w_i + beta k_i zeta + gamma) + alpha^2 L1(zeta)
-        const fe vanish = FSUB(host_pow(zeta, n), one);
-        const fe l1 = FMUL(vanish, fe_inv<Fr>(FMUL(host_from_u64(n), FSUB(zeta, one))));
-        fe cz = alpha;
-        for (int j = 0; j < NW; ++j) cz = FMUL(cz, FADD(FADD(we[j], FMUL(FMUL(pk->k.v[j], zeta), beta)), gamma));
-        cz = FADD(cz, FMUL(fe_sqr<Fr>(alpha), l1));
-        push(w.zpoly, n + 3, cz);
+        const fe vanish = FSUB(host_pow(ze, n), one);
+        const fe l1 = FMUL(vanish, fe_inv<Fr>(FMUL(host_from_u64(n), FSUB(ze, one))));
+        fe cz = al;
+        for (int j = 0; j < NW; ++j) cz = FMUL(cz, FADD(FADD(we[j], FMUL(FMUL(pk->k.v[j], ze), be)), ga));
+        cz = FADD(cz, FMUL(fe_sqr<Fr>(al), l1));
+        push(w.zpoly, S, n + 3, cz);
         // sigma_4(X): -alpha beta z(zeta w) prod_{i<4}(w_i + beta sigma_i + gamma)
-        fe cs = FMUL(FMUL(alpha, beta), proof->perm_next_eval);
-        for (int j = 0; j < NW - 1; ++j) cs = FMUL(cs, FADD(FADD(we[j], FMUL(beta, se[j])), gamma));
-        push(pk->sig_coeffs + (size_t)(NW - 1) * n, n, fe_neg<Fr>(cs));
+        fe cs = FMUL(FMUL(al, be), proof->perm_next_eval);
+        for (int j = 0; j < NW - 1; ++j) cs = FMUL(cs, FADD(FADD(we[j], FMUL(be, se[j])), ga));
+        push(pk->sig_coeffs + (size_t)(NW - 1) * n, 0, n, fe_neg<Fr>(cs));
         // - Z_H(zeta) * sum zeta^((n+2) i) t_i(X)
-        const fe zn2 = FMUL(FMUL(FADD(vanish, one), zeta), zeta);
+        const fe zn2 = FMUL(FMUL(FADD(vanish, one), ze), ze);
         fe ct = fe_neg<Fr>(vanish);
         for (int i = 0; i < NW; ++i) {
-            push(w.split + (size_t)i * S, i < NW - 1 ? n + 3 : n, ct);
+            push(w.split + (size_t)i * S, NW * S, i < NW - 1 ? n + 3 : n, ct);
             ct = FMUL(ct, zn2);
         }
         // batched opening at zeta: lin + v w_0 + ... + v^5 w_4 + v^6 sigma_0 + ... + v^9 sigma_3
         fe cv = one;
         for (int i = 0; i < NW; ++i) {
-            cv = FMUL(cv, v);
-            push(w.wpoly + (size_t)i * S, n + 2, cv);
+            cv = FMUL(cv, v[p]);
+            push(w.wpoly + (size_t)i * S, NW * S, n + 2, cv);
         }
         for (int i = 0; i < NW - 1; ++i) {
-            cv = FMUL(cv, v);
-            push(pk->sig_coeffs + (size_t)i * n, n, cv);
+            cv = FMUL(cv, v[p]);
+            push(pk->sig_coeffs + (size_t)i * n, 0, n, cv);
         }
         la.count = t;
-        la.dyn = &dp->lin_s[0];
+        fill_open_params(&hp[p].open[0], ze);
+        fill_open_params(&hp[p].open[1], zeta_w[p]);
     }
-    fill_open_params(&hp->open[0], zeta);
-    fill_open_params(&hp->open[1], zeta_w);
-    g1_affine open2[2];
-    rc = commit_enqueue(6, w.sdiv + 1, n + 2, S + 8, 2, [&]() -> int {
+    la.dyn = &dp->lin_s[0];
+    la.dstride = D;
+    rc = commit_enqueue(6, w.sdiv + 1, n + 2, S + 8, 2 * k, [&]() -> int {
         int r = push_params();
         if (r != B200_OK) return r;
-        B200_LAUNCH(k_lincomb, grid_for(n + 3, 128), 128, 0, st)(la, n + 3, w.lin);
+        B200_LAUNCH(k_lincomb, dim3(grid_for(n + 3, 128), k), 128, 0, st)(la, n + 3, w.lin, S);
         // opening proofs: commit((batch - batch(zeta)) / (X - zeta)) and commit((z - z(zeta w)) / (X - zeta w))
-        horner_suffix(w.lin, n + 3, zeta, w.sdiv, w.evals + 16, w.hscr, st, &dp->open[0]);
-        horner_suffix(w.zpoly, n + 3, zeta_w, w.sdiv + (S + 8), w.evals + 17, w.hscr, st, &dp->open[1]);
+        HornerStrides hs;
+        hs.k = k;
+        hs.p = S;
+        hs.s = 2 * (S + 8);
+        hs.out = kEvalSlots;
+        hs.dyn = D;
+        horner_suffix(w.lin, n + 3, zeta[0], w.sdiv, w.evals + 16, w.hscr, st, &dp->open[0], hs);
+        horner_suffix(w.zpoly, n + 3, zeta_w[0], w.sdiv + (S + 8), w.evals + 17, w.hscr, st, &dp->open[1], hs);
         return B200_OK;
     });
     if (rc != B200_OK) return rc;
-    if ((rc = commit_collect(c, 2, open2)) != B200_OK) return rc;
-    proof->opening_proof = open2[0];
-    proof->shifted_opening_proof = open2[1];
+    comms.resize(2 * k);
+    if ((rc = commit_collect(bf.msm, 2 * k, comms.data())) != B200_OK) return rc;
+    for (unsigned p = 0; p < k; ++p) {
+        items[p].proof->opening_proof = comms[2 * p];
+        items[p].proof->shifted_opening_proof = comms[2 * p + 1];
+    }
     mark();  // [5] round 5
     if (gset && !gs) gset->proofs_seen = 1;  // this key has now run eagerly on this context: later proofs replay graphs
-    if (h_challenges) {
-        tr.append_commitment(proof->opening_proof);
-        tr.append_commitment(proof->shifted_opening_proof);
+    for (unsigned p = 0; p < k; ++p) {
+        if (!items[p].challenges || items[p].status != B200_OK) continue;
+        SolidityTranscript& tr = trs[p];
+        tr.append_commitment(items[p].proof->opening_proof);
+        tr.append_commitment(items[p].proof->shifted_opening_proof);
         const fe u = tr.get_and_append_challenge();
-        const fe all[6] = {beta, gamma, alpha, zeta, v, u};
-        std::memcpy(h_challenges, all, sizeof(all));
+        const fe all[6] = {beta[p], gamma[p], alpha[p], zeta[p], v[p], u};
+        std::memcpy(items[p].challenges, all, sizeof(all));
     }
     return B200_OK;
+}
+
+// Proofs per prove() call of a batch: as many as half the free device memory holds (the batch buffers the context
+// already has count as free: they are reused), at most kMaxBatchChunk.  Per proof: the workspace, the two NTT scratches
+// and the MSM scratch of its five largest commitments.  B200_PROVE_BATCH_CHUNK overrides it (tests: the bytes out do
+// not depend on the chunk size).
+constexpr size_t kMaxBatchChunk = 64;
+static size_t prove_batch_chunk(Context* c, const ProvingKey* pk, size_t k) {
+    if (const char* e = std::getenv("B200_PROVE_BATCH_CHUNK")) {
+        const long v = std::atol(e);
+        if (v >= 1) return std::min<size_t>((size_t)v, k);
+    }
+    const size_t n = pk->n, m = pk->m;
+    const MsmPlan& pl = pk->srs->plan;
+    const size_t msm_per_commit = n * (size_t)pl.n_digits * 4 * 2 + ((size_t)pl.n_phys << (pl.c - 1)) * sizeof(g1_xyzz) * 4;
+    const size_t per_proof = (workspace_elems(n, 1) + 13 * m) * sizeof(fe) + NW * msm_per_commit;
+    size_t free_b = 0, total_b = 0;
+    if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) free_b = 0;
+    const Context::BatchBufs& b = c->batch;
+    const size_t budget = (free_b + b.ws.cap + b.nscr.cap + b.nscr2.cap) / 2;
+    // the MSM's 32-bit entry index: n * digits * NW * chunk < 2^32
+    const size_t idx_cap = ((size_t)1 << 32) / ((size_t)n * pl.n_digits * NW) - 1;
+    return std::max<size_t>(1, std::min({k, kMaxBatchChunk, budget / per_proof, idx_cap}));
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1329,7 +1519,7 @@ static int link(Context* c, const Bases* srs, const fe* h_a1, size_t len1, const
     }
     fe* d_Q = d_ZS;  // the inversion's scratch is free again after it: quotient evaluations, then coefficients
     const size_t q_len = len - size;
-    rc = commit_enqueue(c, srs, gs, 0, d_Q, q_len, q_len, 1, [&]() -> int {
+    rc = commit_enqueue(c, &c->msm, srs, gs, 0, d_Q, q_len, q_len, 1, [&]() -> int {
         int r;
         B200_CUDA(cudaMemsetAsync(d_flag, 0, 4, st));
         {
@@ -1337,7 +1527,7 @@ static int link(Context* c, const Bases* srs, const fe* h_a1, size_t len1, const
             a.count = 2;
             a.p[0] = d_a1; a.len[0] = (uint32_t)len1; a.s[0] = one;
             a.p[1] = d_a2; a.len[1] = (uint32_t)len2; a.s[1] = fe_neg<Fr>(one);
-            B200_LAUNCH(k_lincomb, grid_for(len, 128), 128, 0, st)(a, len, d_diff);
+            B200_LAUNCH(k_lincomb, grid_for(len, 128), 128, 0, st)(a, len, d_diff, 0);
         }
         fill_powers(d_roots, size, g, root0, st);
         B200_CUDA(cudaMemsetAsync(d_E, 0, N * sizeof(fe), st));
@@ -1354,7 +1544,7 @@ static int link(Context* c, const Bases* srs, const fe* h_a1, size_t len1, const
         return B200_OK;
     });
     if (rc != B200_OK) return rc;
-    if ((rc = commit_collect(c, 1, &out->quotient_commitment)) != B200_OK) return rc;
+    if ((rc = commit_collect(&c->msm, 1, &out->quotient_commitment)) != B200_OK) return rc;
     if (*h_flag) {
         set_error("link: the two wire polynomials differ on the link group (wrong layout or mismatched witnesses)");
         return B200_ERR_UNSATISFIED;
@@ -1370,19 +1560,19 @@ static int link(Context* c, const Bases* srs, const fe* h_a1, size_t len1, const
     hp->lin_s[0] = one;
     hp->lin_s[1] = fe_neg<Fr>(zd);
     fill_open_params(&hp->open, eta);
-    rc = commit_enqueue(c, srs, gs, 1, d_open + 1, len - 1, len - 1, 1, [&]() -> int {
+    rc = commit_enqueue(c, &c->msm, srs, gs, 1, d_open + 1, len - 1, len - 1, 1, [&]() -> int {
         B200_CUDA(cudaMemcpyAsync(dp, hp, sizeof(LinkParams), cudaMemcpyHostToDevice, st));
         LinArgs a{};
         a.count = 2;
         a.p[0] = d_diff; a.len[0] = (uint32_t)len;
         a.p[1] = d_Q; a.len[1] = (uint32_t)q_len;
         a.dyn = &dp->lin_s[0];
-        B200_LAUNCH(k_lincomb, grid_for(len, 128), 128, 0, st)(a, len, d_ident);
+        B200_LAUNCH(k_lincomb, grid_for(len, 128), 128, 0, st)(a, len, d_ident, 0);
         horner_suffix(d_ident, len, eta, d_open, slot, hscr, st, &dp->open);
         return B200_OK;
     });
     if (rc != B200_OK) return rc;
-    if ((rc = commit_collect(c, 1, &out->opening_proof)) != B200_OK) return rc;
+    if ((rc = commit_collect(&c->msm, 1, &out->opening_proof)) != B200_OK) return rc;
     if (gset && !gs) gset->proofs_seen = 1;
     return B200_OK;
 }
@@ -1465,9 +1655,51 @@ int b200_plonk_prove(b200_ctx* ctx, const b200_pk* pk, const uint64_t* wires, co
     if (!ctx || !pk || !wires || !blinders || !proof || (pk->pk->num_inputs && !pub_inputs)) return B200_ERR_INVALID;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
     B200_CUDA(cudaSetDevice(ctx->c.device));
-    return prove(&ctx->c, pk->pk, reinterpret_cast<const fe*>(wires), reinterpret_cast<const fe*>(pub_inputs),
-                 reinterpret_cast<const fe*>(blinders), reinterpret_cast<ProofOut*>(proof),
-                 reinterpret_cast<fe*>(link_poly), reinterpret_cast<fe*>(challenges));
+    ProveItem item{reinterpret_cast<const fe*>(wires),     reinterpret_cast<const fe*>(pub_inputs),
+                   reinterpret_cast<const fe*>(blinders),  reinterpret_cast<ProofOut*>(proof),
+                   reinterpret_cast<fe*>(link_poly),       reinterpret_cast<fe*>(challenges), B200_OK};
+    return prove(&ctx->c, single_bufs(&ctx->c), pk->pk, &item, 1, /*single=*/true);
+    B200_CATCH
+}
+
+int b200_plonk_prove_batch(b200_ctx* ctx, const b200_pk* pk, const b200_prove_item* items, size_t k, int* statuses) {
+    B200_TRY
+    if (!ctx || !pk || (k && !items)) return B200_ERR_INVALID;
+    const ProvingKey* key = pk->pk;
+    std::vector<ProveItem> its(k);
+    for (size_t i = 0; i < k; ++i) {
+        const b200_prove_item& x = items[i];
+        if (!x.wires || !x.blinders || !x.proof || (key->num_inputs && !x.pub_inputs)) {
+            set_error("plonk_prove_batch: item " + std::to_string(i) + " has a NULL pointer");
+            return B200_ERR_INVALID;
+        }
+        its[i] = ProveItem{reinterpret_cast<const fe*>(x.wires), reinterpret_cast<const fe*>(x.pub_inputs),
+                           reinterpret_cast<const fe*>(x.blinders), reinterpret_cast<ProofOut*>(x.proof),
+                           reinterpret_cast<fe*>(x.link_poly), reinterpret_cast<fe*>(x.challenges), B200_OK};
+    }
+    if (k == 0) return B200_OK;
+    std::lock_guard<std::mutex> lk(ctx->c.mu);
+    B200_CUDA(cudaSetDevice(ctx->c.device));
+    const size_t chunk = prove_batch_chunk(&ctx->c, key, k);
+    for (size_t off = 0; off < k; off += chunk) {
+        const unsigned cnt = (unsigned)std::min(chunk, k - off);
+        const int rc = prove(&ctx->c, batch_bufs(&ctx->c), key, its.data() + off, cnt, /*single=*/false);
+        if (rc != B200_OK && rc != B200_ERR_UNSATISFIED) return rc;  // B200_ERR_UNSATISFIED: every item of the chunk, see statuses
+    }
+    size_t bad = 0;
+    for (size_t i = 0; i < k; ++i) {
+        if (its[i].status != B200_OK) {
+            std::memset(items[i].proof, 0, sizeof(b200_proof));
+            ++bad;
+        }
+        if (statuses) statuses[i] = its[i].status;
+    }
+    if (bad) {
+        set_error("WrongQuotientPolyDegree: " + std::to_string(bad) + " of " + std::to_string(k) +
+                  " witnesses do not satisfy the circuit (see statuses)");
+        return B200_ERR_UNSATISFIED;
+    }
+    return B200_OK;
     B200_CATCH
 }
 

@@ -24,7 +24,7 @@ namespace {
 struct Bundle;
 
 struct Job {
-    enum Kind { kProve, kLink } kind = kProve;
+    enum Kind { kProve, kProveBatch, kLink } kind = kProve;
     uint64_t ticket = 0;
     // prove
     const b200_pk* pk = nullptr;
@@ -32,6 +32,9 @@ struct Job {
     std::vector<uint64_t> pub_inputs, blinders;
     b200_proof* proof = nullptr;
     uint64_t* link_poly = nullptr;
+    // prove batch: the items with pub_inputs / blinders pointing into the copies below (pub_inputs, blinders: k each)
+    std::vector<b200_prove_item> items;
+    int* statuses = nullptr;
     // link
     const b200_bases* srs = nullptr;
     const uint64_t *a1 = nullptr, *a2 = nullptr;
@@ -111,6 +114,8 @@ struct b200_pool {
                 d.status = b200_plonk_prove(ctxs[w], job->pk, job->wires,
                                             job->pub_inputs.empty() ? nullptr : job->pub_inputs.data(),
                                             job->blinders.data(), job->proof, job->link_poly, nullptr);
+            } else if (job->kind == Job::kProveBatch) {
+                d.status = b200_plonk_prove_batch(ctxs[w], job->pk, job->items.data(), job->items.size(), job->statuses);
             } else {
                 d.status = b200_plonk_link(ctxs[w], job->srs, job->a1, job->len1, job->a2, job->len2,
                                            job->comm1, job->comm2, job->alignment, job->offset, job->size,
@@ -230,6 +235,36 @@ int b200_pool_submit_prove(b200_pool* pool, const b200_pk* pk, const uint64_t* w
     j->blinders.assign(blinders, blinders + 4 * 17);
     j->proof = proof;
     j->link_poly = link_poly;
+    return pool_push(pool, std::move(j), ticket);
+    B200_CATCH
+}
+
+int b200_pool_submit_prove_batch(b200_pool* pool, const b200_pk* pk, const b200_prove_item* items, size_t k, int* statuses,
+                                 uint64_t* ticket) {
+    B200_TRY
+    if (!pool || !pk || (k && !items) || !ticket) {
+        b200::set_error("pool_submit_prove_batch: null argument");
+        return B200_ERR_INVALID;
+    }
+    const size_t ni = b200_pk_num_inputs(pk);
+    for (size_t i = 0; i < k; ++i)
+        if (!items[i].wires || !items[i].blinders || !items[i].proof || (ni && !items[i].pub_inputs)) {
+            b200::set_error("pool_submit_prove_batch: item " + std::to_string(i) + " has a NULL pointer");
+            return B200_ERR_INVALID;
+        }
+    std::unique_ptr<Job> j(new Job());
+    j->kind = Job::kProveBatch;
+    j->pk = pk;
+    j->statuses = statuses;
+    j->pub_inputs.resize(4 * ni * k);
+    j->blinders.resize(4 * 17 * k);
+    j->items.assign(items, items + k);
+    for (size_t i = 0; i < k; ++i) {  // the worker reads the copies
+        if (ni) std::memcpy(&j->pub_inputs[4 * ni * i], items[i].pub_inputs, 32 * ni);
+        std::memcpy(&j->blinders[4 * 17 * i], items[i].blinders, 32 * 17);
+        j->items[i].pub_inputs = ni ? &j->pub_inputs[4 * ni * i] : nullptr;
+        j->items[i].blinders = &j->blinders[4 * 17 * i];
+    }
     return pool_push(pool, std::move(j), ticket);
     B200_CATCH
 }

@@ -138,6 +138,43 @@ impl GpuProver {
         Ok((proof_from_raw(&raw), hint_from_raw(&raw, &link)))
     }
 
+    /// `prove_with_link_hint` for many circuits (witnesses) of ONE key, proved by one `b200_plonk_prove_batch` job on one
+    /// worker: every kernel launch covers all of them and each commitment round is one batched MSM.  Item i of the result
+    /// is `prove_with_link_hint`'s answer for `circuits[i]` with the same blinders: the proof and hint, or
+    /// `WrongQuotientPolyDegree` for a witness that does not satisfy the circuit.
+    pub fn prove_batch<R: rand::RngCore + rand::CryptoRng>(
+        &self, rng: &mut R, circuits: &[&PlonkCircuit<Fr>], pk: &GpuProvingKey,
+    ) -> Result<Vec<Result<(Proof<Bn254>, LinkingHint<Bn254>), PlonkError>>, PlonkError> {
+        let n = 1usize << pk.log_n;
+        let k = circuits.len();
+        let mut wires = Vec::with_capacity(k);
+        let mut pub_inputs = Vec::with_capacity(k);
+        for cs in circuits {
+            wires.push(cs.witness_table().iter().flat_map(|col| col.iter().flat_map(fr_limbs)).collect::<Vec<u64>>());
+            pub_inputs.push(cs.public_input()?.iter().flat_map(fr_limbs).collect::<Vec<u64>>());
+        }
+        let blinders: Vec<Vec<u64>> = (0..k).map(|_| (0..17).map(|_| Fr::rand(rng)).flat_map(|f| fr_limbs(&f)).collect()).collect();
+        let mut raws: Vec<ffi::b200_proof> = (0..k).map(|_| unsafe { std::mem::zeroed() }).collect();
+        let mut links: Vec<Vec<u64>> = (0..k).map(|_| vec![0u64; (n + 2) * 4]).collect();
+        let items: Vec<ffi::b200_prove_item> = (0..k).map(|i| ffi::b200_prove_item {
+            wires: wires[i].as_ptr(), pub_inputs: pub_inputs[i].as_ptr(), blinders: blinders[i].as_ptr(),
+            proof: &mut raws[i], link_poly: links[i].as_mut_ptr(), challenges: std::ptr::null_mut(),
+        }).collect();
+        let mut statuses: Vec<c_int> = vec![0; k];
+        let mut ticket = 0u64;
+        check(unsafe {
+            ffi::b200_pool_submit_prove_batch(self.pool, pk.raw, items.as_ptr(), k, statuses.as_mut_ptr(), &mut ticket)
+        })?;
+        let rc = unsafe { ffi::b200_pool_wait(self.pool, ticket) }; // buffers above stay alive until here
+        if rc != ffi::B200_ERR_UNSATISFIED {
+            check(rc)?;
+        }
+        Ok((0..k).map(|i| {
+            check(statuses[i])?;
+            Ok((proof_from_raw(&raws[i]), hint_from_raw(&raws[i], &links[i])))
+        }).collect())
+    }
+
     /// replaces `PlonkKzgSnark::link_proofs::<SolidityTranscript>(lhs, rhs, &layout, &pk.commit_key)`
     /// (proof_linking/intent_only.rs:42-47, intent_and_balance.rs:66-72, output_balance.rs)
     pub fn link_proofs(&self, lhs: &LinkingHint<Bn254>, rhs: &LinkingHint<Bn254>, layout: &GroupLayout)

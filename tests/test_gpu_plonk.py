@@ -23,7 +23,9 @@ def setup(ctx, oracle, pyoracle, log_n, seed, num_inputs=7):
     return circ, tau, srs
 
 
-@pytest.mark.parametrize("log_n", [5, 8, 11, 13])
+# every domain from 2^5 to 2^15: the chunked scans (CH = 16) change their level structure across these sizes, e.g. 16,
+# 256 and 4096 chunks fill a top level exactly
+@pytest.mark.parametrize("log_n", [5, 7, 8, 9, 10, 11, 12, 13, 14, 15])
 def test_prove_matches_oracle_bit_exact(ctx, oracle, pyoracle, log_n):
     circ, tau, srs = setup(ctx, oracle, pyoracle, log_n, seed=100 + log_n)
     bases = ctx.load_bases(srs, check_on_curve=True)

@@ -44,7 +44,8 @@ def unsatisfied(circ):
     return bad
 
 
-@pytest.mark.parametrize("log_n,num_inputs", [(2, 0), (3, 2), (10, 0), (10, 5), (13, 4)])
+# n = 16 and 256: a segment of the grand-product scan is exactly one chunk / exactly 16 chunks
+@pytest.mark.parametrize("log_n,num_inputs", [(2, 0), (3, 2), (4, 1), (5, 2), (8, 3), (10, 0), (10, 5), (12, 2), (13, 4)])
 def test_batch_equals_single_proofs(ctx, oracle, pyoracle, log_n, num_inputs):
     circ, srs, bases, pk = make(ctx, oracle, pyoracle, log_n, num_inputs, seed=11 + log_n)
     bls = [synth.splitmix_blinders(7000 + 31 * i + log_n) for i in range(17)]

@@ -239,6 +239,31 @@ int b200_plonk_link(b200_ctx* ctx, const b200_bases* srs, const uint64_t* a1, si
                     unsigned alignment, size_t offset, size_t size, b200_link_proof* proof,
                     uint64_t* eta);
 
+/* One link proof of a batch: the arguments of b200_plonk_link. */
+typedef struct {
+    const uint64_t* a1; size_t len1;      /* host or device pointers, as b200_plonk_link */
+    const uint64_t* a2; size_t len2;
+    const uint64_t* comm1; const uint64_t* comm2;
+    unsigned alignment; size_t offset; size_t size;
+    b200_link_proof* proof;
+    uint64_t* eta;                        /* may be NULL */
+} b200_link_item;
+/* Makes k link proofs together: the division by Z_D runs as one launch per step over all items of one transform size,
+ * the k quotient commitments and the k opening proofs are one batched MSM each over the same SRS bases, and the host
+ * derives every eta in one round trip.  Item i's proof and eta are byte-identical to b200_plonk_link(ctx, srs,
+ * items[i].a1, ...); items may mix lengths, layouts and pointer kinds.
+ * statuses (may be NULL) receives k codes: B200_OK, or B200_ERR_UNSATISFIED for an item whose a1 and a2 differ on the
+ * group (its proof is zeroed, its eta is not written; every other item is still proved).  Returns B200_OK when every item
+ * was proved, B200_ERR_UNSATISFIED when any was not.  An argument error fails the whole call before any device work with
+ * B200_ERR_INVALID, and b200_last_error() names the item: a NULL ctx / srs, a NULL items pointer with k > 0, an item
+ * with a NULL a1 / a2 / comm1 / comm2 / proof pointer, or one that b200_plonk_link refuses (size 0, size >= max(len1,
+ * len2), alignment > 28, max(len1, len2) above the SRS length, or a transform above 2^28).  A CUDA or memory error fails
+ * the whole call too.  k = 0 is accepted.
+ * The batch runs in chunks of as many items as half the free device memory holds (at most 64); the results do not
+ * depend on the chunk size.  It runs eagerly (no CUDA graphs) in the context's batch buffers, the ones
+ * b200_plonk_prove_batch uses: single link proofs and single proofs keep replaying their graphs. */
+int b200_plonk_link_batch(b200_ctx* ctx, const b200_bases* srs, const b200_link_item* items, size_t k, int* statuses);
+
 /* ---- verification (host only; no device is needed or used) -----------------------------------
  * G2 points are 128-byte records x0 || x1 || y0 || y1 (Montgomery Fq), the layout of the ptau file's
  * G2 section read by srs.rs:185-199: g2_h = `UnivariateUniversalParams.h`, g2_tau_h = `.beta_h`.
@@ -342,6 +367,14 @@ int b200_pool_submit_link(b200_pool* pool, const b200_bases* srs, const uint64_t
                           const uint64_t* a2, size_t len2, const uint64_t* comm1, const uint64_t* comm2,
                           unsigned alignment, size_t offset, size_t size, b200_link_proof* proof,
                           uint64_t* ticket);
+/* Queue one `b200_plonk_link_batch(ctx_of_some_worker, srs, items, k, statuses)` as ONE job on one worker.  The items
+ * array and each item's comm1 / comm2 are copied at submit; a1, a2, the proof and eta buffers and statuses (may be
+ * NULL) stay owned by the caller until the ticket has been waited for.  A NULL pointer (pool, srs, ticket, items with
+ * k > 0, or an item's a1 / a2 / comm1 / comm2 / proof) is refused at submit with B200_ERR_INVALID and nothing is queued.
+ * The ticket's status is the call's: B200_ERR_UNSATISFIED when any item was refused (see statuses), B200_ERR_INVALID
+ * for a bad layout or length. */
+int b200_pool_submit_link_batch(b200_pool* pool, const b200_bases* srs, const b200_link_item* items, size_t k,
+                                int* statuses, uint64_t* ticket);
 /* One proof of a bundle, arguments as for b200_pool_submit_prove.  `link_poly` ((2^log_n + 2) x 4 limbs) is required
  * for every proof a link names. */
 typedef struct {

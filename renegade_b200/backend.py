@@ -634,6 +634,81 @@ def link_proofs(ctx: Context, srs: Bases, hint_a: LinkingHint, hint_b: LinkingHi
     return proof, eta
 
 
+class B200LinkItem(C.Structure):
+    """b200_link_item: one link proof of a batch."""
+    _fields_ = [("a1", C.c_void_p), ("len1", C.c_size_t), ("a2", C.c_void_p), ("len2", C.c_size_t),
+                ("comm1", C.c_void_p), ("comm2", C.c_void_p), ("alignment", C.c_uint), ("offset", C.c_size_t),
+                ("size", C.c_size_t), ("proof", C.c_void_p), ("eta", C.c_void_p)]
+
+
+def _link_poly(poly, where: str):
+    """(pointer, length, array or None) of a hint's polynomial: an array of (len, 4) limbs, or (address, len) of one in
+    device or pinned host memory"""
+    if isinstance(poly, tuple):
+        addr, n = poly
+        return C.c_void_p(int(addr)), int(n), None
+    a = np.ascontiguousarray(poly, dtype=np.uint64)
+    if a.ndim != 2 or a.shape[1] != 4:
+        a = a.reshape(-1, 4) if a.size % 4 == 0 else None
+    if a is None:
+        raise ValueError(f"link_proofs_batch: {where} is not a vector of field elements (4 limbs each)")
+    return _ptr(a), a.shape[0], a
+
+
+def _link_items(srs: Bases, triples):
+    """Checks a link batch's arguments (ValueError) and builds its b200_link_item array.  Returns (items, keep): keep[i]
+    holds the arrays item i points into, and its outputs (proof, eta)."""
+    triples = list(triples)
+    srs_len = len(srs)
+    items = (B200LinkItem * max(1, len(triples)))()
+    keep = []
+    for i, t in enumerate(triples):
+        if len(t) != 3:
+            raise ValueError(f"link_proofs_batch: item {i} is not a (hint_a, hint_b, layout) triple")
+        hint_a, hint_b, lay = t
+        p1, n1, a1 = _link_poly(hint_a.linking_wire_poly, f"item {i}'s first polynomial")
+        p2, n2, a2 = _link_poly(hint_b.linking_wire_poly, f"item {i}'s second polynomial")
+        c1 = np.ascontiguousarray(hint_a.linking_wire_comm, dtype=np.uint64).reshape(-1)
+        c2 = np.ascontiguousarray(hint_b.linking_wire_comm, dtype=np.uint64).reshape(-1)
+        if c1.size != 8 or c2.size != 8:
+            raise ValueError(f"link_proofs_batch: item {i}'s commitments must be 8 limbs (x || y) each")
+        n = max(n1, n2)
+        if not 0 < lay.size < n:
+            raise ValueError(f"link_proofs_batch: item {i}'s group of {lay.size} roots does not fit polynomials of {n} "
+                             "coefficients (0 < size < max(len1, len2))")
+        if not 0 <= lay.alignment <= 28 or lay.offset < 0:
+            raise ValueError(f"link_proofs_batch: item {i} has alignment {lay.alignment} and offset {lay.offset} "
+                             "(0 <= alignment <= 28, offset >= 0)")
+        if n > srs_len:
+            raise ValueError(f"link_proofs_batch: item {i} has {n} coefficients, the SRS {srs_len} powers")
+        proof = B200LinkProof()
+        eta = np.zeros(4, dtype=np.uint64)
+        items[i] = B200LinkItem(p1, n1, p2, n2, _ptr(c1), _ptr(c2), lay.alignment, lay.offset, lay.size,
+                                C.cast(C.pointer(proof), C.c_void_p), _ptr(eta))
+        keep.append((a1, a2, c1, c2, proof, eta))
+    return items, keep
+
+
+def _link_batch_results(keep, statuses):
+    st = [int(statuses[i]) for i in range(len(keep))]
+    return [x[4] for x in keep], [x[5] if s == 0 else None for x, s in zip(keep, st)], st
+
+
+def link_proofs_batch(ctx: Context, srs: Bases, triples):
+    """`link_proofs` for many (hint_a, hint_b, layout) triples in ONE call (`b200_plonk_link_batch`).  A hint's
+    linking_wire_poly is an array, or (address, length) of one in device or pinned host memory.  Returns
+    (proofs, etas, statuses): item i's proof and eta equal `link_proofs` of the same triple; statuses[i] is 0, or -7
+    (B200_ERR_UNSATISFIED) when the two polynomials differ on the group, in which case the proof is zeroed and the eta is
+    None.  Argument errors raise ValueError before any device work; other failures raise B200Error."""
+    items, keep = _link_items(srs, triples)
+    k = len(keep)
+    statuses = (C.c_int * max(1, k))()
+    rc = ctx._lib.b200_plonk_link_batch(ctx._h, srs._h, items, k, statuses)
+    if rc not in (0, -7):
+        _lib.check(rc)
+    return _link_batch_results(keep, statuses)
+
+
 def compute_poseidon_hash_batch(ctx: Context, values: np.ndarray) -> np.ndarray:
     """`batch` x `crypto::hash::compute_poseidon_hash(&values[i])` (crates/crypto/src/hash/mod.rs:12-18):
     values has shape (batch, len, 4) Montgomery; returns (batch, 4)."""
@@ -701,6 +776,13 @@ class _PoolBatch:
     held: list
     statuses: Any
     link_hints: bool
+
+
+@dataclass
+class _PoolLinkBatch:
+    """What a queued link batch job writes into: its items' arrays and outputs, and the statuses."""
+    held: list
+    statuses: Any
 
 
 class ProverPool:
@@ -779,6 +861,17 @@ class ProverPool:
         self._keep[ticket.value] = (proof, None, (a1, a2, c1, c2), srs)
         return ticket.value
 
+    def submit_link_batch(self, srs: "Bases", triples, keep=None) -> int:
+        """Queue one `b200_plonk_link_batch` as a single job on one worker; returns the ticket.  Arguments as for
+        `link_proofs_batch`; polynomials given by address stay owned by the caller until `wait(ticket)` returns (pass
+        their owners as `keep`).  `wait(ticket)` returns (proofs, etas, statuses) like `link_proofs_batch`."""
+        items, held = _link_items(srs, triples)
+        statuses = (C.c_int * max(1, len(held)))()
+        ticket = C.c_uint64()
+        _lib.check(self._lib.b200_pool_submit_link_batch(self._h, srs._h, items, len(held), statuses, C.byref(ticket)))
+        self._keep[ticket.value] = (_PoolLinkBatch(held, statuses), None, (items, keep), srs)
+        return ticket.value
+
     def submit_bundle(self, srs: "Bases", proofs, links) -> int:
         """One ticket for a whole proof bundle (`b200_pool_submit_bundle`): `proofs` = [(pk, wires_ptr, pub_inputs,
         blinders)], `links` = [(a, b, GroupLayout)] — link proof between the hints of proofs a and b, forked inside the
@@ -818,9 +911,11 @@ class ProverPool:
         job's own status and message if it failed."""
         rc = self._lib.b200_pool_wait(self._h, ticket)
         proof, link, _, _ = self._keep.pop(ticket, (None, None, None, None))
-        if isinstance(proof, _PoolBatch):  # a batch job: unsatisfied items are reported in its statuses
+        if isinstance(proof, (_PoolBatch, _PoolLinkBatch)):  # a batch job: refused items are reported in its statuses
             if rc not in (0, -7):
                 _lib.check(rc)
+            if isinstance(proof, _PoolLinkBatch):
+                return _link_batch_results(proof.held, proof.statuses)
             return _batch_results(proof.held, proof.statuses, proof.link_hints, False)
         _lib.check(rc)
         return (proof, link) if link is not None else proof

@@ -401,6 +401,52 @@ __global__ void k_any_nonzero(const fe* __restrict__ v, size_t count, uint32_t* 
         if (!fe_is_zero(fe_load_ro(v + i))) atomicOr(flag, 1u);
 }
 
+// ---- link proofs in batches: one descriptor per item, blockIdx.y = item --------------------------------------------
+struct LinkDesc {
+    fe g, root0;        // generator of the layout's 2^alignment roots of unity, and the group's first root g^offset
+    uint64_t roots_at;  // where the item's roots start in the batch's root array
+    uint64_t size;      // roots in the group
+    uint64_t q_len;     // quotient coefficients: len - size
+    uint64_t pad;
+};
+
+// roots[roots_at + i] = root0 * g^i, i < size
+__global__ void k_link_roots(const LinkDesc* __restrict__ d, fe* __restrict__ roots) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const LinkDesc* it = d + blockIdx.y;
+    if (i >= it->size) return;
+    fe base = it->g, acc = it->root0;
+    for (size_t e = i; e; e >>= 1) {
+        if (e & 1) acc = FMUL(acc, base);
+        base = fe_sqr<Fr>(base);
+    }
+    fe_store(roots + it->roots_at + i, acc);
+}
+
+// k_vanishing_on_coset for items of one transform size N: item y's values at out + y * N, its roots from its descriptor
+__global__ void k_vanishing_on_coset_batch(const fe* __restrict__ tw, size_t N, fe g, const fe* __restrict__ roots,
+                                           const LinkDesc* __restrict__ d, fe* __restrict__ out) {
+    const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= N) return;
+    const LinkDesc* it = d + blockIdx.y;
+    const size_t half = N >> 1;
+    fe wj = fe_load_ro(tw + (j < half ? j : j - half));
+    if (j >= half) wj = fe_neg<Fr>(wj);
+    const fe x = FMUL(g, wj);
+    const fe* r = roots + it->roots_at;
+    const size_t count = it->size;
+    fe acc = fe_one<Fr>();
+    for (size_t i = 0; i < count; ++i) acc = FMUL(acc, FSUB(x, fe_load_ro(r + i)));
+    fe_store(out + blockIdx.y * N + j, acc);
+}
+
+// flag[y] |= 1 when item y's coefficients [q_len_y, m) are not all zero (q + y * m): the division was not exact
+__global__ void k_check_zero_tail(const fe* __restrict__ q, size_t m, const LinkDesc* __restrict__ d, uint32_t* flag) {
+    const size_t i = d[blockIdx.y].q_len + (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    if (!fe_is_zero(fe_load_ro(q + blockIdx.y * m + i))) atomicOr(flag + blockIdx.y, 1u);
+}
+
 
 // ---- element-wise Fr vector primitives (the collaborative prover's share arithmetic) ------------------------------
 // out[i] = a[i] (op) b[i]  or  a[i] (op) b[0] when b is a scalar; op: 0 add, 1 sub, 2 mul
@@ -1577,6 +1623,224 @@ static int link(Context* c, const Bases* srs, const fe* h_a1, size_t len1, const
     return B200_OK;
 }
 
+// One link proof of a batch (b200_plonk_link_batch): its inputs, outputs and status (B200_OK, or B200_ERR_UNSATISFIED
+// when the division by Z_D is not exact).  log_N: the transform size link() would pick for it.
+struct LinkItem {
+    const fe *a1, *a2;
+    size_t len1, len2;
+    g1_affine comm1, comm2;
+    unsigned alignment;
+    size_t offset, size;
+    LinkOut* out;
+    fe* eta;
+    unsigned log_N;
+    int status;
+};
+
+// eta of a link proof: link()'s transcript over the two wire commitments and the quotient commitment
+__attribute__((noinline)) static fe link_challenge(const g1_affine& comm1, const g1_affine& comm2, const g1_affine& quot) {
+    SolidityTranscript tr;
+    tr.append_commitment(comm1);
+    tr.append_commitment(comm2);
+    tr.append_commitment(quot);
+    return tr.get_and_append_challenge();
+}
+
+// k link proofs at once, eager, on Context::batch; the items come sorted by log_N.  The same steps as link(), each one
+// launch (or one batched transform / inversion) over many items:
+//  - the differences a1 - a2 of all k items, `L` = max len apart (zero above each item's own length);
+//  - the division, per group of items of one transform size N: item y's data N apart, its roots and q_len read from its
+//    LinkDesc; the quotients then go to one region `Q` = max q_len apart (zero above each item's own q_len);
+//  - ONE batched MSM of the k quotients; the host runs the k transcripts (eta, Z_D(eta)) in one round trip;
+//  - the openings over the common length L (leading zero coefficients change neither p(eta) nor the quotient's
+//    coefficients, and zero scalars add nothing to a commitment), then ONE batched MSM of the k opening proofs.
+// Each item's bytes are link()'s.  An item whose division is not exact is carried through the launches and gets
+// B200_ERR_UNSATISFIED; its outputs are not written.
+static int link_chunk(Context* c, const Bases* srs, LinkItem* const* items, unsigned k) {
+    cudaStream_t st = c->stream;
+    Context::BatchBufs& b = c->batch;
+    int rc;
+    size_t L = 0, Q = 0, n_roots = 0, max_size = 0, max_group = 0;
+    for (unsigned y = 0; y < k; ++y) {
+        const LinkItem& it = *items[y];
+        const size_t len = std::max(it.len1, it.len2);
+        L = std::max(L, len);
+        Q = std::max(Q, len - it.size);
+        n_roots += it.size;
+        max_size = std::max(max_size, it.size);
+    }
+    std::vector<unsigned> grp{0};  // group i: items [grp[i], grp[i + 1]), one transform size each
+    for (unsigned y = 1; y <= k; ++y)
+        if (y == k || items[y]->log_N != items[y - 1]->log_N) {
+            max_group = std::max(max_group, (size_t)(y - grp.back()) << items[y - 1]->log_N);
+            grp.push_back(y);
+        }
+    static_assert(sizeof(LinkDesc) % sizeof(fe) == 0 && sizeof(LinkParams) % sizeof(fe) == 0, "arrays of field elements");
+    const size_t hscr_n = (size_t)k * 4 * (L / CH + 4 * CH + 64);
+    const size_t desc_n = (size_t)k * sizeof(LinkDesc) / sizeof(fe);
+    const size_t flag_n = ((size_t)k * 4 + sizeof(fe) - 1) / sizeof(fe);
+    const size_t kL = (size_t)k * L, kQ = (size_t)k * Q;
+    if ((rc = b.ws.reserve((3 * kL + kQ + 3 * max_group + hscr_n + n_roots + k + desc_n + flag_n) * sizeof(fe))) != B200_OK)
+        return rc;
+    if ((rc = b.nscr.reserve(max_group * sizeof(fe))) != B200_OK) return rc;
+    const size_t desc_bytes = (size_t)k * sizeof(LinkDesc);
+    if ((rc = b.h_small.reserve(desc_bytes + (size_t)k * 4)) != B200_OK) return rc;
+    if ((rc = b.h_params.reserve(k * sizeof(LinkParams))) != B200_OK) return rc;
+    if ((rc = b.d_params.reserve(k * sizeof(LinkParams))) != B200_OK) return rc;
+    std::vector<Domain*> doms(grp.size() - 1);
+    for (size_t g = 0; g + 1 < grp.size(); ++g)
+        if ((rc = get_domain(c, items[grp[g]]->log_N, &doms[g])) != B200_OK) return rc;
+
+    fe* base = reinterpret_cast<fe*>(b.ws.p);
+    fe *d_a1 = base, *d_a2 = d_a1 + kL, *d_diff = d_a2 + kL, *d_quot = d_diff + kL;
+    fe *d_E = d_quot + kQ, *d_Z = d_E + max_group, *d_ZS = d_Z + max_group;  // one group's evaluations, Z_D, scratch
+    fe *hscr = d_ZS + max_group, *d_roots = hscr + hscr_n, *d_tot = d_roots + n_roots;
+    LinkDesc* d_desc = reinterpret_cast<LinkDesc*>(d_tot + k);
+    uint32_t* d_flag = reinterpret_cast<uint32_t*>(d_tot + k + desc_n);
+    fe *d_ident = d_a1, *d_open = d_a2;  // free again once the differences are formed
+    fe* nscr = reinterpret_cast<fe*>(b.nscr.p);
+    LinkDesc* h_desc = reinterpret_cast<LinkDesc*>(b.h_small.p);
+    uint32_t* h_flag = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(b.h_small.p) + desc_bytes);
+    LinkParams* hp = reinterpret_cast<LinkParams*>(b.h_params.p);
+    LinkParams* dp = reinterpret_cast<LinkParams*>(b.d_params.p);
+    constexpr size_t D = sizeof(LinkParams) / sizeof(fe);
+    MsmScratch* msm = &b.msm;
+    msm->host_horner = k < kDeviceHornerFrom;
+    const fe one = fe_one<Fr>();
+
+    size_t at = 0;
+    for (unsigned y = 0; y < k; ++y) {
+        const LinkItem& it = *items[y];
+        LinkDesc& d = h_desc[y];
+        d.g = host_root_of_unity(it.alignment);
+        d.root0 = host_pow(d.g, (uint64_t)it.offset);
+        d.roots_at = at;
+        d.size = it.size;
+        d.q_len = std::max(it.len1, it.len2) - it.size;
+        d.pad = 0;
+        at += it.size;
+    }
+    rc = commit_enqueue(c, msm, srs, nullptr, 0, d_quot, Q, Q, k, [&]() -> int {
+        int r;
+        B200_CUDA(cudaMemsetAsync(d_a1, 0, 2 * kL * sizeof(fe), st));
+        for (unsigned y = 0; y < k; ++y) {  // caller-owned host or device pointers (UVA)
+            B200_CUDA(cudaMemcpyAsync(d_a1 + (size_t)y * L, items[y]->a1, items[y]->len1 * sizeof(fe), cudaMemcpyDefault, st));
+            B200_CUDA(cudaMemcpyAsync(d_a2 + (size_t)y * L, items[y]->a2, items[y]->len2 * sizeof(fe), cudaMemcpyDefault, st));
+        }
+        B200_CUDA(cudaMemcpyAsync(d_desc, h_desc, desc_bytes, cudaMemcpyHostToDevice, st));
+        B200_CUDA(cudaMemsetAsync(d_flag, 0, (size_t)k * 4, st));
+        B200_CUDA(cudaMemsetAsync(d_quot, 0, kQ * sizeof(fe), st));
+        {
+            LinArgs a{};
+            a.count = 2;
+            a.p[0] = d_a1; a.pstride[0] = (uint32_t)L; a.len[0] = (uint32_t)L; a.s[0] = one;
+            a.p[1] = d_a2; a.pstride[1] = (uint32_t)L; a.len[1] = (uint32_t)L; a.s[1] = fe_neg<Fr>(one);
+            B200_LAUNCH(k_lincomb, dim3(grid_for(L, 128), k), 128, 0, st)(a, L, d_diff, L);
+        }
+        B200_LAUNCH(k_link_roots, dim3(grid_for(max_size, 128), k), 128, 0, st)(d_desc, d_roots);
+        for (size_t g = 0; g + 1 < grp.size(); ++g) {
+            const unsigned y0 = grp[g], kg = grp[g + 1] - y0;
+            const Domain* dN = doms[g];
+            const size_t N = (size_t)1 << dN->log_n, kN = (size_t)kg * N;
+            size_t min_q = N;
+            for (unsigned y = y0; y < y0 + kg; ++y) min_q = std::min<size_t>(min_q, h_desc[y].q_len);
+            B200_CUDA(cudaMemsetAsync(d_E, 0, kN * sizeof(fe), st));
+            B200_CUDA(cudaMemcpy2DAsync(d_E, N * sizeof(fe), d_diff + (size_t)y0 * L, L * sizeof(fe), std::min(L, N) * sizeof(fe), kg,
+                                        cudaMemcpyDeviceToDevice, st));
+            if ((r = ntt_device(dN, d_E, nscr, /*inverse=*/0, /*coset=*/1, kg, N, st)) != B200_OK) return r;
+            B200_LAUNCH(k_vanishing_on_coset_batch, dim3(grid_for(N, 128), kg), 128, 0, st)(dN->tw_fwd, N, fe_from_u32<Fr>(5), d_roots,
+                                                                                            d_desc + y0, d_Z);
+            batch_inverse_enqueue(nullptr, d_Z, d_ZS, kN, st);
+            B200_LAUNCH(k_fr_vec_op, grid_for(kN, 256), 256, 0, st)(2, d_E, d_Z, 0, kN, d_ZS);
+            if ((r = ntt_device(dN, d_ZS, nscr, /*inverse=*/1, /*coset=*/1, kg, N, st)) != B200_OK) return r;
+            B200_LAUNCH(k_check_zero_tail, dim3(grid_for(N - min_q, 256), kg), 256, 0, st)(d_ZS, N, d_desc + y0, d_flag + y0);
+            // exact items are zero from q_len on, so min(Q, N) coefficients carry the whole quotient
+            B200_CUDA(cudaMemcpy2DAsync(d_quot + (size_t)y0 * Q, Q * sizeof(fe), d_ZS, N * sizeof(fe), std::min(Q, N) * sizeof(fe), kg,
+                                        cudaMemcpyDeviceToDevice, st));
+        }
+        B200_CUDA(cudaMemcpyAsync(h_flag, d_flag, (size_t)k * 4, cudaMemcpyDeviceToHost, st));
+        return B200_OK;
+    });
+    if (rc != B200_OK) return rc;
+    std::vector<g1_affine> comms(k);
+    if ((rc = commit_collect(msm, k, comms.data())) != B200_OK) return rc;
+    unsigned proved = 0;
+    for (unsigned y = 0; y < k; ++y) {  // the flags were copied before the commitments' window sums on the same stream
+        LinkItem& it = *items[y];
+        LinkParams& p = hp[y];
+        std::memset(&p, 0, sizeof(p));
+        if (h_flag[y]) {  // carried through the opening with harmless parameters
+            it.status = B200_ERR_UNSATISFIED;
+            p.lin_s[0] = one;
+            fill_open_params(&p.open, fe_zero());
+            continue;
+        }
+        ++proved;
+        it.status = B200_OK;
+        it.out->quotient_commitment = comms[y];
+        const fe eta = link_challenge(it.comm1, it.comm2, comms[y]);
+        if (it.eta) *it.eta = eta;
+        fe zd = one, root = h_desc[y].root0;
+        for (size_t i = 0; i < it.size; ++i) {
+            zd = FMUL(zd, FSUB(eta, root));
+            root = FMUL(root, h_desc[y].g);
+        }
+        p.lin_s[0] = one;
+        p.lin_s[1] = fe_neg<Fr>(zd);
+        fill_open_params(&p.open, eta);
+    }
+    if (!proved) return B200_OK;  // see the statuses
+    msm->host_horner = k < kDeviceHornerFrom;
+    rc = commit_enqueue(c, msm, srs, nullptr, 0, d_open + 1, L - 1, L, k, [&]() -> int {
+        B200_CUDA(cudaMemcpyAsync(dp, hp, k * sizeof(LinkParams), cudaMemcpyHostToDevice, st));
+        LinArgs a{};
+        a.count = 2;
+        a.p[0] = d_diff; a.pstride[0] = (uint32_t)L; a.len[0] = (uint32_t)L;
+        a.p[1] = d_quot; a.pstride[1] = (uint32_t)Q; a.len[1] = (uint32_t)Q;
+        a.dyn = &dp->lin_s[0];
+        a.dstride = D;
+        B200_LAUNCH(k_lincomb, dim3(grid_for(L, 128), k), 128, 0, st)(a, L, d_ident, L);
+        HornerStrides hs;
+        hs.k = k;
+        hs.p = hs.s = L;
+        hs.out = 1;
+        hs.dyn = D;
+        horner_suffix(d_ident, L, fe_zero(), d_open, d_tot, hscr, st, &dp->open, hs);
+        return B200_OK;
+    });
+    if (rc != B200_OK) return rc;
+    if ((rc = commit_collect(msm, k, comms.data())) != B200_OK) return rc;
+    for (unsigned y = 0; y < k; ++y)
+        if (items[y]->status == B200_OK) items[y]->out->opening_proof = comms[y];
+    return B200_OK;
+}
+
+// Link proofs per link_chunk() call: as many as half the free device memory holds (the batch buffers the context already
+// has count as free), at most kMaxBatchChunk, and below the MSM's 32-bit entry index.  Sized for the batch's longest
+// polynomial and largest transform: per item the workspace, the NTT scratch and the MSM scratch of one commitment.
+// B200_LINK_BATCH_CHUNK overrides it (tests: the bytes out do not depend on the chunk size).
+static size_t link_batch_chunk(Context* c, const Bases* srs, const std::vector<LinkItem>& its) {
+    const size_t k = its.size();
+    if (const char* e = std::getenv("B200_LINK_BATCH_CHUNK")) {
+        const long v = std::atol(e);
+        if (v >= 1) return std::min<size_t>((size_t)v, k);
+    }
+    size_t L = 0, N = 0;
+    for (const LinkItem& it : its) {
+        L = std::max({L, it.len1, it.len2});
+        N = std::max(N, (size_t)1 << it.log_N);
+    }
+    const MsmPlan& pl = srs->plan;
+    const size_t msm_per_item = L * (size_t)pl.n_digits * 4 * 2 + ((size_t)pl.n_phys << (pl.c - 1)) * sizeof(g1_xyzz) * 4;
+    const size_t per_item = (5 * L + 4 * N + 4 * (L / CH + 4 * CH + 64) + 16) * sizeof(fe) + msm_per_item;
+    size_t free_b = 0, total_b = 0;
+    if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) free_b = 0;
+    const Context::BatchBufs& b = c->batch;
+    const size_t budget = (free_b + b.ws.cap + b.nscr.cap) / 2;
+    const size_t idx_cap = ((size_t)1 << 32) / (L * (size_t)pl.n_digits) - 1;  // L * digits * chunk < 2^32
+    return std::max<size_t>(1, std::min({k, kMaxBatchChunk, budget / per_item, idx_cap}));
+}
+
 }  // namespace b200
 
 // ---------------------------------------------------------------------------------------------
@@ -1627,6 +1891,76 @@ int b200_plonk_link(b200_ctx* ctx, const b200_bases* srs, const uint64_t* a1, si
     std::memcpy(&c2, comm2, 64);
     return link(&ctx->c, srs->b, reinterpret_cast<const fe*>(a1), len1, reinterpret_cast<const fe*>(a2), len2, c1, c2,
                 alignment, offset, size, reinterpret_cast<LinkOut*>(proof), reinterpret_cast<fe*>(eta));
+    B200_CATCH
+}
+
+int b200_plonk_link_batch(b200_ctx* ctx, const b200_bases* srs, const b200_link_item* items, size_t k, int* statuses) {
+    B200_TRY
+    if (!ctx || !srs || (k && !items)) {
+        set_error("plonk_link_batch: null argument");
+        return B200_ERR_INVALID;
+    }
+    // every argument error fails the call before any device work (link()'s B200_ERR_INVALID conditions)
+    std::vector<LinkItem> its(k);
+    for (size_t i = 0; i < k; ++i) {
+        const b200_link_item& x = items[i];
+        const std::string item = "plonk_link_batch: item " + std::to_string(i);
+        if (!x.a1 || !x.a2 || !x.comm1 || !x.comm2 || !x.proof) {
+            set_error(item + " has a NULL pointer");
+            return B200_ERR_INVALID;
+        }
+        const size_t len = std::max(x.len1, x.len2);
+        if (x.size == 0 || x.size >= len || x.alignment > 28 || len > srs->b->n) {
+            set_error(item + ": bad group layout or polynomial length");
+            return B200_ERR_INVALID;
+        }
+        unsigned log_N = 1;
+        while (((size_t)1 << log_N) < len) ++log_N;
+        if (log_N > 28) {
+            set_error(item + ": polynomial too long");
+            return B200_ERR_INVALID;
+        }
+        LinkItem& it = its[i];
+        it.a1 = reinterpret_cast<const fe*>(x.a1);
+        it.a2 = reinterpret_cast<const fe*>(x.a2);
+        it.len1 = x.len1;
+        it.len2 = x.len2;
+        std::memcpy(&it.comm1, x.comm1, 64);
+        std::memcpy(&it.comm2, x.comm2, 64);
+        it.alignment = x.alignment;
+        it.offset = x.offset;
+        it.size = x.size;
+        it.out = reinterpret_cast<LinkOut*>(x.proof);
+        it.eta = reinterpret_cast<fe*>(x.eta);
+        it.log_N = log_N;
+        it.status = B200_OK;
+    }
+    if (k == 0) return B200_OK;
+    std::lock_guard<std::mutex> lk(ctx->c.mu);
+    B200_CUDA(cudaSetDevice(ctx->c.device));
+    // items of one transform size next to each other: a chunk divides each size's items with one launch per step
+    std::vector<LinkItem*> order(k);
+    for (size_t i = 0; i < k; ++i) order[i] = &its[i];
+    std::stable_sort(order.begin(), order.end(), [](const LinkItem* a, const LinkItem* b) { return a->log_N < b->log_N; });
+    const size_t chunk = link_batch_chunk(&ctx->c, srs->b, its);
+    for (size_t off = 0; off < k; off += chunk) {
+        const int rc = link_chunk(&ctx->c, srs->b, order.data() + off, (unsigned)std::min(chunk, k - off));
+        if (rc != B200_OK) return rc;
+    }
+    size_t bad = 0;
+    for (size_t i = 0; i < k; ++i) {
+        if (its[i].status != B200_OK) {
+            std::memset(items[i].proof, 0, sizeof(b200_link_proof));
+            ++bad;
+        }
+        if (statuses) statuses[i] = its[i].status;
+    }
+    if (bad) {
+        set_error("plonk_link_batch: " + std::to_string(bad) + " of " + std::to_string(k) +
+                  " item(s) have wire polynomials that differ on the link group (see statuses)");
+        return B200_ERR_UNSATISFIED;
+    }
+    return B200_OK;
     B200_CATCH
 }
 

@@ -24,7 +24,7 @@ namespace {
 struct Bundle;
 
 struct Job {
-    enum Kind { kProve, kProveBatch, kLink } kind = kProve;
+    enum Kind { kProve, kProveBatch, kLink, kLinkBatch } kind = kProve;
     uint64_t ticket = 0;
     // prove
     const b200_pk* pk = nullptr;
@@ -43,6 +43,9 @@ struct Job {
     unsigned alignment = 0;
     size_t offset = 0, size = 0;
     b200_link_proof* link_proof = nullptr;
+    // link batch: the items with comm1 / comm2 pointing into the copies below (8 limbs each, two per item)
+    std::vector<b200_link_item> link_items;
+    std::vector<uint64_t> link_comms;
     std::shared_ptr<Bundle> bundle;  // set for the sub-jobs of a bundle (they carry no ticket of their own)
 };
 
@@ -116,6 +119,8 @@ struct b200_pool {
                                             job->blinders.data(), job->proof, job->link_poly, nullptr);
             } else if (job->kind == Job::kProveBatch) {
                 d.status = b200_plonk_prove_batch(ctxs[w], job->pk, job->items.data(), job->items.size(), job->statuses);
+            } else if (job->kind == Job::kLinkBatch) {
+                d.status = b200_plonk_link_batch(ctxs[w], job->srs, job->link_items.data(), job->link_items.size(), job->statuses);
             } else {
                 d.status = b200_plonk_link(ctxs[w], job->srs, job->a1, job->len1, job->a2, job->len2,
                                            job->comm1, job->comm2, job->alignment, job->offset, job->size,
@@ -291,6 +296,34 @@ int b200_pool_submit_link(b200_pool* pool, const b200_bases* srs, const uint64_t
     j->offset = offset;
     j->size = size;
     j->link_proof = proof;
+    return pool_push(pool, std::move(j), ticket);
+    B200_CATCH
+}
+
+int b200_pool_submit_link_batch(b200_pool* pool, const b200_bases* srs, const b200_link_item* items, size_t k,
+                                int* statuses, uint64_t* ticket) {
+    B200_TRY
+    if (!pool || !srs || (k && !items) || !ticket) {
+        b200::set_error("pool_submit_link_batch: null argument");
+        return B200_ERR_INVALID;
+    }
+    for (size_t i = 0; i < k; ++i)
+        if (!items[i].a1 || !items[i].a2 || !items[i].comm1 || !items[i].comm2 || !items[i].proof) {
+            b200::set_error("pool_submit_link_batch: item " + std::to_string(i) + " has a NULL pointer");
+            return B200_ERR_INVALID;
+        }
+    std::unique_ptr<Job> j(new Job());
+    j->kind = Job::kLinkBatch;
+    j->srs = srs;
+    j->statuses = statuses;
+    j->link_items.assign(items, items + k);
+    j->link_comms.resize(16 * k);
+    for (size_t i = 0; i < k; ++i) {  // the worker reads the copies
+        std::memcpy(&j->link_comms[16 * i], items[i].comm1, 64);
+        std::memcpy(&j->link_comms[16 * i + 8], items[i].comm2, 64);
+        j->link_items[i].comm1 = &j->link_comms[16 * i];
+        j->link_items[i].comm2 = &j->link_comms[16 * i + 8];
+    }
     return pool_push(pool, std::move(j), ticket);
     B200_CATCH
 }

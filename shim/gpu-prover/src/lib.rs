@@ -6,6 +6,7 @@
 //! | `circuit-types/src/traits.rs:996`  | `PlonkKzgSnark::prove_with_link_hint::<_, _, SolidityTranscript>(rng, &circuit, &pk)` | [`GpuProver::prove_with_link_hint`] |
 //! | `circuit-types/src/traits.rs:1012` | `PlonkKzgSnark::verify::<SolidityTranscript>(&vk, pi, &proof, None)` | [`verify`] (host only) |
 //! | `proof_linking/intent_only.rs:42-47` | `PlonkKzgSnark::link_proofs::<SolidityTranscript>(a, b, &layout, &ck)` | [`GpuProver::link_proofs`] |
+//! | `native_proof_manager.rs:726-782` | the four `link_proofs` calls of `compute_private_settlement_link_proofs` | [`GpuProver::link_proofs_batch`] |
 //! | `primitives/srs.rs:63-71` | `parse_ptau_file` + `powers_of_g` | [`GpuProver::load_srs`] |
 //!
 //! Marshalling rules (SURVEY.md §7 "Rust ABI hazards"): `Fr`/`Fq` are `Fp(BigInt<4>, PhantomData)` holding the
@@ -193,6 +194,48 @@ impl GpuProver {
             quotient_commitment: jf_primitives::pcs::prelude::Commitment(g1_from(&raw.quotient_commitment)),
             opening_proof: jf_primitives::pcs::prelude::UnivariateKzgProof { proof: g1_from(&raw.opening_proof) },
         })
+    }
+
+    /// `link_proofs` for many (lhs, rhs, layout) triples, made by one `b200_plonk_link_batch` job on one worker: the
+    /// division runs as one launch per step over the items of one transform size, and the quotient and opening
+    /// commitments are one batched MSM each.  Item i of the result is `link_proofs`' answer for `links[i]`: the proof, or
+    /// `WrongQuotientPolyDegree` when the two polynomials differ on the group.  E.g. the four link proofs of a private
+    /// match (`compute_private_settlement_link_proofs`, native_proof_manager.rs:726-782) in one call.
+    #[allow(clippy::type_complexity)]
+    pub fn link_proofs_batch(&self, links: &[(&LinkingHint<Bn254>, &LinkingHint<Bn254>, &GroupLayout)])
+        -> Vec<Result<mpc_plonk::proof_system::structs::LinkingProof<Bn254>, PlonkError>> {
+        let k = links.len();
+        let polys: Vec<(Vec<u64>, Vec<u64>)> = links.iter().map(|(l, r, _)| (
+            l.linking_wire_poly.coeffs.iter().flat_map(fr_limbs).collect(),
+            r.linking_wire_poly.coeffs.iter().flat_map(fr_limbs).collect())).collect();
+        let comms: Vec<([u64; 8], [u64; 8])> =
+            links.iter().map(|(l, r, _)| (g1_record(&l.linking_wire_comm.0), g1_record(&r.linking_wire_comm.0))).collect();
+        let mut raws: Vec<ffi::b200_link_proof> = (0..k).map(|_| unsafe { std::mem::zeroed() }).collect();
+        let items: Vec<ffi::b200_link_item> = (0..k).map(|i| ffi::b200_link_item {
+            a1: polys[i].0.as_ptr(), len1: polys[i].0.len() / 4, a2: polys[i].1.as_ptr(), len2: polys[i].1.len() / 4,
+            comm1: comms[i].0.as_ptr(), comm2: comms[i].1.as_ptr(), alignment: links[i].2.alignment as c_uint,
+            offset: links[i].2.offset, size: links[i].2.size, proof: &mut raws[i], eta: std::ptr::null_mut(),
+        }).collect();
+        let mut statuses: Vec<c_int> = vec![0; k];
+        let mut ticket = 0u64;
+        let submitted = check(unsafe {
+            ffi::b200_pool_submit_link_batch(self.pool, self.srs, items.as_ptr(), k, statuses.as_mut_ptr(), &mut ticket)
+        });
+        let rc = match submitted {
+            Ok(()) => unsafe { ffi::b200_pool_wait(self.pool, ticket) }, // buffers above stay alive until here
+            Err(e) => return (0..k).map(|_| Err(PlonkError::InvalidParameters(format!("{e:?}")))).collect(),
+        };
+        if rc != ffi::B200_OK && rc != ffi::B200_ERR_UNSATISFIED {
+            let err = check(rc).unwrap_err();
+            return (0..k).map(|_| Err(PlonkError::InvalidParameters(format!("{err:?}")))).collect();
+        }
+        (0..k).map(|i| {
+            check(statuses[i])?;
+            Ok(mpc_plonk::proof_system::structs::LinkingProof {
+                quotient_commitment: jf_primitives::pcs::prelude::Commitment(g1_from(&raws[i].quotient_commitment)),
+                opening_proof: jf_primitives::pcs::prelude::UnivariateKzgProof { proof: g1_from(&raws[i].opening_proof) },
+            })
+        }).collect()
     }
 
     /// Many `verify` / `verify_link_proof` checks with ONE pairing on this GPU (`b200_plonk_batch_verify`).

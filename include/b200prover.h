@@ -233,7 +233,8 @@ typedef struct {
  * `linking_wire_comm`; (alignment, offset, size) = mpc-relation `GroupLayout`: the group sits on
  * the roots g^(offset + i), i < size, g the generator of the 2^alignment-th roots of unity.
  * eta (may be NULL) receives the Fiat–Shamir challenge.  Fails with B200_ERR_UNSATISFIED when a1 and a2
- * do not agree on the group (no link proof exists: wrong layout or mismatched witnesses). */
+ * do not agree on the group (no link proof exists: wrong layout or mismatched witnesses); *proof is zeroed then and
+ * eta is not written. */
 int b200_plonk_link(b200_ctx* ctx, const b200_bases* srs, const uint64_t* a1, size_t len1,
                     const uint64_t* a2, size_t len2, const uint64_t* comm1, const uint64_t* comm2,
                     unsigned alignment, size_t offset, size_t size, b200_link_proof* proof,

@@ -196,7 +196,7 @@ int splitmix_fr_device(uint64_t seed, size_t first, size_t n, int montgomery, fe
 // (`buffers`: a fingerprint of the addresses the launches refer to).
 constexpr int kProofSegs = 7;
 struct ProofGraphSet {
-    uint64_t key = 0, sub[6] = {}, buffers = 0, last_use = 0;  // proofs: key = the proving key's id; link proofs: see link()
+    uint64_t key = 0, sub[6] = {}, buffers = 0, last_use = 0;  // proofs: key = the proving key's id; link proofs: see link_chunk()
     unsigned proofs_seen = 0;
     bool timing = false;  // captured with the MSM's timing events as graph nodes
     cudaGraphExec_t exec[kProofSegs] = {};

@@ -22,6 +22,7 @@
 #include "b200prover.h"
 #include "device_ctx.h"
 #include "transcript.h"
+#include "verify_terms.h"
 
 namespace b200 {
 
@@ -381,27 +382,7 @@ __global__ void k_check_degree(const fe* __restrict__ q, size_t deg, size_t m, u
     }
 }
 
-// out[j] = prod_i (x_j - roots[i]), x_j = g * w^j the j-th point of the coset g * H_N (tw[k] = w^k, k < N/2)
-__global__ void k_vanishing_on_coset(const fe* __restrict__ tw, size_t N, fe g, const fe* __restrict__ roots, size_t count,
-                                     fe* __restrict__ out) {
-    const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= N) return;
-    const size_t half = N >> 1;
-    fe wj = fe_load_ro(tw + (j < half ? j : j - half));
-    if (j >= half) wj = fe_neg<Fr>(wj);
-    const fe x = FMUL(g, wj);
-    fe acc = fe_one<Fr>();
-    for (size_t i = 0; i < count; ++i) acc = FMUL(acc, FSUB(x, fe_load_ro(roots + i)));
-    fe_store(out + j, acc);
-}
-
-// flag |= 1 when any of the `count` elements is non-zero (single small block)
-__global__ void k_any_nonzero(const fe* __restrict__ v, size_t count, uint32_t* flag) {
-    for (size_t i = threadIdx.x; i < count; i += blockDim.x)
-        if (!fe_is_zero(fe_load_ro(v + i))) atomicOr(flag, 1u);
-}
-
-// ---- link proofs in batches: one descriptor per item, blockIdx.y = item --------------------------------------------
+// ---- link proofs: one descriptor per item, blockIdx.y = item ----------------------------------------------------
 struct LinkDesc {
     fe g, root0;        // generator of the layout's 2^alignment roots of unity, and the group's first root g^offset
     uint64_t roots_at;  // where the item's roots start in the batch's root array
@@ -423,7 +404,8 @@ __global__ void k_link_roots(const LinkDesc* __restrict__ d, fe* __restrict__ ro
     fe_store(roots + it->roots_at + i, acc);
 }
 
-// k_vanishing_on_coset for items of one transform size N: item y's values at out + y * N, its roots from its descriptor
+// out[y * N + j] = prod_i (x_j - roots_y[i]), x_j = g * w^j the j-th point of the coset g * H_N (tw[k] = w^k, k < N/2),
+// for the items y of one transform size N, each with its roots from its descriptor
 __global__ void k_vanishing_on_coset_batch(const fe* __restrict__ tw, size_t N, fe g, const fe* __restrict__ roots,
                                            const LinkDesc* __restrict__ d, fe* __restrict__ out) {
     const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1082,6 +1064,12 @@ static ProverBufs batch_bufs(Context* c) {
 // at 10, 2.85 vs 3.86 ms at 64).
 constexpr unsigned kDeviceHornerFrom = 10;
 
+// MsmScratch::in_graph holds only while a prover call runs: cleared on every way out of it
+struct InGraphReset {
+    MsmScratch& s;
+    ~InGraphReset() { s.in_graph = false; }
+};
+
 // The five prover rounds for k proofs of one key.  Every launch covers all k proofs (see Workspace and the kernels'
 // batch index); every commitment round is ONE batched MSM over the k proofs' polynomials; the host runs the k
 // Fiat–Shamir transcripts between rounds, so a batch makes the five host round trips once.
@@ -1119,10 +1107,7 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
     ProofGraphSet* gset = single ? graph_set_for(c, pk->id) : nullptr;
     ProofGraphSet* gs = gset && gset->proofs_seen > 0 ? gset : nullptr;
     bf.msm->in_graph = gs != nullptr;
-    struct InGraphReset {
-        MsmScratch& s;
-        ~InGraphReset() { s.in_graph = false; }
-    } in_graph_reset{*bf.msm};
+    InGraphReset in_graph_reset{*bf.msm};
     ProofParams* hp = reinterpret_cast<ProofParams*>(bf.h_params->p);  // pinned staging copy, one block per proof
     ProofParams* dp = reinterpret_cast<ProofParams*>(bf.d_params->p);  // what the kernels read
     static_assert(sizeof(ProofParams) % sizeof(fe) == 0, "ProofParams is an array of field elements");
@@ -1499,132 +1484,8 @@ struct LinkOut {
 };
 static_assert(sizeof(LinkOut) == sizeof(b200_link_proof), "link proof layout");
 
-static int link(Context* c, const Bases* srs, const fe* h_a1, size_t len1, const fe* h_a2, size_t len2,
-                const g1_affine& comm1, const g1_affine& comm2, unsigned alignment, size_t offset, size_t size,
-                LinkOut* out, fe* h_eta) {
-    const size_t len = len1 > len2 ? len1 : len2;
-    if (size == 0 || size >= len || alignment > 28 || len > srs->n) {
-        set_error("link: bad group layout or polynomial length");
-        return B200_ERR_INVALID;
-    }
-    cudaStream_t st = c->stream;
-    int rc;
-    // Division by Z_D on an evaluation domain: N = 2^k >= len points of the coset g * H_N (Z_D has no root there).
-    // diff / Z_D pointwise, back to coefficients: the quotient when the division is exact — and exact it is iff the
-    // interpolant's degree is len - 1 - size (p * Z_D - diff has degree < N and vanishes on N points).  Two transforms,
-    // one batch inversion and three element-wise kernels instead of `size` dependent synthetic divisions.
-    unsigned log_N = 1;
-    while (((size_t)1 << log_N) < len) ++log_N;
-    if (log_N > 28) {
-        set_error("link: polynomial too long");
-        return B200_ERR_INVALID;
-    }
-    const size_t N = (size_t)1 << log_N;
-    const size_t L = len + 8, NL = N + 8;
-    const size_t scr = 4 * (L / CH + 4 * CH + 64);
-    if ((rc = c->plonk_ws.reserve((5 * L + 3 * NL + scr + size + 16) * sizeof(fe))) != B200_OK) return rc;
-    if ((rc = c->ntt_scratch.reserve(N * sizeof(fe))) != B200_OK) return rc;
-    if ((rc = c->h_small.reserve(4096)) != B200_OK) return rc;
-    if ((rc = c->h_params.reserve(sizeof(ProofParams))) != B200_OK) return rc;
-    if ((rc = c->d_params.reserve(sizeof(ProofParams))) != B200_OK) return rc;
-    Domain* dN = nullptr;
-    if ((rc = get_domain(c, log_N, &dN)) != B200_OK) return rc;
-    fe* base = reinterpret_cast<fe*>(c->plonk_ws.p);
-    fe *d_a1 = base, *d_a2 = base + L, *d_diff = base + 2 * L, *d_ident = base + 3 * L, *d_open = base + 4 * L;
-    fe *d_E = base + 5 * L, *d_Z = d_E + NL, *d_ZS = d_Z + NL;  // evaluations, Z_D on the coset, inversion scratch / quotient
-    fe* hscr = d_ZS + NL;
-    fe* d_roots = hscr + scr;    // the `size` roots of the group's vanishing polynomial
-    fe* slot = d_roots + size;   // 16 spare elements: evaluation slot, then the exactness flag
-    uint32_t* d_flag = reinterpret_cast<uint32_t*>(slot + 4);
-    fe* nscr = reinterpret_cast<fe*>(c->ntt_scratch.p);
-    uint32_t* h_flag = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(c->h_small.p) + 1024);
-    // the launches depend on (context, SRS, lengths, layout) only: two graph segments, like the prover's rounds
-    const uint64_t sub[6] = {srs->id, (uint64_t)len1, (uint64_t)len2, (uint64_t)alignment, (uint64_t)offset, (uint64_t)size};
-    ProofGraphSet* gset = graph_set_for(c, ~(uint64_t)0, sub);
-    ProofGraphSet* gs = gset && gset->proofs_seen > 0 ? gset : nullptr;
-    c->msm.in_graph = gs != nullptr;
-    struct InGraphReset {
-        MsmScratch& s;
-        ~InGraphReset() { s.in_graph = false; }
-    } in_graph_reset{c->msm};
-    LinkParams* hp = reinterpret_cast<LinkParams*>(c->h_params.p);
-    LinkParams* dp = reinterpret_cast<LinkParams*>(c->d_params.p);
-    static_assert(sizeof(LinkParams) <= sizeof(ProofParams), "one parameter block serves both");
-
-    B200_CUDA(cudaMemcpyAsync(d_a1, h_a1, len1 * sizeof(fe), cudaMemcpyDefault, st));  // caller-owned: outside the graphs
-    B200_CUDA(cudaMemcpyAsync(d_a2, h_a2, len2 * sizeof(fe), cudaMemcpyDefault, st));
-    const fe one = fe_one<Fr>();
-    // roots of the link group's vanishing polynomial: g_a^(offset + i), g_a the generator of the 2^alignment roots of unity
-    const fe g = host_root_of_unity(alignment);
-    std::vector<fe> roots(size);
-    fe root = host_pow(g, (uint64_t)offset);
-    const fe root0 = root;
-    for (size_t i = 0; i < size; ++i) {
-        roots[i] = root;
-        root = FMUL(root, g);
-    }
-    fe* d_Q = d_ZS;  // the inversion's scratch is free again after it: quotient evaluations, then coefficients
-    const size_t q_len = len - size;
-    rc = commit_enqueue(c, &c->msm, srs, gs, 0, d_Q, q_len, q_len, 1, [&]() -> int {
-        int r;
-        B200_CUDA(cudaMemsetAsync(d_flag, 0, 4, st));
-        {
-            LinArgs a{};
-            a.count = 2;
-            a.p[0] = d_a1; a.len[0] = (uint32_t)len1; a.s[0] = one;
-            a.p[1] = d_a2; a.len[1] = (uint32_t)len2; a.s[1] = fe_neg<Fr>(one);
-            B200_LAUNCH(k_lincomb, grid_for(len, 128), 128, 0, st)(a, len, d_diff, 0);
-        }
-        fill_powers(d_roots, size, g, root0, st);
-        B200_CUDA(cudaMemsetAsync(d_E, 0, N * sizeof(fe), st));
-        B200_CUDA(cudaMemcpyAsync(d_E, d_diff, len * sizeof(fe), cudaMemcpyDeviceToDevice, st));
-        if ((r = ntt_device(dN, d_E, nscr, /*inverse=*/0, /*coset=*/1, 1, N, st)) != B200_OK) return r;
-        B200_LAUNCH(k_vanishing_on_coset, grid_for(N, 128), 128, 0, st)(dN->tw_fwd, N, fe_from_u32<Fr>(5), d_roots, size, d_Z);
-        batch_inverse_enqueue(nullptr, d_Z, d_ZS, N, st);
-        B200_LAUNCH(k_fr_vec_op, grid_for(N, 256), 256, 0, st)(2, d_E, d_Z, 0, N, d_Q);
-        if ((r = ntt_device(dN, d_Q, nscr, /*inverse=*/1, /*coset=*/1, 1, N, st)) != B200_OK) return r;
-        // a1 and a2 must agree on every root of the group, i.e. the division is exact: otherwise no link proof verifies
-        // and the reference's prover output would be rejected (ADVICE r1: silent bad proof)
-        B200_LAUNCH(k_any_nonzero, 1, 256, 0, st)(d_Q + q_len, N - q_len, d_flag);
-        B200_CUDA(cudaMemcpyAsync(h_flag, d_flag, 4, cudaMemcpyDeviceToHost, st));
-        return B200_OK;
-    });
-    if (rc != B200_OK) return rc;
-    if ((rc = commit_collect(&c->msm, 1, &out->quotient_commitment)) != B200_OK) return rc;
-    if (*h_flag) {
-        set_error("link: the two wire polynomials differ on the link group (wrong layout or mismatched witnesses)");
-        return B200_ERR_UNSATISFIED;
-    }
-    SolidityTranscript tr;
-    tr.append_commitment(comm1);
-    tr.append_commitment(comm2);
-    tr.append_commitment(out->quotient_commitment);
-    const fe eta = tr.get_and_append_challenge();
-    if (h_eta) *h_eta = eta;
-    fe zd = one;
-    for (size_t i = 0; i < size; ++i) zd = FMUL(zd, FSUB(eta, roots[i]));
-    hp->lin_s[0] = one;
-    hp->lin_s[1] = fe_neg<Fr>(zd);
-    fill_open_params(&hp->open, eta);
-    rc = commit_enqueue(c, &c->msm, srs, gs, 1, d_open + 1, len - 1, len - 1, 1, [&]() -> int {
-        B200_CUDA(cudaMemcpyAsync(dp, hp, sizeof(LinkParams), cudaMemcpyHostToDevice, st));
-        LinArgs a{};
-        a.count = 2;
-        a.p[0] = d_diff; a.len[0] = (uint32_t)len;
-        a.p[1] = d_Q; a.len[1] = (uint32_t)q_len;
-        a.dyn = &dp->lin_s[0];
-        B200_LAUNCH(k_lincomb, grid_for(len, 128), 128, 0, st)(a, len, d_ident, 0);
-        horner_suffix(d_ident, len, eta, d_open, slot, hscr, st, &dp->open);
-        return B200_OK;
-    });
-    if (rc != B200_OK) return rc;
-    if ((rc = commit_collect(&c->msm, 1, &out->opening_proof)) != B200_OK) return rc;
-    if (gset && !gs) gset->proofs_seen = 1;
-    return B200_OK;
-}
-
-// One link proof of a batch (b200_plonk_link_batch): its inputs, outputs and status (B200_OK, or B200_ERR_UNSATISFIED
-// when the division by Z_D is not exact).  log_N: the transform size link() would pick for it.
+// One link proof of a link_chunk() call: its inputs, outputs and status (B200_OK, or B200_ERR_UNSATISFIED when the
+// division by Z_D is not exact).  log_N: the size of the transform its division runs on.
 struct LinkItem {
     const fe *a1, *a2;
     size_t len1, len2;
@@ -1637,28 +1498,60 @@ struct LinkItem {
     int status;
 };
 
-// eta of a link proof: link()'s transcript over the two wire commitments and the quotient commitment
-__attribute__((noinline)) static fe link_challenge(const g1_affine& comm1, const g1_affine& comm2, const g1_affine& quot) {
-    SolidityTranscript tr;
-    tr.append_commitment(comm1);
-    tr.append_commitment(comm2);
-    tr.append_commitment(quot);
-    return tr.get_and_append_challenge();
+// Checks the layout and lengths of one link proof and fills `it` from `x` (whose pointers the caller has checked):
+// B200_ERR_INVALID, with a message that starts with `where`, when no link proof is made for them.
+static int link_item(const Bases* srs, const b200_link_item& x, const std::string& where, LinkItem* it) {
+    const size_t len = std::max(x.len1, x.len2);
+    if (x.size == 0 || x.size >= len || x.alignment > 28 || len > srs->n) {
+        set_error(where + ": bad group layout or polynomial length");
+        return B200_ERR_INVALID;
+    }
+    // Division by Z_D on an evaluation domain: N = 2^log_N >= len points of the coset g * H_N (Z_D has no root there).
+    // diff / Z_D pointwise, back to coefficients: the quotient when the division is exact — and exact it is iff the
+    // interpolant's degree is len - 1 - size (p * Z_D - diff has degree < N and vanishes on N points).  Two transforms,
+    // one batch inversion and a few element-wise kernels instead of `size` dependent synthetic divisions.
+    unsigned log_N = 1;
+    while (((size_t)1 << log_N) < len) ++log_N;
+    if (log_N > 28) {
+        set_error(where + ": polynomial too long");
+        return B200_ERR_INVALID;
+    }
+    it->a1 = reinterpret_cast<const fe*>(x.a1);
+    it->a2 = reinterpret_cast<const fe*>(x.a2);
+    it->len1 = x.len1;
+    it->len2 = x.len2;
+    std::memcpy(&it->comm1, x.comm1, 64);
+    std::memcpy(&it->comm2, x.comm2, 64);
+    it->alignment = x.alignment;
+    it->offset = x.offset;
+    it->size = x.size;
+    it->out = reinterpret_cast<LinkOut*>(x.proof);
+    it->eta = reinterpret_cast<fe*>(x.eta);
+    it->log_N = log_N;
+    it->status = B200_OK;
+    return B200_OK;
 }
 
-// k link proofs at once, eager, on Context::batch; the items come sorted by log_N.  The same steps as link(), each one
-// launch (or one batched transform / inversion) over many items:
+// Out of line: inlined into link_chunk, the transcript's std::vector::insert draws a false -Wstringop-overflow from GCC 13
+__attribute__((noinline)) static fe link_eta(const g1_affine& c1, const g1_affine& c2, const g1_affine& cq) {
+    SolidityTranscript tr;
+    return vt::link_challenge(tr, c1, c2, cq);
+}
+
+// k link proofs at once; the items come sorted by log_N.  Each step is one launch (or one batched transform /
+// inversion) over many items:
 //  - the differences a1 - a2 of all k items, `L` = max len apart (zero above each item's own length);
 //  - the division, per group of items of one transform size N: item y's data N apart, its roots and q_len read from its
 //    LinkDesc; the quotients then go to one region `Q` = max q_len apart (zero above each item's own q_len);
 //  - ONE batched MSM of the k quotients; the host runs the k transcripts (eta, Z_D(eta)) in one round trip;
 //  - the openings over the common length L (leading zero coefficients change neither p(eta) nor the quotient's
 //    coefficients, and zero scalars add nothing to a commitment), then ONE batched MSM of the k opening proofs.
-// Each item's bytes are link()'s.  An item whose division is not exact is carried through the launches and gets
-// B200_ERR_UNSATISFIED; its outputs are not written.
-static int link_chunk(Context* c, const Bases* srs, LinkItem* const* items, unsigned k) {
+// An item whose division is not exact is carried through the launches and gets B200_ERR_UNSATISFIED; its outputs are
+// not written.
+// single: b200_plonk_link (k = 1 on the context's own buffers, its two segments replayed as CUDA graphs from the second
+// call with the same SRS, lengths and layout on); otherwise a batch, eager, on Context::batch.
+static int link_chunk(Context* c, const ProverBufs& bf, const Bases* srs, LinkItem* const* items, unsigned k, bool single) {
     cudaStream_t st = c->stream;
-    Context::BatchBufs& b = c->batch;
     int rc;
     size_t L = 0, Q = 0, n_roots = 0, max_size = 0, max_group = 0;
     for (unsigned y = 0; y < k; ++y) {
@@ -1680,33 +1573,44 @@ static int link_chunk(Context* c, const Bases* srs, LinkItem* const* items, unsi
     const size_t desc_n = (size_t)k * sizeof(LinkDesc) / sizeof(fe);
     const size_t flag_n = ((size_t)k * 4 + sizeof(fe) - 1) / sizeof(fe);
     const size_t kL = (size_t)k * L, kQ = (size_t)k * Q;
-    if ((rc = b.ws.reserve((3 * kL + kQ + 3 * max_group + hscr_n + n_roots + k + desc_n + flag_n) * sizeof(fe))) != B200_OK)
+    if ((rc = bf.ws->reserve((3 * kL + kQ + 3 * max_group + hscr_n + n_roots + k + desc_n + flag_n) * sizeof(fe))) != B200_OK)
         return rc;
-    if ((rc = b.nscr.reserve(max_group * sizeof(fe))) != B200_OK) return rc;
+    if ((rc = bf.nscr->reserve(max_group * sizeof(fe))) != B200_OK) return rc;
     const size_t desc_bytes = (size_t)k * sizeof(LinkDesc);
-    if ((rc = b.h_small.reserve(desc_bytes + (size_t)k * 4)) != B200_OK) return rc;
-    if ((rc = b.h_params.reserve(k * sizeof(LinkParams))) != B200_OK) return rc;
-    if ((rc = b.d_params.reserve(k * sizeof(LinkParams))) != B200_OK) return rc;
+    if ((rc = bf.h_small->reserve(desc_bytes + (size_t)k * 4)) != B200_OK) return rc;
+    if ((rc = bf.h_params->reserve(k * sizeof(LinkParams))) != B200_OK) return rc;
+    if ((rc = bf.d_params->reserve(k * sizeof(LinkParams))) != B200_OK) return rc;
     std::vector<Domain*> doms(grp.size() - 1);
     for (size_t g = 0; g + 1 < grp.size(); ++g)
         if ((rc = get_domain(c, items[grp[g]]->log_N, &doms[g])) != B200_OK) return rc;
 
-    fe* base = reinterpret_cast<fe*>(b.ws.p);
+    fe* base = reinterpret_cast<fe*>(bf.ws->p);
     fe *d_a1 = base, *d_a2 = d_a1 + kL, *d_diff = d_a2 + kL, *d_quot = d_diff + kL;
     fe *d_E = d_quot + kQ, *d_Z = d_E + max_group, *d_ZS = d_Z + max_group;  // one group's evaluations, Z_D, scratch
     fe *hscr = d_ZS + max_group, *d_roots = hscr + hscr_n, *d_tot = d_roots + n_roots;
     LinkDesc* d_desc = reinterpret_cast<LinkDesc*>(d_tot + k);
     uint32_t* d_flag = reinterpret_cast<uint32_t*>(d_tot + k + desc_n);
     fe *d_ident = d_a1, *d_open = d_a2;  // free again once the differences are formed
-    fe* nscr = reinterpret_cast<fe*>(b.nscr.p);
-    LinkDesc* h_desc = reinterpret_cast<LinkDesc*>(b.h_small.p);
-    uint32_t* h_flag = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(b.h_small.p) + desc_bytes);
-    LinkParams* hp = reinterpret_cast<LinkParams*>(b.h_params.p);
-    LinkParams* dp = reinterpret_cast<LinkParams*>(b.d_params.p);
+    fe* nscr = reinterpret_cast<fe*>(bf.nscr->p);
+    LinkDesc* h_desc = reinterpret_cast<LinkDesc*>(bf.h_small->p);
+    uint32_t* h_flag = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(bf.h_small->p) + desc_bytes);
+    LinkParams* hp = reinterpret_cast<LinkParams*>(bf.h_params->p);
+    LinkParams* dp = reinterpret_cast<LinkParams*>(bf.d_params->p);
     constexpr size_t D = sizeof(LinkParams) / sizeof(fe);
-    MsmScratch* msm = &b.msm;
-    msm->host_horner = k < kDeviceHornerFrom;
+    MsmScratch* msm = bf.msm;
     const fe one = fe_one<Fr>();
+
+    // graphs: only once a call with this key has run eagerly on this context.  The launches depend on (context, SRS,
+    // lengths, group size) only, as the layout reaches them through LinkDesc; alignment and offset stay in the key all
+    // the same, so that every layout's first call runs eagerly.
+    const LinkItem& i0 = *items[0];
+    const uint64_t sub[6] = {srs->id, (uint64_t)i0.len1, (uint64_t)i0.len2, (uint64_t)i0.alignment, (uint64_t)i0.offset,
+                             (uint64_t)i0.size};
+    ProofGraphSet* gset = single ? graph_set_for(c, ~(uint64_t)0, sub) : nullptr;
+    ProofGraphSet* gs = gset && gset->proofs_seen > 0 ? gset : nullptr;
+    msm->in_graph = gs != nullptr;
+    InGraphReset in_graph_reset{*msm};
+    if (!single) msm->host_horner = k < kDeviceHornerFrom;
 
     size_t at = 0;
     for (unsigned y = 0; y < k; ++y) {
@@ -1720,13 +1624,14 @@ static int link_chunk(Context* c, const Bases* srs, LinkItem* const* items, unsi
         d.pad = 0;
         at += it.size;
     }
-    rc = commit_enqueue(c, msm, srs, nullptr, 0, d_quot, Q, Q, k, [&]() -> int {
+    // caller-owned host or device pointers (UVA) are copied outside the graphs (their addresses change from call to call)
+    B200_CUDA(cudaMemsetAsync(d_a1, 0, 2 * kL * sizeof(fe), st));
+    for (unsigned y = 0; y < k; ++y) {
+        B200_CUDA(cudaMemcpyAsync(d_a1 + (size_t)y * L, items[y]->a1, items[y]->len1 * sizeof(fe), cudaMemcpyDefault, st));
+        B200_CUDA(cudaMemcpyAsync(d_a2 + (size_t)y * L, items[y]->a2, items[y]->len2 * sizeof(fe), cudaMemcpyDefault, st));
+    }
+    rc = commit_enqueue(c, msm, srs, gs, 0, d_quot, Q, Q, k, [&]() -> int {
         int r;
-        B200_CUDA(cudaMemsetAsync(d_a1, 0, 2 * kL * sizeof(fe), st));
-        for (unsigned y = 0; y < k; ++y) {  // caller-owned host or device pointers (UVA)
-            B200_CUDA(cudaMemcpyAsync(d_a1 + (size_t)y * L, items[y]->a1, items[y]->len1 * sizeof(fe), cudaMemcpyDefault, st));
-            B200_CUDA(cudaMemcpyAsync(d_a2 + (size_t)y * L, items[y]->a2, items[y]->len2 * sizeof(fe), cudaMemcpyDefault, st));
-        }
         B200_CUDA(cudaMemcpyAsync(d_desc, h_desc, desc_bytes, cudaMemcpyHostToDevice, st));
         B200_CUDA(cudaMemsetAsync(d_flag, 0, (size_t)k * 4, st));
         B200_CUDA(cudaMemsetAsync(d_quot, 0, kQ * sizeof(fe), st));
@@ -1753,6 +1658,8 @@ static int link_chunk(Context* c, const Bases* srs, LinkItem* const* items, unsi
             batch_inverse_enqueue(nullptr, d_Z, d_ZS, kN, st);
             B200_LAUNCH(k_fr_vec_op, grid_for(kN, 256), 256, 0, st)(2, d_E, d_Z, 0, kN, d_ZS);
             if ((r = ntt_device(dN, d_ZS, nscr, /*inverse=*/1, /*coset=*/1, kg, N, st)) != B200_OK) return r;
+            // a1 and a2 must agree on every root of the group, i.e. the division is exact: otherwise no link proof
+            // verifies and the reference's prover output would be rejected
             B200_LAUNCH(k_check_zero_tail, dim3(grid_for(N - min_q, 256), kg), 256, 0, st)(d_ZS, N, d_desc + y0, d_flag + y0);
             // exact items are zero from q_len on, so min(Q, N) coefficients carry the whole quotient
             B200_CUDA(cudaMemcpy2DAsync(d_quot + (size_t)y0 * Q, Q * sizeof(fe), d_ZS, N * sizeof(fe), std::min(Q, N) * sizeof(fe), kg,
@@ -1778,20 +1685,14 @@ static int link_chunk(Context* c, const Bases* srs, LinkItem* const* items, unsi
         ++proved;
         it.status = B200_OK;
         it.out->quotient_commitment = comms[y];
-        const fe eta = link_challenge(it.comm1, it.comm2, comms[y]);
+        const fe eta = link_eta(it.comm1, it.comm2, comms[y]);
         if (it.eta) *it.eta = eta;
-        fe zd = one, root = h_desc[y].root0;
-        for (size_t i = 0; i < it.size; ++i) {
-            zd = FMUL(zd, FSUB(eta, root));
-            root = FMUL(root, h_desc[y].g);
-        }
         p.lin_s[0] = one;
-        p.lin_s[1] = fe_neg<Fr>(zd);
+        p.lin_s[1] = fe_neg<Fr>(vt::link_zd(eta, h_desc[y].g, it.offset, it.size));
         fill_open_params(&p.open, eta);
     }
     if (!proved) return B200_OK;  // see the statuses
-    msm->host_horner = k < kDeviceHornerFrom;
-    rc = commit_enqueue(c, msm, srs, nullptr, 0, d_open + 1, L - 1, L, k, [&]() -> int {
+    rc = commit_enqueue(c, msm, srs, gs, 1, d_open + 1, L - 1, L, k, [&]() -> int {
         B200_CUDA(cudaMemcpyAsync(dp, hp, k * sizeof(LinkParams), cudaMemcpyHostToDevice, st));
         LinArgs a{};
         a.count = 2;
@@ -1812,6 +1713,7 @@ static int link_chunk(Context* c, const Bases* srs, LinkItem* const* items, unsi
     if ((rc = commit_collect(msm, k, comms.data())) != B200_OK) return rc;
     for (unsigned y = 0; y < k; ++y)
         if (items[y]->status == B200_OK) items[y]->out->opening_proof = comms[y];
+    if (gset && !gs) gset->proofs_seen = 1;  // both segments have run eagerly: the next call with this key captures them
     return B200_OK;
 }
 
@@ -1884,13 +1786,19 @@ int b200_plonk_link(b200_ctx* ctx, const b200_bases* srs, const uint64_t* a1, si
                     size_t size, b200_link_proof* proof, uint64_t* eta) {
     B200_TRY
     if (!ctx || !srs || !a1 || !a2 || !comm1 || !comm2 || !proof) return B200_ERR_INVALID;
+    LinkItem it;
+    int rc = link_item(srs->b, b200_link_item{a1, len1, a2, len2, comm1, comm2, alignment, offset, size, proof, eta}, "link", &it);
+    if (rc != B200_OK) return rc;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
     B200_CUDA(cudaSetDevice(ctx->c.device));
-    g1_affine c1, c2;
-    std::memcpy(&c1, comm1, 64);
-    std::memcpy(&c2, comm2, 64);
-    return link(&ctx->c, srs->b, reinterpret_cast<const fe*>(a1), len1, reinterpret_cast<const fe*>(a2), len2, c1, c2,
-                alignment, offset, size, reinterpret_cast<LinkOut*>(proof), reinterpret_cast<fe*>(eta));
+    LinkItem* one = &it;
+    if ((rc = link_chunk(&ctx->c, single_bufs(&ctx->c), srs->b, &one, 1, /*single=*/true)) != B200_OK) return rc;
+    if (it.status != B200_OK) {
+        std::memset(proof, 0, sizeof(b200_link_proof));
+        set_error("link: the two wire polynomials differ on the link group (wrong layout or mismatched witnesses)");
+        return B200_ERR_UNSATISFIED;
+    }
+    return B200_OK;
     B200_CATCH
 }
 
@@ -1900,7 +1808,7 @@ int b200_plonk_link_batch(b200_ctx* ctx, const b200_bases* srs, const b200_link_
         set_error("plonk_link_batch: null argument");
         return B200_ERR_INVALID;
     }
-    // every argument error fails the call before any device work (link()'s B200_ERR_INVALID conditions)
+    // every argument error fails the call before any device work (b200_plonk_link's B200_ERR_INVALID conditions)
     std::vector<LinkItem> its(k);
     for (size_t i = 0; i < k; ++i) {
         const b200_link_item& x = items[i];
@@ -1909,31 +1817,8 @@ int b200_plonk_link_batch(b200_ctx* ctx, const b200_bases* srs, const b200_link_
             set_error(item + " has a NULL pointer");
             return B200_ERR_INVALID;
         }
-        const size_t len = std::max(x.len1, x.len2);
-        if (x.size == 0 || x.size >= len || x.alignment > 28 || len > srs->b->n) {
-            set_error(item + ": bad group layout or polynomial length");
-            return B200_ERR_INVALID;
-        }
-        unsigned log_N = 1;
-        while (((size_t)1 << log_N) < len) ++log_N;
-        if (log_N > 28) {
-            set_error(item + ": polynomial too long");
-            return B200_ERR_INVALID;
-        }
-        LinkItem& it = its[i];
-        it.a1 = reinterpret_cast<const fe*>(x.a1);
-        it.a2 = reinterpret_cast<const fe*>(x.a2);
-        it.len1 = x.len1;
-        it.len2 = x.len2;
-        std::memcpy(&it.comm1, x.comm1, 64);
-        std::memcpy(&it.comm2, x.comm2, 64);
-        it.alignment = x.alignment;
-        it.offset = x.offset;
-        it.size = x.size;
-        it.out = reinterpret_cast<LinkOut*>(x.proof);
-        it.eta = reinterpret_cast<fe*>(x.eta);
-        it.log_N = log_N;
-        it.status = B200_OK;
+        const int rc = link_item(srs->b, x, item, &its[i]);
+        if (rc != B200_OK) return rc;
     }
     if (k == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
@@ -1944,7 +1829,8 @@ int b200_plonk_link_batch(b200_ctx* ctx, const b200_bases* srs, const b200_link_
     std::stable_sort(order.begin(), order.end(), [](const LinkItem* a, const LinkItem* b) { return a->log_N < b->log_N; });
     const size_t chunk = link_batch_chunk(&ctx->c, srs->b, its);
     for (size_t off = 0; off < k; off += chunk) {
-        const int rc = link_chunk(&ctx->c, srs->b, order.data() + off, (unsigned)std::min(chunk, k - off));
+        const int rc = link_chunk(&ctx->c, batch_bufs(&ctx->c), srs->b, order.data() + off, (unsigned)std::min(chunk, k - off),
+                                  /*single=*/false);
         if (rc != B200_OK) return rc;
     }
     size_t bad = 0;

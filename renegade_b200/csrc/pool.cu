@@ -35,18 +35,23 @@ struct Job {
     // prove batch: the items with pub_inputs / blinders pointing into the copies below (pub_inputs, blinders: k each)
     std::vector<b200_prove_item> items;
     int* statuses = nullptr;
-    // link
+    // link (one item) and link batch: the items with comm1 / comm2 pointing into the copies below (8 limbs each, two per
+    // item)
     const b200_bases* srs = nullptr;
-    const uint64_t *a1 = nullptr, *a2 = nullptr;
-    size_t len1 = 0, len2 = 0;
-    uint64_t comm1[8], comm2[8];
-    unsigned alignment = 0;
-    size_t offset = 0, size = 0;
-    b200_link_proof* link_proof = nullptr;
-    // link batch: the items with comm1 / comm2 pointing into the copies below (8 limbs each, two per item)
     std::vector<b200_link_item> link_items;
     std::vector<uint64_t> link_comms;
     std::shared_ptr<Bundle> bundle;  // set for the sub-jobs of a bundle (they carry no ticket of their own)
+
+    void set_link_items(const b200_link_item* its, size_t k) {  // the worker reads the copies
+        link_items.assign(its, its + k);
+        link_comms.resize(16 * k);
+        for (size_t i = 0; i < k; ++i) {
+            std::memcpy(&link_comms[16 * i], its[i].comm1, 64);
+            std::memcpy(&link_comms[16 * i + 8], its[i].comm2, 64);
+            link_items[i].comm1 = &link_comms[16 * i];
+            link_items[i].comm2 = &link_comms[16 * i + 8];
+        }
+    }
 };
 
 struct Done {
@@ -88,16 +93,11 @@ struct b200_pool {
         j->kind = Job::kLink;
         j->bundle = b;
         j->srs = b->srs;
-        j->a1 = pa.link_poly;
-        j->len1 = ((size_t)1 << b200_pk_log_n(pa.pk)) + 2;
-        j->a2 = pb.link_poly;
-        j->len2 = ((size_t)1 << b200_pk_log_n(pb.pk)) + 2;
-        std::memcpy(j->comm1, pa.proof->wires_poly_comms[0], sizeof j->comm1);  // `linking_wire_comm` of each hint
-        std::memcpy(j->comm2, pb.proof->wires_poly_comms[0], sizeof j->comm2);
-        j->alignment = l.alignment;
-        j->offset = l.offset;
-        j->size = l.size;
-        j->link_proof = l.proof;
+        // comm1 / comm2: the `linking_wire_comm` of each hint
+        const b200_link_item it{pa.link_poly, ((size_t)1 << b200_pk_log_n(pa.pk)) + 2, pb.link_poly,
+                                ((size_t)1 << b200_pk_log_n(pb.pk)) + 2, pa.proof->wires_poly_comms[0], pb.proof->wires_poly_comms[0],
+                                l.alignment, l.offset, l.size, l.proof, nullptr};
+        j->set_link_items(&it, 1);
         return j;
     }
 
@@ -121,10 +121,10 @@ struct b200_pool {
                 d.status = b200_plonk_prove_batch(ctxs[w], job->pk, job->items.data(), job->items.size(), job->statuses);
             } else if (job->kind == Job::kLinkBatch) {
                 d.status = b200_plonk_link_batch(ctxs[w], job->srs, job->link_items.data(), job->link_items.size(), job->statuses);
-            } else {
-                d.status = b200_plonk_link(ctxs[w], job->srs, job->a1, job->len1, job->a2, job->len2,
-                                           job->comm1, job->comm2, job->alignment, job->offset, job->size,
-                                           job->link_proof, nullptr);
+            } else {  // a single link stays on b200_plonk_link, which replays its CUDA graphs
+                const b200_link_item& x = job->link_items[0];
+                d.status = b200_plonk_link(ctxs[w], job->srs, x.a1, x.len1, x.a2, x.len2, x.comm1, x.comm2, x.alignment,
+                                           x.offset, x.size, x.proof, x.eta);
             }
             if (d.status != B200_OK) d.message = b200_last_error();  // this worker's thread-local message
             bool new_jobs = false;
@@ -286,16 +286,8 @@ int b200_pool_submit_link(b200_pool* pool, const b200_bases* srs, const uint64_t
     std::unique_ptr<Job> j(new Job());
     j->kind = Job::kLink;
     j->srs = srs;
-    j->a1 = a1;
-    j->len1 = len1;
-    j->a2 = a2;
-    j->len2 = len2;
-    std::memcpy(j->comm1, comm1, sizeof j->comm1);
-    std::memcpy(j->comm2, comm2, sizeof j->comm2);
-    j->alignment = alignment;
-    j->offset = offset;
-    j->size = size;
-    j->link_proof = proof;
+    const b200_link_item it{a1, len1, a2, len2, comm1, comm2, alignment, offset, size, proof, nullptr};
+    j->set_link_items(&it, 1);
     return pool_push(pool, std::move(j), ticket);
     B200_CATCH
 }
@@ -316,14 +308,7 @@ int b200_pool_submit_link_batch(b200_pool* pool, const b200_bases* srs, const b2
     j->kind = Job::kLinkBatch;
     j->srs = srs;
     j->statuses = statuses;
-    j->link_items.assign(items, items + k);
-    j->link_comms.resize(16 * k);
-    for (size_t i = 0; i < k; ++i) {  // the worker reads the copies
-        std::memcpy(&j->link_comms[16 * i], items[i].comm1, 64);
-        std::memcpy(&j->link_comms[16 * i + 8], items[i].comm2, 64);
-        j->link_items[i].comm1 = &j->link_comms[16 * i];
-        j->link_items[i].comm2 = &j->link_comms[16 * i + 8];
-    }
+    j->set_link_items(items, k);
     return pool_push(pool, std::move(j), ticket);
     B200_CATCH
 }

@@ -111,6 +111,7 @@ def test_link_proofs_replayed(ctx, oracle, pyoracle):
     bases = ctx.load_bases(srs)
     ctx.use_graphs(True)
     g0 = ctx.graph_launches()
+    kept = []  # every round's hints stay alive: each call reads polynomials at addresses no earlier call used
     for rnd in range(4):
         vals = [(i * 0x9E3779B97F4A7C15 + 777 * rnd + 5) % py.R for i in range(layout.size)]
         hints = []
@@ -120,6 +121,7 @@ def test_link_proofs_replayed(ctx, oracle, pyoracle):
             _, hint = PlonkKzgSnark.prove_with_link_hint(ctx, pk, circ.wires, circ.pub_inputs, synth.splitmix_blinders(seed + rnd))
             pk.free()
             hints.append(hint)
+        kept.append(hints)
         lp, eta = link_proofs(ctx, bases, hints[0], hints[1], layout)
         rc, olp, oeta = oracle.plonk_link(hints[0].linking_wire_poly, hints[1].linking_wire_poly, hints[0].linking_wire_comm,
                                           hints[1].linking_wire_comm, layout.alignment, layout.offset, layout.size, srs)

@@ -48,6 +48,16 @@ def test_link_two_circuits(ctx, oracle, pyoracle):
     with pytest.raises(B200Error) as err:      # the prover refuses: a division by the group's roots is not exact
         link_proofs(ctx, bases, hints[0], hints[1], wrong)
     assert err.value.code == -7
+    # the refused call zeroes the caller's proof buffer and leaves its eta buffer alone
+    import ctypes as C
+    from renegade_b200.backend import B200LinkProof
+    a1, a2, c1, c2 = (np.ascontiguousarray(x, dtype=np.uint64) for x in (hints[0].linking_wire_poly, hints[1].linking_wire_poly,
+                                                                         hints[0].linking_wire_comm, hints[1].linking_wire_comm))
+    junk, eta_buf = B200LinkProof.from_buffer_copy(b"\xa5" * C.sizeof(B200LinkProof)), np.full(4, 7, dtype=np.uint64)
+    vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+    assert (ctx._lib.b200_plonk_link(ctx._h, bases._h, vp(a1), a1.size // 4, vp(a2), a2.size // 4, vp(c1), vp(c2), wrong.alignment,
+                                     wrong.offset, wrong.size, C.byref(junk), vp(eta_buf)) == -7
+            and bytes(junk) == bytes(C.sizeof(B200LinkProof)) and (eta_buf == 7).all())
     rc, _, _ = oracle.plonk_link(hints[0].linking_wire_poly, hints[1].linking_wire_poly, hints[0].linking_wire_comm,
                                  hints[1].linking_wire_comm, wrong.alignment, wrong.offset, wrong.size, srs)
     assert rc == 2

@@ -91,7 +91,7 @@ int b200_srs_parse_ptau(const uint8_t* bytes, size_t len, const uint8_t** g1_rec
  * work), 1 for LATENCY (one MSM at a time: shortest dependent chains; e.g. c = 16 instead of 15 at 2^13
  * points), 8..23 fixes it.  The result does not depend on the window.
  * check_on_curve != 0 repeats the reference's `is_on_curve` assertion (srs.rs:178-179) on the
- * device and fails with B200_ERR_NOT_ON_CURVE. */
+ * device and fails with B200_ERR_NOT_ON_CURVE (a coordinate >= q counts as off the curve). */
 int b200_bases_load(b200_ctx* ctx, const uint8_t* points64, size_t n, int window_bits,
                     int check_on_curve, b200_bases** out);
 /* Same, from points already in device memory (device pointer). */
@@ -268,7 +268,10 @@ int b200_plonk_link_batch(b200_ctx* ctx, const b200_bases* srs, const b200_link_
 /* ---- verification (host only; no device is needed or used) -----------------------------------
  * G2 points are 128-byte records x0 || x1 || y0 || y1 (Montgomery Fq), the layout of the ptau file's
  * G2 section read by srs.rs:185-199: g2_h = `UnivariateUniversalParams.h`, g2_tau_h = `.beta_h`.
- * *accepted = 1 / 0; a malformed (off-curve) proof element is a rejection, not an error. */
+ * *accepted = 1 / 0; a malformed proof element is a rejection, not an error.  Malformed: a G1 point off the curve,
+ * or any field element outside [0, p) (a coordinate >= q; a public input, evaluation or vk.k >= r) — the
+ * Montgomery limbs of a * 2^256 mod p are below p, so v + p is not another encoding of v.  A G2 record with a
+ * coordinate >= q is off the curve: B200_ERR_NOT_ON_CURVE, here and in b200_pairing_check. */
 /* Replaces `PlonkKzgSnark::<Bn254>::verify::<SolidityTranscript>(&vk, public_inputs, &proof, None)`
  * (traits.rs:1012-1018, reached from `SingleProverCircuit::verify`, traits.rs:1003-1019).  The
  * verifying key is passed flat: domain size 2^log_n, num_inputs, k[5], the 13 selector and 5 sigma
@@ -321,9 +324,11 @@ typedef struct {
  * b200_plonk_verify / b200_plonk_verify_link with the same G2 pair.  verdicts (may be NULL): n_proofs + n_links bytes,
  * verdicts[i] = that single verifier's answer for item i; when the combined check fails the failing items are found
  * by bisection over subsets (each step one MSM pair and one pairing).  With verdicts NULL the call stops after the
- * combined check.  An item with an off-curve G1 point is rejected (verdict 0) and left out of the combination.
- * Errors: B200_ERR_NOT_ON_CURVE for an off-curve G2 point; B200_ERR_INVALID for a vk index out of range, log_n > 28,
- * a link with alignment > 28 or size == 0, or a NULL pointer.  Zero items are accepted. */
+ * combined check.  An item with an off-curve G1 point or a field element outside [0, p) is rejected (verdict 0) and
+ * left out of the combination.
+ * Errors: B200_ERR_NOT_ON_CURVE for an off-curve G2 point (a coordinate >= q included); B200_ERR_INVALID for a vk
+ * index out of range, log_n > 28, a link with alignment > 28 or size == 0, or a NULL pointer.  Zero items are
+ * accepted. */
 int b200_plonk_batch_verify(b200_ctx* ctx, const b200_verifying_key* vks, size_t n_vks, const b200_batch_proof* proofs,
                             size_t n_proofs, const b200_batch_link* links, size_t n_links, const uint64_t g2_h[16],
                             const uint64_t g2_tau_h[16], int* all_accepted, uint8_t* verdicts);

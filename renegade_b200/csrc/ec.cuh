@@ -161,7 +161,9 @@ FF_HD g1_xyzz g1_mul_bits(const g1_affine& p, const fe& k, int bits) {
     return acc;
 }
 
+// also false for a coordinate outside [0, q): (x + q, y) would otherwise pass as a second encoding of (x, y)
 FF_HD bool g1_affine_on_curve(const g1_affine& p) {
+    if (!fe_is_canonical<Fq>(p.x) || !fe_is_canonical<Fq>(p.y)) return false;
     if (g1_affine_is_inf(p)) return true;
     fe lhs = fe_sqr<Fq>(p.y);
     fe rhs = fe_add<Fq>(fe_mul<Fq>(fe_sqr<Fq>(p.x), p.x), fe_from_u32<Fq>(3));

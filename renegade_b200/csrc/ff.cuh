@@ -747,6 +747,15 @@ FF_HD bool limbs_ge(const uint32_t* x, const uint32_t* y) {
         if (x[i] != y[i]) return x[i] > y[i];
     return true;
 }
+// The limbs encode an element of the field: a Montgomery residue a 2^256 mod p lies in [0, p).  Everything above maps
+// to the same residue under fe_mul but not under fe_add / fe_sub, so a verifier refuses it where it enters.
+template <class C>
+FF_HD bool fe_is_canonical(const fe& a) {
+    uint32_t m[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) m[i] = C::mod(i);
+    return !limbs_ge(a.l, m);
+}
 FF_HD void limbs_sub(uint32_t* x, const uint32_t* y) {  // x -= y (x >= y)
     int64_t br = 0;
 #pragma unroll

@@ -373,7 +373,10 @@ fq12 final_exponentiation(const fq12& f) {
     return fq12_mul(fq12_frob1(fq12_frob2(y15)), y14);  // q^3 = q o q^2
 }
 
+// false for a coordinate outside [0, q) too, as g1_affine_on_curve
 bool g2_on_curve(const g2_affine& p) {
+    for (const fe* c : {&p.x.a, &p.x.b, &p.y.a, &p.y.b})
+        if (!fe_is_canonical<Fq>(*c)) return false;
     if (p.inf) return true;
     // b' = 3 / (9 + u) = 3 (9 - u) / 82
     const fe inv82 = fe_inv<Fq>(fe_from_u32<Fq>(82));
@@ -503,7 +506,8 @@ int b200_plonk_verify(unsigned log_n, size_t num_inputs, const uint64_t* k, cons
     const g1_affine* sel = reinterpret_cast<const g1_affine*>(selector_comms);
     const g1_affine* sig = reinterpret_cast<const g1_affine*>(sigma_comms);
     const fe* pi = reinterpret_cast<const fe*>(pub_inputs);
-    if (!vt::plonk_points_on_curve(sel, sig, proof)) return B200_OK;  // rejected
+    if (!vt::plonk_points_on_curve(sel, sig, proof) || !vt::plonk_scalars_canonical(kk, pi, num_inputs, proof))
+        return B200_OK;  // rejected
     // ---- challenges (same transcript as the prover, plonk.cu) ------------------------------------------------
     SolidityTranscript tr;
     const vt::PlonkChallenges ch = vt::plonk_challenges(tr, log_n, num_inputs, kk, sel, sig, pi, proof);

@@ -22,7 +22,7 @@
 //   6. Bases (gathered on the device by k_gather_bases, no window tables: they are used once), msm_device_batch with
 //      A and B, and ONE pairing.  If it fails and verdicts are asked for, the failing items are found by bisection:
 //      each step re-merges a subset from the per-item scalars already on the device (masked merge, MSM, one pairing).
-// An item with an off-curve point is rejected and left out of the combination.
+// An item with an off-curve point or a field element outside [0, p) is rejected and left out of the combination.
 #include <cstring>
 #include <mutex>
 #include <vector>
@@ -62,7 +62,7 @@ struct ItemDev {
 };
 struct ItemState {  // what k_prepare leaves for k_scalars
     vt::PlonkChallenges ch;  // link: zeta = eta, beta = Z_D(eta)
-    uint32_t ok;             // every point on the curve (and the transcript fitted its buffer)
+    uint32_t ok;             // every point on the curve, every scalar below r (and the transcript fitted its buffer)
 };
 struct Roots {
     fe g[kMaxAlign + 1];  // generator of the 2^a-th roots of unity
@@ -101,7 +101,8 @@ __global__ void __launch_bounds__(128) k_prepare(const ItemDev* __restrict__ ite
     if (it.kind == 0) {
         const VkDev& vk = vks[it.vk];
         const vt::ProofIn& proof = proofs[it.idx];
-        bool ok = vt::plonk_points_on_curve(vk.sel, vk.sig, proof);
+        bool ok = vt::plonk_points_on_curve(vk.sel, vk.sig, proof) &&
+                  vt::plonk_scalars_canonical(vk.k, pi + it.pi_off, vk.num_inputs, proof);
         SolidityTranscriptT<SpanBytes> tr(SpanBytes{tr_bytes + it.tr_off, 0, it.tr_cap, false});
         out.ch = vt::plonk_challenges(tr, vk.log_n, vk.num_inputs, vk.k, vk.sel, vk.sig, pi + it.pi_off, proof);
         ok = ok && !tr.bytes().overflow;

@@ -82,6 +82,17 @@ FF_HD bool plonk_points_on_curve(const g1_affine* sel, const g1_affine* sig, con
     return ok;
 }
 
+// every scalar the verifier reads must be an element of Fr, i.e. below r: the key's k, the public inputs and the
+// proof's evaluations.  The transcript reduces what it hashes, so v + r would give the same challenges as v.
+FF_HD bool plonk_scalars_canonical(const fe* kk, const fe* pi, size_t num_inputs, const ProofIn& proof) {
+    bool ok = true;
+    for (int i = 0; i < NW; ++i) ok = ok && fe_is_canonical<FrCfg>(kk[i]);
+    for (size_t i = 0; i < num_inputs; ++i) ok = ok && fe_is_canonical<FrCfg>(pi[i]);
+    for (int i = 0; i < NW; ++i) ok = ok && fe_is_canonical<FrCfg>(proof.wires_evals[i]);
+    for (int i = 0; i < NW - 1; ++i) ok = ok && fe_is_canonical<FrCfg>(proof.wire_sigma_evals[i]);
+    return ok && fe_is_canonical<FrCfg>(proof.perm_next_eval);
+}
+
 struct PlonkChallenges {
     fe beta, gamma, alpha, zeta, v, u;
 };

@@ -221,7 +221,7 @@ def parse_ptau_file(ctx: Context, data: bytes, window_bits: int = 0,
     _lib.check(lib.b200_srs_parse_ptau(C.cast(buf, C.c_void_p), len(data), C.byref(rec), C.byref(n)))
     need = MAX_SRS_DEGREE + 1 if count is None else count
     if n.value < need:
-        raise _lib.B200Error(-4, f"ptau: only {n.value} G1 records available, need {need}")
+        raise _lib.B200Error(_lib.B200_ERR_FORMAT, f"ptau: only {n.value} G1 records available, need {need}")
     off = rec.value - C.addressof(buf)
     host = np.frombuffer(data, dtype=np.uint64, count=need * 8, offset=off).reshape(need, 8).copy()
     bases = ctx.load_bases(host, window_bits=window_bits, check_on_curve=check_on_curve)
@@ -285,18 +285,8 @@ class Radix2EvaluationDomain:
 # ---------------------------------------------------------------------------------------------
 # TurboPlonk prover (boundary B2)
 # ---------------------------------------------------------------------------------------------
-class B200Proof(C.Structure):
+class B200Proof(_lib.STRUCTS["b200_proof"]):
     """b200_proof: field order of the reference's `PlonkProof` (plonk_proof_def.rs:197-222)."""
-    _fields_ = [
-        ("wires_poly_comms", (C.c_uint64 * 8) * 5),
-        ("prod_perm_poly_comm", C.c_uint64 * 8),
-        ("split_quot_poly_comms", (C.c_uint64 * 8) * 5),
-        ("opening_proof", C.c_uint64 * 8),
-        ("shifted_opening_proof", C.c_uint64 * 8),
-        ("wires_evals", (C.c_uint64 * 4) * 5),
-        ("wire_sigma_evals", (C.c_uint64 * 4) * 4),
-        ("perm_next_eval", C.c_uint64 * 4),
-    ]
 
     def to_array(self) -> np.ndarray:
         return np.frombuffer(bytes(self), dtype=np.uint64).copy()
@@ -353,21 +343,9 @@ class VerifyingKey:
         return VerifyingKey(pk.log_n, pk.num_inputs, pk.k, pk.selector_comms, pk.sigma_comms, g2_h, g2_tau_h)
 
 
-class B200VerifyingKey(C.Structure):
-    """b200_verifying_key: the flat verifying key of b200_plonk_verify."""
-    _fields_ = [("log_n", C.c_uint), ("num_inputs", C.c_size_t), ("k", C.c_void_p), ("selector_comms", C.c_void_p),
-                ("sigma_comms", C.c_void_p)]
-
-
-class B200BatchProof(C.Structure):
-    """b200_batch_proof: one proof of a batch (index of its key, public inputs, proof)."""
-    _fields_ = [("vk", C.c_uint), ("pub_inputs", C.c_void_p), ("proof", C.c_void_p)]
-
-
-class B200BatchLink(C.Structure):
-    """b200_batch_link: one link proof of a batch."""
-    _fields_ = [("comm1", C.c_void_p), ("comm2", C.c_void_p), ("alignment", C.c_uint), ("offset", C.c_size_t),
-                ("size", C.c_size_t), ("proof", C.c_void_p)]
+B200VerifyingKey = _lib.STRUCTS["b200_verifying_key"]  # the flat verifying key of b200_plonk_verify
+B200BatchProof = _lib.STRUCTS["b200_batch_proof"]      # one proof of a batch (index of its key, public inputs, proof)
+B200BatchLink = _lib.STRUCTS["b200_batch_link"]        # one link proof of a batch
 
 
 def _u64(a, shape=None) -> np.ndarray:
@@ -523,15 +501,12 @@ class PlonkKzgSnark:
         k = len(keep)
         statuses = (C.c_int * max(1, k))()
         rc = ctx._lib.b200_plonk_prove_batch(ctx._h, pk._h, items, k, statuses)
-        if rc not in (0, -7):
+        if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
             _lib.check(rc)
         return _batch_results(keep, statuses, link_hints, want_challenges)
 
 
-class B200ProveItem(C.Structure):
-    """b200_prove_item: one witness of a batch."""
-    _fields_ = [("wires", C.c_void_p), ("pub_inputs", C.c_void_p), ("blinders", C.c_void_p), ("proof", C.c_void_p),
-                ("link_poly", C.c_void_p), ("challenges", C.c_void_p)]
+B200ProveItem = _lib.STRUCTS["b200_prove_item"]  # one witness of a batch
 
 
 def _prove_items(pk: ProvingKey, wires_list, pub_inputs_list, blinders_list, link_hints: bool, want_challenges: bool):
@@ -574,7 +549,7 @@ def _batch_results(keep, statuses, link_hints: bool, want_challenges: bool):
     hints = None
     if link_hints:
         hints = [LinkingHint(linking_wire_poly=x[4], linking_wire_comm=np.array(x[3].wires_poly_comms[0], dtype=np.uint64))
-                 if s == 0 else None for x, s in zip(keep, st)]
+                 if s == _lib.B200_OK else None for x, s in zip(keep, st)]
     if want_challenges:
         return proofs, hints, st, [x[5] for x in keep]
     return proofs, hints, st
@@ -603,9 +578,8 @@ def prove_raw(ctx: Context, pk: ProvingKey, wires_ptr: int, pub_inputs: np.ndarr
     return proof
 
 
-class B200LinkProof(C.Structure):
+class B200LinkProof(_lib.STRUCTS["b200_link_proof"]):
     """b200_link_proof: mpc-plonk `LinkingProof { quotient_commitment, opening_proof }`."""
-    _fields_ = [("quotient_commitment", C.c_uint64 * 8), ("opening_proof", C.c_uint64 * 8)]
 
     def to_array(self) -> np.ndarray:
         return np.frombuffer(bytes(self), dtype=np.uint64).copy()
@@ -634,11 +608,7 @@ def link_proofs(ctx: Context, srs: Bases, hint_a: LinkingHint, hint_b: LinkingHi
     return proof, eta
 
 
-class B200LinkItem(C.Structure):
-    """b200_link_item: one link proof of a batch."""
-    _fields_ = [("a1", C.c_void_p), ("len1", C.c_size_t), ("a2", C.c_void_p), ("len2", C.c_size_t),
-                ("comm1", C.c_void_p), ("comm2", C.c_void_p), ("alignment", C.c_uint), ("offset", C.c_size_t),
-                ("size", C.c_size_t), ("proof", C.c_void_p), ("eta", C.c_void_p)]
+B200LinkItem = _lib.STRUCTS["b200_link_item"]  # one link proof of a batch
 
 
 def _link_poly(poly, where: str):
@@ -691,7 +661,7 @@ def _link_items(srs: Bases, triples):
 
 def _link_batch_results(keep, statuses):
     st = [int(statuses[i]) for i in range(len(keep))]
-    return [x[4] for x in keep], [x[5] if s == 0 else None for x, s in zip(keep, st)], st
+    return [x[4] for x in keep], [x[5] if s == _lib.B200_OK else None for x, s in zip(keep, st)], st
 
 
 def link_proofs_batch(ctx: Context, srs: Bases, triples):
@@ -704,7 +674,7 @@ def link_proofs_batch(ctx: Context, srs: Bases, triples):
     k = len(keep)
     statuses = (C.c_int * max(1, k))()
     rc = ctx._lib.b200_plonk_link_batch(ctx._h, srs._h, items, k, statuses)
-    if rc not in (0, -7):
+    if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
         _lib.check(rc)
     return _link_batch_results(keep, statuses)
 
@@ -758,16 +728,8 @@ ProofLinkingHint = LinkingHint         # `pub type ProofLinkingHint = LinkingHin
 ProverError = _lib.B200Error           # circuit-types/src/errors.rs:33-58: a failing prove surfaces as an error value
 
 
-class BundleProof(C.Structure):
-    """b200_bundle_proof"""
-    _fields_ = [("pk", C.c_void_p), ("wires", C.c_void_p), ("pub_inputs", C.c_void_p), ("num_inputs", C.c_size_t),
-                ("blinders", C.c_void_p), ("proof", C.c_void_p), ("link_poly", C.c_void_p)]
-
-
-class BundleLink(C.Structure):
-    """b200_bundle_link"""
-    _fields_ = [("a", C.c_uint), ("b", C.c_uint), ("alignment", C.c_uint), ("offset", C.c_size_t), ("size", C.c_size_t),
-                ("proof", C.c_void_p)]
+BundleProof = _lib.STRUCTS["b200_bundle_proof"]
+BundleLink = _lib.STRUCTS["b200_bundle_link"]
 
 
 @dataclass
@@ -825,9 +787,9 @@ class ProverPool:
         pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64)
         bl = np.ascontiguousarray(blinders, dtype=np.uint64)
         if pi.size != 4 * pk.num_inputs:
-            raise ProverError(-1, f"submit_prove: {pi.size // 4} public inputs for a key with {pk.num_inputs}")
+            raise ProverError(_lib.B200_ERR_INVALID, f"submit_prove: {pi.size // 4} public inputs for a key with {pk.num_inputs}")
         if bl.size != 4 * 17:
-            raise ProverError(-1, "submit_prove: blinders must be 17 Fr elements")
+            raise ProverError(_lib.B200_ERR_INVALID, "submit_prove: blinders must be 17 Fr elements")
         link = np.zeros((pk.domain_size + 2, 4), dtype=np.uint64) if with_link_poly else None
         ticket = C.c_uint64()
         _lib.check(self._lib.b200_pool_submit_prove(self._h, pk._h, C.c_void_p(wires_ptr), _ptr(pi) if pi.size else None,
@@ -885,7 +847,7 @@ class ProverPool:
             pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64)
             bl = np.ascontiguousarray(blinders, dtype=np.uint64)
             if pi.size != 4 * pk.num_inputs or bl.size != 4 * 17:
-                raise ProverError(-1, "submit_bundle: public inputs / blinders do not match the key")
+                raise ProverError(_lib.B200_ERR_INVALID, "submit_bundle: public inputs / blinders do not match the key")
             proof = B200Proof()
             poly = np.zeros((pk.domain_size + 2, 4), dtype=np.uint64)
             arr_p[i].pk, arr_p[i].wires = pk._h, C.c_void_p(wires_ptr)
@@ -912,7 +874,7 @@ class ProverPool:
         rc = self._lib.b200_pool_wait(self._h, ticket)
         proof, link, _, _ = self._keep.pop(ticket, (None, None, None, None))
         if isinstance(proof, (_PoolBatch, _PoolLinkBatch)):  # a batch job: refused items are reported in its statuses
-            if rc not in (0, -7):
+            if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
                 _lib.check(rc)
             if isinstance(proof, _PoolLinkBatch):
                 return _link_batch_results(proof.held, proof.statuses)

@@ -232,7 +232,7 @@ class SingleProverCircuit:
                 proofs, hints, statuses = srs.pool.wait(tk)
         except _lib.B200Error as e:
             raise ProverError("Plonk", e) from e
-        bad = [i for i, st in enumerate(statuses) if st != 0]
+        bad = [i for i, st in enumerate(statuses) if st != _lib.B200_OK]
         if bad:
             raise ProverError("Plonk", f"WrongQuotientPolyDegree at indices {bad}")
         return list(zip(proofs, hints))

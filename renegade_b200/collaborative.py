@@ -450,7 +450,7 @@ class MultiproverPlonkKzgSnark:
         deg = NW * (n + 1) + 2
         tail = limbs_to_scalars(be.to_limbs(fab.open([q[deg:] for q in quot_c])))  # zero for a satisfied circuit: opening leaks nothing
         if tail[0] == 0 or any(tail[1:]):
-            raise _lib.B200Error(-7, "WrongQuotientPolyDegree: the shared witness does not satisfy the circuit")
+            raise _lib.B200Error(_lib.B200_ERR_UNSATISFIED, "WrongQuotientPolyDegree: the shared witness does not satisfy the circuit")
         total = NW * (n + 1) + 3
         split = [[None] * NW for _ in range(P)]
         for p in range(P):

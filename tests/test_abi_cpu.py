@@ -3,6 +3,7 @@ include/b200prover.h declares, fails loudly without a GPU (no CPU fallback), and
 entry points (ptau parsing, partial-sum combination) behave like the reference's."""
 import ctypes as C
 import os
+import subprocess
 import sys
 import re
 
@@ -18,9 +19,42 @@ def header_symbols():
     return sorted(set(re.findall(r"\b(b200_[a-z0-9_]+)\s*\(", src)))
 
 
-def test_header_matches_binding_list():
+def _gcc(src: str, path, *flags) -> None:
+    path.with_suffix(".c").write_text(src)
+    out = subprocess.run(["gcc", "-std=c11", "-Werror", "-I" + os.path.join(ROOT, "include"), *flags,
+                          str(path.with_suffix(".c")), "-o", str(path)], capture_output=True, text=True)
+    assert out.returncode == 0, out.stderr
+
+
+def test_binding_matches_the_compiler(tmp_path):
+    """The binding _lib derives from include/b200prover.h is what a C compiler makes of the header.  Every parsed
+    signature initialises a pointer to the declared function, so a parse that differs from the declaration does not
+    compile; every ctypes struct has the compiler's size and field offsets and sizes; every scalar type of the mapping
+    has the compiler's size and signedness."""
     from renegade_b200 import _lib
-    assert header_symbols() == sorted(_lib.EXPORTS)
+    _, structs, funcs, _ = _lib.parse_header()
+    assert header_symbols() == sorted(_lib.EXPORTS) and len(funcs) == len(_lib.EXPORTS)
+    decls = [f"static {ret} (*const p_{name})({', '.join(t for _, t in args) or 'void'}) = {name};"
+             for name, ret, args in funcs]
+    _gcc('#include "b200prover.h"\n' + "\n".join(decls) + "\n", tmp_path / "signatures.o", "-c")
+
+    lines = [f'printf("{t} %zu %d\\n", sizeof({t}), ({t})-1 < 0);' for t in _lib.SCALARS]
+    lines.append('printf("void* %zu 0\\n", sizeof(void*));')
+    for s, fields in structs.items():
+        lines.append(f'printf("{s} %zu 0\\n", sizeof({s}));')
+        lines += [f'printf("{s}.{f} %zu %zu\\n", offsetof({s}, {f}), sizeof((({s}*)0)->{f}));' for f, _, _ in fields]
+    _gcc('#include <stdio.h>\n#include <stddef.h>\n#include "b200prover.h"\nint main(void) {\n' + "\n".join(lines) +
+         "\nreturn 0;\n}\n", tmp_path / "layout")
+    got = subprocess.run([str(tmp_path / "layout")], capture_output=True, text=True, check=True).stdout.splitlines()
+
+    want = [f"{t} {C.sizeof(ct)} {int(ct(-1).value < 0)}" for t, ct in _lib.SCALARS.items()]
+    want.append(f"void* {C.sizeof(C.c_void_p)} 0")
+    for s, fields in structs.items():
+        cls = _lib.STRUCTS[s]
+        assert [f for f, _ in cls._fields_] == [f for f, _, _ in fields]
+        want.append(f"{s} {C.sizeof(cls)} 0")
+        want += [f"{s}.{f} {getattr(cls, f).offset} {getattr(cls, f).size}" for f, _, _ in fields]
+    assert got == want
 
 
 def test_library_exports_every_declared_symbol():

@@ -127,13 +127,15 @@ int b200_msm_batch_device(b200_ctx* ctx, const b200_bases* bases, size_t base_of
  * throughput setting; the row/column tree reduction that replaced it has one shape for both uses. */
 int b200_msm_tuning(b200_ctx* ctx, int throughput_mode);
 /* Device-side phase timing (CUDA events recorded on the context's stream).  enable != 0 turns
- * it on for subsequent MSM calls; out_ms (may be NULL) receives the last call's
+ * it on for subsequent MSM calls, the batch provers' commitments included; out_ms (may be NULL)
+ * receives the last single call's (b200_msm*, b200_plonk_prove, b200_plonk_link)
  * {total, sort = count+scan+scatter, bucket accumulation, bucket reduction} in ms. */
 int b200_msm_timing(b200_ctx* ctx, int enable, float out_ms[4]);
 
 /* Running totals of the bucket-accumulation kernel since the last reset while timing is enabled:
  * out = {milliseconds, (point, scalar) pairs, launches}, every MSM call on this context included
- * (the prover's batched commitments too). */
+ * (the prover's batched commitments too, b200_plonk_prove_batch's and b200_plonk_link_batch's
+ * included).  A proof of domain size n adds 4 launches and 13n + 32 pairs. */
 int b200_msm_timing_totals(b200_ctx* ctx, int reset, double out[3]);
 
 /* Sum of k affine points on the host (combining per-GPU partial MSM results after the NCCL

@@ -426,12 +426,18 @@ int b200_msm_timing_totals(b200_ctx* ctx, int reset, double out[3]) {
     B200_TRY
     if (!ctx) return B200_ERR_INVALID;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
+    // the single calls' scratch and the batch calls' (b200_plonk_prove_batch, b200_plonk_link_batch)
+    MsmScratch* const scratches[2] = {&ctx->c.msm, &ctx->c.batch.msm};
     if (out) {
-        out[0] = ctx->c.msm.tot_acc_ms;
-        out[1] = ctx->c.msm.tot_pairs;
-        out[2] = ctx->c.msm.tot_launches;
+        out[0] = out[1] = out[2] = 0;
+        for (const MsmScratch* s : scratches) {
+            out[0] += s->tot_acc_ms;
+            out[1] += s->tot_pairs;
+            out[2] += s->tot_launches;
+        }
     }
-    if (reset) ctx->c.msm.tot_acc_ms = ctx->c.msm.tot_pairs = ctx->c.msm.tot_launches = 0;
+    if (reset)
+        for (MsmScratch* s : scratches) s->tot_acc_ms = s->tot_pairs = s->tot_launches = 0;
     return B200_OK;
     B200_CATCH
 }
@@ -450,6 +456,7 @@ int b200_msm_timing(b200_ctx* ctx, int enable, float out_ms[4]) {
     if (!ctx) return B200_ERR_INVALID;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
     ctx->c.msm.timing = enable != 0;
+    ctx->c.batch.msm.timing = enable != 0;  // the batch calls commit through their own scratch
     if (out_ms)
         for (int i = 0; i < 4; ++i) out_ms[i] = ctx->c.msm.ms[i];
     return B200_OK;

@@ -18,10 +18,12 @@
 //     inversion), prefetching the next 64-byte point while the current addition runs;
 //   * sum_k (k+1) B_k without a running sum: the buckets of a window form a matrix whose row and
 //     column sums carry the weights, so every bucket enters two plain additions (one serial level of
-//     fan-in 8 / 4, then shared-memory binary trees), and the two weighted sums that remain become
-//     c - 1 per-bit sums; the dependent additions of those tails run on four lanes each
-//     (xyzz_add_quad); the last ~2 KB go to the host, which runs the Horner over the bit sums and
-//     the single field inversion of the batch.
+//     fan-in 8 / 4, then the rest of each row / column), and the two weighted sums that remain become
+//     c - 1 per-bit sums.  Throughput plans (the prover's batched commitments) read the buckets from
+//     their segment sums in the serial level and finish with two wide levels of warp-local sums;
+//     latency plans (one MSM alone) combine the buckets first and finish with shared-memory binary
+//     trees whose dependent additions run on four lanes each (xyzz_add_quad).  The last ~2 KB go to
+//     the host, which runs the Horner over the bit sums and the single field inversion of the batch.
 #include <algorithm>
 #include <cstdlib>
 #include <vector>
@@ -291,11 +293,13 @@ __device__ __forceinline__ g1_affine load_entry_point(const g1_affine* tables, s
 // first; bin starts from msm_scan_kernel) hands every warp segments of equal length.  One thread per
 // bucket: a bucket of cnt entries in k segments has rem = cnt % k segments of cnt / k + 1 entries, then
 // k - rem of cnt / k.  Slots are claimed per block (shared-memory ranks, one global atomic per block and
-// length) and the same thread records seg_bucket[s] = bucket owning segment s.
+// length) and the same thread records seg_bucket[s] = bucket owning segment s.  Buckets cut into more than kCombineSeq
+// segments are listed for msm_heavy_combine_kernel.
 __global__ void __launch_bounds__(256) msm_segorder_kernel(const uint32_t* __restrict__ offsets,
                                                            const uint32_t* __restrict__ seg_offsets, uint32_t n_buckets,
                                                            uint32_t* __restrict__ seg_cursor /* kSegBins */,
-                                                           uint32_t* __restrict__ seg_bucket, uint32_t* __restrict__ order) {
+                                                           uint32_t* __restrict__ seg_bucket, uint32_t* __restrict__ order,
+                                                           uint32_t* __restrict__ heavy_count, uint32_t* __restrict__ heavy_list) {
     __shared__ uint32_t s_cnt[kSegBins], s_base[kSegBins];
     if (threadIdx.x < kSegBins) s_cnt[threadIdx.x] = 0;
     __syncthreads();
@@ -311,6 +315,7 @@ __global__ void __launch_bounds__(256) msm_segorder_kernel(const uint32_t* __res
             r0 = atomicAdd(&s_cnt[len], k - rem);
             if (rem) r1 = atomicAdd(&s_cnt[len + 1], rem);
         }
+        if (k > (uint32_t)kCombineSeq) heavy_list[atomicAdd(heavy_count, 1u)] = b;
     }
     __syncthreads();
     if (threadIdx.x < kSegBins && s_cnt[threadIdx.x]) s_base[threadIdx.x] = atomicAdd(&seg_cursor[threadIdx.x], s_cnt[threadIdx.x]);
@@ -440,21 +445,17 @@ __device__ __forceinline__ void xyzz_add_quad(g1_xyzz* sh, uint32_t ia, uint32_t
     }
 }
 
-// bucket = sum of its segment sums: sequential for ordinary buckets, deferred to a block tree
-// (msm_heavy_combine_kernel) for buckets cut into more than kCombineSeq segments.
+// bucket = sum of its segment sums: sequential for ordinary buckets, left to a block tree
+// (msm_heavy_combine_kernel) for buckets cut into more than kCombineSeq segments.  Latency plans only: a throughput
+// plan's serial tree level reads the segment sums itself (bucket_first).
 __global__ void __launch_bounds__(128) msm_bucket_combine_kernel(const g1_xyzz* __restrict__ seg_sums,
                                                                  const uint32_t* __restrict__ seg_offsets,
                                                                  uint32_t n_buckets,
-                                                                 g1_xyzz* __restrict__ buckets,
-                                                                 uint32_t* __restrict__ heavy_count,
-                                                                 uint32_t* __restrict__ heavy_list) {
+                                                                 g1_xyzz* __restrict__ buckets) {
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= n_buckets) return;
     const uint32_t s0 = seg_offsets[b], s1 = seg_offsets[b + 1];
-    if (s1 - s0 > (uint32_t)kCombineSeq) {
-        heavy_list[atomicAdd(heavy_count, 1u)] = b;
-        return;
-    }
+    if (s1 - s0 > (uint32_t)kCombineSeq) return;
     g1_xyzz acc = g1_xyzz_inf();
     if (s0 < s1) {
         acc = g1_xyzz_load(seg_sums + s0);
@@ -491,8 +492,8 @@ __global__ void __launch_bounds__(kReduceThreads) msm_heavy_combine_kernel(const
 // R = row sums, C = column sums.  Every bucket enters exactly two additions (its row tree and its column
 // tree), and the trees are plain sums: all of their work is data-parallel with dependent chains of at most
 // 7 additions per level (fan-in <= 8) — instead of a running sum whose chain is as long as a thread's chunk.
-// What is left is two weighted sums over 2^l / 2^(c-1-l) elements (<= 256 each up to c = 17), one block per
-// window (msm_bitsum_kernel + msm_horner_kernel below).
+// What is left is two weighted sums over 2^l / 2^(c-1-l) elements (<= 256 each up to c = 17), written as c - 1 bit
+// sums: msm_tail_bits_kernel (throughput plans) or msm_bitsum_kernel (latency plans), then msm_horner_kernel or the host.
 //   msm_tree_kernel, one launch per level, both trees side by side:
 //     out[a * inner + b] = sum_{j < T} in[(a * T + j) * inner + b]
 //   row tree: inner = 1 (sums of T neighbours over the flat bucket array; L is a multiple of every T, so a
@@ -504,10 +505,31 @@ struct TreeLevel {
 };
 struct TreeArgs {
     TreeLevel row, col;
+    // throughput plans: the serial level reads the buckets from the accumulation's segment sums (the bucket combine folded
+    // in); nullptr: from the combined buckets in `in` (latency plans, msm_bucket_combine_kernel)
+    const uint32_t* seg_offsets;
+    const g1_xyzz* seg_sums;
 };
 constexpr int kTreeThreads = 128;
 constexpr size_t kSmallTreeBuckets = (size_t)1 << 17;  // latency plans up to this many buckets: fan-in 4 in the serial level, see tree_shape
 constexpr size_t kQuadTreeMaxOutputs = 16384;  // msm_tree_quad_kernel up to this many outputs (65536 lanes), see msm_launch_batch
+
+// Bucket bk's first segment sum (the identity for an empty bucket); its other segment sums are rest[0 .. n_rest).  A bucket
+// with more than kCombineSeq segments, and every bucket of a latency plan, is one point of `buckets`.
+__device__ __forceinline__ g1_xyzz bucket_first(const TreeArgs& a, const g1_xyzz* buckets, size_t bk, const g1_xyzz*& rest,
+                                                uint32_t& n_rest) {
+    n_rest = 0;
+    if (a.seg_offsets) {
+        const uint32_t s0 = a.seg_offsets[bk], k = a.seg_offsets[bk + 1] - s0;
+        if (k <= (uint32_t)kCombineSeq) {
+            if (k == 0) return g1_xyzz_inf();
+            rest = a.seg_sums + s0 + 1;
+            n_rest = k - 1;
+            return g1_xyzz_load(a.seg_sums + s0);
+        }
+    }
+    return g1_xyzz_load(buckets + bk);
+}
 
 __global__ void __launch_bounds__(kTreeThreads) msm_tree_kernel(TreeArgs a) {
     const bool is_row = blockIdx.x < a.row.n_blocks;
@@ -518,14 +540,26 @@ __global__ void __launch_bounds__(kTreeThreads) msm_tree_kernel(TreeArgs a) {
     const size_t first = (((size_t)(t >> lv.inner_log) << lv.t_log) << lv.inner_log) | (t & inner_mask);
     const size_t stride = (size_t)1 << lv.inner_log;
     const uint32_t T = 1u << lv.t_log;
-    const g1_xyzz* p = lv.in + first;
-    g1_xyzz acc = g1_xyzz_load(p);
-    g1_xyzz next = T > 1 ? g1_xyzz_load(p + stride) : acc;
+    // the points added, in order: bucket j's first segment sum, then its other ones, for j < T; the next one is fetched under
+    // the addition of the current one
+    const g1_xyzz* rest = nullptr;
+    uint32_t n_rest, i = 0, j = 0;
+    g1_xyzz acc = g1_xyzz_inf();
+    g1_xyzz next = bucket_first(a, lv.in, first, rest, n_rest);
 #pragma unroll 1
-    for (uint32_t j = 1; j < T; ++j) {
+    while (true) {
         const g1_xyzz cur = next;
-        if (j + 1 < T) next = g1_xyzz_load(p + (size_t)(j + 1) * stride);  // prefetch under the addition
+        bool more = true;
+        if (i < n_rest) {
+            next = g1_xyzz_load(rest + i++);
+        } else if (++j < T) {
+            next = bucket_first(a, lv.in, first + (size_t)j * stride, rest, n_rest);
+            i = 0;
+        } else {
+            more = false;
+        }
         acc = g1_add(acc, cur);
+        if (!more) break;
     }
     g1_xyzz_store(lv.out + t, acc);
 }
@@ -567,7 +601,7 @@ __global__ void __launch_bounds__(kThreads) msm_tree_quad_kernel(TreeArgs a) {
     if (on) fe_store(reinterpret_cast<fe*>(lv.out + t) + q, fe_load(F + 4u * sa + q));
 }
 
-// Second (and last) level of both trees: what the serial level leaves — 2^g partial sums per row / column, g <= 8 —
+// Latency plans: second (and last) level of both trees: what the serial level leaves — 2^g partial sums per row / column, g <= 8 —
 // is folded by a binary tree in shared memory, one addition per step on the critical path instead of 2^g - 1.
 //   rows:    out[O] = sum_j in[O * G + j]                                  (G = 2^g partials of a row are contiguous)
 //   columns: out[w * L + lo] = sum_j in[(w * G + j) * L + lo]             (the G partial rows of window w)
@@ -629,7 +663,7 @@ __global__ void __launch_bounds__(kBlockTreeThreads) msm_blocktree_kernel(BlockT
     if (j == 0 && O < p.n_out) g1_xyzz_store(p.out + O, QUAD ? sh[t] : v);
 }
 
-// What is left per window are the two weighted sums.  A dependent XYZZ addition costs a warp the latency of its
+// Latency plans: what is left per window are the two weighted sums.  A dependent XYZZ addition costs a warp the latency of its
 // chained field products whatever else the SM does, so this tail is arranged for the SHORTEST dependent chain, with
 // every independent piece on its own SM:
 //     L * sum_hi hi R[hi] + sum_lo (lo + 1) C[lo] = sum_b 2^b T_b,   b < c - 1,
@@ -724,6 +758,99 @@ __global__ void __launch_bounds__(32) msm_horner_kernel(const g1_xyzz* __restric
         v = g1_add(v, o);
     }
     if (lane == 0) g1_xyzz_store(window_sums + window, v);
+}
+
+// ---- throughput plans: the reduction after the serial level as two wide levels of warp-local sums ------------------
+// Both levels are many small independent sums, so they are laid out as throughput work: a sum of cnt points goes to a
+// group of S = 2^s_log aligned lanes of one warp (rows / columns: S = cnt / 8, at least 4 and at most 32; bit sums: 32); lane k folds points
+// k, k + S, ... one after the other and the group's lanes meet in log2(S) shuffle levels.  No shared memory, no block
+// barrier, a few warps per block: the blocks hold an SM no longer than their own additions take.
+//   msm_tail_kernel        R[O] and C[O] from the serial level's G = 2^g partials of row / column O
+//   msm_tail_bits_kernel   the c - 1 bit sums T_b of each window from R and C (the weights of msm_bitsum_kernel)
+constexpr int kTailThreads = 128;
+constexpr uint32_t kTailFoldLog = 3;  // points folded one after the other by a lane before the shuffle levels
+
+// log2 of the lanes that sum 2^cnt_log points: 2^cnt_log / 8, at least 4 (the small windows of small proofs: shorter
+// chains, at c = 17 the same) and at most 32
+constexpr uint32_t tail_group_log(uint32_t cnt_log) {
+    return cnt_log <= 2u ? cnt_log : cnt_log <= kTailFoldLog + 2u ? 2u : cnt_log - kTailFoldLog < 5u ? cnt_log - kTailFoldLog : 5u;
+}
+
+// Sum of at(0) .. at(cnt - 1) by the group of 2^s_log lanes this lane is lane k of; the result is valid in lane k = 0.
+// Every lane of the warp calls it (the shuffles are warp-wide): lanes with nothing to add pass cnt = 0.
+template <class F>
+__device__ __forceinline__ g1_xyzz group_sum(uint32_t k, uint32_t s_log, uint32_t cnt, F at) {
+    const uint32_t S = 1u << s_log;
+    g1_xyzz acc = g1_xyzz_inf();
+    if (k < cnt) {
+        g1_xyzz next = g1_xyzz_load(at(k));
+#pragma unroll 1
+        for (uint32_t i = k + S;; i += S) {
+            const g1_xyzz cur = next;
+            if (i < cnt) next = g1_xyzz_load(at(i));  // prefetch under the addition
+            acc = xyzz_add(acc, cur);
+            if (i >= cnt) break;
+        }
+    }
+#pragma unroll 1
+    for (uint32_t d = S >> 1; d > 0; d >>= 1) {
+        g1_xyzz o = xyzz_shfl_down(acc, d);
+        if (k >= d) o = g1_xyzz_inf();  // only lanes k < d carry on; the others must not pick up the next group's points
+        acc = xyzz_add(acc, o);
+    }
+    return acc;
+}
+
+struct TailPart {
+    const g1_xyzz* in;
+    g1_xyzz* out;
+    uint32_t n_out, g_log, s_log, n_warps;
+};
+struct TailArgs {
+    TailPart row, col;
+    uint32_t l_log;
+};
+
+//   rows:    R[O] = sum_j in[O * G + j]                        (G partials of a row are contiguous)
+//   columns: C[w * L + lo] = sum_j in[(w * G + j) * L + lo]    (the G partial rows of window w)
+__global__ void __launch_bounds__(kTailThreads) msm_tail_kernel(TailArgs a) {
+    const uint32_t warp = (blockIdx.x * kTailThreads + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
+    if (warp >= a.row.n_warps + a.col.n_warps) return;  // whole warps
+    const bool is_row = warp < a.row.n_warps;
+    const TailPart& p = is_row ? a.row : a.col;
+    const uint32_t idx = ((is_row ? warp : warp - a.row.n_warps) << 5) | lane;
+    const uint32_t O = idx >> p.s_log, k = idx & ((1u << p.s_log) - 1u);
+    const bool on = O < p.n_out;
+    const uint32_t lo_mask = (1u << a.l_log) - 1u;
+    const g1_xyzz sum = group_sum(k, p.s_log, on ? 1u << p.g_log : 0u, [&](uint32_t j) {
+        return is_row ? p.in + (((size_t)O << p.g_log) | j)
+                      : p.in + (((((size_t)(O >> a.l_log) << p.g_log) | j) << a.l_log) | (O & lo_mask));
+    });
+    if (on && k == 0) g1_xyzz_store(p.out + O, sum);
+}
+
+// bit_sums[w][b], b < c - 1 = l + r: T_b = the C[lo] of window w whose weight lo + 1 has bit b set, plus the R[hi] whose
+// weight hi * L has bit b set (bit b - l of hi); bit l of lo + 1 is set only in lo + 1 = L.  One warp per bit sum.
+__global__ void __launch_bounds__(kTailThreads) msm_tail_bits_kernel(const g1_xyzz* __restrict__ C, uint32_t l_log,
+                                                                     const g1_xyzz* __restrict__ R, uint32_t r_log,
+                                                                     uint32_t n_out, g1_xyzz* __restrict__ bit_sums) {
+    const uint32_t O = (blockIdx.x * kTailThreads + threadIdx.x) >> 5, k = threadIdx.x & 31u;
+    if (O >= n_out) return;  // whole warps
+    const uint32_t n_bits = l_log + r_log, w = O / n_bits, b = O % n_bits;
+    const g1_xyzz* Cw = C + ((size_t)w << l_log);
+    const g1_xyzz* Rw = R + ((size_t)w << r_log);
+    // column side (b < l): the j-th weight with bit b set is v = (j >> b) << (b + 1) | 1 << b | j mod 2^b, j < L / 2;
+    // row side (b >= l): the same over hi with bit b - l, after C[L - 1] when b = l
+    const uint32_t extra = b == l_log ? 1u : 0u;
+    const uint32_t cnt = b < l_log ? 1u << (l_log - 1) : extra + (r_log ? 1u << (r_log - 1) : 0u);
+    const uint32_t bb = b < l_log ? b : b - l_log, low_mask = (1u << bb) - 1u;
+    const g1_xyzz sum = group_sum(k, 5u, cnt, [&](uint32_t j) {
+        if (j < extra) return Cw + ((1u << l_log) - 1u);
+        j -= extra;
+        const uint32_t v = ((j >> bb) << (bb + 1)) | (1u << bb) | (j & low_mask);
+        return b < l_log ? Cw + (v - 1u) : Rw + v;
+    });
+    if (k == 0) g1_xyzz_store(bit_sums + O, sum);
 }
 
 // ---- window tables: table[j][i] = 2^(shift*j) * P_i (affine) -------------------------------------
@@ -953,8 +1080,8 @@ int bases_create(const g1_affine* h_points, size_t n, int c_override, int check_
 }
 
 // Bits of the column index (l) and of the row index (r), and how each tree splits them: `a` bits by the serial
-// level (fan-in <= 8 per thread: the throughput part, two additions per bucket), the rest (<= 8 bits) by the
-// shared-memory binary tree of msm_blocktree_kernel.
+// level (fan-in <= 8 per thread: the throughput part, two additions per bucket), the rest (<= 8 bits) by
+// msm_tail_kernel (throughput plans) or the shared-memory binary tree of msm_blocktree_kernel (latency plans).
 static void tree_shape(int c, int latency, size_t n_buckets, int* l_log, int* r_log, int* a_row, int* a_col) {
     const int bits = c - 1;
     const int l = (bits + 1) / 2, r = bits - l;
@@ -1105,7 +1232,8 @@ int msm_launch_batch(const Bases* b, size_t base_off, const fe* d_scalars, size_
     B200_LAUNCH(msm_scatter_kernel, grid_n, bs, 0, st)(d_scalars, n, stride, montgomery, pl, (uint32_t)base_off,
                                               (uint32_t)buckets_per_msm, cursor, entries);
     B200_LAUNCH(msm_segorder_kernel, (unsigned)((n_buckets + 255) / 256), 256, 0, st)(offsets, seg_offsets, (uint32_t)n_buckets,
-                                                                             stt->seg_starts, seg_bucket, seg_order);
+                                                                             stt->seg_starts, seg_bucket, seg_order,
+                                                                             &stt->heavy_count, heavy_list);
     // the long kernels of the MSM go to the low-priority companion stream (see b200_init)
     cudaStream_t hv = s->hv_stream ? s->hv_stream : st;
     stamp(1);
@@ -1119,27 +1247,58 @@ int msm_launch_batch(const Bases* b, size_t base_off, const fe* d_scalars, size_
         cudaEventRecord(s->hv_join, hv);
         cudaStreamWaitEvent(st, s->hv_join, 0);
     }
-    B200_LAUNCH(msm_bucket_combine_kernel, (unsigned)((n_buckets + 127) / 128), 128, 0, st)(
-        seg_sums, seg_offsets, (uint32_t)n_buckets, buckets, &stt->heavy_count, heavy_list);
+    if (pl.latency)
+        B200_LAUNCH(msm_bucket_combine_kernel, (unsigned)((n_buckets + 127) / 128), 128, 0, st)(seg_sums, seg_offsets,
+                                                                                              (uint32_t)n_buckets, buckets);
     B200_LAUNCH(msm_heavy_combine_kernel, (unsigned)std::min<size_t>(max_heavy, 4 * sm_count()), kReduceThreads, 0, st)(
         seg_sums, seg_offsets, &stt->heavy_count, heavy_list, buckets);
     stamp(2);
-    {
+    const unsigned n_bits = (unsigned)(pl.c - 1);
+    g1_xyzz* bit_sums = (g1_xyzz*)s->bit_sums.p;
+    g1_xyzz* t0 = (g1_xyzz*)s->tree.p;
+    g1_xyzz *row_p = t0, *col_p = t0 + row_l1, *R = col_p + col_l1, *Cs = R + n_R;
+    if (!pl.latency) {
+        // serial level over the segment sums (both sides even at fan-in 1: nothing else reads the buckets), then the two
+        // warp-sum levels of msm_tail_kernel / msm_tail_bits_kernel
+        TreeArgs a;
+        a.row = TreeLevel{buckets, row_p, (uint32_t)row_l1, (uint32_t)a_row, 0, 0};
+        a.col = TreeLevel{buckets, col_p, (uint32_t)col_l1, (uint32_t)a_col, (uint32_t)l_log, 0};
+        a.row.n_blocks = (a.row.n_out + kTreeThreads - 1) / kTreeThreads;
+        a.col.n_blocks = (a.col.n_out + kTreeThreads - 1) / kTreeThreads;
+        a.seg_offsets = seg_offsets;
+        a.seg_sums = seg_sums;
+        B200_LAUNCH(msm_tree_kernel, a.row.n_blocks + a.col.n_blocks, kTreeThreads, 0, st)(a);
+        TailArgs ta;
+        ta.l_log = (uint32_t)l_log;
+        const uint32_t gr = (uint32_t)(l_log - a_row), gc = (uint32_t)(r_log - a_col);
+        ta.row = TailPart{row_p, R, (uint32_t)n_R, gr, 0, 0};
+        ta.col = TailPart{col_p, Cs, (uint32_t)n_C, gc, 0, 0};
+        for (TailPart* p : {&ta.row, &ta.col}) {
+            p->s_log = tail_group_log(p->g_log);
+            p->n_warps = (uint32_t)((((size_t)p->n_out << p->s_log) + 31) / 32);
+        }
+        const uint32_t tail_warps = ta.row.n_warps + ta.col.n_warps;
+        B200_LAUNCH(msm_tail_kernel, (tail_warps * 32 + kTailThreads - 1) / kTailThreads, kTailThreads, 0, st)(ta);
+        // c - 1 bit sums per window are too few to fill the GPU and end a lone MSM's chain: a whole warp each
+        const uint32_t n_out = (uint32_t)(n_windows * n_bits);
+        B200_LAUNCH(msm_tail_bits_kernel, (n_out * 32 + kTailThreads - 1) / kTailThreads, kTailThreads, 0, st)(
+            Cs, (uint32_t)l_log, R, (uint32_t)r_log, n_out, bit_sums);
+    } else {
         const bool quad = quad_mode() >= 1;
-        g1_xyzz* t0 = (g1_xyzz*)s->tree.p;
-        g1_xyzz *row_p = t0, *col_p = t0 + row_l1, *R = col_p + col_l1, *Cs = R + n_R;
         const g1_xyzz *row_in = buckets, *col_in = buckets;
         if (a_row || a_col) {  // serial level: out[a * inner + b] = sum_{j < 2^a} in[(a * 2^a + j) * inner + b]
             TreeArgs a;
             a.row = TreeLevel{buckets, row_p, a_row ? (uint32_t)row_l1 : 0u, (uint32_t)a_row, 0, 0};
             a.col = TreeLevel{buckets, col_p, a_col ? (uint32_t)col_l1 : 0u, (uint32_t)a_col, (uint32_t)l_log, 0};
+            a.seg_offsets = nullptr;
+            a.seg_sums = nullptr;
             a.row.n_blocks = (a.row.n_out + kTreeThreads - 1) / kTreeThreads;
             a.col.n_blocks = (a.col.n_out + kTreeThreads - 1) / kTreeThreads;
             // four lanes per output only where the level is a latency chain: a latency plan (one MSM alone) with fewer outputs
             // than the machine has lanes.  As throughput work the quad form just adds its exchange overhead: used everywhere
             // it slowed the 2^20-point MSM's reduce and the headline, and with the size rule alone the pool's small
             // statements were slower than with the tail kernels only
-            if (quad_mode() >= 2 && pl.latency && (size_t)a.row.n_out + a.col.n_out <= kQuadTreeMaxOutputs) {
+            if (quad_mode() >= 2 && (size_t)a.row.n_out + a.col.n_out <= kQuadTreeMaxOutputs) {
                 constexpr unsigned kQ = kTreeThreads / 4;  // outputs per block
                 a.row.n_blocks = (a.row.n_out + kQ - 1) / kQ;
                 a.col.n_blocks = (a.col.n_out + kQ - 1) / kQ;
@@ -1165,16 +1324,14 @@ int msm_launch_batch(const Bases* b, size_t base_off, const fe* d_scalars, size_
             if (gc) col_in = Cs;
         }
         // row_in: R[window][2^r_log], col_in: C[window][2^l_log]
-        const unsigned n_bits = (unsigned)(pl.c - 1);
-        g1_xyzz* bit_sums = (g1_xyzz*)s->bit_sums.p;
         if (quad) B200_LAUNCH(msm_bitsum_kernel<true>, dim3(n_bits, (unsigned)n_windows), kBitThreads, 0, st)(col_in, (uint32_t)l_log, row_in,
                                                                                                      (uint32_t)r_log, bit_sums);
         else B200_LAUNCH(msm_bitsum_kernel<false>, dim3(n_bits, (unsigned)n_windows), kBitThreads, 0, st)(col_in, (uint32_t)l_log, row_in,
                                                                                                       (uint32_t)r_log, bit_sums);
-        // The last step, sum_b 2^b T_b, is a chain of c - 2 dependent doublings whoever runs it, and a host core runs it an
-        // order of magnitude faster than a lone warp.  The host takes it (msm_finish_batch) unless the sums are consumed on the device.
-        if (!use_host_horner(s)) B200_LAUNCH(msm_horner_kernel, (unsigned)n_windows, 32, 0, st)(bit_sums, n_bits, window_sums);
     }
+    // The last step, sum_b 2^b T_b, is a chain of c - 2 dependent doublings whoever runs it, and a host core runs it an
+    // order of magnitude faster than a lone warp.  The host takes it (msm_finish_batch) unless the sums are consumed on the device.
+    if (!use_host_horner(s)) B200_LAUNCH(msm_horner_kernel, (unsigned)n_windows, 32, 0, st)(bit_sums, n_bits, window_sums);
     B200_CUDA(cudaGetLastError());
     stamp(3);
     if (use_host_horner(s))

@@ -334,6 +334,23 @@ typedef struct {
 int b200_plonk_batch_verify(b200_ctx* ctx, const b200_verifying_key* vks, size_t n_vks, const b200_batch_proof* proofs,
                             size_t n_proofs, const b200_batch_link* links, size_t n_links, const uint64_t g2_h[16],
                             const uint64_t g2_tau_h[16], int* all_accepted, uint8_t* verdicts);
+/* verdicts[i] (n_proofs + n_links bytes, proofs first) = b200_plonk_verify / b200_plonk_verify_link's answer for item i,
+ * each item checked on its own, e(A_i, [tau]_2) == e(B_i, [1]_2), with no random combination and no bisection: the cost
+ * does not depend on how many items fail.  The pairings run on the device, one thread per item.  Arguments, errors and
+ * rejections of malformed items exactly as b200_plonk_batch_verify; verdicts may be NULL only when there are no items. */
+int b200_plonk_verify_each(b200_ctx* ctx, const b200_verifying_key* vks, size_t n_vks, const b200_batch_proof* proofs,
+                           size_t n_proofs, const b200_batch_link* links, size_t n_links, const uint64_t g2_h[16],
+                           const uint64_t g2_tau_h[16], uint8_t* verdicts);
+/* n_checks independent checks, all against the same m G2 points: is_one[c] = [ prod_{j<m} e(P_{c,j}, Q_j) == 1 ],
+ * g1_points = n_checks x m 64-byte records (host), g2_points = m 128-byte records.  is_one[c] equals what
+ * b200_pairing_check returns for check c's m pairs.  Where b200_pairing_check would fail for some check (a point off
+ * the curve, a coordinate >= q), the call fails with the same code and b200_last_error() names the first such check
+ * (an off-curve G2 point fails every check: the message names the point).  At most 8 pairs per check (m <= 8, else
+ * B200_ERR_INVALID); m = 0 makes every check 1.  The G2 points are validated and their Miller-loop lines computed on
+ * the host; the G1 checks, the Miller loops and the final exponentiations run on the device, one thread per check.
+ * NULL pointers: B200_ERR_INVALID (g1_points / is_one may be NULL when there are no checks). */
+int b200_pairing_check_many(b200_ctx* ctx, const uint64_t* g2_points, size_t m, const uint64_t* g1_points,
+                            size_t n_checks, uint8_t* is_one);
 
 /* Wall-clock milliseconds of the last proof's phases on this context: round 1, round 2, round 3
  * (coset NTTs + quotient + split), round 3 commitments, round 4, round 5, then two spare slots. */

@@ -353,6 +353,9 @@ def _u64(a, shape=None) -> np.ndarray:
     return a.reshape(shape) if shape is not None else a
 
 
+PAIRING_MAX_PAIRS = 8  # pairs per check of b200_pairing_check_many
+
+
 def pairing_check(g1_points, g2_points) -> bool:
     """prod e(P_i, Q_i) == 1 (`b200_pairing_check`; host only).  P_i: 8 x uint64, Q_i: 16 x uint64."""
     lib = _lib.load()
@@ -365,6 +368,26 @@ def pairing_check(g1_points, g2_points) -> bool:
     return bool(one.value)
 
 
+def pairing_check_many(ctx: Context, g2_points, g1_points) -> np.ndarray:
+    """n independent pairing checks against the same m G2 points on `ctx`'s device (`b200_pairing_check_many`):
+    out[c] = prod_j e(g1_points[c, j], g2_points[j]) == 1.  g2_points: (m, 16) uint64, g1_points: (n, m, 8) uint64,
+    m <= PAIRING_MAX_PAIRS.  Each answer equals `pairing_check` over the check's m pairs."""
+    q = _u64(g2_points)
+    if q.ndim != 2 or q.shape[1] != 16:
+        raise ValueError("g2_points: (m, 16) uint64")
+    m = q.shape[0]
+    p = _u64(g1_points)
+    if p.ndim != 3 or p.shape[1:] != (m, 8):
+        raise ValueError("g1_points: (n, m, 8) uint64 with m = len(g2_points)")
+    if m > PAIRING_MAX_PAIRS:
+        raise ValueError("at most %d pairs per check" % PAIRING_MAX_PAIRS)
+    n = p.shape[0]
+    out = np.zeros(max(1, n), dtype=np.uint8)
+    _lib.check(ctx._lib.b200_pairing_check_many(ctx._h, _ptr(q) if m else None, m, _ptr(p) if p.size else None, n,
+                                                 out.ctypes.data_as(C.c_void_p)))
+    return out[:n].astype(bool)
+
+
 def verify_link_proof(comm_a: np.ndarray, comm_b: np.ndarray, proof: "B200LinkProof", layout: "GroupLayout",
                       g2_h: np.ndarray, g2_tau_h: np.ndarray) -> bool:
     """`PlonkKzgSnark::verify_link_proof::<SolidityTranscript>` (proof_linking/intent_only.rs:77-84)."""
@@ -373,6 +396,70 @@ def verify_link_proof(comm_a: np.ndarray, comm_b: np.ndarray, proof: "B200LinkPr
                                                   layout.size, C.byref(proof), _ptr(_u64(g2_h)), _ptr(_u64(g2_tau_h)),
                                                   C.byref(ok)))
     return bool(ok.value)
+
+
+class _VerifyBatch:
+    """The Python argument checks and the C structs of `batch_verify` and `verify_each`: the distinct verifying keys, the
+    proofs whose public-input count matches their key (the others are False verdicts without a device call), the
+    links and the one G2 pair.  `args` are the C call's arguments from ctx on, up to the outputs."""
+
+    def __init__(self, vks, pub_inputs, proofs, links, g2):
+        vks, pub_inputs, proofs, links = list(vks), list(pub_inputs), list(proofs), list(links)
+        if not (len(vks) == len(pub_inputs) == len(proofs)):
+            raise ValueError("one verifying key and one public-input vector per proof")
+        g2_pairs = {(_u64(vk.g2_h).tobytes(), _u64(vk.g2_tau_h).tobytes()) for vk in vks}
+        if g2 is not None:
+            g2_pairs.add((_u64(g2[0]).tobytes(), _u64(g2[1]).tobytes()))
+        if len(g2_pairs) > 1:
+            raise ValueError("the verifying keys of one batch must share the G2 pair (h, beta_h)")
+        self.n_proofs = len(proofs)
+        self.n_items = len(proofs) + len(links)
+        if not g2_pairs:
+            if self.n_items:
+                raise ValueError("links without proofs need g2=(g2_h, g2_tau_h)")
+            return
+        g2_h, g2_tau_h = (np.frombuffer(b, dtype=np.uint64).copy() for b in next(iter(g2_pairs)))
+        self.keep = [g2_h, g2_tau_h]  # the arrays the C structs point into stay alive as long as this object
+        # distinct verifying keys
+        vk_index, c_vks = {}, []
+        for vk in vks:
+            arrs = (_u64(vk.k, (5, 4)), _u64(vk.selector_comms, (13, 8)), _u64(vk.sigma_comms, (5, 8)))
+            key = (vk.log_n, vk.num_inputs) + tuple(a.tobytes() for a in arrs)
+            if key not in vk_index:
+                vk_index[key] = len(c_vks)
+                self.keep.append(arrs)
+                c_vks.append(B200VerifyingKey(vk.log_n, vk.num_inputs, *(_ptr(a) for a in arrs)))
+        c_proofs, self.proof_pos = [], []
+        for i, (vk, pi, proof) in enumerate(zip(vks, pub_inputs, proofs)):
+            p = _u64(pi, (-1, 4))
+            if p.shape[0] != vk.num_inputs:
+                continue  # not accepted (the reference's verifier errors on a wrong public-input count)
+            self.keep.append(p)
+            key = (vk.log_n, vk.num_inputs) + tuple(
+                a.tobytes() for a in (_u64(vk.k, (5, 4)), _u64(vk.selector_comms, (13, 8)), _u64(vk.sigma_comms, (5, 8))))
+            c_proofs.append(B200BatchProof(vk_index[key], _ptr(p) if p.size else None, C.cast(C.pointer(proof), C.c_void_p)))
+            self.proof_pos.append(i)
+        c_links = []
+        for comm_a, comm_b, lproof, layout in links:
+            a, b = _u64(comm_a), _u64(comm_b)
+            self.keep.append((a, b))
+            c_links.append(B200BatchLink(_ptr(a), _ptr(b), layout.alignment, layout.offset, layout.size,
+                                         C.cast(C.pointer(lproof), C.c_void_p)))
+        self.c_proofs, self.c_links = c_proofs, c_links
+        self.n_c = len(c_proofs) + len(c_links)
+        arrays = ((B200VerifyingKey * max(1, len(c_vks)))(*c_vks), (B200BatchProof * max(1, len(c_proofs)))(*c_proofs),
+                  (B200BatchLink * max(1, len(c_links)))(*c_links))
+        self.keep.append(arrays)
+        self.args = (arrays[0], len(c_vks), arrays[1], len(c_proofs), arrays[2], len(c_links), _ptr(g2_h), _ptr(g2_tau_h))
+
+    def verdicts(self, c_verdicts) -> list:
+        """The C call's verdicts at the caller's item positions; a proof left out is False."""
+        out = [False] * self.n_items
+        for j, i in enumerate(self.proof_pos):
+            out[i] = bool(c_verdicts[j])
+        for j in range(len(self.c_links)):
+            out[self.n_proofs + j] = bool(c_verdicts[len(self.c_proofs) + j])
+        return out
 
 
 class PlonkKzgSnark:
@@ -401,60 +488,25 @@ class PlonkKzgSnark:
         ValueError); `g2 = (g2_h, g2_tau_h)` supplies it when there are only links.  Returns (all_ok, verdicts) with
         verdicts[i] the single verifier's answer for item i, proofs first, then links.  A wrong public-input count is
         a False verdict, as in `verify`."""
-        vks, pub_inputs, proofs, links = list(vks), list(pub_inputs), list(proofs), list(links)
-        if not (len(vks) == len(pub_inputs) == len(proofs)):
-            raise ValueError("one verifying key and one public-input vector per proof")
-        g2_pairs = {(_u64(vk.g2_h).tobytes(), _u64(vk.g2_tau_h).tobytes()) for vk in vks}
-        if g2 is not None:
-            g2_pairs.add((_u64(g2[0]).tobytes(), _u64(g2[1]).tobytes()))
-        if len(g2_pairs) > 1:
-            raise ValueError("the verifying keys of one batch must share the G2 pair (h, beta_h)")
-        n_items = len(proofs) + len(links)
-        if not g2_pairs:
-            if n_items:
-                raise ValueError("links without proofs need g2=(g2_h, g2_tau_h)")
+        b = _VerifyBatch(vks, pub_inputs, proofs, links, g2)
+        if b.n_items == 0:
             return True, []
-        g2_h, g2_tau_h = (np.frombuffer(b, dtype=np.uint64).copy() for b in next(iter(g2_pairs)))
-        keep = []  # the arrays the C structs point into stay alive until the call returns
-        # distinct verifying keys
-        vk_index, c_vks = {}, []
-        for vk in vks:
-            arrs = (_u64(vk.k, (5, 4)), _u64(vk.selector_comms, (13, 8)), _u64(vk.sigma_comms, (5, 8)))
-            key = (vk.log_n, vk.num_inputs) + tuple(a.tobytes() for a in arrs)
-            if key not in vk_index:
-                vk_index[key] = len(c_vks)
-                keep.append(arrs)
-                c_vks.append(B200VerifyingKey(vk.log_n, vk.num_inputs, *(_ptr(a) for a in arrs)))
-        c_proofs, proof_pos = [], []
-        for i, (vk, pi, proof) in enumerate(zip(vks, pub_inputs, proofs)):
-            p = _u64(pi, (-1, 4))
-            if p.shape[0] != vk.num_inputs:
-                continue  # not accepted (the reference's verifier errors on a wrong public-input count)
-            keep.append(p)
-            key = (vk.log_n, vk.num_inputs) + tuple(
-                a.tobytes() for a in (_u64(vk.k, (5, 4)), _u64(vk.selector_comms, (13, 8)), _u64(vk.sigma_comms, (5, 8))))
-            c_proofs.append(B200BatchProof(vk_index[key], _ptr(p) if p.size else None, C.cast(C.pointer(proof), C.c_void_p)))
-            proof_pos.append(i)
-        c_links = []
-        for comm_a, comm_b, lproof, layout in links:
-            a, b = _u64(comm_a), _u64(comm_b)
-            keep.append((a, b))
-            c_links.append(B200BatchLink(_ptr(a), _ptr(b), layout.alignment, layout.offset, layout.size,
-                                         C.cast(C.pointer(lproof), C.c_void_p)))
-        arr_vks = (B200VerifyingKey * max(1, len(c_vks)))(*c_vks)
-        arr_proofs = (B200BatchProof * max(1, len(c_proofs)))(*c_proofs)
-        arr_links = (B200BatchLink * max(1, len(c_links)))(*c_links)
-        n_c = len(c_proofs) + len(c_links)
-        verdicts = (C.c_uint8 * max(1, n_c))()
+        verdicts = (C.c_uint8 * max(1, b.n_c))()
         ok = C.c_int(0)
-        _lib.check(ctx._lib.b200_plonk_batch_verify(ctx._h, arr_vks, len(c_vks), arr_proofs, len(c_proofs), arr_links,
-                                                    len(c_links), _ptr(g2_h), _ptr(g2_tau_h), C.byref(ok), verdicts))
-        out = [False] * n_items
-        for j, i in enumerate(proof_pos):
-            out[i] = bool(verdicts[j])
-        for j in range(len(c_links)):
-            out[len(proofs) + j] = bool(verdicts[len(c_proofs) + j])
-        return bool(ok.value) and len(c_proofs) == len(proofs), out
+        _lib.check(ctx._lib.b200_plonk_batch_verify(ctx._h, *b.args, C.byref(ok), verdicts))
+        return bool(ok.value) and len(b.c_proofs) == b.n_proofs, b.verdicts(verdicts)
+
+    @staticmethod
+    def verify_each(ctx: Context, vks, pub_inputs, proofs, links=(), g2=None) -> list:
+        """The verdicts of `batch_verify`, each item checked on its own with its own pairing on `ctx`'s device
+        (`b200_plonk_verify_each`): no bisection, so the cost does not depend on how many items fail.  Same arguments
+        and argument errors as `batch_verify`; returns the list of verdicts, proofs first, then links."""
+        b = _VerifyBatch(vks, pub_inputs, proofs, links, g2)
+        if b.n_items == 0:
+            return []
+        verdicts = (C.c_uint8 * max(1, b.n_c))()
+        _lib.check(ctx._lib.b200_plonk_verify_each(ctx._h, *b.args, verdicts))
+        return b.verdicts(verdicts)
 
     @staticmethod
     def preprocess(ctx: Context, srs: Bases, log_n: int, num_inputs: int, selectors: np.ndarray,

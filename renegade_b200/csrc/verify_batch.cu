@@ -23,12 +23,19 @@
 //      A and B, and ONE pairing.  If it fails and verdicts are asked for, the failing items are found by bisection:
 //      each step re-merges a subset from the per-item scalars already on the device (masked merge, MSM, one pairing).
 // An item with an off-curve point or a field element outside [0, p) is rejected and left out of the combination.
+//
+// b200_plonk_verify_each runs steps 1 and 2 (Batch::stage), then k_scalars with rho = 1, k_item_points (A_i and -B_i of
+// each item) and the device pairing (k_pairing_many over the lines of [tau]_2 and [1]_2 prepared on the host,
+// pairing.cuh): every item is checked on its own, so the cost does not depend on how many fail.  b200_pairing_check_many
+// exposes the pairing kernel itself.
 #include <cstring>
 #include <mutex>
+#include <string>
 #include <vector>
 
 #include "b200prover.h"
 #include "device_ctx.h"
+#include "pairing.cuh"
 #include "transcript.h"
 #include "verify_terms.h"
 
@@ -38,6 +45,7 @@ namespace {
 
 using Fr = FrCfg;
 constexpr int kMaxAlign = 28;
+constexpr int kMaxPairs = 8;  // pairs per check of b200_pairing_check_many
 
 struct VkDev {  // one distinct verifying key
     fe k[vt::NW];
@@ -142,25 +150,27 @@ __global__ void __launch_bounds__(128) k_prepare(const ItemDev* __restrict__ ite
 __global__ void __launch_bounds__(128) k_scalars(const ItemDev* __restrict__ items, size_t k, const VkDev* __restrict__ vks,
                                                  const vt::ProofIn* __restrict__ proofs, const fe* __restrict__ pi,
                                                  const fe* __restrict__ wtab, const fe* __restrict__ den_inv,
-                                                 const ItemState* __restrict__ st, Seed seed, fe* __restrict__ rec) {
+                                                 const ItemState* __restrict__ st, Seed seed, bool unit_weights,
+                                                 fe* __restrict__ rec) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= k) return;
     const ItemState s = st[i];
     if (!s.ok) return;  // rejected: its record stays zero
-    // rho_i = keccak(seed || i) mod r
-    uint8_t h[32];
-    {
+    // rho_i = keccak(seed || i) mod r, or 1 for an item checked on its own
+    fe rho = fe_one<Fr>();
+    if (!unit_weights) {
+        uint8_t h[32];
         Keccak256 kc;
         kc.absorb(seed.b, 32);
         uint8_t be[8];
         for (int b = 0; b < 8; ++b) be[b] = (uint8_t)((uint64_t)i >> (56 - 8 * b));
         kc.absorb(be, 8);
         kc.finish(h);
+        rho = fe_zero();
+        const fe c256 = fe_from_u32<Fr>(256);
+        for (int b = 0; b < 32; ++b) rho = fe_add<Fr>(fe_mul<Fr>(rho, c256), fe_from_u32<Fr>(h[b]));
+        if (fe_is_zero(rho)) rho = fe_one<Fr>();
     }
-    fe rho = fe_zero();
-    const fe c256 = fe_from_u32<Fr>(256);
-    for (int b = 0; b < 32; ++b) rho = fe_add<Fr>(fe_mul<Fr>(rho, c256), fe_from_u32<Fr>(h[b]));
-    if (fe_is_zero(rho)) rho = fe_one<Fr>();
     const ItemDev it = items[i];
     DevSink sink{rec + i * kRec, rho};
     if (it.kind == 0) {
@@ -232,7 +242,88 @@ __global__ void __launch_bounds__(kMergeThreads) k_merge_shared(const uint32_t* 
     }
 }
 
+// ---- per-item checks (b200_plonk_verify_each) ---------------------------------------------------------------------
+// One warp per item: lane s multiplies the point of slot s by its coefficients of A and of B (double-and-add over the
+// canonical scalar), five shuffle levels add the 32 products (g1_add's exact paths for the identity and P == -Q), and
+// lane 0 stores (A_i, -B_i) in affine form, the G1 side of the item's check e(A_i, [tau]_2) e(-B_i, [1]_2) == 1.  The two
+// inversions are Fermat's, in lane 0: ~500 field products, next to ~10^5 for the item's pairing.  A rejected item has
+// a zero record, so both of its sums are the identity.
+constexpr int kItemThreads = 128;
+FF_D g1_xyzz xyzz_shfl_down(const g1_xyzz& p, int off) {
+    g1_xyzz r;
+    for (int w = 0; w < 8; ++w) {
+        r.x.l[w] = __shfl_down_sync(0xffffffffu, p.x.l[w], off);
+        r.y.l[w] = __shfl_down_sync(0xffffffffu, p.y.l[w], off);
+        r.zz.l[w] = __shfl_down_sync(0xffffffffu, p.zz.l[w], off);
+        r.zzz.l[w] = __shfl_down_sync(0xffffffffu, p.zzz.l[w], off);
+    }
+    return r;
+}
+__global__ void __launch_bounds__(kItemThreads) k_item_points(const ItemDev* __restrict__ items, size_t k,
+                                                              const VkDev* __restrict__ vks,
+                                                              const vt::ProofIn* __restrict__ proofs,
+                                                              const LinkDev* __restrict__ links, const fe* __restrict__ rec,
+                                                              g1_affine* __restrict__ out) {
+    const size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / 32;  // the same for the whole warp
+    const int lane = threadIdx.x & 31;
+    if (i >= k) return;
+    const ItemDev it = items[i];
+    g1_affine p;
+    p.x = p.y = fe_zero();
+    if (it.kind == 0) {
+        if (lane < vt::kProofPoints) p = vt::proof_point(proofs[it.idx], lane);
+        else if (lane < vt::kSlotSig) p = vks[it.vk].sel[lane - vt::kSlotSel];
+        else if (lane < vt::kSlotG) p = vks[it.vk].sig[lane - vt::kSlotSig];
+        else p = vt::g1_generator();
+    } else if (lane < vt::kLinkPoints) {
+        p = links[it.idx].pt[lane];
+    }
+    g1_xyzz a = g1_mul_bits(p, fe_from_mont<Fr>(fe_load(rec + i * kRec + lane)), 254);
+    g1_xyzz b = g1_mul_bits(p, fe_from_mont<Fr>(fe_load(rec + i * kRec + vt::kSlots + lane)), 254);
+    for (int off = 16; off; off >>= 1) {
+        const g1_xyzz oa = xyzz_shfl_down(a, off), ob = xyzz_shfl_down(b, off);
+        a = g1_add(a, oa);
+        b = g1_add(b, ob);
+    }
+    if (lane == 0) {
+        g1_affine_store(out + 2 * i, g1_to_affine(a));
+        g1_affine_store(out + 2 * i + 1, g1_affine_neg(g1_to_affine(b)));
+    }
+}
+
+// is_one[c] = 1 / 0 for check c: prod_j e(g1[c m + j], Q_j) == 1, or 2 when one of its G1 points is off the curve or has
+// a coordinate >= q.  One thread per check; every thread reads the same prepared lines (L1 broadcast).
+constexpr int kPairThreads = 64;
+__global__ void __launch_bounds__(kPairThreads) k_pairing_many(const G2Prepared* __restrict__ q, int m,
+                                                               const g1_affine* __restrict__ g1, size_t n, PairingConsts pc,
+                                                               uint8_t* __restrict__ is_one) {
+    const size_t c = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= n) return;
+    g1_affine p[kMaxPairs];
+    bool ok = true;
+    for (int j = 0; j < m; ++j) {
+        p[j] = g1[c * m + j];
+        ok = ok && g1_affine_on_curve(p[j]);
+    }
+    if (!ok) {
+        is_one[c] = 2;
+        return;
+    }
+    is_one[c] = fq12_is_one(final_exponentiation(miller_loop_prepared(q, p, m), pc)) ? 1 : 0;
+}
+
+// verdict_i = ok_i && the item's pairing check holds
+__global__ void k_verdicts(const ItemState* __restrict__ st, const uint8_t* __restrict__ is_one, size_t k,
+                           uint8_t* __restrict__ verdicts) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < k) verdicts[i] = st[i].ok && is_one[i] == 1 ? 1 : 0;
+}
+
 inline unsigned grid_of(size_t n, unsigned bs) { return (unsigned)((n + bs - 1) / bs); }
+
+void pairing_many_enqueue(const G2Prepared* q, int m, const g1_affine* g1, size_t n, uint8_t* is_one, cudaStream_t st) {
+    B200_LAUNCH(k_pairing_many, grid_of(n, kPairThreads), kPairThreads, 0, st)(q, m, g1, n, pairing_consts(), is_one);
+}
 
 template <class T>
 int upload(DevBuf* d, const std::vector<T>& h, cudaStream_t st) {
@@ -293,7 +384,155 @@ struct Batch {
         // the whole set fails and its lower half passes: the upper half fails (the check is a product over the items)
         return bisect(hi, g2_tau_h, g2_h, verdicts);
     }
+
+    // Staging, uploads, k_prepare and the inversion of the denominators, for k >= 1 items whose arguments passed
+    // check_items: what both entry points run first.
+    int stage(const b200_verifying_key* in_vks, size_t n_vks, const b200_batch_proof* in_proofs, size_t n_proofs,
+              const b200_batch_link* in_links, size_t n_links) {
+        cudaStream_t st = c->stream;
+        k = n_proofs + n_links;
+        this->n_vks = (unsigned)n_vks;
+        // ---- host staging: keys, items, public inputs, layouts ---------------------------------------------------------
+        std::vector<VkDev> hv(n_vks);
+        std::vector<fe> hw;  // per key: w and the table start
+        size_t wtab_n = 0;
+        for (size_t v = 0; v < n_vks; ++v) {
+            VkDev& d = hv[v];
+            std::memcpy(d.k, in_vks[v].k, sizeof(d.k));
+            std::memcpy(d.sel, in_vks[v].selector_comms, sizeof(d.sel));
+            std::memcpy(d.sig, in_vks[v].sigma_comms, sizeof(d.sig));
+            d.log_n = in_vks[v].log_n;
+            d.num_inputs = in_vks[v].num_inputs;
+            d.w = host_root_of_unity(d.log_n);
+            const uint64_t n = (uint64_t)1 << d.log_n;
+            fe nf = fe_zero();
+            nf.l[0] = (uint32_t)n;
+            nf.l[1] = (uint32_t)(n >> 32);
+            d.n_mont = fe_to_mont<Fr>(nf);
+            d.wtab_off = wtab_n;
+            wtab_n += d.num_inputs ? d.num_inputs : 1;
+        }
+        std::vector<ItemDev> hi(k);
+        std::vector<vt::ProofIn> hp(n_proofs);
+        std::vector<LinkDev> hl(n_links);
+        std::vector<fe> hpi;
+        size_t den_n = 0, tr_n = 0, base_n = 0;
+        std::vector<std::vector<uint32_t>> per_vk(n_vks);
+        for (size_t p = 0; p < n_proofs; ++p) {
+            const VkDev& vk = hv[in_proofs[p].vk];
+            std::memcpy(&hp[p], in_proofs[p].proof, sizeof(vt::ProofIn));
+            ItemDev& it = hi[p];
+            it.kind = 0;
+            it.idx = (uint32_t)p;
+            it.vk = in_proofs[p].vk;
+            it.base_off = (uint32_t)base_n;
+            base_n += vt::kProofPoints;
+            it.pi_off = hpi.size();
+            const fe* pi = reinterpret_cast<const fe*>(in_proofs[p].pub_inputs);
+            hpi.insert(hpi.end(), pi, pi + vk.num_inputs);
+            it.den_off = den_n;
+            den_n += vk.num_inputs ? vk.num_inputs : 1;
+            it.tr_off = tr_n;
+            it.tr_cap = vt::plonk_transcript_bytes(vk.num_inputs);
+            tr_n += it.tr_cap;
+            per_vk[it.vk].push_back((uint32_t)p);
+        }
+        for (size_t l = 0; l < n_links; ++l) {
+            LinkDev& d = hl[l];
+            std::memcpy(&d.pt[vt::kLinkC1], in_links[l].comm1, 64);
+            std::memcpy(&d.pt[vt::kLinkC2], in_links[l].comm2, 64);
+            std::memcpy(&d.pt[vt::kLinkCq], in_links[l].proof->quotient_commitment, 64);
+            std::memcpy(&d.pt[vt::kLinkPi], in_links[l].proof->opening_proof, 64);
+            d.offset = in_links[l].offset;
+            d.size = in_links[l].size;
+            d.alignment = in_links[l].alignment;
+            ItemDev& it = hi[n_proofs + l];
+            std::memset(&it, 0, sizeof(it));
+            it.kind = 1;
+            it.idx = (uint32_t)l;
+            it.base_off = (uint32_t)base_n;
+            base_n += vt::kLinkPoints;
+        }
+        // shared bases after the items' own: 18 per key, then G
+        shared0 = base_n;
+        n_bases = base_n + n_vks * vt::kVkPoints + 1;
+        if (n_bases > 0xffffffffu) return B200_ERR_INVALID;
+        std::vector<g1_affine> hshared;
+        for (size_t v = 0; v < n_vks; ++v) {
+            hshared.insert(hshared.end(), hv[v].sel, hv[v].sel + vt::NS);
+            hshared.insert(hshared.end(), hv[v].sig, hv[v].sig + vt::NW);
+        }
+        hshared.push_back(vt::g1_generator());
+        std::vector<uint32_t> hvk_items, hvk_start(n_vks + 1, 0);
+        for (size_t v = 0; v < n_vks; ++v) {
+            hvk_start[v] = (uint32_t)hvk_items.size();
+            hvk_items.insert(hvk_items.end(), per_vk[v].begin(), per_vk[v].end());
+        }
+        hvk_start[n_vks] = (uint32_t)hvk_items.size();
+        Roots roots;
+        for (int a = 0; a <= kMaxAlign; ++a) roots.g[a] = host_root_of_unity((unsigned)a);
+
+        int rc;
+        if ((rc = upload(&items, hi, st)) || (rc = upload(&vks, hv, st)) || (rc = upload(&proofs, hp, st)) ||
+            (rc = upload(&links, hl, st)) || (rc = upload(&pi, hpi, st)) || (rc = upload(&vk_items, hvk_items, st)) ||
+            (rc = upload(&vk_start, hvk_start, st)) || (rc = wtab.reserve(wtab_n * sizeof(fe))) ||
+            (rc = tr.reserve(tr_n + 1)) || (rc = den.reserve(den_n * sizeof(fe) + 32)) ||
+            (rc = den_tmp.reserve(den_n * sizeof(fe) + 32)) || (rc = state.reserve(k * sizeof(ItemState))) ||
+            (rc = digest.reserve(k * 32)) || (rc = rec.reserve(k * kRec * sizeof(fe))) ||
+            (rc = bases_pts.reserve(n_bases * sizeof(g1_affine))) || (rc = scal.reserve(2 * n_bases * sizeof(fe))) ||
+            (rc = mask.reserve(k)))
+            return rc;
+        // w^j tables of the keys
+        for (size_t v = 0; v < n_vks; ++v)
+            fill_powers((fe*)wtab.p + hv[v].wtab_off, hv[v].num_inputs ? hv[v].num_inputs : 1, hv[v].w, fe_one<Fr>(), st);
+        B200_CUDA(cudaMemcpyAsync((g1_affine*)bases_pts.p + shared0, hshared.data(), hshared.size() * sizeof(g1_affine),
+                                  cudaMemcpyHostToDevice, st));
+        B200_CUDA(cudaMemsetAsync(rec.p, 0, k * kRec * sizeof(fe), st));
+
+        // ---- 1. prepare, 2. invert ------------------------------------------------------------------------------------
+        B200_LAUNCH(k_prepare, grid_of(k, 128), 128, 0, st)((const ItemDev*)items.p, k, (const VkDev*)vks.p,
+                                                           (const vt::ProofIn*)proofs.p, (const LinkDev*)links.p,
+                                                           (const fe*)pi.p, (const fe*)wtab.p, (uint8_t*)tr.p,
+                                                           (fe*)den.p, roots, (ItemState*)state.p, (uint8_t*)digest.p);
+        if (den_n) batch_inverse_enqueue(nullptr, (fe*)den.p, (fe*)den_tmp.p, den_n, st);
+        return B200_OK;
+    }
 };
+
+// The NULL checks of both entry points (the output pointers apart)
+bool args_present(const b200_ctx* ctx, const b200_verifying_key* vks, size_t n_vks, const b200_batch_proof* proofs,
+                  size_t n_proofs, const b200_batch_link* links, size_t n_links, const uint64_t* g2_h,
+                  const uint64_t* g2_tau_h) {
+    return ctx && (!n_vks || vks) && (!n_proofs || proofs) && (!n_links || links) && g2_h && g2_tau_h &&
+           n_vks <= 0xffffffffu && n_proofs + n_links <= 0xffffffffu;
+}
+
+// The entries' argument checks of both entry points; b200_last_error() names `who`
+int check_items(const char* who, const b200_verifying_key* vks, size_t n_vks, const b200_batch_proof* proofs,
+                size_t n_proofs, const b200_batch_link* links, size_t n_links, const uint64_t g2_h[16],
+                const uint64_t g2_tau_h[16]) {
+    const std::string w(who);
+    for (size_t v = 0; v < n_vks; ++v)
+        if (vks[v].log_n > kMaxAlign || !vks[v].k || !vks[v].selector_comms || !vks[v].sigma_comms) {
+            set_error(w + ": bad verifying key");
+            return B200_ERR_INVALID;
+        }
+    for (size_t p = 0; p < n_proofs; ++p)
+        if (proofs[p].vk >= n_vks || !proofs[p].proof || (vks[proofs[p].vk].num_inputs && !proofs[p].pub_inputs)) {
+            set_error(w + ": bad proof entry (vk index, proof or public inputs)");
+            return B200_ERR_INVALID;
+        }
+    for (size_t l = 0; l < n_links; ++l)
+        if (!links[l].comm1 || !links[l].comm2 || !links[l].proof || links[l].alignment > kMaxAlign || links[l].size == 0) {
+            set_error(w + ": bad link entry");
+            return B200_ERR_INVALID;
+        }
+    if (!g2_records_on_curve(g2_tau_h, g2_h)) {
+        set_error(w + ": G2 point not on curve");
+        return B200_ERR_NOT_ON_CURVE;
+    }
+    return B200_OK;
+}
 
 }  // namespace
 
@@ -305,29 +544,11 @@ extern "C" int b200_plonk_batch_verify(b200_ctx* ctx, const b200_verifying_key* 
                                        size_t n_proofs, const b200_batch_link* links, size_t n_links, const uint64_t g2_h[16],
                                        const uint64_t g2_tau_h[16], int* all_accepted, uint8_t* verdicts) {
     B200_TRY
-    if (!ctx || (n_vks && !vks) || (n_proofs && !proofs) || (n_links && !links) || !g2_h || !g2_tau_h || !all_accepted ||
-        n_vks > 0xffffffffu || n_proofs + n_links > 0xffffffffu)
+    if (!args_present(ctx, vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h) || !all_accepted)
         return B200_ERR_INVALID;
     *all_accepted = 0;
-    for (size_t v = 0; v < n_vks; ++v)
-        if (vks[v].log_n > kMaxAlign || !vks[v].k || !vks[v].selector_comms || !vks[v].sigma_comms) {
-            set_error("batch_verify: bad verifying key");
-            return B200_ERR_INVALID;
-        }
-    for (size_t p = 0; p < n_proofs; ++p)
-        if (proofs[p].vk >= n_vks || !proofs[p].proof || (vks[proofs[p].vk].num_inputs && !proofs[p].pub_inputs)) {
-            set_error("batch_verify: bad proof entry (vk index, proof or public inputs)");
-            return B200_ERR_INVALID;
-        }
-    for (size_t l = 0; l < n_links; ++l)
-        if (!links[l].comm1 || !links[l].comm2 || !links[l].proof || links[l].alignment > kMaxAlign || links[l].size == 0) {
-            set_error("batch_verify: bad link entry");
-            return B200_ERR_INVALID;
-        }
-    if (!g2_records_on_curve(g2_tau_h, g2_h)) {
-        set_error("batch_verify: G2 point not on curve");
-        return B200_ERR_NOT_ON_CURVE;
-    }
+    int rc = check_items("batch_verify", vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h);
+    if (rc != B200_OK) return rc;
     const size_t k = n_proofs + n_links;
     if (k == 0) {
         *all_accepted = 1;
@@ -338,112 +559,7 @@ extern "C" int b200_plonk_batch_verify(b200_ctx* ctx, const b200_verifying_key* 
     cudaStream_t st = ctx->c.stream;
     Batch bt;
     bt.c = &ctx->c;
-    bt.k = k;
-    bt.n_vks = (unsigned)n_vks;
-
-    // ---- host staging: keys, items, public inputs, layouts ---------------------------------------------------------
-    std::vector<VkDev> hv(n_vks);
-    std::vector<fe> hw;  // per key: w and the table start
-    size_t wtab_n = 0;
-    for (size_t v = 0; v < n_vks; ++v) {
-        VkDev& d = hv[v];
-        std::memcpy(d.k, vks[v].k, sizeof(d.k));
-        std::memcpy(d.sel, vks[v].selector_comms, sizeof(d.sel));
-        std::memcpy(d.sig, vks[v].sigma_comms, sizeof(d.sig));
-        d.log_n = vks[v].log_n;
-        d.num_inputs = vks[v].num_inputs;
-        d.w = host_root_of_unity(d.log_n);
-        const uint64_t n = (uint64_t)1 << d.log_n;
-        fe nf = fe_zero();
-        nf.l[0] = (uint32_t)n;
-        nf.l[1] = (uint32_t)(n >> 32);
-        d.n_mont = fe_to_mont<Fr>(nf);
-        d.wtab_off = wtab_n;
-        wtab_n += d.num_inputs ? d.num_inputs : 1;
-    }
-    std::vector<ItemDev> hi(k);
-    std::vector<vt::ProofIn> hp(n_proofs);
-    std::vector<LinkDev> hl(n_links);
-    std::vector<fe> hpi;
-    size_t den_n = 0, tr_n = 0, base_n = 0;
-    std::vector<std::vector<uint32_t>> per_vk(n_vks);
-    for (size_t p = 0; p < n_proofs; ++p) {
-        const VkDev& vk = hv[proofs[p].vk];
-        std::memcpy(&hp[p], proofs[p].proof, sizeof(vt::ProofIn));
-        ItemDev& it = hi[p];
-        it.kind = 0;
-        it.idx = (uint32_t)p;
-        it.vk = proofs[p].vk;
-        it.base_off = (uint32_t)base_n;
-        base_n += vt::kProofPoints;
-        it.pi_off = hpi.size();
-        const fe* pi = reinterpret_cast<const fe*>(proofs[p].pub_inputs);
-        hpi.insert(hpi.end(), pi, pi + vk.num_inputs);
-        it.den_off = den_n;
-        den_n += vk.num_inputs ? vk.num_inputs : 1;
-        it.tr_off = tr_n;
-        it.tr_cap = vt::plonk_transcript_bytes(vk.num_inputs);
-        tr_n += it.tr_cap;
-        per_vk[it.vk].push_back((uint32_t)p);
-    }
-    for (size_t l = 0; l < n_links; ++l) {
-        LinkDev& d = hl[l];
-        std::memcpy(&d.pt[vt::kLinkC1], links[l].comm1, 64);
-        std::memcpy(&d.pt[vt::kLinkC2], links[l].comm2, 64);
-        std::memcpy(&d.pt[vt::kLinkCq], links[l].proof->quotient_commitment, 64);
-        std::memcpy(&d.pt[vt::kLinkPi], links[l].proof->opening_proof, 64);
-        d.offset = links[l].offset;
-        d.size = links[l].size;
-        d.alignment = links[l].alignment;
-        ItemDev& it = hi[n_proofs + l];
-        std::memset(&it, 0, sizeof(it));
-        it.kind = 1;
-        it.idx = (uint32_t)l;
-        it.base_off = (uint32_t)base_n;
-        base_n += vt::kLinkPoints;
-    }
-    // shared bases after the items' own: 18 per key, then G
-    bt.shared0 = base_n;
-    bt.n_bases = base_n + n_vks * vt::kVkPoints + 1;
-    if (bt.n_bases > 0xffffffffu) return B200_ERR_INVALID;
-    std::vector<g1_affine> hshared;
-    for (size_t v = 0; v < n_vks; ++v) {
-        hshared.insert(hshared.end(), hv[v].sel, hv[v].sel + vt::NS);
-        hshared.insert(hshared.end(), hv[v].sig, hv[v].sig + vt::NW);
-    }
-    hshared.push_back(vt::g1_generator());
-    std::vector<uint32_t> hvk_items, hvk_start(n_vks + 1, 0);
-    for (size_t v = 0; v < n_vks; ++v) {
-        hvk_start[v] = (uint32_t)hvk_items.size();
-        hvk_items.insert(hvk_items.end(), per_vk[v].begin(), per_vk[v].end());
-    }
-    hvk_start[n_vks] = (uint32_t)hvk_items.size();
-    Roots roots;
-    for (int a = 0; a <= kMaxAlign; ++a) roots.g[a] = host_root_of_unity((unsigned)a);
-
-    int rc;
-    if ((rc = upload(&bt.items, hi, st)) || (rc = upload(&bt.vks, hv, st)) || (rc = upload(&bt.proofs, hp, st)) ||
-        (rc = upload(&bt.links, hl, st)) || (rc = upload(&bt.pi, hpi, st)) || (rc = upload(&bt.vk_items, hvk_items, st)) ||
-        (rc = upload(&bt.vk_start, hvk_start, st)) || (rc = bt.wtab.reserve(wtab_n * sizeof(fe))) ||
-        (rc = bt.tr.reserve(tr_n + 1)) || (rc = bt.den.reserve(den_n * sizeof(fe) + 32)) ||
-        (rc = bt.den_tmp.reserve(den_n * sizeof(fe) + 32)) || (rc = bt.state.reserve(k * sizeof(ItemState))) ||
-        (rc = bt.digest.reserve(k * 32)) || (rc = bt.rec.reserve(k * kRec * sizeof(fe))) ||
-        (rc = bt.bases_pts.reserve(bt.n_bases * sizeof(g1_affine))) || (rc = bt.scal.reserve(2 * bt.n_bases * sizeof(fe))) ||
-        (rc = bt.mask.reserve(k)))
-        return rc;
-    // w^j tables of the keys
-    for (size_t v = 0; v < n_vks; ++v)
-        fill_powers((fe*)bt.wtab.p + hv[v].wtab_off, hv[v].num_inputs ? hv[v].num_inputs : 1, hv[v].w, fe_one<Fr>(), st);
-    B200_CUDA(cudaMemcpyAsync((g1_affine*)bt.bases_pts.p + bt.shared0, hshared.data(), hshared.size() * sizeof(g1_affine),
-                              cudaMemcpyHostToDevice, st));
-    B200_CUDA(cudaMemsetAsync(bt.rec.p, 0, k * kRec * sizeof(fe), st));
-
-    // ---- 1. prepare, 2. invert ------------------------------------------------------------------------------------
-    B200_LAUNCH(k_prepare, grid_of(k, 128), 128, 0, st)((const ItemDev*)bt.items.p, k, (const VkDev*)bt.vks.p,
-                                                       (const vt::ProofIn*)bt.proofs.p, (const LinkDev*)bt.links.p,
-                                                       (const fe*)bt.pi.p, (const fe*)bt.wtab.p, (uint8_t*)bt.tr.p,
-                                                       (fe*)bt.den.p, roots, (ItemState*)bt.state.p, (uint8_t*)bt.digest.p);
-    if (den_n) batch_inverse_enqueue(nullptr, (fe*)bt.den.p, (fe*)bt.den_tmp.p, den_n, st);
+    if ((rc = bt.stage(vks, n_vks, proofs, n_proofs, links, n_links)) != B200_OK) return rc;
     B200_LAUNCH(k_gather_bases, grid_of(k, 128), 128, 0, st)((const ItemDev*)bt.items.p, k, (const vt::ProofIn*)bt.proofs.p,
                                                             (const LinkDev*)bt.links.p, (g1_affine*)bt.bases_pts.p);
     B200_CUDA(cudaGetLastError());
@@ -467,7 +583,7 @@ extern "C" int b200_plonk_batch_verify(b200_ctx* ctx, const b200_verifying_key* 
     B200_LAUNCH(k_scalars, grid_of(k, 128), 128, 0, st)((const ItemDev*)bt.items.p, k, (const VkDev*)bt.vks.p,
                                                        (const vt::ProofIn*)bt.proofs.p, (const fe*)bt.pi.p,
                                                        (const fe*)bt.wtab.p, (const fe*)bt.den.p,
-                                                       (const ItemState*)bt.state.p, seed, (fe*)bt.rec.p);
+                                                       (const ItemState*)bt.state.p, seed, false, (fe*)bt.rec.p);
     B200_CUDA(cudaGetLastError());
     // ---- 5, 6. bases without tables, merged scalars, MSM pair, one pairing ------------------------------------------
     if ((rc = bases_create_device((const g1_affine*)bt.bases_pts.p, bt.n_bases, 1, st, &bt.bases, 0)) != B200_OK) return rc;
@@ -484,6 +600,87 @@ extern "C" int b200_plonk_batch_verify(b200_ctx* ctx, const b200_verifying_key* 
         for (size_t i = 0; i < k; ++i) verdicts[i] = mask[i];
         if (!ok && (rc = bt.bisect(valid, g2_tau_h, g2_h, verdicts)) != B200_OK) return rc;
     }
+    return B200_OK;
+    B200_CATCH
+}
+
+extern "C" int b200_plonk_verify_each(b200_ctx* ctx, const b200_verifying_key* vks, size_t n_vks, const b200_batch_proof* proofs,
+                                      size_t n_proofs, const b200_batch_link* links, size_t n_links, const uint64_t g2_h[16],
+                                      const uint64_t g2_tau_h[16], uint8_t* verdicts) {
+    B200_TRY
+    const size_t k = n_proofs + n_links;
+    if (!args_present(ctx, vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h) || (k && !verdicts))
+        return B200_ERR_INVALID;
+    int rc = check_items("verify_each", vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h);
+    if (rc != B200_OK || k == 0) return rc;
+    // Q = ([tau]_2, [1]_2), prepared on the host (both are on the curve: check_items)
+    std::vector<G2Prepared> q(2);
+    g2_prepare_record(g2_tau_h, &q[0]);
+    g2_prepare_record(g2_h, &q[1]);
+    std::lock_guard<std::mutex> lk(ctx->c.mu);
+    B200_CUDA(cudaSetDevice(ctx->c.device));
+    cudaStream_t st = ctx->c.stream;
+    Batch bt;
+    bt.c = &ctx->c;
+    if ((rc = bt.stage(vks, n_vks, proofs, n_proofs, links, n_links)) != B200_OK) return rc;
+    DevBuf d_q, d_ab, d_one, d_verdicts;
+    if ((rc = upload(&d_q, q, st)) || (rc = d_ab.reserve(2 * k * sizeof(g1_affine))) || (rc = d_one.reserve(k)) ||
+        (rc = d_verdicts.reserve(k)))
+        return rc;
+    // each item's coefficients with rho = 1, its A_i and -B_i, and its own two-pair check
+    B200_LAUNCH(k_scalars, grid_of(k, 128), 128, 0, st)((const ItemDev*)bt.items.p, k, (const VkDev*)bt.vks.p,
+                                                       (const vt::ProofIn*)bt.proofs.p, (const fe*)bt.pi.p,
+                                                       (const fe*)bt.wtab.p, (const fe*)bt.den.p,
+                                                       (const ItemState*)bt.state.p, Seed{}, true, (fe*)bt.rec.p);
+    B200_LAUNCH(k_item_points, grid_of(32 * k, kItemThreads), kItemThreads, 0, st)(
+        (const ItemDev*)bt.items.p, k, (const VkDev*)bt.vks.p, (const vt::ProofIn*)bt.proofs.p, (const LinkDev*)bt.links.p,
+        (const fe*)bt.rec.p, (g1_affine*)d_ab.p);
+    pairing_many_enqueue((const G2Prepared*)d_q.p, 2, (const g1_affine*)d_ab.p, k, (uint8_t*)d_one.p, st);
+    B200_LAUNCH(k_verdicts, grid_of(k, 128), 128, 0, st)((const ItemState*)bt.state.p, (const uint8_t*)d_one.p, k,
+                                                        (uint8_t*)d_verdicts.p);
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaMemcpyAsync(verdicts, d_verdicts.p, k, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    return B200_OK;
+    B200_CATCH
+}
+
+extern "C" int b200_pairing_check_many(b200_ctx* ctx, const uint64_t* g2_points, size_t m, const uint64_t* g1_points,
+                                       size_t n_checks, uint8_t* is_one) {
+    B200_TRY
+    if (!ctx || (m && !g2_points) || (m && n_checks && !g1_points) || (n_checks && !is_one)) return B200_ERR_INVALID;
+    if (m > (size_t)kMaxPairs) {
+        set_error("pairing_check_many: more than " + std::to_string(kMaxPairs) + " pairs per check");
+        return B200_ERR_INVALID;
+    }
+    // the m schedules, then the n_checks x m G1 points: one upload
+    const size_t q_bytes = m * sizeof(G2Prepared), p_bytes = n_checks * m * sizeof(g1_affine);
+    std::vector<uint8_t> h(q_bytes + p_bytes);
+    for (size_t j = 0; j < m; ++j)
+        if (!g2_prepare_record(g2_points + 16 * j, reinterpret_cast<G2Prepared*>(h.data()) + j)) {
+            set_error("pairing_check_many: G2 point " + std::to_string(j) + " not on curve");
+            return B200_ERR_NOT_ON_CURVE;
+        }
+    if (n_checks == 0) return B200_OK;
+    if (p_bytes) std::memcpy(h.data() + q_bytes, g1_points, p_bytes);
+    std::lock_guard<std::mutex> lk(ctx->c.mu);
+    B200_CUDA(cudaSetDevice(ctx->c.device));
+    cudaStream_t st = ctx->c.stream;
+    DevBuf d_in, d_out;
+    int rc;
+    if ((rc = upload(&d_in, h, st)) || (rc = d_out.reserve(n_checks))) return rc;
+    pairing_many_enqueue((const G2Prepared*)d_in.p, (int)m, (const g1_affine*)((const uint8_t*)d_in.p + q_bytes), n_checks,
+                         (uint8_t*)d_out.p, st);
+    B200_CUDA(cudaGetLastError());
+    std::vector<uint8_t> out(n_checks);
+    B200_CUDA(cudaMemcpyAsync(out.data(), d_out.p, n_checks, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    for (size_t c = 0; c < n_checks; ++c)
+        if (out[c] > 1) {
+            set_error("pairing_check_many: check " + std::to_string(c) + ": G1 point not on curve");
+            return B200_ERR_NOT_ON_CURVE;
+        }
+    std::memcpy(is_one, out.data(), n_checks);
     return B200_OK;
     B200_CATCH
 }

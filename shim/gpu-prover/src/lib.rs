@@ -245,32 +245,55 @@ impl GpuProver {
     pub fn batch_verify(&self, vks: &[BatchVerifyingKey], proofs: &[(usize, &[Fr], &Proof<Bn254>)],
                         links: &[(&G1Affine, &G1Affine, &mpc_plonk::proof_system::structs::LinkingProof<Bn254>, &GroupLayout)],
                         g2_h: &[u64; 16], g2_tau_h: &[u64; 16]) -> Result<Vec<bool>, PlonkError> {
-        let flat: Vec<(Vec<u64>, Vec<u64>, Vec<u64>)> = vks.iter().map(|v| (
-            v.k.iter().flat_map(fr_limbs).collect(),
-            v.selector_comms.iter().flat_map(g1_record).collect(),
-            v.sigma_comms.iter().flat_map(g1_record).collect())).collect();
-        let c_vks: Vec<ffi::b200_verifying_key> = vks.iter().zip(&flat).map(|(v, (k, sel, sig))| ffi::b200_verifying_key {
-            log_n: v.log_n, num_inputs: v.num_inputs, k: k.as_ptr(), selector_comms: sel.as_ptr(), sigma_comms: sig.as_ptr(),
-        }).collect();
-        let pis: Vec<Vec<u64>> = proofs.iter().map(|(_, pi, _)| pi.iter().flat_map(fr_limbs).collect()).collect();
-        let raws: Vec<ffi::b200_proof> = proofs.iter().map(|(_, _, p)| proof_to_raw(p)).collect();
-        let c_proofs: Vec<ffi::b200_batch_proof> = proofs.iter().zip(pis.iter().zip(&raws)).map(|((vk, _, _), (pi, raw))| {
-            ffi::b200_batch_proof { vk: *vk as c_uint, pub_inputs: pi.as_ptr(), proof: raw }
-        }).collect();
-        let lflat: Vec<([u64; 8], [u64; 8], ffi::b200_link_proof)> = links.iter().map(|(a, b, lp, _)| (g1_record(a), g1_record(b),
-            ffi::b200_link_proof { quotient_commitment: g1_record(&lp.quotient_commitment.0), opening_proof: g1_record(&lp.opening_proof.proof) })).collect();
-        let c_links: Vec<ffi::b200_batch_link> = links.iter().zip(&lflat).map(|((_, _, _, lay), (a, b, lp))| ffi::b200_batch_link {
-            comm1: a.as_ptr(), comm2: b.as_ptr(), alignment: lay.alignment as c_uint, offset: lay.offset, size: lay.size, proof: lp,
-        }).collect();
         let mut verdicts = vec![0u8; proofs.len() + links.len()];
         let mut all: c_int = 0;
-        check(unsafe {
+        with_batch(vks, proofs, links, |c_vks, c_proofs, c_links| check(unsafe {
             ffi::b200_plonk_batch_verify(ffi::b200_pool_ctx(self.pool, 0), c_vks.as_ptr(), c_vks.len(), c_proofs.as_ptr(),
                                          c_proofs.len(), c_links.as_ptr(), c_links.len(), g2_h.as_ptr(), g2_tau_h.as_ptr(),
                                          &mut all, verdicts.as_mut_ptr())
-        })?;
+        }))?;
         Ok(verdicts.into_iter().map(|v| v == 1).collect())
     }
+
+    /// The same verdicts as `batch_verify`, each item checked on its own with its own pairing on this GPU
+    /// (`b200_plonk_verify_each`): no bisection, so the cost does not depend on how many items fail.
+    #[allow(clippy::type_complexity)]
+    pub fn verify_each(&self, vks: &[BatchVerifyingKey], proofs: &[(usize, &[Fr], &Proof<Bn254>)],
+                       links: &[(&G1Affine, &G1Affine, &mpc_plonk::proof_system::structs::LinkingProof<Bn254>, &GroupLayout)],
+                       g2_h: &[u64; 16], g2_tau_h: &[u64; 16]) -> Result<Vec<bool>, PlonkError> {
+        let mut verdicts = vec![0u8; proofs.len() + links.len()];
+        with_batch(vks, proofs, links, |c_vks, c_proofs, c_links| check(unsafe {
+            ffi::b200_plonk_verify_each(ffi::b200_pool_ctx(self.pool, 0), c_vks.as_ptr(), c_vks.len(), c_proofs.as_ptr(),
+                                        c_proofs.len(), c_links.as_ptr(), c_links.len(), g2_h.as_ptr(), g2_tau_h.as_ptr(),
+                                        verdicts.as_mut_ptr())
+        }))?;
+        Ok(verdicts.into_iter().map(|v| v == 1).collect())
+    }
+}
+
+/// The C structs of a batch of `verify` / `verify_link_proof` items, alive while `f` runs.
+#[allow(clippy::type_complexity)]
+fn with_batch<R>(vks: &[BatchVerifyingKey], proofs: &[(usize, &[Fr], &Proof<Bn254>)],
+                 links: &[(&G1Affine, &G1Affine, &mpc_plonk::proof_system::structs::LinkingProof<Bn254>, &GroupLayout)],
+                 f: impl FnOnce(&[ffi::b200_verifying_key], &[ffi::b200_batch_proof], &[ffi::b200_batch_link]) -> R) -> R {
+    let flat: Vec<(Vec<u64>, Vec<u64>, Vec<u64>)> = vks.iter().map(|v| (
+        v.k.iter().flat_map(fr_limbs).collect(),
+        v.selector_comms.iter().flat_map(g1_record).collect(),
+        v.sigma_comms.iter().flat_map(g1_record).collect())).collect();
+    let c_vks: Vec<ffi::b200_verifying_key> = vks.iter().zip(&flat).map(|(v, (k, sel, sig))| ffi::b200_verifying_key {
+        log_n: v.log_n, num_inputs: v.num_inputs, k: k.as_ptr(), selector_comms: sel.as_ptr(), sigma_comms: sig.as_ptr(),
+    }).collect();
+    let pis: Vec<Vec<u64>> = proofs.iter().map(|(_, pi, _)| pi.iter().flat_map(fr_limbs).collect()).collect();
+    let raws: Vec<ffi::b200_proof> = proofs.iter().map(|(_, _, p)| proof_to_raw(p)).collect();
+    let c_proofs: Vec<ffi::b200_batch_proof> = proofs.iter().zip(pis.iter().zip(&raws)).map(|((vk, _, _), (pi, raw))| {
+        ffi::b200_batch_proof { vk: *vk as c_uint, pub_inputs: pi.as_ptr(), proof: raw }
+    }).collect();
+    let lflat: Vec<([u64; 8], [u64; 8], ffi::b200_link_proof)> = links.iter().map(|(a, b, lp, _)| (g1_record(a), g1_record(b),
+        ffi::b200_link_proof { quotient_commitment: g1_record(&lp.quotient_commitment.0), opening_proof: g1_record(&lp.opening_proof.proof) })).collect();
+    let c_links: Vec<ffi::b200_batch_link> = links.iter().zip(&lflat).map(|((_, _, _, lay), (a, b, lp))| ffi::b200_batch_link {
+        comm1: a.as_ptr(), comm2: b.as_ptr(), alignment: lay.alignment as c_uint, offset: lay.offset, size: lay.size, proof: lp,
+    }).collect();
+    f(&c_vks, &c_proofs, &c_links)
 }
 
 /// The flat verifying key of one circuit, as `verify` takes it.

@@ -355,7 +355,8 @@ class PlonkCircuit:
     def public_input(self) -> List[int]:
         return [self.witness_values[v] for v in self.pub_input_vars]
 
-    def finalize_for_arithmetization(self, min_log_n: int = 2, wires_only: bool = False) -> SynthCircuit:
+    def finalize_for_arithmetization(self, min_log_n: int = 2, wires_only: bool = False,
+                                     witness_only: bool = False) -> SynthCircuit:
         """Public-input gates first, zero padding to the next power of two, one copy-constraint cycle per variable
         (upstream: `finalize_for_arithmetization`, traits.rs:847,991).  Returns the flat tables the C ABI takes.
 
@@ -393,6 +394,15 @@ class PlonkCircuit:
         # only the 5 x n value table changes): skip the selector columns and the copy permutation, keep their fingerprint
         gate_sels = [tuple(row.gate.selectors()) for row in rows]
         digest = hash((n, tuple(tuple(row.wires) for row in rows), tuple(gate_sels))) or 1
+        # `witness_only` (a key made by `preprocess_wiring` holds the wiring too): per proof only the witness vector goes
+        # to the device, and the 5 x n value table is never built on the host
+        if witness_only:
+            pub = self.public_input()
+            self._finalized = True
+            return SynthCircuit(log_n=log_n, num_inputs=len(pub), k=to_mont_array([pow(5, i, R) for i in range(N_WIRES)]),
+                                selectors=None, perm=None, wires=None, pub_inputs=to_mont_array(pub), n_gates=n_gates,
+                                selectors_int=None, wires_int=None, pub_inputs_int=pub, structure_digest=digest,
+                                witness=to_mont_array(self.witness_values))
         wires_int = [[self.witness_values[row.wires[w]] for row in rows] for w in range(N_WIRES)]
         pub = self.public_input()
         k_int = [pow(5, i, R) for i in range(N_WIRES)]
@@ -415,7 +425,9 @@ class PlonkCircuit:
         return SynthCircuit(log_n=log_n, num_inputs=len(pub), k=to_mont_array(k_int),
                             selectors=np.stack([to_mont_array(col) for col in sel]), perm=perm, wires=wires,
                             pub_inputs=pub_arr, n_gates=n_gates, selectors_int=sel, wires_int=wires_int, pub_inputs_int=pub,
-                            structure_digest=digest)
+                            structure_digest=digest,
+                            wire_vars=np.array([row.wires for row in rows], dtype=np.uint32).T.copy(),
+                            witness=to_mont_array(self.witness_values))
 
 
 # ---------------------------------------------------------------------------------------------

@@ -94,6 +94,44 @@ int main(int argc, char** argv) {
             fprintf(stderr, "pool proof %d differs from the direct proof\n", i);
             return 5;
         }
+
+    /* The same circuit handed over as a host like the reference's holds it: the wiring (the variable on every wire
+     * position) and the witness vector.  Here they are recovered from the job's tables: one variable per cycle of the
+     * copy permutation.  A key made from the wiring proves from the witness vector alone; proof and public inputs must
+     * equal those of b200_plonk_prove on the 5 x n table under the same key, directly, as a batch and through the pool. */
+    unsigned* wire_vars = (unsigned*)malloc(5 * n * sizeof(unsigned));
+    uint64_t* witness = (uint64_t*)malloc(5 * n * 32);
+    size_t num_vars = 0;
+    memset(wire_vars, 0xFF, 5 * n * sizeof(unsigned));
+    for (size_t p = 0; p < 5 * n; ++p) {
+        if (wire_vars[p] != 0xFFFFFFFFu) continue;
+        memcpy(witness + 4 * num_vars, wires + 4 * p, 32);
+        for (size_t q = p; wire_vars[q] == 0xFFFFFFFFu; q = (size_t)perm[q]) wire_vars[q] = (unsigned)num_vars;
+        ++num_vars;
+    }
+    b200_pk* wpk = NULL;
+    CHECK(b200_plonk_preprocess_wiring(ctx, bases, log_n, num_inputs, selectors, wire_vars, num_vars, k, &wpk));
+    if (b200_pk_num_vars(wpk) != num_vars || b200_pk_num_vars(pk) != 0) {
+        fprintf(stderr, "b200_pk_num_vars: wrong answer\n");
+        return 6;
+    }
+    b200_proof from_table, from_witness[4];
+    uint64_t* pub_out = (uint64_t*)calloc(4 * (num_inputs + 1) * 4, 8);
+    CHECK(b200_plonk_prove(ctx, wpk, wires, pub_inputs, blinders, &from_table, NULL, NULL));
+    CHECK(b200_plonk_prove_witness(ctx, wpk, witness, blinders, &from_witness[0], NULL, NULL, pub_out));
+    b200_witness_item items[2] = {{witness, blinders, &from_witness[1], NULL, NULL, pub_out + 4 * num_inputs},
+                                  {witness, blinders, &from_witness[2], NULL, NULL, pub_out + 8 * num_inputs}};
+    int statuses[2];
+    CHECK(b200_plonk_prove_witness_batch(ctx, wpk, items, 2, statuses));
+    CHECK(b200_pool_submit_prove_witness(pool, wpk, witness, blinders, &from_witness[3], NULL, pub_out + 12 * num_inputs, &tickets[0]));
+    CHECK(b200_pool_wait(pool, tickets[0]));
+    for (int i = 0; i < 4; ++i)
+        if (memcmp(&from_witness[i], &from_table, sizeof(proof)) != 0 ||
+            memcmp(pub_out + 4 * num_inputs * i, pub_inputs, 32 * num_inputs) != 0) {
+            fprintf(stderr, "witness proof %d differs from the proof on the expanded table\n", i);
+            return 6;
+        }
+    b200_pk_free(ctx, wpk);
     b200_pool_destroy(pool);
 
     FILE* o = fopen(argv[2], "wb");

@@ -178,6 +178,23 @@ int b200_known_dlog_bases_device(b200_ctx* ctx, uint64_t seed, size_t first, siz
 int b200_plonk_preprocess(b200_ctx* ctx, const b200_bases* srs, unsigned log_n, size_t num_inputs,
                           const uint64_t* selectors_evals, const uint64_t* perm, const uint64_t* k,
                           b200_pk** out);
+/* b200_plonk_preprocess from the circuit's wiring (`PlonkCircuit::wire_variables` after finalize_for_arithmetization)
+ * instead of the permutation derived from it:
+ *   wire_vars   5 x n variable indices (32 bits each), wire_vars[i*n + j] = the variable on wire i of row j, each < num_vars;
+ *   num_vars    length of the witness vector a proof of this key takes (1 <= num_vars < 2^32).
+ * The copy permutation is derived on the device: the positions p = i*n + j of one variable, in ascending p, form one
+ * cycle, each mapped to the next and the last to the first (a variable used once maps to itself; variable numbers no
+ * position uses are allowed).  The key is the key b200_plonk_preprocess builds from that permutation (same verifying key)
+ * and additionally keeps wire_vars resident (20n bytes), so that proofs can be made from witness vectors
+ * (b200_plonk_prove_witness).  Public input j is the witness value of the variable on the output wire (wire 4) of row j,
+ * j < num_inputs: the public-input gates constrain w4 = public input.
+ * B200_ERR_INVALID for an index >= num_vars (b200_last_error names the first such position) and for num_vars outside
+ * [1, 2^32).  The grouping is a radix sort (CUB); its launches are not counted by b200_kernel_launches. */
+int b200_plonk_preprocess_wiring(b200_ctx* ctx, const b200_bases* srs, unsigned log_n, size_t num_inputs,
+                                 const uint64_t* selectors_evals, const unsigned* wire_vars, size_t num_vars,
+                                 const uint64_t* k, b200_pk** out);
+/* Length of the witness vector of a key made by b200_plonk_preprocess_wiring; 0 for a key made by b200_plonk_preprocess. */
+size_t b200_pk_num_vars(const b200_pk* pk);
 /* VerifyingKey commitments: 13 selector + 5 sigma commitments, 64 B each. */
 int b200_pk_verifying_key(const b200_pk* pk, uint64_t* selector_comms, uint64_t* sigma_comms);
 /* Shape of a key: number of public inputs and log2 of the domain size it was preprocessed for. */
@@ -198,6 +215,17 @@ void b200_pk_free(b200_ctx* ctx, b200_pk* pk);
 int b200_plonk_prove(b200_ctx* ctx, const b200_pk* pk, const uint64_t* wires,
                      const uint64_t* pub_inputs, const uint64_t* blinders, b200_proof* proof,
                      uint64_t* link_poly, uint64_t* challenges);
+
+/* b200_plonk_prove from the witness vector (`PlonkCircuit::witness`: num_vars x 4 limbs, Montgomery, host or device
+ * pointer) of a key made by b200_plonk_preprocess_wiring.  The wire table is gathered on the device from the key's
+ * resident wiring, so a proof uploads num_vars x 32 bytes instead of 5n x 32 and the host never builds the table.
+ * proof, link_poly and challenges are byte-identical to b200_plonk_prove on the expanded table
+ * wires[i*n + j] = witness[wire_vars[i*n + j]] with the public inputs read from the witness.
+ * pub_inputs_out (may be NULL) receives the key's num_inputs public inputs.  A device witness (read in place when it is
+ * 16-byte aligned) costs one extra stream synchronisation: its public inputs are read back before the transcript starts.
+ * B200_ERR_INVALID for a key without wiring or a NULL ctx / pk / witness / blinders / proof. */
+int b200_plonk_prove_witness(b200_ctx* ctx, const b200_pk* pk, const uint64_t* witness, const uint64_t* blinders,
+                             b200_proof* proof, uint64_t* link_poly, uint64_t* challenges, uint64_t* pub_inputs_out);
 
 /* One witness of a batch: the arguments of b200_plonk_prove. */
 typedef struct {
@@ -220,6 +248,20 @@ typedef struct {
  * 400 MB at 2^16; at most 64); the results do not depend on the chunk size.  A batch runs eagerly (no CUDA graphs) in
  * buffers of its own on the context, kept for the next batch: single proofs keep replaying their graphs. */
 int b200_plonk_prove_batch(b200_ctx* ctx, const b200_pk* pk, const b200_prove_item* items, size_t k, int* statuses);
+
+/* One witness vector of a batch: the arguments of b200_plonk_prove_witness. */
+typedef struct {
+    const uint64_t* witness;    /* num_vars x 4 limbs, host or device pointer */
+    const uint64_t* blinders;   /* 17, draw order as b200_plonk_prove */
+    b200_proof* proof;
+    uint64_t* link_poly;        /* may be NULL; (n + 2) x 4 limbs */
+    uint64_t* challenges;       /* may be NULL; beta gamma alpha zeta v u */
+    uint64_t* pub_inputs_out;   /* may be NULL; the key's num_inputs values */
+} b200_witness_item;
+/* b200_plonk_prove_batch with the items given as witness vectors of a key made by b200_plonk_preprocess_wiring: one
+ * launch gathers the wire tables of a whole chunk.  Item i's outputs are byte-identical to b200_plonk_prove_witness's;
+ * statuses, return codes and chunking exactly as b200_plonk_prove_batch (B200_ERR_INVALID also for a key without wiring). */
+int b200_plonk_prove_witness_batch(b200_ctx* ctx, const b200_pk* pk, const b200_witness_item* items, size_t k, int* statuses);
 
 /* Flat link proof, field order of mpc-plonk `LinkingProof { quotient_commitment, opening_proof }`
  * (crates/relayer-types/types-proofs/src/mocks.rs:28-30). */
@@ -380,6 +422,12 @@ b200_ctx* b200_pool_ctx(b200_pool* pool, unsigned worker);
 int b200_pool_submit_prove(b200_pool* pool, const b200_pk* pk, const uint64_t* wires,
                            const uint64_t* pub_inputs, size_t num_inputs, const uint64_t* blinders,
                            b200_proof* proof, uint64_t* link_poly, uint64_t* ticket);
+/* Queue one `b200_plonk_prove_witness(ctx_of_some_worker, pk, witness, blinders, proof, link_poly, NULL, pub_inputs_out)`.
+ * The blinders are copied at submit; the witness vector and the output buffers stay owned by the caller until the ticket
+ * has been waited for.  B200_ERR_INVALID at submit for a NULL pool / pk / witness / blinders / proof / ticket or a key
+ * without wiring. */
+int b200_pool_submit_prove_witness(b200_pool* pool, const b200_pk* pk, const uint64_t* witness, const uint64_t* blinders,
+                                   b200_proof* proof, uint64_t* link_poly, uint64_t* pub_inputs_out, uint64_t* ticket);
 /* Queue one `b200_plonk_prove_batch(ctx_of_some_worker, pk, items, k, statuses)` as ONE job on one worker.  The items'
  * pub_inputs and blinders are copied at submit (the items array too); wires, the proof / link_poly / challenges buffers
  * and statuses (may be NULL) stay owned by the caller until the ticket has been waited for.  The ticket's status is the

@@ -313,6 +313,11 @@ class ProvingKey:
     def domain_size(self) -> int:
         return 1 << self.log_n
 
+    @property
+    def num_vars(self) -> int:
+        """Length of the witness vector a proof of this key takes; 0 for a key without wiring (`preprocess`)."""
+        return int(self._ctx._lib.b200_pk_num_vars(self._h))
+
     def free(self):
         if self._h:
             self._ctx._lib.b200_pk_free(self._ctx._h, self._h)
@@ -520,6 +525,70 @@ class PlonkKzgSnark:
         return ProvingKey(ctx, h, log_n, num_inputs, kk)
 
     @staticmethod
+    def preprocess_wiring(ctx: Context, srs: Bases, log_n: int, num_inputs: int, selectors: np.ndarray,
+                          wire_vars: np.ndarray, num_vars: int, k: np.ndarray) -> ProvingKey:
+        """`preprocess` from the circuit's wiring (b200_plonk_preprocess_wiring): wire_vars[i, j] = the variable on wire i of
+        row j (5 x n, < num_vars).  The copy permutation is derived on the device and the key keeps the wiring, so its
+        proofs are made from witness vectors (`prove_witness`)."""
+        sel = np.ascontiguousarray(selectors, dtype=np.uint64).reshape(13, 1 << log_n, 4)
+        wv = np.ascontiguousarray(wire_vars, dtype=np.uint32).reshape(5 << log_n)
+        kk = np.ascontiguousarray(k, dtype=np.uint64).reshape(5, 4)
+        h = C.c_void_p()
+        _lib.check(ctx._lib.b200_plonk_preprocess_wiring(ctx._h, srs._h, log_n, num_inputs, _ptr(sel), wv.ctypes.data_as(C.c_void_p), num_vars,
+                                                         _ptr(kk), C.byref(h)))
+        return ProvingKey(ctx, h, log_n, num_inputs, kk)
+
+    @staticmethod
+    def prove_witness(ctx: Context, pk: ProvingKey, witness, blinders: np.ndarray, want_challenges: bool = False):
+        """`prove_with_link_hint` from the witness vector (b200_plonk_prove_witness) of a key made by `preprocess_wiring`:
+        witness is the num_vars x 4 array, or the address of one in device or pinned host memory (int).  Returns
+        (proof, LinkingHint, pub_inputs[, challenges]); proof, hint and challenges equal `prove_with_link_hint` on the
+        expanded wire table."""
+        n = pk.domain_size
+        wit, wit_ptr = _witness_arg(pk, witness, "prove_witness")
+        bl = np.ascontiguousarray(blinders, dtype=np.uint64).reshape(17, 4)
+        proof = B200Proof()
+        link = np.zeros((n + 2, 4), dtype=np.uint64)
+        ch = np.zeros((6, 4), dtype=np.uint64)
+        pub = np.zeros((pk.num_inputs, 4), dtype=np.uint64)
+        _lib.check(ctx._lib.b200_plonk_prove_witness(ctx._h, pk._h, wit_ptr, _ptr(bl), C.byref(proof), _ptr(link),
+                                                     _ptr(ch) if want_challenges else None, _ptr(pub) if pub.size else None))
+        hint = LinkingHint(linking_wire_poly=link, linking_wire_comm=np.array(proof.wires_poly_comms[0], dtype=np.uint64))
+        return (proof, hint, pub, ch) if want_challenges else (proof, hint, pub)
+
+    @staticmethod
+    def prove_witness_batch(ctx: Context, pk: ProvingKey, witness_list, blinders_list, link_hints: bool = False,
+                            want_challenges: bool = False):
+        """`prove_batch` with the items given as witness vectors (b200_plonk_prove_witness_batch).  Returns
+        (proofs, hints, statuses, pub_inputs[, challenges]), item i as `prove_witness` of the same arguments."""
+        witness_list, blinders_list = list(witness_list), list(blinders_list)
+        if len(witness_list) != len(blinders_list):
+            raise ValueError(f"prove_witness_batch: {len(witness_list)} witness vectors and {len(blinders_list)} blinder vectors")
+        k, n = len(witness_list), pk.domain_size
+        items = (B200WitnessItem * max(1, k))()
+        keep, pubs = [], []
+        for i, (witness, blinders) in enumerate(zip(witness_list, blinders_list)):
+            wit, wit_ptr = _witness_arg(pk, witness, f"prove_witness_batch: item {i}")
+            bl = np.ascontiguousarray(blinders, dtype=np.uint64)
+            if bl.size != 17 * 4:
+                raise ValueError(f"prove_witness_batch: item {i} has {bl.size // 4} blinders, the prover draws 17")
+            proof = B200Proof()
+            link = np.zeros((n + 2, 4), dtype=np.uint64) if link_hints else None
+            ch = np.zeros((6, 4), dtype=np.uint64) if want_challenges else None
+            pub = np.zeros((pk.num_inputs, 4), dtype=np.uint64)
+            items[i] = B200WitnessItem(wit_ptr, _ptr(bl), C.cast(C.pointer(proof), C.c_void_p),
+                                       _ptr(link) if link is not None else None, _ptr(ch) if ch is not None else None,
+                                       _ptr(pub) if pub.size else None)
+            keep.append((wit, None, bl, proof, link, ch))
+            pubs.append(pub)
+        statuses = (C.c_int * max(1, k))()
+        rc = ctx._lib.b200_plonk_prove_witness_batch(ctx._h, pk._h, items, k, statuses)
+        if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
+            _lib.check(rc)
+        res = _batch_results(keep, statuses, link_hints, want_challenges)
+        return res[:3] + (pubs,) + res[3:]
+
+    @staticmethod
     def prove_with_link_hint(ctx: Context, pk: ProvingKey, wires: np.ndarray, pub_inputs: np.ndarray,
                              blinders: np.ndarray, want_challenges: bool = False):
         """Returns (proof, LinkingHint[, challenges]).  `blinders` are the 17 field elements the
@@ -559,6 +628,17 @@ class PlonkKzgSnark:
 
 
 B200ProveItem = _lib.STRUCTS["b200_prove_item"]  # one witness of a batch
+B200WitnessItem = _lib.STRUCTS["b200_witness_item"]  # one witness vector of a batch
+
+
+def _witness_arg(pk: ProvingKey, witness, where: str):
+    """A witness vector as (array kept alive or None, pointer): an array of the key's num_vars elements, or an address."""
+    if isinstance(witness, (int, np.integer)):
+        return None, C.c_void_p(int(witness))
+    wit = np.ascontiguousarray(witness, dtype=np.uint64)
+    if wit.size != 4 * pk.num_vars:
+        raise ValueError(f"{where}: the witness has {wit.size // 4} elements, the key takes {pk.num_vars}")
+    return wit, _ptr(wit)
 
 
 def _prove_items(pk: ProvingKey, wires_list, pub_inputs_list, blinders_list, link_hints: bool, want_challenges: bool):
@@ -793,6 +873,13 @@ class _PoolBatch:
 
 
 @dataclass
+class _PoolWitness:
+    """What a queued witness job writes into."""
+    proof: Any
+    pub_inputs: np.ndarray
+
+
+@dataclass
 class _PoolLinkBatch:
     """What a queued link batch job writes into: its items' arrays and outputs, and the statuses."""
     held: list
@@ -848,6 +935,28 @@ class ProverPool:
                                                     pi.size // 4, _ptr(bl), C.byref(proof),
                                                     _ptr(link) if link is not None else None, C.byref(ticket)))
         self._keep[ticket.value] = (proof, link, keep, pk)
+        return ticket.value
+
+    def submit_prove_witness(self, pk: "ProvingKey", witness, blinders: np.ndarray, with_link_poly: bool = False,
+                             keep=None) -> int:
+        """Queue one proof from a witness vector (array, or address in pinned host or device memory kept valid until
+        `wait(ticket)` returns) of a key made by `preprocess_wiring`; returns the ticket.  `wait(ticket)` returns
+        (proof, pub_inputs), or (proof, link_poly, pub_inputs) with `with_link_poly`."""
+        try:
+            wit, wit_ptr = _witness_arg(pk, witness, "submit_prove_witness")
+        except ValueError as e:
+            raise ProverError(_lib.B200_ERR_INVALID, str(e))
+        bl = np.ascontiguousarray(blinders, dtype=np.uint64)
+        if bl.size != 4 * 17:
+            raise ProverError(_lib.B200_ERR_INVALID, "submit_prove_witness: blinders must be 17 Fr elements")
+        proof = B200Proof()
+        pub = np.zeros((pk.num_inputs, 4), dtype=np.uint64)
+        link = np.zeros((pk.domain_size + 2, 4), dtype=np.uint64) if with_link_poly else None
+        ticket = C.c_uint64()
+        _lib.check(self._lib.b200_pool_submit_prove_witness(self._h, pk._h, wit_ptr, _ptr(bl), C.byref(proof),
+                                                            _ptr(link) if link is not None else None,
+                                                            _ptr(pub) if pub.size else None, C.byref(ticket)))
+        self._keep[ticket.value] = (_PoolWitness(proof, pub), link, (wit, keep), pk)
         return ticket.value
 
     def submit_prove_batch(self, pk: "ProvingKey", wires_list, pub_inputs_list, blinders_list, link_hints: bool = False,
@@ -932,6 +1041,8 @@ class ProverPool:
                 return _link_batch_results(proof.held, proof.statuses)
             return _batch_results(proof.held, proof.statuses, proof.link_hints, False)
         _lib.check(rc)
+        if isinstance(proof, _PoolWitness):
+            return (proof.proof, proof.pub_inputs) if link is None else (proof.proof, link, proof.pub_inputs)
         return (proof, link) if link is not None else proof
 
     def wait_all(self) -> None:

@@ -126,8 +126,12 @@ def setup_preprocessed_keys(circuit: type) -> Tuple[ProvingKey, VerifyingKey]:
         if circ.n + 3 > len(srs.powers_of_g):
             raise ProverError("Plonk", f"circuit {name} needs {circ.n + 3} SRS powers, {len(srs.powers_of_g)} loaded")
         try:
-            pk = PlonkKzgSnark.preprocess(srs.ctx, srs.powers_of_g, circ.log_n, circ.num_inputs, circ.selectors, circ.perm,
-                                          circ.k)
+            if getattr(circuit, "prove_from_witness", False):
+                pk = PlonkKzgSnark.preprocess_wiring(srs.ctx, srs.powers_of_g, circ.log_n, circ.num_inputs, circ.selectors,
+                                                     circ.wire_vars, circ.num_vars, circ.k)
+            else:
+                pk = PlonkKzgSnark.preprocess(srs.ctx, srs.powers_of_g, circ.log_n, circ.num_inputs, circ.selectors, circ.perm,
+                                              circ.k)
         except _lib.B200Error as e:
             raise ProverError("Plonk", e) from e
         pair = (pk, VerifyingKey.from_proving_key(pk, srs.g2_h, srs.g2_tau_h))
@@ -139,6 +143,11 @@ def setup_preprocessed_keys(circuit: type) -> Tuple[ProvingKey, VerifyingKey]:
 class SingleProverCircuit:
     """traits.rs:868-1020.  Subclasses give `name()`, `synthesize`, `statement_scalars`, `dummy_instance` and, when they
     take part in proof linking, `proof_linking_groups()` / `generate_layout`."""
+
+    # Opt-in: the key is built from the circuit's wiring (`preprocess_wiring`) and every proof is made from the witness
+    # vector (`prove_witness`): the host never builds the 5 x n value table.  The constraint system's
+    # `finalize_for_arithmetization` must then give `wire_vars` / `witness` and take `witness_only=True`.
+    prove_from_witness = False
 
     # ---- what a circuit provides --------------------------------------------------------------------------
     @classmethod
@@ -199,6 +208,13 @@ class SingleProverCircuit:
         pk, circ = cls._arithmetize(witness, statement)
         srs = system_srs()
         try:
+            if cls.prove_from_witness:
+                if srs.pool is None:
+                    return PlonkKzgSnark.prove_witness(srs.ctx, pk, circ.witness, draw_blinders(rng))[:2]
+                proof, link, _ = srs.pool.wait(srs.pool.submit_prove_witness(pk, circ.witness, draw_blinders(rng),
+                                                                             with_link_poly=True))
+                return proof, LinkingHint(linking_wire_poly=link,
+                                          linking_wire_comm=np.array(proof.wires_poly_comms[0], dtype=np.uint64))
             if srs.pool is None:
                 return PlonkKzgSnark.prove_with_link_hint(srs.ctx, pk, circ.wires, circ.pub_inputs, draw_blinders(rng))
             wires = np.ascontiguousarray(circ.wires, dtype=np.uint64)
@@ -220,12 +236,16 @@ class SingleProverCircuit:
             return []
         arith = [cls._arithmetize(w, s) for w, s in instances]
         pk = arith[0][0]
-        wires = [np.ascontiguousarray(c.wires, dtype=np.uint64) for _, c in arith]
-        pis = [c.pub_inputs for _, c in arith]
         blinders = [draw_blinders(rng) for _ in arith]
         srs = system_srs()
+        if not cls.prove_from_witness:
+            wires = [np.ascontiguousarray(c.wires, dtype=np.uint64) for _, c in arith]
+            pis = [c.pub_inputs for _, c in arith]
         try:
-            if srs.pool is None:
+            if cls.prove_from_witness:  # one batch call on the SRS context (the pool has no witness batch job)
+                proofs, hints, statuses, _ = PlonkKzgSnark.prove_witness_batch(srs.ctx, pk, [c.witness for _, c in arith],
+                                                                               blinders, link_hints=True)
+            elif srs.pool is None:
                 proofs, hints, statuses = PlonkKzgSnark.prove_batch(srs.ctx, pk, wires, pis, blinders, link_hints=True)
             else:
                 tk = srs.pool.submit_prove_batch(pk, wires, pis, blinders, link_hints=True)
@@ -247,7 +267,10 @@ class SingleProverCircuit:
             # the key holds the witness-independent structure; per proof only the value tables are arithmetized
             # (SURVEY 8(f) f4), with a fingerprint of the structure to compare against the key's
             try:
-                circ = cs.finalize_for_arithmetization(wires_only=True) if keyed else cs.finalize_for_arithmetization()
+                if cls.prove_from_witness:
+                    circ = cs.finalize_for_arithmetization(witness_only=True)
+                else:
+                    circ = cs.finalize_for_arithmetization(wires_only=True) if keyed else cs.finalize_for_arithmetization()
             except TypeError:  # a constraint system without the wires-only form
                 circ = cs.finalize_for_arithmetization()
         except ProverError:

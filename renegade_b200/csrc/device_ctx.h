@@ -246,6 +246,11 @@ struct Context {
 
 int get_domain(Context* c, unsigned log_n, Domain** out);
 
+// d_perm[p] = the next position (ascending, cyclic) that carries the variable d_wire_vars[p] carries, for the `count` wire
+// positions of a circuit: the copy-constraint permutation k_sigma_evals takes (wiring.cu).  Synchronises `st`.
+// B200_ERR_INVALID, naming the first position, for a variable index >= num_vars.
+int wiring_permutation(const uint32_t* d_wire_vars, size_t count, size_t num_vars, uint64_t* d_perm, cudaStream_t st);
+
 }  // namespace b200
 
 // opaque handle types of the C ABI

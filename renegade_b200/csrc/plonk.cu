@@ -52,6 +52,24 @@ __global__ void k_sigma_evals(const uint64_t* __restrict__ perm, const fe* __res
     fe_store(out + t, FMUL(k.v[tgt / n], fe_load_ro(dom + tgt % n)));
 }
 
+// ---- wire table from the witness vector ------------------------------------------------------------
+// wires_ev[p][t] = witness_p[wire_vars[t]] for every wire position t = i*n + j of every proof p of a chunk (blockIdx.y), and
+// the public inputs — the values on the output wire of rows 0..num_inputs-1 — into the head of pi_poly[p].  The index
+// loads and the stores are coalesced; the 32-byte elements come through the read-only path.
+constexpr size_t kMaxBatchChunk = 64;  // proofs per prover call of a batch, at most
+struct WitnessPtrs {
+    const fe* v[kMaxBatchChunk];
+};
+__global__ void k_gather_wires(const uint32_t* __restrict__ wire_vars, WitnessPtrs wit, size_t n, size_t num_inputs,
+                               fe* __restrict__ wires_ev, fe* __restrict__ pi_poly, size_t pstride) {
+    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= NW * n) return;
+    const size_t p = blockIdx.y;
+    const fe x = fe_load_ro(wit.v[p] + __ldg(wire_vars + t));
+    fe_store(wires_ev + p * NW * n + t, x);
+    if (t >= (NW - 1) * n && t - (NW - 1) * n < num_inputs) fe_store(pi_poly + p * pstride + (t - (NW - 1) * n), x);
+}
+
 // out[i] = n * (x_i - 1)   (inverted afterwards: L_1(x) / Z_H(x) = 1 / (n (x - 1)))
 __global__ void k_l1_denominators(const fe* __restrict__ pts, size_t m, fe n_mont, fe* __restrict__ out) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -539,9 +557,15 @@ struct ProvingKey {
     fe zh_inv[8];
     fe group_gen;
     g1_affine sel_comms[NS], sig_comms[NW];
+    // keys made from the wiring (b200_plonk_preprocess_wiring) keep it: the variable on every wire position (device, NW x n),
+    // the length of the witness vector, and the variables of the public inputs (host: the transcript starts with them)
+    uint32_t* wire_vars = nullptr;
+    size_t num_vars = 0;
+    std::vector<uint32_t> pub_vars;
     ~ProvingKey() {
         for (fe* p : {sel_coeffs, sig_coeffs, sig_evals, ce_sel, ce_sig, dom, coset_pts, l1_inv, cscale, cscale_inv})
             if (p) cudaFree(p);
+        if (wire_vars) cudaFree(wire_vars);
     }
 };
 
@@ -783,8 +807,10 @@ static int coset_evals(const ProvingKey* pk, const Domain* dn, const fe* src, si
     return ntt_device(dn, dst, scratch, /*inverse=*/0, /*coset=*/0, count * (unsigned)pk->nc, n, st);
 }
 
+// The copy permutation comes from the caller (h_perm) or, with h_perm null, is derived on the device from the wiring
+// (h_wire_vars, num_vars), which the key then keeps.
 static int preprocess(Context* c, const Bases* srs, unsigned log_n, size_t num_inputs, const fe* h_selectors,
-                      const uint64_t* h_perm, const fe* h_k, ProvingKey** out) {
+                      const uint64_t* h_perm, const uint32_t* h_wire_vars, size_t num_vars, const fe* h_k, ProvingKey** out) {
     const size_t n = (size_t)1 << log_n;
     // 6 cosets (6n > 5n + 7 points) from n = 16 on; all 8 for the tiny domains, where 6n would not exceed
     // the quotient's degree by enough to keep the degree check meaningful
@@ -866,7 +892,15 @@ static int preprocess(Context* c, const Bases* srs, unsigned log_n, size_t num_i
     cudaMemcpyAsync(pk->sel_coeffs, h_selectors, NS * n * sizeof(fe), cudaMemcpyHostToDevice, st);
     if ((rc = ntt_device(dn, pk->sel_coeffs, scratch, 1, 0, NS, n, st)) != B200_OK) return fail(rc);
     // sigmas: permutation -> evaluations (kept for the grand product) -> coefficients
-    cudaMemcpyAsync(d_perm, h_perm, NW * n * 8, cudaMemcpyHostToDevice, st);
+    if (h_perm) {
+        cudaMemcpyAsync(d_perm, h_perm, NW * n * 8, cudaMemcpyHostToDevice, st);
+    } else {
+        if (cudaMalloc(&pk->wire_vars, NW * n * sizeof(uint32_t)) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaMalloc(wiring)"));
+        cudaMemcpyAsync(pk->wire_vars, h_wire_vars, NW * n * sizeof(uint32_t), cudaMemcpyHostToDevice, st);
+        if ((rc = wiring_permutation(pk->wire_vars, NW * n, num_vars, d_perm, st)) != B200_OK) return fail(rc);
+        pk->num_vars = num_vars;
+        pk->pub_vars.assign(h_wire_vars + (NW - 1) * n, h_wire_vars + (NW - 1) * n + num_inputs);
+    }
     B200_LAUNCH(k_sigma_evals, grid_for(NW * n, 256), 256, 0, st)(d_perm, pk->dom, n, pk->k, pk->sig_evals);
     cudaMemcpyAsync(pk->sig_coeffs, pk->sig_evals, NW * n * sizeof(fe), cudaMemcpyDeviceToDevice, st);
     if ((rc = ntt_device(dn, pk->sig_coeffs, scratch, 1, 0, NW, n, st)) != B200_OK) return fail(rc);
@@ -1033,14 +1067,26 @@ static void fill_open_params(OpenParams* o, fe z) {
 // One proof of a prover call: its inputs, its outputs, and its status (B200_OK, or B200_ERR_UNSATISFIED when the witness
 // does not satisfy the circuit).
 struct ProveItem {
-    const fe* wires;
-    const fe* pub_inputs;
+    const fe* wires;       // the 5 x n table, or null: the table is gathered from `witness` through the key's wiring
+    const fe* pub_inputs;  // with a witness: filled in by prove()
     const fe* blinders;
     ProofOut* proof;
     fe* link_poly;
     fe* challenges;
     int status;
+    const fe* witness = nullptr;   // num_vars elements, host or device pointer
+    fe* pub_inputs_out = nullptr;  // with a witness, may be null: receives the public inputs
 };
+
+// A pointer the device can read in place (cudaMalloc'ed or managed memory), as opposed to host memory
+static bool device_readable(const void* p) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+        cudaGetLastError();
+        return false;
+    }
+    return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+}
 
 // The buffers a prover call runs in: the context's own (single proofs; their captured graphs refer to these addresses)
 // or the context's batch set (Context::batch), which batches grow instead.
@@ -1084,7 +1130,9 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
     int rc;
     const size_t flags_bytes = ((size_t)k * 4 + 63) / 64 * 64;  // h_small: the k degree flags, then k x 2 NW evaluations
     if ((rc = bf.ws->reserve(workspace_elems(n, k) * sizeof(fe))) != B200_OK) return rc;
-    if ((rc = bf.nscr->reserve((size_t)k * 7 * m * sizeof(fe))) != B200_OK) return rc;
+    const bool from_witness = items[0].witness != nullptr;  // every item of a call has the same kind of input
+    // the NTT scratch doubles as the staging area of the witness vectors: the gather has read them before round 1 uses it
+    if ((rc = bf.nscr->reserve((size_t)k * std::max(7 * m, from_witness ? pk->num_vars : 0) * sizeof(fe))) != B200_OK) return rc;
     if ((rc = bf.nscr2->reserve((size_t)k * 6 * m * sizeof(fe))) != B200_OK) return rc;
     if ((rc = bf.h_small->reserve(std::max<size_t>(4096, flags_bytes + (size_t)k * 2 * NW * sizeof(fe)))) != B200_OK) return rc;
     if ((rc = bf.h_params->reserve(k * sizeof(ProofParams))) != B200_OK) return rc;
@@ -1132,6 +1180,56 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
         if (phase < 8) c->plonk_ms[phase++] = std::chrono::duration<float, std::milli>(now - t_prev).count();
         t_prev = now;
     };
+    // ---- inputs -------------------------------------------------------------------------------------
+    // caller-owned buffers are copied outside the graphs (their addresses change from proof to proof)
+    B200_CUDA(cudaMemsetAsync(w.wpoly, 0, (NW + 1) * k * S * sizeof(fe), st));  // wire slots and the public-input slots behind them
+    std::vector<fe> pubs;  // the public inputs of witness items
+    if (from_witness) {
+        const size_t nv = pk->num_vars, ni = pk->num_inputs;
+        pubs.resize((size_t)k * ni);
+        bool any_device = false;
+        for (unsigned p0 = 0; p0 < k; p0 += kMaxBatchChunk) {
+            const unsigned cnt = std::min<unsigned>(k - p0, kMaxBatchChunk);
+            WitnessPtrs wit{};
+            for (unsigned q = 0; q < cnt; ++q) {
+                const unsigned p = p0 + q;
+                const bool in_place = device_readable(items[p].witness) && (uintptr_t)items[p].witness % alignof(fe) == 0;
+                if (in_place) {
+                    wit.v[q] = items[p].witness;
+                } else {  // host memory (or a device pointer the 16-byte loads cannot take): staged
+                    fe* stage = nscr + (size_t)p * nv;
+                    B200_CUDA(cudaMemcpyAsync(stage, items[p].witness, nv * sizeof(fe), cudaMemcpyDefault, st));
+                    wit.v[q] = stage;
+                }
+                fe* pub = pubs.data() + (size_t)p * ni;
+                if (!device_readable(items[p].witness)) {
+                    for (size_t i = 0; i < ni; ++i) pub[i] = items[p].witness[pk->pub_vars[i]];
+                } else if (ni) {
+                    any_device = true;
+                }
+            }
+            B200_LAUNCH(k_gather_wires, dim3(grid_for(NW * n, 256), cnt), 256, 0, st)(
+                pk->wire_vars, wit, n, ni, w.wires_ev + (size_t)p0 * NW * n, w.pi_poly + (size_t)p0 * S, S);
+        }
+        if (any_device) {  // the transcript starts with the public inputs: one read-back and wait for device witnesses
+            for (unsigned p = 0; p < k; ++p)
+                if (device_readable(items[p].witness))
+                    B200_CUDA(cudaMemcpyAsync(pubs.data() + (size_t)p * ni, w.pi_poly + (size_t)p * S, ni * sizeof(fe),
+                                              cudaMemcpyDeviceToHost, st));
+            B200_CUDA(cudaStreamSynchronize(st));
+        }
+        for (unsigned p = 0; p < k; ++p) {
+            items[p].pub_inputs = pubs.data() + (size_t)p * ni;
+            if (items[p].pub_inputs_out && ni) std::memcpy(items[p].pub_inputs_out, items[p].pub_inputs, ni * sizeof(fe));
+        }
+    } else {
+        for (unsigned p = 0; p < k; ++p)  // host or device pointer (UVA)
+            B200_CUDA(cudaMemcpyAsync(w.wires_ev + (size_t)p * NW * n, items[p].wires, NW * n * sizeof(fe), cudaMemcpyDefault, st));
+        if (pk->num_inputs)
+            for (unsigned p = 0; p < k; ++p)
+                B200_CUDA(cudaMemcpyAsync(w.pi_poly + (size_t)p * S, items[p].pub_inputs, pk->num_inputs * sizeof(fe),
+                                          cudaMemcpyHostToDevice, st));
+    }
     std::vector<SolidityTranscript> trs(k);
     for (unsigned p = 0; p < k; ++p) {
         items[p].status = B200_OK;
@@ -1146,14 +1244,6 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
     }
 
     // ---- round 1 ------------------------------------------------------------------------------------
-    // caller-owned buffers are copied outside the graphs (their addresses change from proof to proof)
-    for (unsigned p = 0; p < k; ++p)  // host or device pointer (UVA)
-        B200_CUDA(cudaMemcpyAsync(w.wires_ev + (size_t)p * NW * n, items[p].wires, NW * n * sizeof(fe), cudaMemcpyDefault, st));
-    B200_CUDA(cudaMemsetAsync(w.wpoly, 0, (NW + 1) * k * S * sizeof(fe), st));  // wire slots and the public-input slots behind them
-    if (pk->num_inputs)
-        for (unsigned p = 0; p < k; ++p)
-            B200_CUDA(cudaMemcpyAsync(w.pi_poly + (size_t)p * S, items[p].pub_inputs, pk->num_inputs * sizeof(fe),
-                                      cudaMemcpyHostToDevice, st));
     for (unsigned p = 0; p < k; ++p)
         for (int i = 0; i < NW; ++i) {
             hp[p].blind_w[i][0] = items[p].blinders[2 * i];
@@ -1450,7 +1540,6 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
 // already has count as free: they are reused), at most kMaxBatchChunk.  Per proof: the workspace, the two NTT scratches
 // and the MSM scratch of its five largest commitments.  B200_PROVE_BATCH_CHUNK overrides it (tests: the bytes out do
 // not depend on the chunk size).
-constexpr size_t kMaxBatchChunk = 64;
 static size_t prove_batch_chunk(Context* c, const ProvingKey* pk, size_t k) {
     if (const char* e = std::getenv("B200_PROVE_BATCH_CHUNK")) {
         const long v = std::atol(e);
@@ -1459,7 +1548,8 @@ static size_t prove_batch_chunk(Context* c, const ProvingKey* pk, size_t k) {
     const size_t n = pk->n, m = pk->m;
     const MsmPlan& pl = pk->srs->plan;
     const size_t msm_per_commit = n * (size_t)pl.n_digits * 4 * 2 + ((size_t)pl.n_phys << (pl.c - 1)) * sizeof(g1_xyzz) * 4;
-    const size_t per_proof = (workspace_elems(n, 1) + 13 * m) * sizeof(fe) + NW * msm_per_commit;
+    // (a witness vector is staged in the first NTT scratch, 7m elements unless the vector is longer)
+    const size_t per_proof = (workspace_elems(n, 1) + 6 * m + std::max(7 * m, pk->num_vars)) * sizeof(fe) + NW * msm_per_commit;
     size_t free_b = 0, total_b = 0;
     if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) free_b = 0;
     const Context::BatchBufs& b = c->batch;
@@ -1763,8 +1853,29 @@ int b200_plonk_preprocess(b200_ctx* ctx, const b200_bases* srs, unsigned log_n, 
     std::lock_guard<std::mutex> lk(ctx->c.mu);
     B200_CUDA(cudaSetDevice(ctx->c.device));
     ProvingKey* pk = nullptr;
-    int rc = preprocess(&ctx->c, srs->b, log_n, num_inputs, reinterpret_cast<const fe*>(selectors_evals), perm,
+    int rc = preprocess(&ctx->c, srs->b, log_n, num_inputs, reinterpret_cast<const fe*>(selectors_evals), perm, nullptr, 0,
                         reinterpret_cast<const fe*>(k), &pk);
+    if (rc != B200_OK) return rc;
+    *out = new b200_pk{pk};
+    return B200_OK;
+    B200_CATCH
+}
+
+int b200_plonk_preprocess_wiring(b200_ctx* ctx, const b200_bases* srs, unsigned log_n, size_t num_inputs,
+                                 const uint64_t* selectors_evals, const unsigned* wire_vars, size_t num_vars, const uint64_t* k,
+                                 b200_pk** out) {
+    static_assert(sizeof(unsigned) == sizeof(uint32_t), "wire_vars holds 32-bit indices");
+    B200_TRY
+    if (!ctx || !srs || !selectors_evals || !wire_vars || !k || !out) return B200_ERR_INVALID;
+    if (num_vars == 0 || num_vars >> 32) {
+        set_error("preprocess_wiring: num_vars must be in [1, 2^32)");
+        return B200_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lk(ctx->c.mu);
+    B200_CUDA(cudaSetDevice(ctx->c.device));
+    ProvingKey* pk = nullptr;
+    int rc = preprocess(&ctx->c, srs->b, log_n, num_inputs, reinterpret_cast<const fe*>(selectors_evals), nullptr,
+                        reinterpret_cast<const uint32_t*>(wire_vars), num_vars, reinterpret_cast<const fe*>(k), &pk);
     if (rc != B200_OK) return rc;
     *out = new b200_pk{pk};
     return B200_OK;
@@ -1780,6 +1891,7 @@ int b200_pk_verifying_key(const b200_pk* pk, uint64_t* selector_comms, uint64_t*
 
 size_t b200_pk_num_inputs(const b200_pk* pk) { return pk ? pk->pk->num_inputs : 0; }
 unsigned b200_pk_log_n(const b200_pk* pk) { return pk ? pk->pk->log_n : 0; }
+size_t b200_pk_num_vars(const b200_pk* pk) { return pk ? pk->pk->num_vars : 0; }
 
 int b200_plonk_link(b200_ctx* ctx, const b200_bases* srs, const uint64_t* a1, size_t len1, const uint64_t* a2,
                     size_t len2, const uint64_t* comm1, const uint64_t* comm2, unsigned alignment, size_t offset,
@@ -1882,6 +1994,56 @@ int b200_plonk_prove(b200_ctx* ctx, const b200_pk* pk, const uint64_t* wires, co
     B200_CATCH
 }
 
+// A key that proves from witness vectors, or B200_ERR_INVALID
+static int require_wiring(const b200_pk* pk, const char* who) {
+    if (pk->pk->wire_vars) return B200_OK;
+    set_error(std::string(who) + ": the key holds no wiring (made by b200_plonk_preprocess, not b200_plonk_preprocess_wiring)");
+    return B200_ERR_INVALID;
+}
+
+int b200_plonk_prove_witness(b200_ctx* ctx, const b200_pk* pk, const uint64_t* witness, const uint64_t* blinders,
+                             b200_proof* proof, uint64_t* link_poly, uint64_t* challenges, uint64_t* pub_inputs_out) {
+    B200_TRY
+    if (!ctx || !pk || !witness || !blinders || !proof) return B200_ERR_INVALID;
+    const int ok = require_wiring(pk, "plonk_prove_witness");
+    if (ok != B200_OK) return ok;
+    std::lock_guard<std::mutex> lk(ctx->c.mu);
+    B200_CUDA(cudaSetDevice(ctx->c.device));
+    ProveItem item{nullptr, nullptr, reinterpret_cast<const fe*>(blinders), reinterpret_cast<ProofOut*>(proof),
+                   reinterpret_cast<fe*>(link_poly), reinterpret_cast<fe*>(challenges), B200_OK,
+                   reinterpret_cast<const fe*>(witness), reinterpret_cast<fe*>(pub_inputs_out)};
+    return prove(&ctx->c, single_bufs(&ctx->c), pk->pk, &item, 1, /*single=*/true);
+    B200_CATCH
+}
+
+// The k items of a batch in chunks; statuses and return code as b200_plonk_prove_batch documents them.
+static int prove_batch_items(b200_ctx* ctx, const ProvingKey* key, std::vector<ProveItem>& its, int* statuses) {
+    const size_t k = its.size();
+    if (k == 0) return B200_OK;
+    std::lock_guard<std::mutex> lk(ctx->c.mu);
+    B200_CUDA(cudaSetDevice(ctx->c.device));
+    const size_t chunk = prove_batch_chunk(&ctx->c, key, k);
+    for (size_t off = 0; off < k; off += chunk) {
+        const unsigned cnt = (unsigned)std::min(chunk, k - off);
+        const int rc = prove(&ctx->c, batch_bufs(&ctx->c), key, its.data() + off, cnt, /*single=*/false);
+        if (rc != B200_OK && rc != B200_ERR_UNSATISFIED) return rc;  // B200_ERR_UNSATISFIED: every item of the chunk, see statuses
+    }
+    size_t bad = 0;
+    for (size_t i = 0; i < k; ++i) {
+        if (its[i].status != B200_OK) {
+            std::memset(its[i].proof, 0, sizeof(b200_proof));
+            ++bad;
+        }
+        if (statuses) statuses[i] = its[i].status;
+    }
+    if (bad) {
+        set_error("WrongQuotientPolyDegree: " + std::to_string(bad) + " of " + std::to_string(k) +
+                  " witnesses do not satisfy the circuit (see statuses)");
+        return B200_ERR_UNSATISFIED;
+    }
+    return B200_OK;
+}
+
 int b200_plonk_prove_batch(b200_ctx* ctx, const b200_pk* pk, const b200_prove_item* items, size_t k, int* statuses) {
     B200_TRY
     if (!ctx || !pk || (k && !items)) return B200_ERR_INVALID;
@@ -1897,29 +2059,27 @@ int b200_plonk_prove_batch(b200_ctx* ctx, const b200_pk* pk, const b200_prove_it
                            reinterpret_cast<const fe*>(x.blinders), reinterpret_cast<ProofOut*>(x.proof),
                            reinterpret_cast<fe*>(x.link_poly), reinterpret_cast<fe*>(x.challenges), B200_OK};
     }
-    if (k == 0) return B200_OK;
-    std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
-    const size_t chunk = prove_batch_chunk(&ctx->c, key, k);
-    for (size_t off = 0; off < k; off += chunk) {
-        const unsigned cnt = (unsigned)std::min(chunk, k - off);
-        const int rc = prove(&ctx->c, batch_bufs(&ctx->c), key, its.data() + off, cnt, /*single=*/false);
-        if (rc != B200_OK && rc != B200_ERR_UNSATISFIED) return rc;  // B200_ERR_UNSATISFIED: every item of the chunk, see statuses
-    }
-    size_t bad = 0;
+    return prove_batch_items(ctx, key, its, statuses);
+    B200_CATCH
+}
+
+int b200_plonk_prove_witness_batch(b200_ctx* ctx, const b200_pk* pk, const b200_witness_item* items, size_t k, int* statuses) {
+    B200_TRY
+    if (!ctx || !pk || (k && !items)) return B200_ERR_INVALID;
+    const int ok = require_wiring(pk, "plonk_prove_witness_batch");
+    if (ok != B200_OK) return ok;
+    std::vector<ProveItem> its(k);
     for (size_t i = 0; i < k; ++i) {
-        if (its[i].status != B200_OK) {
-            std::memset(items[i].proof, 0, sizeof(b200_proof));
-            ++bad;
+        const b200_witness_item& x = items[i];
+        if (!x.witness || !x.blinders || !x.proof) {
+            set_error("plonk_prove_witness_batch: item " + std::to_string(i) + " has a NULL pointer");
+            return B200_ERR_INVALID;
         }
-        if (statuses) statuses[i] = its[i].status;
+        its[i] = ProveItem{nullptr, nullptr, reinterpret_cast<const fe*>(x.blinders), reinterpret_cast<ProofOut*>(x.proof),
+                           reinterpret_cast<fe*>(x.link_poly), reinterpret_cast<fe*>(x.challenges), B200_OK,
+                           reinterpret_cast<const fe*>(x.witness), reinterpret_cast<fe*>(x.pub_inputs_out)};
     }
-    if (bad) {
-        set_error("WrongQuotientPolyDegree: " + std::to_string(bad) + " of " + std::to_string(k) +
-                  " witnesses do not satisfy the circuit (see statuses)");
-        return B200_ERR_UNSATISFIED;
-    }
-    return B200_OK;
+    return prove_batch_items(ctx, pk->pk, its, statuses);
     B200_CATCH
 }
 

@@ -24,14 +24,15 @@ namespace {
 struct Bundle;
 
 struct Job {
-    enum Kind { kProve, kProveBatch, kLink, kLinkBatch } kind = kProve;
+    enum Kind { kProve, kProveWitness, kProveBatch, kLink, kLinkBatch } kind = kProve;
     uint64_t ticket = 0;
-    // prove
+    // prove (wires: the table) and prove witness (wires: the witness vector)
     const b200_pk* pk = nullptr;
     const uint64_t* wires = nullptr;
     std::vector<uint64_t> pub_inputs, blinders;
     b200_proof* proof = nullptr;
     uint64_t* link_poly = nullptr;
+    uint64_t* pub_inputs_out = nullptr;
     // prove batch: the items with pub_inputs / blinders pointing into the copies below (pub_inputs, blinders: k each)
     std::vector<b200_prove_item> items;
     int* statuses = nullptr;
@@ -117,6 +118,9 @@ struct b200_pool {
                 d.status = b200_plonk_prove(ctxs[w], job->pk, job->wires,
                                             job->pub_inputs.empty() ? nullptr : job->pub_inputs.data(),
                                             job->blinders.data(), job->proof, job->link_poly, nullptr);
+            } else if (job->kind == Job::kProveWitness) {
+                d.status = b200_plonk_prove_witness(ctxs[w], job->pk, job->wires, job->blinders.data(), job->proof, job->link_poly,
+                                                    nullptr, job->pub_inputs_out);
             } else if (job->kind == Job::kProveBatch) {
                 d.status = b200_plonk_prove_batch(ctxs[w], job->pk, job->items.data(), job->items.size(), job->statuses);
             } else if (job->kind == Job::kLinkBatch) {
@@ -240,6 +244,29 @@ int b200_pool_submit_prove(b200_pool* pool, const b200_pk* pk, const uint64_t* w
     j->blinders.assign(blinders, blinders + 4 * 17);
     j->proof = proof;
     j->link_poly = link_poly;
+    return pool_push(pool, std::move(j), ticket);
+    B200_CATCH
+}
+
+int b200_pool_submit_prove_witness(b200_pool* pool, const b200_pk* pk, const uint64_t* witness, const uint64_t* blinders,
+                                   b200_proof* proof, uint64_t* link_poly, uint64_t* pub_inputs_out, uint64_t* ticket) {
+    B200_TRY
+    if (!pool || !pk || !witness || !blinders || !proof || !ticket) {
+        b200::set_error("pool_submit_prove_witness: null argument");
+        return B200_ERR_INVALID;
+    }
+    if (b200_pk_num_vars(pk) == 0) {
+        b200::set_error("pool_submit_prove_witness: the key holds no wiring (made by b200_plonk_preprocess)");
+        return B200_ERR_INVALID;
+    }
+    std::unique_ptr<Job> j(new Job());
+    j->kind = Job::kProveWitness;
+    j->pk = pk;
+    j->wires = witness;
+    j->blinders.assign(blinders, blinders + 4 * 17);
+    j->proof = proof;
+    j->link_poly = link_poly;
+    j->pub_inputs_out = pub_inputs_out;
     return pool_push(pool, std::move(j), ticket);
     B200_CATCH
 }

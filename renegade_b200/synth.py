@@ -52,6 +52,14 @@ class SynthCircuit:
     # process; 0 = not computed.  A constraint system may also be finalized `wires_only` (selectors / perm left None)
     # when the caller only needs the per-proof tables: the key already holds the structure.
     structure_digest: int = 0
+    # the circuit as wiring + witness vector (b200_plonk_preprocess_wiring / b200_plonk_prove_witness):
+    # wires[i, j] = witness[wire_vars[i, j]].  A constraint system may be finalized `witness_only` (wires left None too).
+    wire_vars: np.ndarray = None   # (5, n) uint32: the variable on wire i of row j
+    witness: np.ndarray = None     # (num_vars, 4) Montgomery
+
+    @property
+    def num_vars(self) -> int:
+        return 0 if self.witness is None else len(self.witness)
 
     @property
     def n(self) -> int:
@@ -179,7 +187,8 @@ def synth_circuit(log_n: int, num_inputs: int = 17, seed: int = 0xB200, fill: fl
         selectors=np.stack([to_mont_array(col) for col in sel]), perm=perm,
         wires=np.stack([to_mont_array(col) for col in wires_int]),
         pub_inputs=to_mont_array(pub_inputs), n_gates=n_gates,
-        selectors_int=sel, wires_int=wires_int, pub_inputs_int=pub_inputs)
+        selectors_int=sel, wires_int=wires_int, pub_inputs_int=pub_inputs,
+        wire_vars=np.array(wire_var, dtype=np.uint32), witness=to_mont_array(values))
 
 
 def splitmix_blinders(seed: int, count: int = 17) -> np.ndarray:

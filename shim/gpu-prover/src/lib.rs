@@ -5,6 +5,8 @@
 //! | `circuit-types/src/traits.rs:850`  | `PlonkKzgSnark::preprocess(&SYSTEM_SRS, &cs)` | [`GpuProver::preprocess`] |
 //! | `circuit-types/src/traits.rs:996`  | `PlonkKzgSnark::prove_with_link_hint::<_, _, SolidityTranscript>(rng, &circuit, &pk)` | [`GpuProver::prove_with_link_hint`] |
 //! | `circuit-types/src/traits.rs:1012` | `PlonkKzgSnark::verify::<SolidityTranscript>(&vk, pi, &proof, None)` | [`verify`] (host only) |
+//! | `circuit-types/src/traits.rs:850`  | the same, keeping the wiring on the device | [`GpuProver::preprocess_wiring`] |
+//! | `circuit-types/src/traits.rs:996`  | the same, from `cs.witness()` instead of the 5 x n value table | [`GpuProver::prove_from_witness`] |
 //! | `proof_linking/intent_only.rs:42-47` | `PlonkKzgSnark::link_proofs::<SolidityTranscript>(a, b, &layout, &ck)` | [`GpuProver::link_proofs`] |
 //! | `native_proof_manager.rs:726-782` | the four `link_proofs` calls of `compute_private_settlement_link_proofs` | [`GpuProver::link_proofs_batch`] |
 //! | `primitives/srs.rs:63-71` | `parse_ptau_file` + `powers_of_g` | [`GpuProver::load_srs`] |
@@ -16,7 +18,8 @@
 //! panics, aborts or unwinds across the boundary.
 //!
 //! NOT compiled in the build image (no cargo there).  `mpc_relation::PlonkCircuit` accessors used below
-//! (`selector_evals`, `wire_permutation_flat`, `witness_table`) are thin getters over fields the fork already has.
+//! (`selector_evals`, `wire_permutation_flat`, `witness_table`, `wire_variables`, `witness`) are thin getters over fields
+//! the fork already has.
 #![allow(unsafe_code)]
 pub mod ffi;
 
@@ -134,6 +137,45 @@ impl GpuProver {
         check(unsafe {
             ffi::b200_pool_submit_prove(self.pool, pk.raw, wires.as_ptr(), pub_inputs.as_ptr(), pk.num_inputs, blinders.as_ptr(),
                                         &mut raw, link.as_mut_ptr(), &mut ticket)
+        })?;
+        check(unsafe { ffi::b200_pool_wait(self.pool, ticket) })?; // buffers above stay alive until here
+        Ok((proof_from_raw(&raw), hint_from_raw(&raw, &link)))
+    }
+
+    /// `preprocess` from the circuit's wiring: the device derives the copy permutation from `cs.wire_variables()` (5 x n
+    /// variable indices) and the key keeps them, so that its proofs are made by `prove_from_witness`.  Same verifying key
+    /// as a key preprocessed from the permutation whose cycles run through each variable's positions in ascending order.
+    pub fn preprocess_wiring(&self, cs: &PlonkCircuit<Fr>) -> Result<GpuProvingKey, PlonkError> {
+        let n = cs.eval_domain_size()?;
+        let selectors: Vec<u64> = cs.selector_evals().iter().flat_map(|col| col.iter().flat_map(fr_limbs)).collect(); // 13 x n
+        let wire_vars: Vec<c_uint> = cs.wire_variables().iter().flat_map(|col| col.iter().map(|v| *v as c_uint)).collect(); // 5 x n
+        let k: Vec<u64> = cs.coset_representatives().iter().flat_map(fr_limbs).collect();
+        let ctx = unsafe { ffi::b200_pool_ctx(self.pool, 0) };
+        let mut pk = std::ptr::null_mut();
+        check(unsafe {
+            ffi::b200_plonk_preprocess_wiring(ctx, self.srs, n.trailing_zeros(), cs.num_inputs(), selectors.as_ptr(),
+                                              wire_vars.as_ptr(), cs.num_vars(), k.as_ptr(), &mut pk)
+        })?;
+        Ok(GpuProvingKey { raw: pk, num_inputs: cs.num_inputs(), log_n: n.trailing_zeros() })
+    }
+
+    /// `prove_with_link_hint` for a key made by `preprocess_wiring`: the witness vector (`cs.witness()`, num_vars
+    /// elements) is all that crosses the boundary; the 5 x n value table is gathered on the device.
+    pub fn prove_from_witness<R: rand::RngCore + rand::CryptoRng>(
+        &self, rng: &mut R, cs: &PlonkCircuit<Fr>, pk: &GpuProvingKey,
+    ) -> Result<(Proof<Bn254>, LinkingHint<Bn254>), PlonkError> {
+        let n = 1usize << pk.log_n;
+        let witness: Vec<u64> = cs.witness().iter().flat_map(fr_limbs).collect(); // num_vars
+        if witness.len() != 4 * unsafe { ffi::b200_pk_num_vars(pk.raw) } {
+            return Err(PlonkError::InvalidParameters("witness length differs from the key's num_vars".into()));
+        }
+        let blinders: Vec<u64> = (0..17).map(|_| Fr::rand(rng)).flat_map(|f| fr_limbs(&f)).collect();
+        let mut raw: ffi::b200_proof = unsafe { std::mem::zeroed() };
+        let mut link = vec![0u64; (n + 2) * 4];
+        let mut ticket = 0u64;
+        check(unsafe {
+            ffi::b200_pool_submit_prove_witness(self.pool, pk.raw, witness.as_ptr(), blinders.as_ptr(), &mut raw,
+                                                link.as_mut_ptr(), std::ptr::null_mut(), &mut ticket)
         })?;
         check(unsafe { ffi::b200_pool_wait(self.pool, ticket) })?; // buffers above stay alive until here
         Ok((proof_from_raw(&raw), hint_from_raw(&raw, &link)))

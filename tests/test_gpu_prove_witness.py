@@ -24,10 +24,10 @@ def load_srs(ctx, oracle, pyoracle, n):
     return ctx.load_bases(oracle.srs_from_tau(tau, n + 3))
 
 
-def keys(ctx, bases, circ):
-    """(key from the wiring, key from the permutation the wiring implies)"""
+def keys(ctx, bases, circ, num_vars=None):
+    """(key from the wiring, key from the permutation the wiring implies); num_vars: the witness's length by default"""
     wpk = PlonkKzgSnark.preprocess_wiring(ctx, bases, circ.log_n, circ.num_inputs, circ.selectors, circ.wire_vars,
-                                          circ.num_vars, circ.k)
+                                          circ.num_vars if num_vars is None else num_vars, circ.k)
     pk = PlonkKzgSnark.preprocess(ctx, bases, circ.log_n, circ.num_inputs, circ.selectors,
                                   wiring_permutation(circ.wire_vars), circ.k)
     return wpk, pk

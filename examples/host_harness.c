@@ -8,6 +8,7 @@
  *   k[5][4], selectors[13][n][4], perm[5n], wires[5][n][4], pub_inputs[num_inputs][4], blinders[17][4],
  *   srs[n_srs][8]                                     (all u64)
  * Output file: b200_proof (1152 bytes) || link polynomial ((n+2) x 4 u64) || 18 VK commitments.
+ * Optional bundle file: the two proofs (2 x 1152 bytes) || the link proof (128 bytes) of the witness bundle below.
  *
  *   gcc -O2 -Iinclude examples/host_harness.c -Lrenegade_b200 -lb200prover -Wl,-rpath,'$ORIGIN/../renegade_b200' -o examples/host_harness
  */
@@ -37,8 +38,8 @@ static uint64_t* read_u64s(FILE* f, size_t count) {
 }
 
 int main(int argc, char** argv) {
-    if (argc != 3) {
-        fprintf(stderr, "usage: %s job.bin proof.bin\n", argv[0]);
+    if (argc != 3 && argc != 4) {
+        fprintf(stderr, "usage: %s job.bin proof.bin [bundle.bin]\n", argv[0]);
         return 1;
     }
     FILE* f = fopen(argv[1], "rb");
@@ -131,6 +132,32 @@ int main(int argc, char** argv) {
             fprintf(stderr, "witness proof %d differs from the proof on the expanded table\n", i);
             return 6;
         }
+
+    /* A bundle of witness vectors through the pool, the shape a relayer settles: two proofs of the key from the wiring
+     * (the second with its 17 blinders in reverse order) and one link proof between them on rows num_inputs ..
+     * num_inputs + 3, where both carry the same witness values.  Each proof must equal the direct one. */
+    uint64_t* blinders_rev = (uint64_t*)malloc(17 * 32);
+    for (int i = 0; i < 17; ++i) memcpy(blinders_rev + 4 * i, blinders + 4 * (16 - i), 32);
+    uint64_t* bundle_polys = (uint64_t*)calloc(2 * (n + 2) * 4, 8);
+    b200_proof bundled[2], direct_rev;
+    b200_link_proof bundled_link;
+    const b200_bundle_witness bw[2] = {{wpk, witness, blinders, &bundled[0], bundle_polys, NULL},
+                                       {wpk, witness, blinders_rev, &bundled[1], bundle_polys + (n + 2) * 4, NULL}};
+    const b200_bundle_link blink = {0, 1, log_n, num_inputs, 4, &bundled_link};
+    CHECK(b200_pool_submit_bundle_witness(pool, bases, bw, 2, &blink, 1, &tickets[0]));
+    CHECK(b200_pool_wait(pool, tickets[0]));
+    CHECK(b200_plonk_prove_witness(ctx, wpk, witness, blinders_rev, &direct_rev, NULL, NULL, NULL));
+    if (memcmp(&bundled[0], &from_table, sizeof(proof)) != 0 || memcmp(&bundled[1], &direct_rev, sizeof(proof)) != 0) {
+        fprintf(stderr, "witness bundle proof differs from the direct proof\n");
+        return 7;
+    }
+    if (argc == 4) { /* the bundle's two proofs and its link proof, for the caller to check against the oracle */
+        FILE* ob = fopen(argv[3], "wb");
+        if (!ob) { perror("bundle out"); return 1; }
+        fwrite(bundled, sizeof(b200_proof), 2, ob);
+        fwrite(&bundled_link, sizeof(bundled_link), 1, ob);
+        fclose(ob);
+    }
     b200_pk_free(ctx, wpk);
     b200_pool_destroy(pool);
 

@@ -477,6 +477,31 @@ typedef struct {
  * the ticket has been waited for. */
 int b200_pool_submit_bundle(b200_pool* pool, const b200_bases* srs, const b200_bundle_proof* proofs, size_t n_proofs,
                             const b200_bundle_link* links, size_t n_links, uint64_t* ticket);
+/* One proof of a bundle given as a witness vector, arguments as for b200_pool_submit_prove_witness: pk is a key made by
+ * b200_plonk_preprocess_wiring, witness its num_vars x 4 limbs (host or device pointer).  `link_poly` ((2^log_n + 2) x 4
+ * limbs) is required for every proof a link names; `pub_inputs_out` (may be NULL) receives the key's num_inputs values. */
+typedef struct {
+    const b200_pk* pk;
+    const uint64_t* witness;
+    const uint64_t* blinders;
+    b200_proof* proof;
+    uint64_t* link_poly;
+    uint64_t* pub_inputs_out;
+} b200_bundle_witness;
+/* b200_pool_submit_bundle with the proofs given as witness vectors: each proof runs as one
+ * b200_plonk_prove_witness on some worker; the links, the ticket and its status are exactly b200_pool_submit_bundle's
+ * (links forked once every proof is in, first failure wins, an unsatisfied proof forks no links).  The arrays and the
+ * blinders are copied at submit; the witness vectors and the output buffers stay owned by the caller until the ticket has
+ * been waited for.  B200_ERR_INVALID at submit, with nothing queued, for a NULL pointer, a key without wiring
+ * (b200_pk_num_vars == 0), or a link naming a missing proof or one without link_poly. */
+int b200_pool_submit_bundle_witness(b200_pool* pool, const b200_bases* srs, const b200_bundle_witness* proofs,
+                                    size_t n_proofs, const b200_bundle_link* links, size_t n_links, uint64_t* ticket);
+/* Queue one `b200_plonk_prove_witness_batch(ctx_of_some_worker, pk, items, k, statuses)` as ONE job on one worker.  The
+ * items array and each item's blinders are copied at submit; the witness vectors, the output buffers and statuses (may be
+ * NULL) stay owned by the caller until the ticket has been waited for.  Refusals at submit, statuses and the ticket's
+ * status as b200_pool_submit_prove_batch (B200_ERR_INVALID at submit also for a key without wiring). */
+int b200_pool_submit_prove_witness_batch(b200_pool* pool, const b200_pk* pk, const b200_witness_item* items, size_t k,
+                                         int* statuses, uint64_t* ticket);
 /* Blocks until the job is done and returns ITS status (B200_OK or the error the prove/link call
  * returned; b200_last_error() of the waiting thread then holds the job's message).  A ticket can
  * be waited for once. */
@@ -518,6 +543,21 @@ int b200_box_submit_prove(b200_box* box, const b200_box_pk* pk, const uint64_t* 
 int b200_box_submit_bundle(b200_box* box, const b200_box_srs* srs, const b200_box_pk* const* pks,
                            const b200_bundle_proof* proofs, size_t n_proofs, const b200_bundle_link* links,
                            size_t n_links, uint64_t* ticket);
+/* b200_plonk_preprocess_wiring on every device: a box key whose proofs can be made from witness vectors. */
+int b200_box_preprocess_wiring(b200_box* box, const b200_box_srs* srs, unsigned log_n, size_t num_inputs,
+                               const uint64_t* selectors_evals, const unsigned* wire_vars, size_t num_vars,
+                               const uint64_t* k, b200_box_pk** out);
+/* b200_pool_submit_prove_witness on one device of the box.  A witness in device memory runs on the device that holds it
+ * (the least loaded of the box entries with that ordinal); host, pinned and managed witnesses go to the least-loaded
+ * device.  B200_ERR_INVALID for a witness on a device outside the box, a key of another box or a key without wiring. */
+int b200_box_submit_prove_witness(b200_box* box, const b200_box_pk* pk, const uint64_t* witness, const uint64_t* blinders,
+                                  b200_proof* proof, uint64_t* link_poly, uint64_t* pub_inputs_out, uint64_t* ticket);
+/* b200_pool_submit_bundle_witness on one device of the box: `pks[i]` is the box key of proofs[i] (the `pk` field of the
+ * entries is ignored).  The bundle stays on one device, chosen as for b200_box_submit_prove_witness; a bundle whose
+ * device-memory witnesses lie on two different devices is refused with B200_ERR_INVALID. */
+int b200_box_submit_bundle_witness(b200_box* box, const b200_box_srs* srs, const b200_box_pk* const* pks,
+                                   const b200_bundle_witness* proofs, size_t n_proofs, const b200_bundle_link* links,
+                                   size_t n_links, uint64_t* ticket);
 int b200_box_wait(b200_box* box, uint64_t ticket);
 /* Index (into the `devices` array) of the device a ticket ran on, -1 for a bad ticket. */
 int b200_box_ticket_device(const b200_box* box, uint64_t ticket);

@@ -561,26 +561,8 @@ class PlonkKzgSnark:
                             want_challenges: bool = False):
         """`prove_batch` with the items given as witness vectors (b200_plonk_prove_witness_batch).  Returns
         (proofs, hints, statuses, pub_inputs[, challenges]), item i as `prove_witness` of the same arguments."""
-        witness_list, blinders_list = list(witness_list), list(blinders_list)
-        if len(witness_list) != len(blinders_list):
-            raise ValueError(f"prove_witness_batch: {len(witness_list)} witness vectors and {len(blinders_list)} blinder vectors")
-        k, n = len(witness_list), pk.domain_size
-        items = (B200WitnessItem * max(1, k))()
-        keep, pubs = [], []
-        for i, (witness, blinders) in enumerate(zip(witness_list, blinders_list)):
-            wit, wit_ptr = _witness_arg(pk, witness, f"prove_witness_batch: item {i}")
-            bl = np.ascontiguousarray(blinders, dtype=np.uint64)
-            if bl.size != 17 * 4:
-                raise ValueError(f"prove_witness_batch: item {i} has {bl.size // 4} blinders, the prover draws 17")
-            proof = B200Proof()
-            link = np.zeros((n + 2, 4), dtype=np.uint64) if link_hints else None
-            ch = np.zeros((6, 4), dtype=np.uint64) if want_challenges else None
-            pub = np.zeros((pk.num_inputs, 4), dtype=np.uint64)
-            items[i] = B200WitnessItem(wit_ptr, _ptr(bl), C.cast(C.pointer(proof), C.c_void_p),
-                                       _ptr(link) if link is not None else None, _ptr(ch) if ch is not None else None,
-                                       _ptr(pub) if pub.size else None)
-            keep.append((wit, None, bl, proof, link, ch))
-            pubs.append(pub)
+        items, keep, pubs = _witness_items(pk, witness_list, blinders_list, link_hints, want_challenges, "prove_witness_batch")
+        k = len(keep)
         statuses = (C.c_int * max(1, k))()
         rc = ctx._lib.b200_plonk_prove_witness_batch(ctx._h, pk._h, items, k, statuses)
         if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
@@ -639,6 +621,32 @@ def _witness_arg(pk: ProvingKey, witness, where: str):
     if wit.size != 4 * pk.num_vars:
         raise ValueError(f"{where}: the witness has {wit.size // 4} elements, the key takes {pk.num_vars}")
     return wit, _ptr(wit)
+
+
+def _witness_items(pk: ProvingKey, witness_list, blinders_list, link_hints: bool, want_challenges: bool, where: str):
+    """Checks a witness batch's arguments (ValueError) and builds its b200_witness_item array.  Returns (items, keep,
+    pub_inputs): keep[i] as `_prove_items` gives it, pub_inputs[i] the array item i's public inputs are written to."""
+    witness_list, blinders_list = list(witness_list), list(blinders_list)
+    if len(witness_list) != len(blinders_list):
+        raise ValueError(f"{where}: {len(witness_list)} witness vectors and {len(blinders_list)} blinder vectors")
+    k, n = len(witness_list), pk.domain_size
+    items = (B200WitnessItem * max(1, k))()
+    keep, pubs = [], []
+    for i, (witness, blinders) in enumerate(zip(witness_list, blinders_list)):
+        wit, wit_ptr = _witness_arg(pk, witness, f"{where}: item {i}")
+        bl = np.ascontiguousarray(blinders, dtype=np.uint64)
+        if bl.size != 17 * 4:
+            raise ValueError(f"{where}: item {i} has {bl.size // 4} blinders, the prover draws 17")
+        proof = B200Proof()
+        link = np.zeros((n + 2, 4), dtype=np.uint64) if link_hints else None
+        ch = np.zeros((6, 4), dtype=np.uint64) if want_challenges else None
+        pub = np.zeros((pk.num_inputs, 4), dtype=np.uint64)
+        items[i] = B200WitnessItem(wit_ptr, _ptr(bl), C.cast(C.pointer(proof), C.c_void_p),
+                                   _ptr(link) if link is not None else None, _ptr(ch) if ch is not None else None,
+                                   _ptr(pub) if pub.size else None)
+        keep.append((wit, None, bl, proof, link, ch))
+        pubs.append(pub)
+    return items, keep, pubs
 
 
 def _prove_items(pk: ProvingKey, wires_list, pub_inputs_list, blinders_list, link_hints: bool, want_challenges: bool):
@@ -862,6 +870,78 @@ ProverError = _lib.B200Error           # circuit-types/src/errors.rs:33-58: a fa
 
 BundleProof = _lib.STRUCTS["b200_bundle_proof"]
 BundleLink = _lib.STRUCTS["b200_bundle_link"]
+BundleWitness = _lib.STRUCTS["b200_bundle_witness"]
+
+
+def _bundle_links(links, n_proofs: int, where: str):
+    """The b200_bundle_link array of a bundle and the link proofs it writes into; a link naming a proof outside the
+    bundle raises ProverError before any device call."""
+    arr_l = (BundleLink * max(len(links), 1))()
+    out_links = []
+    for i, (a, b, lay) in enumerate(links):
+        if not (0 <= a < n_proofs and 0 <= b < n_proofs):
+            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: link {i} names proof ({a}, {b}) of a bundle of {n_proofs}")
+        lp = B200LinkProof()
+        arr_l[i].a, arr_l[i].b, arr_l[i].alignment, arr_l[i].offset, arr_l[i].size = a, b, lay.alignment, lay.offset, lay.size
+        arr_l[i].proof = C.cast(C.pointer(lp), C.c_void_p)
+        out_links.append(lp)
+    return arr_l, out_links
+
+
+def _bundle_witness_arrays(proofs, links, resolve, where: str):
+    """Arrays of a witness bundle: `proofs` = [(key, witness, blinders)], resolve(key) -> (C handle, the key's shape:
+    domain_size, num_inputs, num_vars).  Blinder lengths, keys without wiring, witness lengths and link indices are
+    checked here (ProverError) before any device call.  Returns (b200_bundle_witness array, link array, objects to keep
+    alive, (proofs, link polys, link proofs, pub_inputs) the jobs write into)."""
+    arr_p = (BundleWitness * max(len(proofs), 1))()
+    keep, out_proofs, out_polys, out_pubs = [], [], [], []
+    for i, (key, witness, blinders) in enumerate(proofs):
+        h, shape = resolve(key)
+        if shape.num_vars == 0:
+            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: the key of proof {i} holds no wiring (made by preprocess)")
+        try:
+            wit, wit_ptr = _witness_arg(shape, witness, f"{where}: proof {i}")
+        except ValueError as e:
+            raise ProverError(_lib.B200_ERR_INVALID, str(e))
+        bl = np.ascontiguousarray(blinders, dtype=np.uint64)
+        if bl.size != 4 * 17:
+            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: proof {i} has {bl.size // 4} blinders, the prover draws 17")
+        proof = B200Proof()
+        poly = np.zeros((shape.domain_size + 2, 4), dtype=np.uint64)
+        pub = np.zeros((shape.num_inputs, 4), dtype=np.uint64)
+        arr_p[i].pk, arr_p[i].witness, arr_p[i].blinders = h, wit_ptr, _ptr(bl)
+        arr_p[i].proof, arr_p[i].link_poly = C.cast(C.pointer(proof), C.c_void_p), _ptr(poly)
+        arr_p[i].pub_inputs_out = _ptr(pub) if pub.size else None
+        keep += [wit, bl, key]
+        out_proofs.append(proof)
+        out_polys.append(poly)
+        out_pubs.append(pub)
+    arr_l, out_links = _bundle_links(links, len(proofs), where)
+    return arr_p, arr_l, keep, (out_proofs, out_polys, out_links, out_pubs)
+
+
+def _bundle_table_arrays(proofs, links, resolve, where: str):
+    """`_bundle_witness_arrays` for a bundle of wire tables: `proofs` = [(key, wires_ptr, pub_inputs, blinders)].
+    Returns (b200_bundle_proof array, link array, objects to keep alive, (proofs, link polys, link proofs))."""
+    arr_p = (BundleProof * max(len(proofs), 1))()
+    keep, out_proofs, out_polys = [], [], []
+    for i, (key, wires_ptr, pub_inputs, blinders) in enumerate(proofs):
+        h, shape = resolve(key)
+        pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64)
+        bl = np.ascontiguousarray(blinders, dtype=np.uint64)
+        if pi.size != 4 * shape.num_inputs or bl.size != 4 * 17:
+            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: public inputs / blinders do not match the key")
+        proof = B200Proof()
+        poly = np.zeros((shape.domain_size + 2, 4), dtype=np.uint64)
+        arr_p[i].pk, arr_p[i].wires = h, C.c_void_p(wires_ptr)
+        arr_p[i].pub_inputs = pi.ctypes.data_as(C.c_void_p) if pi.size else None
+        arr_p[i].num_inputs, arr_p[i].blinders = pi.size // 4, bl.ctypes.data_as(C.c_void_p)
+        arr_p[i].proof, arr_p[i].link_poly = C.cast(C.pointer(proof), C.c_void_p), poly.ctypes.data_as(C.c_void_p)
+        keep += [pi, bl, key]
+        out_proofs.append(proof)
+        out_polys.append(poly)
+    arr_l, out_links = _bundle_links(links, len(proofs), where)
+    return arr_p, arr_l, keep, (out_proofs, out_polys, out_links)
 
 
 @dataclass
@@ -877,6 +957,12 @@ class _PoolWitness:
     """What a queued witness job writes into."""
     proof: Any
     pub_inputs: np.ndarray
+
+
+@dataclass
+class _PoolWitnessBatch(_PoolBatch):
+    """What a queued witness batch job writes into: as a batch job, and each item's public inputs."""
+    pub_inputs: list = None
 
 
 @dataclass
@@ -1000,32 +1086,40 @@ class ProverPool:
         blinders)], `links` = [(a, b, GroupLayout)] — link proof between the hints of proofs a and b, forked inside the
         pool once every proof is in (native_proof_manager.rs:526-584, 726-782).  `wait(ticket)` returns
         ([B200Proof], [link polys], [B200LinkProof])."""
-        n_p, n_l = len(proofs), len(links)
-        arr_p = (BundleProof * n_p)()
-        arr_l = (BundleLink * max(n_l, 1))()
-        keep, out_proofs, out_polys, out_links = [], [], [], []
-        for i, (pk, wires_ptr, pub_inputs, blinders) in enumerate(proofs):
-            pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64)
-            bl = np.ascontiguousarray(blinders, dtype=np.uint64)
-            if pi.size != 4 * pk.num_inputs or bl.size != 4 * 17:
-                raise ProverError(_lib.B200_ERR_INVALID, "submit_bundle: public inputs / blinders do not match the key")
-            proof = B200Proof()
-            poly = np.zeros((pk.domain_size + 2, 4), dtype=np.uint64)
-            arr_p[i].pk, arr_p[i].wires = pk._h, C.c_void_p(wires_ptr)
-            arr_p[i].pub_inputs = pi.ctypes.data_as(C.c_void_p) if pi.size else None
-            arr_p[i].num_inputs, arr_p[i].blinders = pi.size // 4, bl.ctypes.data_as(C.c_void_p)
-            arr_p[i].proof, arr_p[i].link_poly = C.cast(C.pointer(proof), C.c_void_p), poly.ctypes.data_as(C.c_void_p)
-            keep += [pi, bl, pk]
-            out_proofs.append(proof)
-            out_polys.append(poly)
-        for i, (a, b, lay) in enumerate(links):
-            lp = B200LinkProof()
-            arr_l[i].a, arr_l[i].b, arr_l[i].alignment, arr_l[i].offset, arr_l[i].size = a, b, lay.alignment, lay.offset, lay.size
-            arr_l[i].proof = C.cast(C.pointer(lp), C.c_void_p)
-            out_links.append(lp)
+        arr_p, arr_l, keep, out = _bundle_table_arrays(proofs, links, lambda pk: (pk._h, pk), "submit_bundle")
         ticket = C.c_uint64()
-        _lib.check(self._lib.b200_pool_submit_bundle(self._h, srs._h, arr_p, n_p, arr_l, n_l, C.byref(ticket)))
-        self._keep[ticket.value] = ((out_proofs, out_polys, out_links), None, keep, srs)
+        _lib.check(self._lib.b200_pool_submit_bundle(self._h, srs._h, arr_p, len(proofs), arr_l, len(links), C.byref(ticket)))
+        self._keep[ticket.value] = (out, None, keep, srs)
+        return ticket.value
+
+    def submit_bundle_witness(self, srs: "Bases", proofs, links) -> int:
+        """`submit_bundle` with every proof given as a witness vector (`b200_pool_submit_bundle_witness`): `proofs` =
+        [(pk, witness, blinders)], pk a key made by `preprocess_wiring`, witness an array or an address (pinned host or
+        device memory, kept valid until `wait(ticket)` returns) as `submit_prove_witness` takes.  `wait(ticket)` returns
+        ([B200Proof], [link polys], [B200LinkProof], [pub_inputs])."""
+        arr_p, arr_l, keep, out = _bundle_witness_arrays(proofs, links, lambda pk: (pk._h, pk), "submit_bundle_witness")
+        ticket = C.c_uint64()
+        _lib.check(self._lib.b200_pool_submit_bundle_witness(self._h, srs._h if srs is not None else None, arr_p, len(proofs),
+                                                             arr_l, len(links), C.byref(ticket)))
+        self._keep[ticket.value] = (out, None, keep, srs)
+        return ticket.value
+
+    def submit_prove_witness_batch(self, pk: "ProvingKey", witnesses, blinders_list, link_hints: bool = False,
+                                   keep=None) -> int:
+        """Queue one `b200_plonk_prove_witness_batch` as a single job on one worker; returns the ticket.  Arguments as
+        for `PlonkKzgSnark.prove_witness_batch`; witnesses given by address stay owned by the caller until `wait(ticket)`
+        returns (pass their owners as `keep`).  `wait(ticket)` returns (proofs, hints, statuses, pub_inputs) like
+        `prove_witness_batch`."""
+        if pk.num_vars == 0:
+            raise ProverError(_lib.B200_ERR_INVALID, "submit_prove_witness_batch: the key holds no wiring (made by preprocess)")
+        try:
+            items, held, pubs = _witness_items(pk, witnesses, blinders_list, link_hints, False, "submit_prove_witness_batch")
+        except ValueError as e:
+            raise ProverError(_lib.B200_ERR_INVALID, str(e))
+        statuses = (C.c_int * max(1, len(held)))()
+        ticket = C.c_uint64()
+        _lib.check(self._lib.b200_pool_submit_prove_witness_batch(self._h, pk._h, items, len(held), statuses, C.byref(ticket)))
+        self._keep[ticket.value] = (_PoolWitnessBatch(held, statuses, link_hints, pubs), None, (items, keep), pk)
         return ticket.value
 
     def wait(self, ticket: int):
@@ -1039,6 +1133,8 @@ class ProverPool:
                 _lib.check(rc)
             if isinstance(proof, _PoolLinkBatch):
                 return _link_batch_results(proof.held, proof.statuses)
+            if isinstance(proof, _PoolWitnessBatch):
+                return _batch_results(proof.held, proof.statuses, proof.link_hints, False) + (proof.pub_inputs,)
             return _batch_results(proof.held, proof.statuses, proof.link_hints, False)
         _lib.check(rc)
         if isinstance(proof, _PoolWitness):
@@ -1070,6 +1166,14 @@ class ProverPool:
             pass
 
 
+@dataclass
+class _BoxKeyShape:
+    """What the box's Python side needs to know of a box key: output sizes and the witness length."""
+    domain_size: int
+    num_inputs: int
+    num_vars: int
+
+
 class ProverBox:
     """`b200_box`: every GPU of the box behind one object — one prover pool per device, the SRS tables and the proving
     keys replicated on each, jobs routed to the least-loaded device.  The single-process counterpart of running one
@@ -1081,6 +1185,7 @@ class ProverBox:
         h = C.c_void_p()
         _lib.check(self._lib.b200_box_create(arr, len(devices), workers_per_device, C.byref(h)))
         self._h, self._keep, self.devices = h, {}, list(devices)
+        self._shapes = {}  # key handle -> _BoxKeyShape, for the keys this box made
 
     def load_srs(self, points: np.ndarray, window_bits: int = 0, check_on_curve: bool = False):
         pts = np.ascontiguousarray(points, dtype=np.uint64).reshape(-1, 8)
@@ -1094,7 +1199,72 @@ class ProverBox:
         kk = np.ascontiguousarray(k, dtype=np.uint64).reshape(5, 4)
         h = C.c_void_p()
         _lib.check(self._lib.b200_box_preprocess(self._h, srs, log_n, num_inputs, _ptr(sel), _ptr(pm), _ptr(kk), C.byref(h)))
+        self._shapes[h.value] = _BoxKeyShape(1 << log_n, num_inputs, 0)
         return h
+
+    def preprocess_wiring(self, srs, log_n: int, num_inputs: int, selectors: np.ndarray, wire_vars: np.ndarray, num_vars: int,
+                          k: np.ndarray):
+        """`PlonkKzgSnark.preprocess_wiring` on every device (`b200_box_preprocess_wiring`): a box key whose proofs are
+        made from witness vectors."""
+        sel = np.ascontiguousarray(selectors, dtype=np.uint64).reshape(13, 1 << log_n, 4)
+        wv = np.ascontiguousarray(wire_vars, dtype=np.uint32).reshape(5 << log_n)
+        kk = np.ascontiguousarray(k, dtype=np.uint64).reshape(5, 4)
+        h = C.c_void_p()
+        _lib.check(self._lib.b200_box_preprocess_wiring(self._h, srs, log_n, num_inputs, _ptr(sel), wv.ctypes.data_as(C.c_void_p),
+                                                        num_vars, _ptr(kk), C.byref(h)))
+        self._shapes[h.value] = _BoxKeyShape(1 << log_n, num_inputs, num_vars)
+        return h
+
+    def _resolve(self, pk):
+        """(handle, shape) of a key this box made; ProverError for any other."""
+        shape = self._shapes.get(getattr(pk, "value", pk))
+        if shape is None:
+            raise ProverError(_lib.B200_ERR_INVALID, "box: the key was not made by this box")
+        return pk, shape
+
+    def submit_prove_witness(self, pk, witness, blinders: np.ndarray, with_link_poly: bool = False, keep=None) -> int:
+        """`ProverPool.submit_prove_witness` on the box (`b200_box_submit_prove_witness`): a witness in device memory runs
+        on its own device, any other on the least-loaded one.  `wait(ticket)` returns (proof, pub_inputs), or (proof,
+        link_poly, pub_inputs) with `with_link_poly`."""
+        _, shape = self._resolve(pk)
+        try:
+            wit, wit_ptr = _witness_arg(shape, witness, "box.submit_prove_witness")
+        except ValueError as e:
+            raise ProverError(_lib.B200_ERR_INVALID, str(e))
+        bl = np.ascontiguousarray(blinders, dtype=np.uint64)
+        if bl.size != 4 * 17:
+            raise ProverError(_lib.B200_ERR_INVALID, "box.submit_prove_witness: blinders must be 17 Fr elements")
+        proof = B200Proof()
+        pub = np.zeros((shape.num_inputs, 4), dtype=np.uint64)
+        link = np.zeros((shape.domain_size + 2, 4), dtype=np.uint64) if with_link_poly else None
+        ticket = C.c_uint64()
+        _lib.check(self._lib.b200_box_submit_prove_witness(self._h, pk, wit_ptr, _ptr(bl), C.byref(proof),
+                                                           _ptr(link) if link is not None else None,
+                                                           _ptr(pub) if pub.size else None, C.byref(ticket)))
+        self._keep[ticket.value] = (_PoolWitness(proof, pub), link, (wit, keep), bl)
+        return ticket.value
+
+    def submit_bundle(self, srs, proofs, links) -> int:
+        """`ProverPool.submit_bundle` on the least-loaded device (`b200_box_submit_bundle`): `proofs` = [(box key,
+        wires_ptr, pub_inputs, blinders)].  `wait(ticket)` returns ([B200Proof], [link polys], [B200LinkProof])."""
+        arr_p, arr_l, keep, out = _bundle_table_arrays(proofs, links, self._resolve, "box.submit_bundle")
+        pks = (C.c_void_p * max(len(proofs), 1))(*[p[0] for p in proofs])
+        ticket = C.c_uint64()
+        _lib.check(self._lib.b200_box_submit_bundle(self._h, srs, pks, arr_p, len(proofs), arr_l, len(links), C.byref(ticket)))
+        self._keep[ticket.value] = (out, None, (keep, pks))
+        return ticket.value
+
+    def submit_bundle_witness(self, srs, proofs, links) -> int:
+        """`ProverPool.submit_bundle_witness` on one device of the box (`b200_box_submit_bundle_witness`): `proofs` = [(box
+        key, witness, blinders)]; device-memory witnesses pin the bundle to their device (all on one).  `wait(ticket)`
+        returns ([B200Proof], [link polys], [B200LinkProof], [pub_inputs])."""
+        arr_p, arr_l, keep, out = _bundle_witness_arrays(proofs, links, self._resolve, "box.submit_bundle_witness")
+        pks = (C.c_void_p * max(len(proofs), 1))(*[p[0] for p in proofs])
+        ticket = C.c_uint64()
+        _lib.check(self._lib.b200_box_submit_bundle_witness(self._h, srs, pks, arr_p, len(proofs), arr_l, len(links),
+                                                            C.byref(ticket)))
+        self._keep[ticket.value] = (out, None, (keep, pks))
+        return ticket.value
 
     def verifying_key(self, pk):
         sel, sig = np.zeros((13, 8), dtype=np.uint64), np.zeros((5, 8), dtype=np.uint64)
@@ -1117,6 +1287,8 @@ class ProverBox:
         rc = self._lib.b200_box_wait(self._h, ticket)
         proof, link, *_ = self._keep.pop(ticket, (None, None))
         _lib.check(rc)
+        if isinstance(proof, _PoolWitness):
+            return (proof.proof, proof.pub_inputs) if link is None else (proof.proof, link, proof.pub_inputs)
         return (proof, link) if link is not None else proof
 
     def ticket_device(self, ticket: int) -> int:
@@ -1124,6 +1296,7 @@ class ProverBox:
 
     def free_pk(self, pk):
         self._lib.b200_box_pk_free(self._h, pk)
+        self._shapes.pop(getattr(pk, "value", pk), None)
 
     def free_srs(self, srs):
         self._lib.b200_box_srs_free(self._h, srs)

@@ -7,6 +7,7 @@
 // overlap the throughput-bound kernels of the others.
 //
 // Host-only code (std::thread) above the same C ABI the single-context entry points use.
+#include <algorithm>
 #include <condition_variable>
 #include <cstring>
 #include <deque>
@@ -24,7 +25,7 @@ namespace {
 struct Bundle;
 
 struct Job {
-    enum Kind { kProve, kProveWitness, kProveBatch, kLink, kLinkBatch } kind = kProve;
+    enum Kind { kProve, kProveWitness, kProveBatch, kProveWitnessBatch, kLink, kLinkBatch } kind = kProve;
     uint64_t ticket = 0;
     // prove (wires: the table) and prove witness (wires: the witness vector)
     const b200_pk* pk = nullptr;
@@ -35,6 +36,8 @@ struct Job {
     uint64_t* pub_inputs_out = nullptr;
     // prove batch: the items with pub_inputs / blinders pointing into the copies below (pub_inputs, blinders: k each)
     std::vector<b200_prove_item> items;
+    // prove witness batch: the items with blinders pointing into the copies in `blinders` (k of them)
+    std::vector<b200_witness_item> witness_items;
     int* statuses = nullptr;
     // link (one item) and link batch: the items with comm1 / comm2 pointing into the copies below (8 limbs each, two per
     // item)
@@ -63,10 +66,17 @@ struct Done {
 // A bundle: proofs first, then — once all of them are in — the link proofs between their wire-0 polynomials; one
 // ticket for the whole thing.  The device-side shape of `NativeProofManager::handle_proof_job` for the settlement jobs
 // (native_proof_manager.rs:526-584: prove, then `compute_*_link_proofs`, :726-782 forking the link proofs).
+// Both bundle entry points (wire tables and witness vectors) share it: a link job needs only each proof's key, proof and
+// link polynomial.
+struct BundleHint {
+    const b200_pk* pk;
+    b200_proof* proof;
+    uint64_t* link_poly;
+};
 struct Bundle {
     uint64_t ticket = 0;
     const b200_bases* srs = nullptr;
-    std::vector<b200_bundle_proof> proofs;
+    std::vector<BundleHint> proofs;
     std::vector<b200_bundle_link> links;
     size_t pending = 0;     // sub-jobs of the current phase still queued or running
     bool linking = false;   // false: proof phase, true: link phase
@@ -88,8 +98,8 @@ struct b200_pool {
     bool stopping = false;
 
     static std::unique_ptr<Job> make_link_job(const std::shared_ptr<Bundle>& b, const b200_bundle_link& l) {
-        const b200_bundle_proof& pa = b->proofs[l.a];
-        const b200_bundle_proof& pb = b->proofs[l.b];
+        const BundleHint& pa = b->proofs[l.a];
+        const BundleHint& pb = b->proofs[l.b];
         std::unique_ptr<Job> j(new Job());
         j->kind = Job::kLink;
         j->bundle = b;
@@ -123,6 +133,9 @@ struct b200_pool {
                                                     nullptr, job->pub_inputs_out);
             } else if (job->kind == Job::kProveBatch) {
                 d.status = b200_plonk_prove_batch(ctxs[w], job->pk, job->items.data(), job->items.size(), job->statuses);
+            } else if (job->kind == Job::kProveWitnessBatch) {
+                d.status = b200_plonk_prove_witness_batch(ctxs[w], job->pk, job->witness_items.data(), job->witness_items.size(),
+                                                          job->statuses);
             } else if (job->kind == Job::kLinkBatch) {
                 d.status = b200_plonk_link_batch(ctxs[w], job->srs, job->link_items.data(), job->link_items.size(), job->statuses);
             } else {  // a single link stays on b200_plonk_link, which replays its CUDA graphs
@@ -301,6 +314,36 @@ int b200_pool_submit_prove_batch(b200_pool* pool, const b200_pk* pk, const b200_
     B200_CATCH
 }
 
+int b200_pool_submit_prove_witness_batch(b200_pool* pool, const b200_pk* pk, const b200_witness_item* items, size_t k,
+                                         int* statuses, uint64_t* ticket) {
+    B200_TRY
+    if (!pool || !pk || (k && !items) || !ticket) {
+        b200::set_error("pool_submit_prove_witness_batch: null argument");
+        return B200_ERR_INVALID;
+    }
+    if (b200_pk_num_vars(pk) == 0) {
+        b200::set_error("pool_submit_prove_witness_batch: the key holds no wiring (made by b200_plonk_preprocess)");
+        return B200_ERR_INVALID;
+    }
+    for (size_t i = 0; i < k; ++i)
+        if (!items[i].witness || !items[i].blinders || !items[i].proof) {
+            b200::set_error("pool_submit_prove_witness_batch: item " + std::to_string(i) + " has a NULL pointer");
+            return B200_ERR_INVALID;
+        }
+    std::unique_ptr<Job> j(new Job());
+    j->kind = Job::kProveWitnessBatch;
+    j->pk = pk;
+    j->statuses = statuses;
+    j->blinders.resize(4 * 17 * k);
+    j->witness_items.assign(items, items + k);
+    for (size_t i = 0; i < k; ++i) {  // the worker reads the copies
+        std::memcpy(&j->blinders[4 * 17 * i], items[i].blinders, 32 * 17);
+        j->witness_items[i].blinders = &j->blinders[4 * 17 * i];
+    }
+    return pool_push(pool, std::move(j), ticket);
+    B200_CATCH
+}
+
 int b200_pool_submit_link(b200_pool* pool, const b200_bases* srs, const uint64_t* a1, size_t len1,
                           const uint64_t* a2, size_t len2, const uint64_t* comm1, const uint64_t* comm2,
                           unsigned alignment, size_t offset, size_t size, b200_link_proof* proof,
@@ -340,6 +383,39 @@ int b200_pool_submit_link_batch(b200_pool* pool, const b200_bases* srs, const b2
     B200_CATCH
 }
 
+// The part of a bundle submission both entry points share: check the links against the proofs' hints, then queue the
+// proof jobs (each already filled in but for its `bundle`) under one ticket.  Nothing is queued on a refusal.
+static int bundle_push(b200_pool* pool, const char* who, const b200_bases* srs, std::vector<BundleHint> hints,
+                       const b200_bundle_link* links, size_t n_links, std::vector<std::unique_ptr<Job>> jobs, uint64_t* ticket) {
+    for (size_t i = 0; i < n_links; ++i) {
+        const b200_bundle_link& l = links[i];
+        if (l.a >= hints.size() || l.b >= hints.size() || !l.proof || !hints[l.a].link_poly || !hints[l.b].link_poly) {
+            b200::set_error(std::string(who) + ": a link names a proof that is missing or has no link_poly buffer");
+            return B200_ERR_INVALID;
+        }
+    }
+    std::shared_ptr<Bundle> b(new Bundle());
+    b->srs = srs;
+    b->proofs = std::move(hints);
+    b->links.assign(links, links + n_links);
+    b->pending = jobs.size();
+    for (auto& j : jobs) j->bundle = b;
+    {
+        std::lock_guard<std::mutex> lk(pool->mu);
+        if (pool->stopping) {
+            b200::set_error("pool: shutting down");
+            return B200_ERR_INVALID;
+        }
+        b->ticket = pool->next_ticket++;
+        *ticket = b->ticket;
+        pool->n_submitted += jobs.size();
+        pool->inflight.insert(b->ticket);
+        for (auto& j : jobs) pool->queue.push_back(std::move(j));
+    }
+    pool->cv_job.notify_all();
+    return B200_OK;
+}
+
 int b200_pool_submit_bundle(b200_pool* pool, const b200_bases* srs, const b200_bundle_proof* proofs, size_t n_proofs,
                             const b200_bundle_link* links, size_t n_links, uint64_t* ticket) {
     B200_TRY
@@ -355,24 +431,13 @@ int b200_pool_submit_bundle(b200_pool* pool, const b200_bases* srs, const b200_b
             return B200_ERR_INVALID;
         }
     }
-    for (size_t i = 0; i < n_links; ++i) {
-        const b200_bundle_link& l = links[i];
-        if (l.a >= n_proofs || l.b >= n_proofs || !l.proof || !proofs[l.a].link_poly || !proofs[l.b].link_poly) {
-            b200::set_error("pool_submit_bundle: a link names a proof that is missing or has no link_poly buffer");
-            return B200_ERR_INVALID;
-        }
-    }
-    std::shared_ptr<Bundle> b(new Bundle());
-    b->srs = srs;
-    b->proofs.assign(proofs, proofs + n_proofs);
-    b->links.assign(links, links + n_links);
-    b->pending = n_proofs;
+    std::vector<BundleHint> hints;
     std::vector<std::unique_ptr<Job>> jobs;
     for (size_t i = 0; i < n_proofs; ++i) {
         const b200_bundle_proof& p = proofs[i];
+        hints.push_back({p.pk, p.proof, p.link_poly});
         std::unique_ptr<Job> j(new Job());
         j->kind = Job::kProve;
-        j->bundle = b;
         j->pk = p.pk;
         j->wires = p.wires;
         j->pub_inputs.assign(p.pub_inputs, p.pub_inputs + 4 * p.num_inputs);
@@ -381,20 +446,45 @@ int b200_pool_submit_bundle(b200_pool* pool, const b200_bases* srs, const b200_b
         j->link_poly = p.link_poly;
         jobs.push_back(std::move(j));
     }
-    {
-        std::lock_guard<std::mutex> lk(pool->mu);
-        if (pool->stopping) {
-            b200::set_error("pool: shutting down");
+    return bundle_push(pool, "pool_submit_bundle", srs, std::move(hints), links, n_links, std::move(jobs), ticket);
+    B200_CATCH
+}
+
+int b200_pool_submit_bundle_witness(b200_pool* pool, const b200_bases* srs, const b200_bundle_witness* proofs,
+                                    size_t n_proofs, const b200_bundle_link* links, size_t n_links, uint64_t* ticket) {
+    B200_TRY
+    if (!pool || !proofs || n_proofs == 0 || (n_links && (!links || !srs)) || !ticket) {
+        b200::set_error("pool_submit_bundle_witness: null argument");
+        return B200_ERR_INVALID;
+    }
+    for (size_t i = 0; i < n_proofs; ++i) {
+        const b200_bundle_witness& p = proofs[i];
+        if (!p.pk || !p.witness || !p.blinders || !p.proof) {
+            b200::set_error("pool_submit_bundle_witness: proof " + std::to_string(i) + " has a NULL pointer");
             return B200_ERR_INVALID;
         }
-        b->ticket = pool->next_ticket++;
-        *ticket = b->ticket;
-        pool->n_submitted += n_proofs;
-        pool->inflight.insert(b->ticket);
-        for (auto& j : jobs) pool->queue.push_back(std::move(j));
+        if (b200_pk_num_vars(p.pk) == 0) {
+            b200::set_error("pool_submit_bundle_witness: the key of proof " + std::to_string(i) +
+                            " holds no wiring (made by b200_plonk_preprocess)");
+            return B200_ERR_INVALID;
+        }
     }
-    pool->cv_job.notify_all();
-    return B200_OK;
+    std::vector<BundleHint> hints;
+    std::vector<std::unique_ptr<Job>> jobs;
+    for (size_t i = 0; i < n_proofs; ++i) {
+        const b200_bundle_witness& p = proofs[i];
+        hints.push_back({p.pk, p.proof, p.link_poly});
+        std::unique_ptr<Job> j(new Job());
+        j->kind = Job::kProveWitness;
+        j->pk = p.pk;
+        j->wires = p.witness;
+        j->blinders.assign(p.blinders, p.blinders + 4 * 17);
+        j->proof = p.proof;
+        j->link_poly = p.link_poly;
+        j->pub_inputs_out = p.pub_inputs_out;
+        jobs.push_back(std::move(j));
+    }
+    return bundle_push(pool, "pool_submit_bundle_witness", srs, std::move(hints), links, n_links, std::move(jobs), ticket);
     B200_CATCH
 }
 
@@ -479,15 +569,18 @@ struct b200_box_srs {
 };
 struct b200_box_pk {
     std::vector<b200_pk*> per_dev;
+    const b200_box* owner = nullptr;  // the box that made it
 };
 
 namespace {
 constexpr int kBoxTicketShift = 48;  // ticket = device index << 48 | the device pool's ticket
 
-int box_least_loaded(b200_box* box) {
+// ordinal >= 0: only the box entries on that CUDA device are candidates
+int box_least_loaded(b200_box* box, int ordinal = -1) {
     int best = 0;
     uint64_t best_load = ~0ull;
     for (size_t i = 0; i < box->pools.size(); ++i) {
+        if (ordinal >= 0 && box->devices[i] != ordinal) continue;
         uint64_t st[4];
         if (b200_pool_stats(box->pools[i], st) != B200_OK) continue;
         const uint64_t load = st[0] - st[1];  // submitted - completed
@@ -497,6 +590,37 @@ int box_least_loaded(b200_box* box) {
         }
     }
     return best;
+}
+
+// The box entry the witness vectors ws[0..n) run on: a witness in device memory pins its jobs to that device (the least
+// loaded of the box entries with its ordinal); host, pinned and managed memory can be read from any device.  Refused: a
+// device outside the box, or device witnesses on two different devices.
+int box_witness_device(b200_box* box, const char* who, const uint64_t* const* ws, size_t n, int* out) {
+    int ordinal = -1;
+    for (size_t i = 0; i < n; ++i) {
+        cudaPointerAttributes a{};
+        if (cudaPointerGetAttributes(&a, ws[i]) != cudaSuccess) {
+            cudaGetLastError();  // a pointer CUDA does not know is ordinary host memory
+            continue;
+        }
+        if (a.type != cudaMemoryTypeDevice) continue;
+        if (ordinal >= 0 && a.device != ordinal) {
+            b200::set_error(std::string(who) + ": the witnesses lie on two devices (" + std::to_string(ordinal) + " and " +
+                            std::to_string(a.device) + "); a bundle runs on one");
+            return B200_ERR_INVALID;
+        }
+        ordinal = a.device;
+    }
+    if (ordinal >= 0 && std::find(box->devices.begin(), box->devices.end(), ordinal) == box->devices.end()) {
+        b200::set_error(std::string(who) + ": the witness lies on device " + std::to_string(ordinal) + ", which is not in the box");
+        return B200_ERR_INVALID;
+    }
+    *out = box_least_loaded(box, ordinal);
+    return B200_OK;
+}
+
+bool box_owns(const b200_box* box, const b200_box_pk* pk) {
+    return pk && pk->owner == box && pk->per_dev.size() == box->pools.size();
 }
 }  // namespace
 
@@ -574,6 +698,7 @@ int b200_box_preprocess(b200_box* box, const b200_box_srs* srs, unsigned log_n, 
     if (!box || !srs || !out || srs->per_dev.size() != box->pools.size()) return B200_ERR_INVALID;
     std::unique_ptr<b200_box_pk> pk(new b200_box_pk());
     pk->per_dev.assign(box->pools.size(), nullptr);
+    pk->owner = box;
     for (size_t i = 0; i < box->pools.size(); ++i) {
         const int rc = b200_plonk_preprocess(b200_pool_ctx(box->pools[i], 0), srs->per_dev[i], log_n, num_inputs, selectors_evals, perm, k,
                                              &pk->per_dev[i]);
@@ -626,6 +751,77 @@ int b200_box_submit_bundle(b200_box* box, const b200_box_srs* srs, const b200_bo
     }
     uint64_t t = 0;
     const int rc = b200_pool_submit_bundle(box->pools[d], srs ? srs->per_dev[d] : nullptr, local.data(), n_proofs, links, n_links, &t);
+    if (rc != B200_OK) return rc;
+    *ticket = ((uint64_t)d << kBoxTicketShift) | t;
+    return B200_OK;
+    B200_CATCH
+}
+
+int b200_box_preprocess_wiring(b200_box* box, const b200_box_srs* srs, unsigned log_n, size_t num_inputs,
+                               const uint64_t* selectors_evals, const unsigned* wire_vars, size_t num_vars, const uint64_t* k,
+                               b200_box_pk** out) {
+    B200_TRY
+    if (!box || !srs || !out || srs->per_dev.size() != box->pools.size()) {
+        b200::set_error("box_preprocess_wiring: null argument or SRS of another box");
+        return B200_ERR_INVALID;
+    }
+    std::unique_ptr<b200_box_pk> pk(new b200_box_pk());
+    pk->per_dev.assign(box->pools.size(), nullptr);
+    pk->owner = box;
+    for (size_t i = 0; i < box->pools.size(); ++i) {
+        const int rc = b200_plonk_preprocess_wiring(b200_pool_ctx(box->pools[i], 0), srs->per_dev[i], log_n, num_inputs,
+                                                    selectors_evals, wire_vars, num_vars, k, &pk->per_dev[i]);
+        if (rc != B200_OK) {
+            b200_box_pk_free(box, pk.release());
+            return rc;
+        }
+    }
+    *out = pk.release();
+    return B200_OK;
+    B200_CATCH
+}
+
+int b200_box_submit_prove_witness(b200_box* box, const b200_box_pk* pk, const uint64_t* witness, const uint64_t* blinders,
+                                  b200_proof* proof, uint64_t* link_poly, uint64_t* pub_inputs_out, uint64_t* ticket) {
+    B200_TRY
+    if (!box || !witness || !ticket || !box_owns(box, pk)) {
+        b200::set_error("box_submit_prove_witness: null argument or key of another box");
+        return B200_ERR_INVALID;
+    }
+    int d = 0;
+    int rc = box_witness_device(box, "box_submit_prove_witness", &witness, 1, &d);
+    if (rc != B200_OK) return rc;
+    uint64_t t = 0;
+    rc = b200_pool_submit_prove_witness(box->pools[d], pk->per_dev[d], witness, blinders, proof, link_poly, pub_inputs_out, &t);
+    if (rc != B200_OK) return rc;
+    *ticket = ((uint64_t)d << kBoxTicketShift) | t;
+    return B200_OK;
+    B200_CATCH
+}
+
+int b200_box_submit_bundle_witness(b200_box* box, const b200_box_srs* srs, const b200_box_pk* const* pks,
+                                   const b200_bundle_witness* proofs, size_t n_proofs, const b200_bundle_link* links,
+                                   size_t n_links, uint64_t* ticket) {
+    B200_TRY
+    if (!box || !pks || !proofs || n_proofs == 0 || !ticket || (n_links && (!srs || srs->per_dev.size() != box->pools.size()))) {
+        b200::set_error("box_submit_bundle_witness: null argument");
+        return B200_ERR_INVALID;
+    }
+    std::vector<const uint64_t*> ws(n_proofs);
+    for (size_t i = 0; i < n_proofs; ++i) {
+        if (!box_owns(box, pks[i]) || !proofs[i].witness) {
+            b200::set_error("box_submit_bundle_witness: proof " + std::to_string(i) + " has no witness or a key of another box");
+            return B200_ERR_INVALID;
+        }
+        ws[i] = proofs[i].witness;
+    }
+    int d = 0;  // a bundle stays on one device: its link proofs need its proofs' polynomials
+    int rc = box_witness_device(box, "box_submit_bundle_witness", ws.data(), n_proofs, &d);
+    if (rc != B200_OK) return rc;
+    std::vector<b200_bundle_witness> local(proofs, proofs + n_proofs);
+    for (size_t i = 0; i < n_proofs; ++i) local[i].pk = pks[i]->per_dev[d];
+    uint64_t t = 0;
+    rc = b200_pool_submit_bundle_witness(box->pools[d], srs ? srs->per_dev[d] : nullptr, local.data(), n_proofs, links, n_links, &t);
     if (rc != B200_OK) return rc;
     *ticket = ((uint64_t)d << kBoxTicketShift) | t;
     return B200_OK;

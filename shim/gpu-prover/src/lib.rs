@@ -7,6 +7,7 @@
 //! | `circuit-types/src/traits.rs:1012` | `PlonkKzgSnark::verify::<SolidityTranscript>(&vk, pi, &proof, None)` | [`verify`] (host only) |
 //! | `circuit-types/src/traits.rs:850`  | the same, keeping the wiring on the device | [`GpuProver::preprocess_wiring`] |
 //! | `circuit-types/src/traits.rs:996`  | the same, from `cs.witness()` instead of the 5 x n value table | [`GpuProver::prove_from_witness`] |
+//! | `circuit-types/src/traits.rs:996`  | the same for many witnesses of one key, in one pool job | [`GpuProver::prove_from_witness_batch`] |
 //! | `proof_linking/intent_only.rs:42-47` | `PlonkKzgSnark::link_proofs::<SolidityTranscript>(a, b, &layout, &ck)` | [`GpuProver::link_proofs`] |
 //! | `native_proof_manager.rs:726-782` | the four `link_proofs` calls of `compute_private_settlement_link_proofs` | [`GpuProver::link_proofs_batch`] |
 //! | `primitives/srs.rs:63-71` | `parse_ptau_file` + `powers_of_g` | [`GpuProver::load_srs`] |
@@ -207,6 +208,41 @@ impl GpuProver {
         let mut ticket = 0u64;
         check(unsafe {
             ffi::b200_pool_submit_prove_batch(self.pool, pk.raw, items.as_ptr(), k, statuses.as_mut_ptr(), &mut ticket)
+        })?;
+        let rc = unsafe { ffi::b200_pool_wait(self.pool, ticket) }; // buffers above stay alive until here
+        if rc != ffi::B200_ERR_UNSATISFIED {
+            check(rc)?;
+        }
+        Ok((0..k).map(|i| {
+            check(statuses[i])?;
+            Ok((proof_from_raw(&raws[i]), hint_from_raw(&raws[i], &links[i])))
+        }).collect())
+    }
+
+    /// `prove_batch` for a key made by `preprocess_wiring`: one `b200_plonk_prove_witness_batch` job on one worker, each
+    /// circuit handing over only its witness vector (`cs.witness()`).  Item i of the result is `prove_from_witness`'s
+    /// answer for `circuits[i]` with the same blinders, or `WrongQuotientPolyDegree` for an unsatisfied witness.
+    pub fn prove_from_witness_batch<R: rand::RngCore + rand::CryptoRng>(
+        &self, rng: &mut R, circuits: &[&PlonkCircuit<Fr>], pk: &GpuProvingKey,
+    ) -> Result<Vec<Result<(Proof<Bn254>, LinkingHint<Bn254>), PlonkError>>, PlonkError> {
+        let n = 1usize << pk.log_n;
+        let k = circuits.len();
+        let num_vars = unsafe { ffi::b200_pk_num_vars(pk.raw) };
+        let witnesses: Vec<Vec<u64>> = circuits.iter().map(|cs| cs.witness().iter().flat_map(fr_limbs).collect()).collect();
+        if witnesses.iter().any(|w| w.len() != 4 * num_vars) {
+            return Err(PlonkError::InvalidParameters("witness length differs from the key's num_vars".into()));
+        }
+        let blinders: Vec<Vec<u64>> = (0..k).map(|_| (0..17).map(|_| Fr::rand(rng)).flat_map(|f| fr_limbs(&f)).collect()).collect();
+        let mut raws: Vec<ffi::b200_proof> = (0..k).map(|_| unsafe { std::mem::zeroed() }).collect();
+        let mut links: Vec<Vec<u64>> = (0..k).map(|_| vec![0u64; (n + 2) * 4]).collect();
+        let items: Vec<ffi::b200_witness_item> = (0..k).map(|i| ffi::b200_witness_item {
+            witness: witnesses[i].as_ptr(), blinders: blinders[i].as_ptr(), proof: &mut raws[i],
+            link_poly: links[i].as_mut_ptr(), challenges: std::ptr::null_mut(), pub_inputs_out: std::ptr::null_mut(),
+        }).collect();
+        let mut statuses: Vec<c_int> = vec![0; k];
+        let mut ticket = 0u64;
+        check(unsafe {
+            ffi::b200_pool_submit_prove_witness_batch(self.pool, pk.raw, items.as_ptr(), k, statuses.as_mut_ptr(), &mut ticket)
         })?;
         let rc = unsafe { ffi::b200_pool_wait(self.pool, ticket) }; // buffers above stay alive until here
         if rc != ffi::B200_ERR_UNSATISFIED {

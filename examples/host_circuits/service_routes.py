@@ -100,13 +100,29 @@ def main():
     ap.add_argument("--password", required=True)
     ap.add_argument("--srs", required=True, help="ptau file (the reference's srs/srs00 chunks concatenated, or any prefix holding 2^14 + 3 powers)")
     ap.add_argument("--g2", help="256-byte file: the two G2 records h || tau*h (only needed by verifiers)")
+    ap.add_argument("--check-srs", action="store_true",
+                    help="check the loaded powers against h, tau*h (from --g2, else from the ptau's section 3) on the "
+                         "device, and refuse to start on an SRS that fails")
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--workers", type=int, default=6)
     args = ap.parse_args()
     pool = ProverPool(args.device, workers=args.workers)
     ctx = pool.context(0)
-    params = rb.parse_ptau_file(ctx, open(args.srs, "rb").read(), count=(1 << 14) + 3)
-    g2 = np.frombuffer(open(args.g2, "rb").read(), dtype=np.uint64) if args.g2 else np.zeros(32, dtype=np.uint64)
+    data = open(args.srs, "rb").read()
+    params = rb.parse_ptau_file(ctx, data, count=(1 << 14) + 3)
+    if args.g2:
+        g2 = np.frombuffer(open(args.g2, "rb").read(), dtype=np.uint64)
+    elif args.check_srs:
+        g2 = np.concatenate(rb.read_ptau_g2(data))
+    else:
+        g2 = np.zeros(32, dtype=np.uint64)
+    if args.check_srs:
+        report = rb.check_srs(ctx, params.powers_of_g, g2[:16], g2[16:32])
+        if not report.valid:
+            params.powers_of_g.free()
+            pool.close()
+            raise SystemExit(f"--check-srs: {args.srs} is not a consistent SRS for this G2 pair: {report}")
+        print(f"SRS checked: {len(params.powers_of_g)} powers consistent with h, tau*h", flush=True)
     ct.set_system_srs(ctx, params.powers_of_g, g2[:16], g2[16:32], pool=pool)
     for c in st.REGISTERED:  # `NativeProofManager::preprocess_circuits` (native_proof_manager.rs:305-331)
         c.proving_key()

@@ -102,6 +102,39 @@ size_t b200_bases_len(const b200_bases* bases);
 /* plan[0..3] = window bits c, digits per scalar, physical bucket windows, precomputed tables */
 void b200_bases_plan(const b200_bases* bases, int plan[4]);
 
+/* Replaces read_ptau_section3 (srs.rs:147-157): the first two G2 records of the section that follows section 2
+ * (located by section 2's declared size, as the reference seeks to its end): h = tau^0 H, beta_h = tau^1 H, 128-byte
+ * records x0||x1||y0||y1 Montgomery, the layout every verifier here takes.  Header checks as b200_srs_parse_ptau.
+ * B200_ERR_FORMAT (b200_last_error says which) for a file that ends before section 3's two records, a section number
+ * other than 3, a section 3 declared shorter than the two records, or a section 2 size that would leave the buffer;
+ * B200_ERR_NOT_ON_CURVE for a record off the twist (a coordinate >= q included).  Host only. */
+int b200_srs_parse_ptau_g2(const uint8_t* bytes, size_t len, uint64_t g2_h[16], uint64_t g2_tau_h[16]);
+
+/* *in_subgroup = [ Q is a point of the twist of order r ] ([r]Q == O; the identity counts as not in the subgroup).
+ * B200_ERR_NOT_ON_CURVE off the twist.  Host only. */
+int b200_g2_in_subgroup(const uint64_t rec[16], int* in_subgroup);
+
+typedef struct {
+    uint64_t consistent;     /* 1: the combined check passed, e(sum rho^i P_i, tau H) == e(sum rho^i P_{i+1}, H), i < n-1 */
+    uint64_t g1_generator;   /* P_0 == (1, 2), the G the verifiers use */
+    uint64_t g2_subgroup;    /* h and beta_h both of order r */
+    uint64_t n_bad;          /* with locate and consistent == 0: number of failing pairs (P_i, P_{i+1}); else 0 */
+    uint64_t bad[8];         /* the first min(n_bad, 8) failing pair indices i, ascending */
+} b200_srs_report;
+
+/* Checks the first n powers of a loaded SRS against the G2 pair: that they are P_i = tau^i P_0 for the tau of
+ * beta_h = tau h.  rho = keccak256("b200 srs check v1" || seed[32] || n as u64 big-endian || g2_h || g2_tau_h) read
+ * big-endian mod r (1 if 0); the two weight vectors rho^i are filled on the device, both sums are one batch-2 MSM over
+ * the resident bases on the context's stream (counted by b200_msm_timing_totals), and the pairing runs on the host.
+ * The seed must be unknown to whoever made the file; then an inconsistent SRS passes with probability at most n / r.
+ * With locate != 0 and a failed combined check, every consecutive pair e(P_i, tau H) == e(P_{i+1}, H) is checked on its
+ * own on the device, one thread per pair, and n_bad / bad are filled (an off-curve point fails the pairs it is in).
+ * The SRS is valid exactly when consistent && g1_generator && g2_subgroup.
+ * B200_ERR_INVALID: NULL ctx / srs / g2 / seed / out, n == 0 or n > b200_bases_len(srs).  B200_ERR_NOT_ON_CURVE for a G2
+ * record off the twist.  n == 1 checks the generator and the subgroup only (consistent = 1). */
+int b200_srs_check(b200_ctx* ctx, const b200_bases* srs, size_t n, const uint64_t g2_h[16], const uint64_t g2_tau_h[16],
+                   const uint8_t seed[32], int locate, b200_srs_report* out);
+
 /* ---- MSM ------------------------------------------------------------------------------- */
 /* out = sum_{i<n} scalars[i] * bases[base_off + i].
  * Replaces `VariableBaseMSM::msm_bigint(&bases[..], &scalars[..])` followed by

@@ -7,7 +7,7 @@ it is missing or no CUDA device is visible (there is no CPU fallback)."""
 from . import _lib  # noqa: F401
 from .backend import (  # noqa: F401
     Bases, Context, Radix2EvaluationDomain, UnivariateKzgPCS, UnivariateUniversalParams,
-    VariableBaseMSM, parse_ptau_file, MAX_SRS_DEGREE,
+    VariableBaseMSM, parse_ptau_file, MAX_SRS_DEGREE, SrsReport, check_srs, read_ptau_g2,
 )
 
 __version__ = "0.1.0"

@@ -204,16 +204,29 @@ class Bases:
 @dataclass
 class UnivariateUniversalParams:
     """jf-primitives `UnivariateUniversalParams<Bn254>` as built at srs.rs:70: the G1 powers
-    live on the device; `powers_of_g_host` keeps the raw 64-byte records for inspection."""
+    live on the device; `powers_of_g_host` keeps the raw 64-byte records for inspection.  `h` / `beta_h` are the
+    two G2 records of section 3 (16 x uint64 each), None for a truncated file that ends before them."""
     powers_of_g: Bases
     powers_of_g_host: np.ndarray
+    h: np.ndarray | None = None
+    beta_h: np.ndarray | None = None
+
+
+def read_ptau_g2(data: bytes):
+    """srs.rs:147-157 (`read_ptau_section3`): (h, beta_h), the first two G2 records of section 3, 16 x uint64 each
+    (`b200_srs_parse_ptau_g2`: header checks as parse_ptau_file, both records on the twist).  Host only."""
+    lib = _lib.load()
+    h, beta_h = np.zeros(16, dtype=np.uint64), np.zeros(16, dtype=np.uint64)
+    _lib.check(lib.b200_srs_parse_ptau_g2(data, len(data), _ptr(h), _ptr(beta_h)))
+    return h, beta_h
 
 
 def parse_ptau_file(ctx: Context, data: bytes, window_bits: int = 0,
                     check_on_curve: bool = True, count: int | None = None) -> UnivariateUniversalParams:
     """srs.rs:63-71: header/section checks, MAX_SRS_DEGREE+1 G1 powers, on-curve assertion
     (srs.rs:178-179, run on the device).  `count` overrides the number of powers kept (the
-    reference always keeps MAX_SRS_DEGREE + 1; smaller values serve truncated test files)."""
+    reference always keeps MAX_SRS_DEGREE + 1; smaller values serve truncated test files).  `h` / `beta_h` are read
+    from section 3 when the file holds it (read_ptau_g2), else left None; a G2 record there off the twist raises."""
     lib = _lib.load()
     buf = (C.c_char * len(data)).from_buffer_copy(data)
     rec = C.c_void_p()
@@ -222,10 +235,59 @@ def parse_ptau_file(ctx: Context, data: bytes, window_bits: int = 0,
     need = MAX_SRS_DEGREE + 1 if count is None else count
     if n.value < need:
         raise _lib.B200Error(_lib.B200_ERR_FORMAT, f"ptau: only {n.value} G1 records available, need {need}")
+    try:
+        g2 = read_ptau_g2(data)
+    except _lib.B200Error as e:  # no section 3 (the truncated files accepted above): no G2 pair; a bad record raises
+        if e.code != _lib.B200_ERR_FORMAT:
+            raise
+        g2 = (None, None)
     off = rec.value - C.addressof(buf)
     host = np.frombuffer(data, dtype=np.uint64, count=need * 8, offset=off).reshape(need, 8).copy()
     bases = ctx.load_bases(host, window_bits=window_bits, check_on_curve=check_on_curve)
-    return UnivariateUniversalParams(powers_of_g=bases, powers_of_g_host=host)
+    return UnivariateUniversalParams(powers_of_g=bases, powers_of_g_host=host, h=g2[0], beta_h=g2[1])
+
+
+def g2_in_subgroup(rec) -> bool:
+    """[r]Q == O for a 128-byte G2 record (`b200_g2_in_subgroup`; the identity is not in the subgroup).  Host only."""
+    out = C.c_int(0)
+    _lib.check(_lib.load().b200_g2_in_subgroup(_ptr(_u64(rec, 16)), C.byref(out)))
+    return bool(out.value)
+
+
+SRS_REPORT_MAX_BAD = 8  # failing pair indices b200_srs_report lists
+
+
+@dataclass
+class SrsReport:
+    """`b200_srs_report`: the SRS is valid exactly when `valid` (consistent powers, P_0 = G, h and beta_h of order r).
+    `bad` lists the first failing pairs (P_i, P_{i+1}) by i, ascending, of `n_bad` in all (located only on request)."""
+    consistent: bool
+    g1_generator: bool
+    g2_subgroup: bool
+    n_bad: int
+    bad: list
+
+    @property
+    def valid(self) -> bool:
+        return self.consistent and self.g1_generator and self.g2_subgroup
+
+
+def check_srs(ctx: Context, bases: Bases, h, beta_h, n: int | None = None, seed: bytes | None = None,
+              locate: bool = True) -> SrsReport:
+    """Checks that the first n (default: all) loaded powers are tau^i G for the tau of beta_h = tau h, with one batch-2
+    MSM on the device and one pairing (`b200_srs_check`).  The weights are the powers of a rho drawn from `seed`
+    (32 bytes; None draws `secrets.token_bytes(32)`), which must be unknown to whoever made the file.  With `locate`,
+    a failed check is followed by every consecutive pair checked on its own on the device, which fills `n_bad` / `bad`."""
+    import secrets
+    n = len(bases) if n is None else n
+    seed = secrets.token_bytes(32) if seed is None else bytes(seed)
+    if len(seed) != 32:
+        raise ValueError("seed: 32 bytes")
+    rep = _lib.STRUCTS["b200_srs_report"]()
+    _lib.check(ctx._lib.b200_srs_check(ctx._h, bases._h, n, _ptr(_u64(h, 16)), _ptr(_u64(beta_h, 16)), seed, int(locate),
+                                       C.byref(rep)))
+    return SrsReport(consistent=bool(rep.consistent), g1_generator=bool(rep.g1_generator), g2_subgroup=bool(rep.g2_subgroup),
+                     n_bad=int(rep.n_bad), bad=[int(rep.bad[i]) for i in range(min(int(rep.n_bad), SRS_REPORT_MAX_BAD))])
 
 
 class VariableBaseMSM:

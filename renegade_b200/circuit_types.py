@@ -32,7 +32,8 @@ from typing import Any, Dict, List, Optional, Tuple
 import numpy as np
 
 from . import _lib
-from .backend import (B200Proof, Bases, Context, LinkingHint, PlonkKzgSnark, ProvingKey, VerifyingKey)
+from .backend import (B200Proof, Bases, Context, LinkingHint, PlonkKzgSnark, ProvingKey, VerifyingKey, check_srs,
+                      parse_ptau_file, read_ptau_g2)
 from .fields import SCALAR_FIELD_MODULUS, scalars_to_limbs
 
 PlonkProof = B200Proof                    # circuit-types/src/lib.rs:72-101
@@ -40,7 +41,8 @@ ProofLinkingHint = LinkingHint
 
 
 class ProverError(Exception):
-    """circuit-types/src/errors.rs:33-47.  `kind` is one of "Circuit", "Plonk", "Verification"."""
+    """circuit-types/src/errors.rs:33-47.  `kind` is one of "Circuit", "Plonk", "Verification", or "Srs" (an SRS that
+    failed `SystemSrs.from_ptau`'s check; `detail` is its SrsReport)."""
 
     def __init__(self, kind: str, detail: Any):
         super().__init__(f"{kind}({detail})")
@@ -59,6 +61,21 @@ class SystemSrs:
     g2_h: np.ndarray
     g2_tau_h: np.ndarray
     pool: Any = None   # optional ProverPool: proofs then run `workers` at a time, one request thread per ticket
+
+    @staticmethod
+    def from_ptau(ctx: Context, data: bytes, count: Optional[int] = None, check: bool = True, pool=None) -> "SystemSrs":
+        """The whole SRS from one ptau file: the G1 powers (`count` of them, default MAX_SRS_DEGREE + 1) loaded on the
+        device, h / beta_h from its section 3, and with `check` the powers checked against them on the device
+        (`check_srs`, fresh random weights); then installed as SYSTEM_SRS (`set_system_srs`).  An SRS that fails the
+        check raises ProverError("Srs", report) and nothing is installed."""
+        params = parse_ptau_file(ctx, data, count=count)
+        h, beta_h = (params.h, params.beta_h) if params.h is not None else read_ptau_g2(data)
+        if check:
+            report = check_srs(ctx, params.powers_of_g, h, beta_h)
+            if not report.valid:
+                params.powers_of_g.free()
+                raise ProverError("Srs", report)
+        return set_system_srs(ctx, params.powers_of_g, h, beta_h, pool=pool)
 
 
 _SYSTEM_SRS: Optional[SystemSrs] = None

@@ -286,6 +286,51 @@ int b200_srs_parse_ptau(const uint8_t* bytes, size_t len, const uint8_t** g1_rec
     B200_CATCH
 }
 
+int b200_srs_parse_ptau_g2(const uint8_t* bytes, size_t len, uint64_t g2_h[16], uint64_t g2_tau_h[16]) {
+    B200_TRY
+    if (!bytes || !g2_h || !g2_tau_h) return B200_ERR_INVALID;
+    // header, section 1 and section 2's header: the checks of b200_srs_parse_ptau, which leaves g1 just past the latter
+    const uint8_t* g1 = nullptr;
+    size_t n_records = 0;
+    int rc = b200_srs_parse_ptau(bytes, len, &g1, &n_records);
+    if (rc != B200_OK) return rc;
+    size_t off = (size_t)(g1 - bytes);
+    uint64_t size;
+    rd_u64(bytes, len, off - 8, &size);
+    if (size > len - off) {  // untrusted 64-bit length, as for section 1
+        set_error("ptau: section 2 longer than the file");
+        return B200_ERR_FORMAT;
+    }
+    off += (size_t)size;
+    // section 3 (srs.rs:147-157): its header, then h and beta_h
+    uint32_t sec;
+    if (!rd_u32(bytes, len, off, &sec) || !rd_u64(bytes, len, off + 4, &size)) {
+        set_error("ptau: the file ends before section 3");
+        return B200_ERR_FORMAT;
+    }
+    if (sec != 3) {
+        set_error("Invalid section number");
+        return B200_ERR_FORMAT;
+    }
+    off += 12;
+    if (size < 256) {
+        set_error("ptau: section 3 is shorter than its two G2 records");
+        return B200_ERR_FORMAT;
+    }
+    if (len - off < 256) {
+        set_error("ptau: the file ends inside section 3's two G2 records");
+        return B200_ERR_FORMAT;
+    }
+    std::memcpy(g2_h, bytes + off, 128);
+    std::memcpy(g2_tau_h, bytes + off + 128, 128);
+    if (!g2_record_on_curve(g2_h) || !g2_record_on_curve(g2_tau_h)) {
+        set_error("ptau: section 3: G2 point not on curve");
+        return B200_ERR_NOT_ON_CURVE;
+    }
+    return B200_OK;
+    B200_CATCH
+}
+
 int b200_bases_load(b200_ctx* ctx, const uint8_t* points64, size_t n, int window_bits, int check_on_curve,
                     b200_bases** out) {
     B200_TRY

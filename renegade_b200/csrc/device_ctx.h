@@ -246,6 +246,9 @@ struct Context {
 
 int get_domain(Context* c, unsigned log_n, Domain** out);
 
+// a 128-byte G2 record x0 || x1 || y0 || y1 (Montgomery) is on the twist, every coordinate below q (verify.cu)
+bool g2_record_on_curve(const uint64_t rec[16]);
+
 // d_perm[p] = the next position (ascending, cyclic) that carries the variable d_wire_vars[p] carries, for the `count` wire
 // positions of a circuit: the copy-constraint permutation k_sigma_evals takes (wiring.cu).  Synchronises `st`.
 // B200_ERR_INVALID, naming the first position, for a variable index >= num_vars.

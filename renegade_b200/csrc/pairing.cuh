@@ -270,6 +270,8 @@ void g2_prepare(const g2_affine& q, G2Prepared* out);
 // host (verify.cu): the same for a 128-byte record x0 || x1 || y0 || y1 (Montgomery); false, and nothing prepared, when
 // the point is off the curve or a coordinate is >= q
 bool g2_prepare_record(const uint64_t rec[16], G2Prepared* out);
+// host (verify.cu): the point of a 128-byte record (all zero: the identity); false when it is off the curve
+bool g2_load_record(const uint64_t rec[16], g2_affine* out);
 
 // f <- f * (the line evaluated at P = (px, py)); the sparse operand first: fq12_mul skips its zero coefficients
 FF_HD void line_eval_mul(fq12* f, const G2Line& l, const fe& px, const fe& py) {

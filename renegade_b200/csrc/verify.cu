@@ -231,6 +231,13 @@ bool g2_prepare_record(const uint64_t rec[16], G2Prepared* out) {
     return true;
 }
 
+bool g2_load_record(const uint64_t rec[16], g2_affine* out) {
+    *out = g2_load(rec);
+    return g2_on_curve(*out);
+}
+
+bool g2_record_on_curve(const uint64_t rec[16]) { return g2_on_curve(g2_load(rec)); }
+
 bool g2_records_on_curve(const uint64_t g2_tau_h[16], const uint64_t g2_h[16]) {
     return g2_on_curve(g2_load(g2_tau_h)) && g2_on_curve(g2_load(g2_h));
 }

@@ -347,6 +347,31 @@ impl GpuProver {
         }))?;
         Ok(verdicts.into_iter().map(|v| v == 1).collect())
     }
+
+    /// Checks the first `n` powers of the loaded SRS against `(g2_h, g2_tau_h)` on this GPU (`b200_srs_check`): one
+    /// batch-2 MSM and one pairing, with weights drawn from `seed`, which must be unknown to whoever made the file.
+    /// With `locate`, a failed check also names the failing pairs (P_i, P_{i+1}).  Valid exactly when
+    /// `consistent && g1_generator && g2_subgroup`.
+    pub fn check_srs(&self, n: usize, g2_h: &[u64; 16], g2_tau_h: &[u64; 16], seed: &[u8; 32], locate: bool)
+        -> Result<ffi::b200_srs_report, PlonkError> {
+        if self.srs.is_null() {
+            return Err(PlonkError::InvalidParameters("check_srs: no SRS loaded".into()));
+        }
+        let mut report: ffi::b200_srs_report = unsafe { std::mem::zeroed() };
+        check(unsafe {
+            ffi::b200_srs_check(ffi::b200_pool_ctx(self.pool, 0), self.srs, n, g2_h.as_ptr(), g2_tau_h.as_ptr(), seed.as_ptr(),
+                                locate as c_int, &mut report)
+        })?;
+        Ok(report)
+    }
+}
+
+/// replaces `read_ptau_section3` (srs.rs:147-157): `(h, beta_h)`, the two G2 records of the ptau's section 3 in the
+/// layout `verify` takes; both are checked to lie on the twist.  Host only.
+pub fn parse_ptau_g2(ptau_bytes: &[u8]) -> Result<([u64; 16], [u64; 16]), PlonkError> {
+    let (mut h, mut beta_h) = ([0u64; 16], [0u64; 16]);
+    check(unsafe { ffi::b200_srs_parse_ptau_g2(ptau_bytes.as_ptr(), ptau_bytes.len(), h.as_mut_ptr(), beta_h.as_mut_ptr()) })?;
+    Ok((h, beta_h))
 }
 
 /// The C structs of a batch of `verify` / `verify_link_proof` items, alive while `f` runs.

@@ -504,10 +504,10 @@ typedef struct {
 } b200_bundle_link;
 /* Queue a whole proof bundle under ONE ticket: the `n_proofs` proofs run through the pool; when all of them are in,
  * the `n_links` link proofs are forked onto the pool; the ticket completes after the last link proof (or with the
- * first failure).  Replaces the settlement arms of `NativeProofManager::handle_proof_job`
- * (native_proof_manager.rs:526-584) with `compute_private_settlement_link_proofs` (:726-782): e.g. a private match =
- * 5 proofs + 4 links.  The arrays are copied at submit; the buffers they point to stay owned by the caller until
- * the ticket has been waited for. */
+ * first failure).  A bundle links only proofs made inside it (e.g. 5 proofs + 4 links of one private match); a
+ * settlement linked against hints kept from earlier validity proofs is b200_pool_submit_settlement
+ * (b200settlement.h).  The arrays are copied at submit; the buffers they point to stay owned by the caller until the
+ * ticket has been waited for. */
 int b200_pool_submit_bundle(b200_pool* pool, const b200_bases* srs, const b200_bundle_proof* proofs, size_t n_proofs,
                             const b200_bundle_link* links, size_t n_links, uint64_t* ticket);
 /* One proof of a bundle given as a witness vector, arguments as for b200_pool_submit_prove_witness: pk is a key made by

@@ -670,6 +670,47 @@ class PlonkKzgSnark:
             _lib.check(rc)
         return _batch_results(keep, statuses, link_hints, want_challenges)
 
+    @staticmethod
+    def prove_settlement(ctx: Context, srs: Bases, pk: ProvingKey, wires, pub_inputs, blinders, links):
+        """A settlement in ONE call (`b200_plonk_prove_settlement`): proves the statement, then links every stored hint to
+        the statement's own hint as one link batch.  wires: the 5 x n table (array) or its address in device or pinned
+        host memory (int); links = [(LinkingHint, GroupLayout)], each hint's linking_wire_poly an array or (address,
+        length) of one in device or pinned host memory.  Returns (proof, link_proofs, statuses): the proof equals
+        `prove_with_link_hint`'s, link i equals `link_proofs(hint_i, settlement hint, layout_i)`; statuses[0] is the
+        proof's, statuses[1 + i] link i's (0, or -7 = B200_ERR_UNSATISFIED: an unsatisfied witness zeroes everything, a
+        stale hint zeroes its own link proof).  Argument errors raise ProverError before any library call."""
+        w, w_ptr = _wires_arg(pk.domain_size, wires, "prove_settlement")
+        pi, bl = _settlement_inputs(pk.num_inputs, pub_inputs, blinders, "prove_settlement")
+        arr, held, out = _settlement_links(links, len(srs), pk.domain_size, "prove_settlement")
+        proof = B200Proof()
+        st = (C.c_int * (len(out) + 1))()
+        rc = ctx._lib.b200_plonk_prove_settlement(ctx._h, srs._h, pk._h, w_ptr, _ptr(pi) if pi.size else None, _ptr(bl),
+                                                  C.byref(proof), None, arr, len(out), st)
+        if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
+            _lib.check(rc)
+        return proof, out, list(st)
+
+    @staticmethod
+    def prove_settlement_witness(ctx: Context, srs: Bases, pk: ProvingKey, witness, blinders, links):
+        """`prove_settlement` from the settlement's witness vector (`b200_plonk_prove_settlement_witness`) of a key made by
+        `preprocess_wiring`: witness as `prove_witness` takes it.  Returns (proof, link_proofs, statuses, pub_inputs)."""
+        if pk.num_vars == 0:
+            raise ProverError(_lib.B200_ERR_INVALID, "prove_settlement_witness: the key holds no wiring (made by preprocess)")
+        try:
+            wit, wit_ptr = _witness_arg(pk, witness, "prove_settlement_witness")
+        except ValueError as e:
+            raise ProverError(_lib.B200_ERR_INVALID, str(e))
+        _, bl = _settlement_inputs(0, (), blinders, "prove_settlement_witness")
+        arr, held, out = _settlement_links(links, len(srs), pk.domain_size, "prove_settlement_witness")
+        proof = B200Proof()
+        pub = np.zeros((pk.num_inputs, 4), dtype=np.uint64)
+        st = (C.c_int * (len(out) + 1))()
+        rc = ctx._lib.b200_plonk_prove_settlement_witness(ctx._h, srs._h, pk._h, wit_ptr, _ptr(bl), C.byref(proof), None,
+                                                          _ptr(pub) if pub.size else None, arr, len(out), st)
+        if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
+            _lib.check(rc)
+        return proof, out, list(st), pub
+
 
 B200ProveItem = _lib.STRUCTS["b200_prove_item"]  # one witness of a batch
 B200WitnessItem = _lib.STRUCTS["b200_witness_item"]  # one witness vector of a batch
@@ -879,6 +920,81 @@ def link_proofs_batch(ctx: Context, srs: Bases, triples):
     if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
         _lib.check(rc)
     return _link_batch_results(keep, statuses)
+
+
+SettlementLink = _lib.STRUCTS["b200_settlement_link"]  # one stored hint of a settlement and its group
+
+
+def _wires_arg(n: int, wires, where: str):
+    """A 5 x n wire table as (array kept alive or None, pointer): an array, or an address."""
+    if isinstance(wires, (int, np.integer)):
+        return None, C.c_void_p(int(wires))
+    w = np.ascontiguousarray(wires, dtype=np.uint64)
+    if w.size != 5 * n * 4:
+        raise ProverError(_lib.B200_ERR_INVALID, f"{where}: the wire table has {w.size // 4} elements, the key needs 5 x {n}")
+    return w, _ptr(w)
+
+
+def _settlement_inputs(num_inputs: int, pub_inputs, blinders, where: str):
+    """The public inputs and the 17 blinders of a settlement, checked (ProverError)."""
+    pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64).reshape(-1, 4)
+    if pi.shape[0] != num_inputs:
+        raise ProverError(_lib.B200_ERR_INVALID, f"{where}: {pi.shape[0]} public inputs for a key with {num_inputs}")
+    bl = np.ascontiguousarray(blinders, dtype=np.uint64)
+    if bl.size != 17 * 4:
+        raise ProverError(_lib.B200_ERR_INVALID, f"{where}: {bl.size // 4} blinders, the prover draws 17")
+    return pi, bl
+
+
+def _settlement_links(links, srs_len, n: int, where: str):
+    """Checks a settlement's links = [(LinkingHint, GroupLayout)] against a key of domain size n (ProverError naming the
+    link; srs_len None skips the SRS length check) and builds their b200_settlement_link array.  Returns (array, arrays
+    to keep alive, link proofs)."""
+    links = list(links)
+    arr = (SettlementLink * max(1, len(links)))()
+    held, out = [], []
+    for i, t in enumerate(links):
+        if len(t) != 2:
+            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: link {i} is not a (hint, layout) pair")
+        hint, lay = t
+        try:
+            p, ln, a = _link_poly(hint.linking_wire_poly, f"link {i}'s hint")
+        except ValueError as e:
+            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: {e}")
+        c = np.ascontiguousarray(hint.linking_wire_comm, dtype=np.uint64).reshape(-1)
+        if c.size != 8:
+            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: link {i}'s hint commitment must be 8 limbs (x || y)")
+        m = max(ln, n + 2)
+        if not 0 < lay.size < m:
+            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: link {i}'s group of {lay.size} roots does not fit "
+                                                     f"polynomials of {m} coefficients")
+        if not 0 <= lay.alignment <= 28 or lay.offset < 0:
+            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: link {i} has alignment {lay.alignment} and offset "
+                                                     f"{lay.offset} (0 <= alignment <= 28, offset >= 0)")
+        if srs_len is not None and m > srs_len:
+            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: link {i} has {m} coefficients, the SRS {srs_len} powers")
+        lp = B200LinkProof()
+        arr[i] = SettlementLink(p, ln, _ptr(c), lay.alignment, lay.offset, lay.size, C.cast(C.pointer(lp), C.c_void_p), None)
+        held += [a, c, hint]
+        out.append(lp)
+    return arr, held, out
+
+
+@dataclass
+class _PoolSettlement:
+    """What a queued settlement job writes into, and what it reads until the wait."""
+    proof: Any
+    links: list
+    statuses: Any
+    pub_inputs: Any  # None for a wire-table settlement
+    held: list
+
+
+def _settlement_results(s: "_PoolSettlement", rc: int):
+    if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
+        _lib.check(rc)
+    st = [int(s.statuses[i]) for i in range(len(s.links) + 1)]
+    return (s.proof, s.links, st) if s.pub_inputs is None else (s.proof, s.links, st, s.pub_inputs)
 
 
 def compute_poseidon_hash_batch(ctx: Context, values: np.ndarray) -> np.ndarray:
@@ -1184,12 +1300,53 @@ class ProverPool:
         self._keep[ticket.value] = (_PoolWitnessBatch(held, statuses, link_hints, pubs), None, (items, keep), pk)
         return ticket.value
 
+    def submit_settlement(self, srs: "Bases", pk: "ProvingKey", wires, pub_inputs, blinders, links, keep=None) -> int:
+        """Queue one `PlonkKzgSnark.prove_settlement` as ONE job on one worker (`b200_pool_submit_settlement`); returns the
+        ticket.  Arguments as `prove_settlement` takes them; a wire table or hint given by address stays owned by the
+        caller until `wait(ticket)` returns (pass its owner as `keep`).  `wait(ticket)` returns (proof, link_proofs,
+        statuses) like `prove_settlement`."""
+        w, w_ptr = _wires_arg(pk.domain_size, wires, "submit_settlement")
+        pi, bl = _settlement_inputs(pk.num_inputs, pub_inputs, blinders, "submit_settlement")
+        arr, held, out = _settlement_links(links, len(srs), pk.domain_size, "submit_settlement")
+        proof = B200Proof()
+        item = BundleProof(pk._h, w_ptr, _ptr(pi) if pi.size else None, pi.shape[0], _ptr(bl),
+                           C.cast(C.pointer(proof), C.c_void_p), None)
+        st = (C.c_int * (len(out) + 1))()
+        ticket = C.c_uint64()
+        _lib.check(self._lib.b200_pool_submit_settlement(self._h, srs._h, C.byref(item), arr, len(out), st, C.byref(ticket)))
+        self._keep[ticket.value] = (_PoolSettlement(proof, out, st, None, [w, pi, bl, arr, held, keep]), None, None, (pk, srs))
+        return ticket.value
+
+    def submit_settlement_witness(self, srs: "Bases", pk: "ProvingKey", witness, blinders, links, keep=None) -> int:
+        """`submit_settlement` from the settlement's witness vector (`b200_pool_submit_settlement_witness`), arguments as
+        `PlonkKzgSnark.prove_settlement_witness` takes them.  `wait(ticket)` returns (proof, link_proofs, statuses,
+        pub_inputs)."""
+        if pk.num_vars == 0:
+            raise ProverError(_lib.B200_ERR_INVALID, "submit_settlement_witness: the key holds no wiring (made by preprocess)")
+        try:
+            wit, wit_ptr = _witness_arg(pk, witness, "submit_settlement_witness")
+        except ValueError as e:
+            raise ProverError(_lib.B200_ERR_INVALID, str(e))
+        _, bl = _settlement_inputs(0, (), blinders, "submit_settlement_witness")
+        arr, held, out = _settlement_links(links, len(srs), pk.domain_size, "submit_settlement_witness")
+        proof = B200Proof()
+        pub = np.zeros((pk.num_inputs, 4), dtype=np.uint64)
+        item = BundleWitness(pk._h, wit_ptr, _ptr(bl), C.cast(C.pointer(proof), C.c_void_p), None, _ptr(pub) if pub.size else None)
+        st = (C.c_int * (len(out) + 1))()
+        ticket = C.c_uint64()
+        _lib.check(self._lib.b200_pool_submit_settlement_witness(self._h, srs._h, C.byref(item), arr, len(out), st,
+                                                                 C.byref(ticket)))
+        self._keep[ticket.value] = (_PoolSettlement(proof, out, st, pub, [wit, bl, arr, held, keep]), None, None, (pk, srs))
+        return ticket.value
+
     def wait(self, ticket: int):
         """Blocks until the job is done; returns its B200Proof (or (B200Proof, link_poly) when the job was
         submitted with `with_link_poly`, or the B200LinkProof of a link job); raises B200Error with the
         job's own status and message if it failed."""
         rc = self._lib.b200_pool_wait(self._h, ticket)
         proof, link, _, _ = self._keep.pop(ticket, (None, None, None, None))
+        if isinstance(proof, _PoolSettlement):  # a settlement: refused links and an unsatisfied proof are in its statuses
+            return _settlement_results(proof, rc)
         if isinstance(proof, (_PoolBatch, _PoolLinkBatch)):  # a batch job: refused items are reported in its statuses
             if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
                 _lib.check(rc)
@@ -1328,6 +1485,45 @@ class ProverBox:
         self._keep[ticket.value] = (out, None, (keep, pks))
         return ticket.value
 
+    def submit_settlement(self, srs, pk, wires, pub_inputs, blinders, links, keep=None) -> int:
+        """`ProverPool.submit_settlement` on one device of the box (`b200_box_submit_settlement`): pk a box key, srs a box
+        SRS.  A wire table or hint polynomial in device memory pins the job to its device (all of them on one); otherwise
+        the job goes to the least-loaded device.  `wait(ticket)` returns (proof, link_proofs, statuses)."""
+        _, shape = self._resolve(pk)
+        w, w_ptr = _wires_arg(shape.domain_size, wires, "box.submit_settlement")
+        pi, bl = _settlement_inputs(shape.num_inputs, pub_inputs, blinders, "box.submit_settlement")
+        arr, held, out = _settlement_links(links, None, shape.domain_size, "box.submit_settlement")
+        proof = B200Proof()
+        item = BundleProof(None, w_ptr, _ptr(pi) if pi.size else None, pi.shape[0], _ptr(bl),
+                           C.cast(C.pointer(proof), C.c_void_p), None)
+        st = (C.c_int * (len(out) + 1))()
+        ticket = C.c_uint64()
+        _lib.check(self._lib.b200_box_submit_settlement(self._h, srs, pk, C.byref(item), arr, len(out), st, C.byref(ticket)))
+        self._keep[ticket.value] = (_PoolSettlement(proof, out, st, None, [w, pi, bl, arr, held, keep]), None)
+        return ticket.value
+
+    def submit_settlement_witness(self, srs, pk, witness, blinders, links, keep=None) -> int:
+        """`submit_settlement` from a witness vector (`b200_box_submit_settlement_witness`); the witness counts among the
+        job's device pointers.  `wait(ticket)` returns (proof, link_proofs, statuses, pub_inputs)."""
+        _, shape = self._resolve(pk)
+        if shape.num_vars == 0:
+            raise ProverError(_lib.B200_ERR_INVALID, "box.submit_settlement_witness: the key holds no wiring (made by preprocess)")
+        try:
+            wit, wit_ptr = _witness_arg(shape, witness, "box.submit_settlement_witness")
+        except ValueError as e:
+            raise ProverError(_lib.B200_ERR_INVALID, str(e))
+        _, bl = _settlement_inputs(0, (), blinders, "box.submit_settlement_witness")
+        arr, held, out = _settlement_links(links, None, shape.domain_size, "box.submit_settlement_witness")
+        proof = B200Proof()
+        pub = np.zeros((shape.num_inputs, 4), dtype=np.uint64)
+        item = BundleWitness(None, wit_ptr, _ptr(bl), C.cast(C.pointer(proof), C.c_void_p), None, _ptr(pub) if pub.size else None)
+        st = (C.c_int * (len(out) + 1))()
+        ticket = C.c_uint64()
+        _lib.check(self._lib.b200_box_submit_settlement_witness(self._h, srs, pk, C.byref(item), arr, len(out), st,
+                                                                C.byref(ticket)))
+        self._keep[ticket.value] = (_PoolSettlement(proof, out, st, pub, [wit, bl, arr, held, keep]), None)
+        return ticket.value
+
     def verifying_key(self, pk):
         sel, sig = np.zeros((13, 8), dtype=np.uint64), np.zeros((5, 8), dtype=np.uint64)
         _lib.check(self._lib.b200_box_pk_verifying_key(pk, _ptr(sel), _ptr(sig)))
@@ -1348,6 +1544,8 @@ class ProverBox:
     def wait(self, ticket: int):
         rc = self._lib.b200_box_wait(self._h, ticket)
         proof, link, *_ = self._keep.pop(ticket, (None, None))
+        if isinstance(proof, _PoolSettlement):
+            return _settlement_results(proof, rc)
         _lib.check(rc)
         if isinstance(proof, _PoolWitness):
             return (proof.proof, proof.pub_inputs) if link is None else (proof.proof, link, proof.pub_inputs)

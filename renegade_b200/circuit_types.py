@@ -32,7 +32,7 @@ from typing import Any, Dict, List, Optional, Tuple
 import numpy as np
 
 from . import _lib
-from .backend import (B200Proof, Bases, Context, LinkingHint, PlonkKzgSnark, ProvingKey, VerifyingKey, check_srs,
+from .backend import (B200Proof, Bases, Context, GroupLayout, LinkingHint, PlonkKzgSnark, ProvingKey, VerifyingKey, check_srs,
                       parse_ptau_file, read_ptau_g2)
 from .fields import SCALAR_FIELD_MODULUS, scalars_to_limbs
 
@@ -244,6 +244,40 @@ class SingleProverCircuit:
             raise ProverError("Plonk", e) from e
 
     @classmethod
+    def prove_settlement(cls, witness, statement, hints, rng=None, pool=None, srs_bases=None):
+        """A settlement arm of `NativeProofManager::handle_proof_job` (native_proof_manager.rs:514-660) in ONE call:
+        `singleprover_prove_with_hint` of this statement, then `link_proofs(hint, &settlement_hint, &layout)` for every
+        (stored hint, link group id) in `hints` (validity hint first, intent_and_balance.rs:57-72), the group layouts
+        taken from `get_circuit_layout()`.  One settlement job on `pool` (default: the system SRS's pool), else one call
+        on the SRS context; `srs_bases` defaults to the system SRS.  The proof and link proofs equal
+        `prove_with_link_hint` + `link_proofs` with the same rng.  Returns (proof, [link proofs]); an unsatisfied witness
+        or a hint that differs from the statement on its group (a stale hint) raises ProverError("Plonk") naming it."""
+        return settlement_result(hints, *cls.prove_settlement_statuses(witness, statement, hints, rng, pool, srs_bases))
+
+    @classmethod
+    def prove_settlement_statuses(cls, witness, statement, hints, rng=None, pool=None, srs_bases=None):
+        """`prove_settlement` without the raising: (proof, link proofs, statuses), statuses[0] the proof's and
+        statuses[1 + i] hint i's (0, or B200_ERR_UNSATISFIED)."""
+        pk, circ = cls._arithmetize(witness, statement)
+        layouts = cls.get_circuit_layout()
+        links = [(h, GroupLayout(layouts[g].alignment, layouts[g].offset, layouts[g].size)) for h, g in hints]
+        srs = system_srs()
+        pool = srs.pool if pool is None else pool
+        bases = srs_bases or srs.powers_of_g
+        blinders = draw_blinders(rng)
+        try:
+            if cls.prove_from_witness:
+                res = (pool.wait(pool.submit_settlement_witness(bases, pk, circ.witness, blinders, links)) if pool is not None
+                       else PlonkKzgSnark.prove_settlement_witness(srs.ctx, bases, pk, circ.witness, blinders, links))
+            else:
+                res = (pool.wait(pool.submit_settlement(bases, pk, circ.wires, circ.pub_inputs, blinders, links))
+                       if pool is not None
+                       else PlonkKzgSnark.prove_settlement(srs.ctx, bases, pk, circ.wires, circ.pub_inputs, blinders, links))
+        except _lib.B200Error as e:
+            raise ProverError("Plonk", e) from e
+        return res[:3]
+
+    @classmethod
     def prove_batch_with_link_hint(cls, instances, rng=None) -> List[Tuple[PlonkProof, ProofLinkingHint]]:
         """Many (witness, statement) pairs of this circuit: each is synthesised on the host, then ONE batch call
         (`PlonkKzgSnark.prove_batch`, or one pool job when the SRS has a pool) proves them all.  Raises ProverError naming
@@ -319,6 +353,22 @@ def singleprover_prove(circuit: type, witness, statement, rng=None) -> PlonkProo
 
 def singleprover_prove_with_hint(circuit: type, witness, statement, rng=None) -> Tuple[PlonkProof, ProofLinkingHint]:
     return circuit.prove_with_link_hint(witness, statement, rng)
+
+
+def settlement_result(hints, proof, link_proofs, statuses):
+    """(proof, link proofs) of a settlement whose statuses are all B200_OK; else ProverError("Plonk") naming the failure:
+    an unsatisfied settlement witness, or the hints that differ from the statement on their link group (stale hints)."""
+    if statuses[0] != _lib.B200_OK:
+        raise ProverError("Plonk", "WrongQuotientPolyDegree: the settlement witness does not satisfy the circuit")
+    stale = [f"hint {i} (group {hints[i][1]})" for i in range(len(hints)) if statuses[1 + i] != _lib.B200_OK]
+    if stale:
+        raise ProverError("Plonk", f"{', '.join(stale)}: differs from the settlement on its link group (a stale hint)")
+    return proof, link_proofs
+
+
+def singleprover_prove_settlement(circuit: type, witness, statement, hints, rng=None):
+    """`SingleProverCircuit.prove_settlement`: (proof, [link proofs]) of a settlement against its stored hints."""
+    return circuit.prove_settlement(witness, statement, hints, rng)
 
 
 def singleprover_prove_batch(circuit: type, instances, rng=None) -> List[PlonkProof]:

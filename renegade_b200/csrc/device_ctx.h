@@ -16,6 +16,7 @@
 #include "ff.cuh"
 
 #include "b200prover.h"  // error codes
+#include "b200settlement.h"  // settlement_check
 
 namespace b200 {
 
@@ -253,6 +254,11 @@ bool g2_record_on_curve(const uint64_t rec[16]);
 // positions of a circuit: the copy-constraint permutation k_sigma_evals takes (wiring.cu).  Synchronises `st`.
 // B200_ERR_INVALID, naming the first position, for a variable index >= num_vars.
 int wiring_permutation(const uint32_t* d_wire_vars, size_t count, size_t num_vars, uint64_t* d_perm, cudaStream_t st);
+
+// The link and key checks of b200_plonk_prove_settlement[_witness] (witness: the key must hold wiring), for a pool to make
+// at submit: B200_OK, or B200_ERR_INVALID with a message that starts with `who` and names the link.
+int settlement_check(const b200_bases* srs, const b200_pk* pk, bool witness, const b200_settlement_link* links, size_t n_links,
+                     const char* who);
 
 }  // namespace b200
 

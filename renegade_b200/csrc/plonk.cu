@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "b200prover.h"
+#include "b200settlement.h"
 #include "device_ctx.h"
 #include "transcript.h"
 #include "verify_terms.h"
@@ -1833,6 +1834,23 @@ static size_t link_batch_chunk(Context* c, const Bases* srs, const std::vector<L
     return std::max<size_t>(1, std::min({k, kMaxBatchChunk, budget / per_item, idx_cap}));
 }
 
+// The items of a link batch on the context's batch buffers (the caller holds the context's lock): items of one transform
+// size next to each other, so that a chunk divides each size's items with one launch per step.  Each item's status says
+// whether its proof was made; the outputs of the others are not written.
+static int link_batch_run(Context* c, const Bases* srs, std::vector<LinkItem>& its) {
+    const size_t k = its.size();
+    if (k == 0) return B200_OK;
+    std::vector<LinkItem*> order(k);
+    for (size_t i = 0; i < k; ++i) order[i] = &its[i];
+    std::stable_sort(order.begin(), order.end(), [](const LinkItem* a, const LinkItem* b) { return a->log_N < b->log_N; });
+    const size_t chunk = link_batch_chunk(c, srs, its);
+    for (size_t off = 0; off < k; off += chunk) {
+        const int rc = link_chunk(c, batch_bufs(c), srs, order.data() + off, (unsigned)std::min(chunk, k - off), /*single=*/false);
+        if (rc != B200_OK) return rc;
+    }
+    return B200_OK;
+}
+
 }  // namespace b200
 
 // ---------------------------------------------------------------------------------------------
@@ -1843,6 +1861,91 @@ using namespace b200;
 struct b200_pk {
     ProvingKey* pk;
 };
+
+namespace b200 {
+
+// ---------------------------------------------------------------------------------------------
+// settlements — the settlement arms of `NativeProofManager::handle_proof_job` (native_proof_manager.rs:514-660): prove
+// the statement, then link each hint the job brings (validity first, settlement second) to the statement's hint
+// ---------------------------------------------------------------------------------------------
+
+// The link items of a settlement of the key `pk`: each caller hint first, the settlement's n + 2 coefficients second
+// (a2 and comm2 are filled in once the proof is made).  Every argument check of the settlement entry points but the
+// proof's own pointers: B200_ERR_INVALID, with a message that starts with `who`, before any device work.
+static int settlement_items(const b200_bases* srs, const b200_pk* pk, bool witness, const b200_settlement_link* links,
+                            size_t n_links, const std::string& who, std::vector<LinkItem>* its) {
+    if (!srs || !pk || (n_links && !links)) {
+        set_error(who + ": NULL srs, key or links");
+        return B200_ERR_INVALID;
+    }
+    if (witness && !pk->pk->wire_vars) {
+        set_error(who + ": the key holds no wiring (made by b200_plonk_preprocess, not b200_plonk_preprocess_wiring)");
+        return B200_ERR_INVALID;
+    }
+    static const uint64_t kNoComm[8] = {};
+    its->resize(n_links);
+    for (size_t i = 0; i < n_links; ++i) {
+        const b200_settlement_link& l = links[i];
+        const std::string where = who + ": link " + std::to_string(i);
+        if (!l.hint_poly || !l.hint_comm || !l.proof) {
+            set_error(where + " has a NULL hint_poly, hint_comm or proof");
+            return B200_ERR_INVALID;
+        }
+        const b200_link_item x{l.hint_poly, l.hint_len, nullptr, pk->pk->n + 2, l.hint_comm, kNoComm,
+                               l.alignment, l.offset, l.size, l.proof, l.eta};
+        const int rc = link_item(srs->b, x, where, &(*its)[i]);
+        if (rc != B200_OK) return rc;
+    }
+    return B200_OK;
+}
+
+int settlement_check(const b200_bases* srs, const b200_pk* pk, bool witness, const b200_settlement_link* links, size_t n_links,
+                     const char* who) {
+    std::vector<LinkItem> its;
+    return settlement_items(srs, pk, witness, links, n_links, who, &its);
+}
+
+// Both settlement entry points once their arguments are checked: the proof (b200_plonk_prove's path, graphs included),
+// then the links as one batch against P, read where prove() left it in the single-proof workspace (proof 0's wire 0,
+// n + 2 coefficients; the link batch runs in the batch buffers and does not touch it).
+static int prove_settlement(b200_ctx* ctx, const Bases* srs, const ProvingKey* pk, ProveItem* item, std::vector<LinkItem>& its,
+                            int* statuses, const std::string& who) {
+    std::lock_guard<std::mutex> lk(ctx->c.mu);
+    B200_CUDA(cudaSetDevice(ctx->c.device));
+    int rc = prove(&ctx->c, single_bufs(&ctx->c), pk, item, 1, /*single=*/true);
+    if (rc == B200_ERR_UNSATISFIED) {
+        std::memset(item->proof, 0, sizeof(b200_proof));
+        for (LinkItem& it : its) std::memset(it.out, 0, sizeof(LinkOut));
+        if (statuses)
+            for (size_t i = 0; i <= its.size(); ++i) statuses[i] = B200_ERR_UNSATISFIED;
+        set_error(who + ": WrongQuotientPolyDegree: the settlement witness does not satisfy the circuit (no link proof made)");
+        return rc;
+    }
+    if (rc != B200_OK) return rc;
+    const fe* d_p = carve(reinterpret_cast<fe*>(ctx->c.plonk_ws.p), pk->n, 1).wpoly;
+    for (LinkItem& it : its) {
+        it.a2 = d_p;
+        it.comm2 = item->proof->wires_poly_comms[0];
+    }
+    if ((rc = link_batch_run(&ctx->c, srs, its)) != B200_OK) return rc;
+    if (statuses) statuses[0] = B200_OK;
+    std::string bad;
+    for (size_t i = 0; i < its.size(); ++i) {
+        if (its[i].status != B200_OK) {
+            std::memset(its[i].out, 0, sizeof(LinkOut));
+            bad += (bad.empty() ? "" : ", ") + std::to_string(i);
+        }
+        if (statuses) statuses[1 + i] = its[i].status;
+    }
+    if (!bad.empty()) {
+        set_error(who + ": the proof was made; the hint of link(s) " + bad +
+                  " differs from the settlement's link polynomial on its group (a stale hint or a wrong layout; see statuses)");
+        return B200_ERR_UNSATISFIED;
+    }
+    return B200_OK;
+}
+
+}  // namespace b200
 
 extern "C" {
 
@@ -1935,16 +2038,8 @@ int b200_plonk_link_batch(b200_ctx* ctx, const b200_bases* srs, const b200_link_
     if (k == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
     B200_CUDA(cudaSetDevice(ctx->c.device));
-    // items of one transform size next to each other: a chunk divides each size's items with one launch per step
-    std::vector<LinkItem*> order(k);
-    for (size_t i = 0; i < k; ++i) order[i] = &its[i];
-    std::stable_sort(order.begin(), order.end(), [](const LinkItem* a, const LinkItem* b) { return a->log_N < b->log_N; });
-    const size_t chunk = link_batch_chunk(&ctx->c, srs->b, its);
-    for (size_t off = 0; off < k; off += chunk) {
-        const int rc = link_chunk(&ctx->c, batch_bufs(&ctx->c), srs->b, order.data() + off, (unsigned)std::min(chunk, k - off),
-                                  /*single=*/false);
-        if (rc != B200_OK) return rc;
-    }
+    const int rc = link_batch_run(&ctx->c, srs->b, its);
+    if (rc != B200_OK) return rc;
     size_t bad = 0;
     for (size_t i = 0; i < k; ++i) {
         if (its[i].status != B200_OK) {
@@ -2013,6 +2108,45 @@ int b200_plonk_prove_witness(b200_ctx* ctx, const b200_pk* pk, const uint64_t* w
                    reinterpret_cast<fe*>(link_poly), reinterpret_cast<fe*>(challenges), B200_OK,
                    reinterpret_cast<const fe*>(witness), reinterpret_cast<fe*>(pub_inputs_out)};
     return prove(&ctx->c, single_bufs(&ctx->c), pk->pk, &item, 1, /*single=*/true);
+    B200_CATCH
+}
+
+int b200_plonk_prove_settlement(b200_ctx* ctx, const b200_bases* srs, const b200_pk* pk, const uint64_t* wires,
+                                const uint64_t* pub_inputs, const uint64_t* blinders, b200_proof* proof, uint64_t* link_poly,
+                                const b200_settlement_link* links, size_t n_links, int* statuses) {
+    B200_TRY
+    const std::string who = "plonk_prove_settlement";
+    if (!ctx || !pk || !wires || !blinders || !proof || (pk->pk->num_inputs && !pub_inputs)) {
+        set_error(who + ": NULL argument");
+        return B200_ERR_INVALID;
+    }
+    std::vector<LinkItem> its;
+    const int rc = settlement_items(srs, pk, /*witness=*/false, links, n_links, who, &its);
+    if (rc != B200_OK) return rc;
+    ProveItem item{reinterpret_cast<const fe*>(wires),     reinterpret_cast<const fe*>(pub_inputs),
+                   reinterpret_cast<const fe*>(blinders),  reinterpret_cast<ProofOut*>(proof),
+                   reinterpret_cast<fe*>(link_poly),       nullptr, B200_OK};
+    return prove_settlement(ctx, srs->b, pk->pk, &item, its, statuses, who);
+    B200_CATCH
+}
+
+int b200_plonk_prove_settlement_witness(b200_ctx* ctx, const b200_bases* srs, const b200_pk* pk, const uint64_t* witness,
+                                        const uint64_t* blinders, b200_proof* proof, uint64_t* link_poly,
+                                        uint64_t* pub_inputs_out, const b200_settlement_link* links, size_t n_links,
+                                        int* statuses) {
+    B200_TRY
+    const std::string who = "plonk_prove_settlement_witness";
+    if (!ctx || !pk || !witness || !blinders || !proof) {
+        set_error(who + ": NULL argument");
+        return B200_ERR_INVALID;
+    }
+    std::vector<LinkItem> its;
+    const int rc = settlement_items(srs, pk, /*witness=*/true, links, n_links, who, &its);
+    if (rc != B200_OK) return rc;
+    ProveItem item{nullptr, nullptr, reinterpret_cast<const fe*>(blinders), reinterpret_cast<ProofOut*>(proof),
+                   reinterpret_cast<fe*>(link_poly), nullptr, B200_OK,
+                   reinterpret_cast<const fe*>(witness), reinterpret_cast<fe*>(pub_inputs_out)};
+    return prove_settlement(ctx, srs->b, pk->pk, &item, its, statuses, who);
     B200_CATCH
 }
 

@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "b200prover.h"
+#include "b200settlement.h"
 #include "device_ctx.h"
 
 namespace {
@@ -25,7 +26,7 @@ namespace {
 struct Bundle;
 
 struct Job {
-    enum Kind { kProve, kProveWitness, kProveBatch, kProveWitnessBatch, kLink, kLinkBatch } kind = kProve;
+    enum Kind { kProve, kProveWitness, kProveBatch, kProveWitnessBatch, kLink, kLinkBatch, kSettlement, kSettlementWitness } kind = kProve;
     uint64_t ticket = 0;
     // prove (wires: the table) and prove witness (wires: the witness vector)
     const b200_pk* pk = nullptr;
@@ -45,6 +46,18 @@ struct Job {
     std::vector<b200_link_item> link_items;
     std::vector<uint64_t> link_comms;
     std::shared_ptr<Bundle> bundle;  // set for the sub-jobs of a bundle (they carry no ticket of their own)
+    // settlement (pk, wires, pub_inputs, blinders, proof, link_poly, pub_inputs_out, srs, statuses as above): the links
+    // with hint_comm pointing into the copies in `link_comms` (8 limbs per link)
+    std::vector<b200_settlement_link> settlement_links;
+
+    void set_settlement_links(const b200_settlement_link* ls, size_t k) {  // the worker reads the copies
+        settlement_links.assign(ls, ls + k);
+        link_comms.resize(8 * k);
+        for (size_t i = 0; i < k; ++i) {
+            std::memcpy(&link_comms[8 * i], ls[i].hint_comm, 64);
+            settlement_links[i].hint_comm = &link_comms[8 * i];
+        }
+    }
 
     void set_link_items(const b200_link_item* its, size_t k) {  // the worker reads the copies
         link_items.assign(its, its + k);
@@ -64,8 +77,9 @@ struct Done {
 };
 
 // A bundle: proofs first, then — once all of them are in — the link proofs between their wire-0 polynomials; one
-// ticket for the whole thing.  The device-side shape of `NativeProofManager::handle_proof_job` for the settlement jobs
-// (native_proof_manager.rs:526-584: prove, then `compute_*_link_proofs`, :726-782 forking the link proofs).
+// ticket for the whole thing.  Its links name proofs of the same bundle only; a settlement linked against hints kept from
+// earlier proofs (the settlement arms of `NativeProofManager::handle_proof_job`, native_proof_manager.rs:514-660) is a
+// settlement job (kSettlement), one call of b200_plonk_prove_settlement.
 // Both bundle entry points (wire tables and witness vectors) share it: a link job needs only each proof's key, proof and
 // link polynomial.
 struct BundleHint {
@@ -136,6 +150,16 @@ struct b200_pool {
             } else if (job->kind == Job::kProveWitnessBatch) {
                 d.status = b200_plonk_prove_witness_batch(ctxs[w], job->pk, job->witness_items.data(), job->witness_items.size(),
                                                           job->statuses);
+            } else if (job->kind == Job::kSettlement) {
+                d.status = b200_plonk_prove_settlement(ctxs[w], job->srs, job->pk, job->wires,
+                                                       job->pub_inputs.empty() ? nullptr : job->pub_inputs.data(),
+                                                       job->blinders.data(), job->proof, job->link_poly,
+                                                       job->settlement_links.data(), job->settlement_links.size(), job->statuses);
+            } else if (job->kind == Job::kSettlementWitness) {
+                d.status = b200_plonk_prove_settlement_witness(ctxs[w], job->srs, job->pk, job->wires, job->blinders.data(),
+                                                               job->proof, job->link_poly, job->pub_inputs_out,
+                                                               job->settlement_links.data(), job->settlement_links.size(),
+                                                               job->statuses);
             } else if (job->kind == Job::kLinkBatch) {
                 d.status = b200_plonk_link_batch(ctxs[w], job->srs, job->link_items.data(), job->link_items.size(), job->statuses);
             } else {  // a single link stays on b200_plonk_link, which replays its CUDA graphs
@@ -488,6 +512,61 @@ int b200_pool_submit_bundle_witness(b200_pool* pool, const b200_bases* srs, cons
     B200_CATCH
 }
 
+int b200_pool_submit_settlement(b200_pool* pool, const b200_bases* srs, const b200_bundle_proof* proof,
+                                const b200_settlement_link* links, size_t n_links, int* statuses, uint64_t* ticket) {
+    B200_TRY
+    const char* who = "pool_submit_settlement";
+    if (!pool || !proof || !ticket || !proof->pk || !proof->wires || !proof->blinders || !proof->proof ||
+        (proof->num_inputs && !proof->pub_inputs)) {
+        b200::set_error(std::string(who) + ": null argument");
+        return B200_ERR_INVALID;
+    }
+    if (proof->num_inputs != b200_pk_num_inputs(proof->pk)) {  // the worker reads exactly pk.num_inputs elements
+        b200::set_error(std::string(who) + ": num_inputs does not match the proving key");
+        return B200_ERR_INVALID;
+    }
+    const int rc = b200::settlement_check(srs, proof->pk, /*witness=*/false, links, n_links, who);
+    if (rc != B200_OK) return rc;
+    std::unique_ptr<Job> j(new Job());
+    j->kind = Job::kSettlement;
+    j->srs = srs;
+    j->pk = proof->pk;
+    j->wires = proof->wires;
+    j->pub_inputs.assign(proof->pub_inputs, proof->pub_inputs + 4 * proof->num_inputs);
+    j->blinders.assign(proof->blinders, proof->blinders + 4 * 17);
+    j->proof = proof->proof;
+    j->link_poly = proof->link_poly;
+    j->statuses = statuses;
+    j->set_settlement_links(links, n_links);
+    return pool_push(pool, std::move(j), ticket);
+    B200_CATCH
+}
+
+int b200_pool_submit_settlement_witness(b200_pool* pool, const b200_bases* srs, const b200_bundle_witness* proof,
+                                        const b200_settlement_link* links, size_t n_links, int* statuses, uint64_t* ticket) {
+    B200_TRY
+    const char* who = "pool_submit_settlement_witness";
+    if (!pool || !proof || !ticket || !proof->pk || !proof->witness || !proof->blinders || !proof->proof) {
+        b200::set_error(std::string(who) + ": null argument");
+        return B200_ERR_INVALID;
+    }
+    const int rc = b200::settlement_check(srs, proof->pk, /*witness=*/true, links, n_links, who);
+    if (rc != B200_OK) return rc;
+    std::unique_ptr<Job> j(new Job());
+    j->kind = Job::kSettlementWitness;
+    j->srs = srs;
+    j->pk = proof->pk;
+    j->wires = proof->witness;
+    j->blinders.assign(proof->blinders, proof->blinders + 4 * 17);
+    j->proof = proof->proof;
+    j->link_poly = proof->link_poly;
+    j->pub_inputs_out = proof->pub_inputs_out;
+    j->statuses = statuses;
+    j->set_settlement_links(links, n_links);
+    return pool_push(pool, std::move(j), ticket);
+    B200_CATCH
+}
+
 int b200_pool_wait(b200_pool* pool, uint64_t ticket) {
     B200_TRY
     if (!pool || ticket == 0) {
@@ -592,9 +671,9 @@ int box_least_loaded(b200_box* box, int ordinal = -1) {
     return best;
 }
 
-// The box entry the witness vectors ws[0..n) run on: a witness in device memory pins its jobs to that device (the least
-// loaded of the box entries with its ordinal); host, pinned and managed memory can be read from any device.  Refused: a
-// device outside the box, or device witnesses on two different devices.
+// The box entry a job reading ws[0..n) (witness vectors, wire tables, hint polynomials) runs on: a pointer into device
+// memory pins the job to that device (the least loaded of the box entries with its ordinal); host, pinned and managed
+// memory can be read from any device.  Refused: a device outside the box, or device pointers on two different devices.
 int box_witness_device(b200_box* box, const char* who, const uint64_t* const* ws, size_t n, int* out) {
     int ordinal = -1;
     for (size_t i = 0; i < n; ++i) {
@@ -606,7 +685,7 @@ int box_witness_device(b200_box* box, const char* who, const uint64_t* const* ws
         if (a.type != cudaMemoryTypeDevice) continue;
         if (ordinal >= 0 && a.device != ordinal) {
             b200::set_error(std::string(who) + ": the witnesses lie on two devices (" + std::to_string(ordinal) + " and " +
-                            std::to_string(a.device) + "); a bundle runs on one");
+                            std::to_string(a.device) + "); a bundle or settlement runs on one");
             return B200_ERR_INVALID;
         }
         ordinal = a.device;
@@ -822,6 +901,60 @@ int b200_box_submit_bundle_witness(b200_box* box, const b200_box_srs* srs, const
     for (size_t i = 0; i < n_proofs; ++i) local[i].pk = pks[i]->per_dev[d];
     uint64_t t = 0;
     rc = b200_pool_submit_bundle_witness(box->pools[d], srs ? srs->per_dev[d] : nullptr, local.data(), n_proofs, links, n_links, &t);
+    if (rc != B200_OK) return rc;
+    *ticket = ((uint64_t)d << kBoxTicketShift) | t;
+    return B200_OK;
+    B200_CATCH
+}
+
+// The device a box settlement runs on: its input (wire table or witness) and every hint polynomial count
+static int box_settlement_device(b200_box* box, const char* who, const b200_box_srs* srs, const b200_box_pk* pk,
+                                 const uint64_t* input, const b200_settlement_link* links, size_t n_links, int* out) {
+    if (!box_owns(box, pk) || !srs || srs->per_dev.size() != box->pools.size() || !input || (n_links && !links)) {
+        b200::set_error(std::string(who) + ": null argument, or a key or SRS of another box");
+        return B200_ERR_INVALID;
+    }
+    std::vector<const uint64_t*> ptrs{input};
+    for (size_t i = 0; i < n_links; ++i)
+        if (links[i].hint_poly) ptrs.push_back(links[i].hint_poly);  // a NULL one is refused by the pool's checks
+    return box_witness_device(box, who, ptrs.data(), ptrs.size(), out);
+}
+
+int b200_box_submit_settlement(b200_box* box, const b200_box_srs* srs, const b200_box_pk* pk, const b200_bundle_proof* proof,
+                               const b200_settlement_link* links, size_t n_links, int* statuses, uint64_t* ticket) {
+    B200_TRY
+    if (!box || !proof || !ticket) {
+        b200::set_error("box_submit_settlement: null argument");
+        return B200_ERR_INVALID;
+    }
+    int d = 0;
+    int rc = box_settlement_device(box, "box_submit_settlement", srs, pk, proof->wires, links, n_links, &d);
+    if (rc != B200_OK) return rc;
+    b200_bundle_proof local = *proof;
+    local.pk = pk->per_dev[d];
+    uint64_t t = 0;
+    rc = b200_pool_submit_settlement(box->pools[d], srs->per_dev[d], &local, links, n_links, statuses, &t);
+    if (rc != B200_OK) return rc;
+    *ticket = ((uint64_t)d << kBoxTicketShift) | t;
+    return B200_OK;
+    B200_CATCH
+}
+
+int b200_box_submit_settlement_witness(b200_box* box, const b200_box_srs* srs, const b200_box_pk* pk,
+                                       const b200_bundle_witness* proof, const b200_settlement_link* links, size_t n_links,
+                                       int* statuses, uint64_t* ticket) {
+    B200_TRY
+    if (!box || !proof || !ticket) {
+        b200::set_error("box_submit_settlement_witness: null argument");
+        return B200_ERR_INVALID;
+    }
+    int d = 0;
+    int rc = box_settlement_device(box, "box_submit_settlement_witness", srs, pk, proof->witness, links, n_links, &d);
+    if (rc != B200_OK) return rc;
+    b200_bundle_witness local = *proof;
+    local.pk = pk->per_dev[d];
+    uint64_t t = 0;
+    rc = b200_pool_submit_settlement_witness(box->pools[d], srs->per_dev[d], &local, links, n_links, statuses, &t);
     if (rc != B200_OK) return rc;
     *ticket = ((uint64_t)d << kBoxTicketShift) | t;
     return B200_OK;

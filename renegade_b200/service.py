@@ -209,6 +209,8 @@ class ProverService:
         route = self.routes[path]
         witness = route.decode_witness(body["witness"])
         statement = route.decode_statement(body["statement"])
+        if self.pool is not None and route.response in ("settlement", "private_settlement"):
+            return self._settle(route, witness, statement, body)
         proof, hint = route.circuit.prove_with_link_hint(witness, statement)
         with self._lock:
             self.stats["proofs"] += 1
@@ -240,6 +242,21 @@ class ProverService:
                 self.stats["link_proofs"] += len(jobs)
             return out
         raise ValueError(f"unknown response kind {route.response}")
+
+    def _settle(self, route: Route, witness, statement, body: Dict[str, Any]) -> Dict[str, Any]:
+        """A settlement route on the pool: ONE settlement job proves the statement and links every hint of the request
+        (`SingleProverCircuit.prove_settlement`), with no host round trip between the proof and its links."""
+        hints = [(decode_link_hint(body[req_field]), group) for req_field, _, group in route.links]
+        res = route.circuit.prove_settlement_statuses(witness, statement, hints, pool=self.pool, srs_bases=self.srs_bases)
+        with self._lock:  # counted as on the two-step path: the proof once made, the link proofs once all are made
+            self.stats["proofs"] += res[2][0] == _lib.B200_OK
+        proof, link_proofs = ct.settlement_result(hints, *res)
+        with self._lock:
+            self.stats["link_proofs"] += len(link_proofs)
+        out = {"proof": encode_proof(proof)}
+        for (_, resp_field, _), lp in zip(route.links, link_proofs):
+            out[resp_field] = encode_link_proof(lp)
+        return out
 
     def _submit_link(self, a: LinkingHint, b: LinkingHint, layout: GroupLayout):
         """Queue one link proof; returns a function that waits for it."""

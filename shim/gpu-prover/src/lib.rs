@@ -10,6 +10,7 @@
 //! | `circuit-types/src/traits.rs:996`  | the same for many witnesses of one key, in one pool job | [`GpuProver::prove_from_witness_batch`] |
 //! | `proof_linking/intent_only.rs:42-47` | `PlonkKzgSnark::link_proofs::<SolidityTranscript>(a, b, &layout, &ck)` | [`GpuProver::link_proofs`] |
 //! | `native_proof_manager.rs:726-782` | the four `link_proofs` calls of `compute_private_settlement_link_proofs` | [`GpuProver::link_proofs_batch`] |
+//! | `native_proof_manager.rs:514-660` | a settlement arm: `singleprover_prove_with_hint`, then `link_proofs` against each stored hint | [`GpuProver::prove_settlement`], [`GpuProver::prove_settlement_from_witness`] |
 //! | `primitives/srs.rs:63-71` | `parse_ptau_file` + `powers_of_g` | [`GpuProver::load_srs`] |
 //!
 //! Marshalling rules (SURVEY.md §7 "Rust ABI hazards"): `Fr`/`Fq` are `Fp(BigInt<4>, PhantomData)` holding the
@@ -23,6 +24,7 @@
 //! the fork already has.
 #![allow(unsafe_code)]
 pub mod ffi;
+pub mod ffi_settlement;
 
 use ark_bn254::{Bn254, Fq, Fr, G1Affine};
 use ark_ff::{BigInt, UniformRand};
@@ -314,6 +316,69 @@ impl GpuProver {
                 opening_proof: jf_primitives::pcs::prelude::UnivariateKzgProof { proof: g1_from(&raws[i].opening_proof) },
             })
         }).collect()
+    }
+
+    /// A settlement arm of `NativeProofManager::handle_proof_job` (native_proof_manager.rs:514-660) as ONE pool job
+    /// (`b200_pool_submit_settlement`): `singleprover_prove_with_hint` of the settlement statement, then `link_proofs(hint,
+    /// &settlement_hint, layout)` for every stored hint the job brings (validity hint first, intent_and_balance.rs:57-72),
+    /// as one link batch that reads the settlement hint from device memory.  The proof and link proofs equal
+    /// `prove_with_link_hint` + `link_proofs` with the same rng draws.  A stale hint (one that differs from the
+    /// settlement on its group) or an unsatisfied witness is `WrongQuotientPolyDegree`; `b200_last_error` names the link.
+    pub fn prove_settlement<R: rand::RngCore + rand::CryptoRng>(
+        &self, rng: &mut R, cs: &PlonkCircuit<Fr>, pk: &GpuProvingKey, hints: &[(&LinkingHint<Bn254>, &GroupLayout)],
+    ) -> Result<(Proof<Bn254>, Vec<mpc_plonk::proof_system::structs::LinkingProof<Bn254>>), PlonkError> {
+        let wires: Vec<u64> = cs.witness_table().iter().flat_map(|col| col.iter().flat_map(fr_limbs)).collect(); // 5 x n
+        let pub_inputs: Vec<u64> = cs.public_input()?.iter().flat_map(fr_limbs).collect();
+        let blinders: Vec<u64> = (0..17).map(|_| Fr::rand(rng)).flat_map(|f| fr_limbs(&f)).collect();
+        self.settle(hints, |raw, links, statuses, ticket| unsafe {
+            let proof = ffi::b200_bundle_proof { pk: pk.raw, wires: wires.as_ptr(), pub_inputs: pub_inputs.as_ptr(),
+                                                 num_inputs: pk.num_inputs, blinders: blinders.as_ptr(), proof: raw,
+                                                 link_poly: std::ptr::null_mut() };
+            ffi_settlement::b200_pool_submit_settlement(self.pool, self.srs, &proof, links.as_ptr(), links.len(), statuses, ticket)
+        })
+    }
+
+    /// `prove_settlement` for a key made by `preprocess_wiring`: only the witness vector crosses the boundary
+    /// (`b200_pool_submit_settlement_witness`).
+    pub fn prove_settlement_from_witness<R: rand::RngCore + rand::CryptoRng>(
+        &self, rng: &mut R, cs: &PlonkCircuit<Fr>, pk: &GpuProvingKey, hints: &[(&LinkingHint<Bn254>, &GroupLayout)],
+    ) -> Result<(Proof<Bn254>, Vec<mpc_plonk::proof_system::structs::LinkingProof<Bn254>>), PlonkError> {
+        let witness: Vec<u64> = cs.witness().iter().flat_map(fr_limbs).collect(); // num_vars
+        if witness.len() != 4 * unsafe { ffi::b200_pk_num_vars(pk.raw) } {
+            return Err(PlonkError::InvalidParameters("witness length differs from the key's num_vars".into()));
+        }
+        let blinders: Vec<u64> = (0..17).map(|_| Fr::rand(rng)).flat_map(|f| fr_limbs(&f)).collect();
+        self.settle(hints, |raw, links, statuses, ticket| unsafe {
+            let proof = ffi::b200_bundle_witness { pk: pk.raw, witness: witness.as_ptr(), blinders: blinders.as_ptr(), proof: raw,
+                                                   link_poly: std::ptr::null_mut(), pub_inputs_out: std::ptr::null_mut() };
+            ffi_settlement::b200_pool_submit_settlement_witness(self.pool, self.srs, &proof, links.as_ptr(), links.len(), statuses, ticket)
+        })
+    }
+
+    /// The part both settlement wrappers share: the link array, the submission (`submit`), the wait and the results.
+    #[allow(clippy::type_complexity)]
+    fn settle(&self, hints: &[(&LinkingHint<Bn254>, &GroupLayout)],
+              submit: impl FnOnce(*mut ffi::b200_proof, &[ffi_settlement::b200_settlement_link], *mut c_int, *mut u64) -> c_int)
+        -> Result<(Proof<Bn254>, Vec<mpc_plonk::proof_system::structs::LinkingProof<Bn254>>), PlonkError> {
+        let k = hints.len();
+        let polys: Vec<Vec<u64>> = hints.iter().map(|(h, _)| h.linking_wire_poly.coeffs.iter().flat_map(fr_limbs).collect()).collect();
+        let comms: Vec<[u64; 8]> = hints.iter().map(|(h, _)| g1_record(&h.linking_wire_comm.0)).collect();
+        let mut raws: Vec<ffi::b200_link_proof> = (0..k).map(|_| unsafe { std::mem::zeroed() }).collect();
+        let links: Vec<ffi_settlement::b200_settlement_link> = (0..k).map(|i| ffi_settlement::b200_settlement_link {
+            hint_poly: polys[i].as_ptr(), hint_len: polys[i].len() / 4, hint_comm: comms[i].as_ptr(),
+            alignment: hints[i].1.alignment as c_uint, offset: hints[i].1.offset, size: hints[i].1.size, proof: &mut raws[i],
+            eta: std::ptr::null_mut(),
+        }).collect();
+        let mut raw: ffi::b200_proof = unsafe { std::mem::zeroed() };
+        let mut statuses: Vec<c_int> = vec![0; k + 1];
+        let mut ticket = 0u64;
+        check(submit(&mut raw, &links, statuses.as_mut_ptr(), &mut ticket))?;
+        check(unsafe { ffi::b200_pool_wait(self.pool, ticket) })?; // buffers above stay alive until here
+        let proofs = raws.iter().map(|r| mpc_plonk::proof_system::structs::LinkingProof {
+            quotient_commitment: jf_primitives::pcs::prelude::Commitment(g1_from(&r.quotient_commitment)),
+            opening_proof: jf_primitives::pcs::prelude::UnivariateKzgProof { proof: g1_from(&r.opening_proof) },
+        }).collect();
+        Ok((proof_from_raw(&raw), proofs))
     }
 
     /// Many `verify` / `verify_link_proof` checks with ONE pairing on this GPU (`b200_plonk_batch_verify`).

@@ -1,10 +1,11 @@
-"""ctypes binding of libb200prover.so, derived from its C ABI, include/b200prover.h and include/b200settlement.h.
+"""ctypes binding of libb200prover.so, derived from its C ABI, include/b200prover.h, include/b200settlement.h and
+include/b200verifyjobs.h.
 
 The headers are parsed once, at import, and are the only description of the ABI here: `EXPORTS` lists the core
-header's entry points in header order, `SETTLEMENT_EXPORTS` those of the settlement header, `B200_OK` / `B200_ERR_*` are
-the core header's `#define`s, `STRUCTS` holds one ctypes class per struct of either header (by C name), and `load()`
-gives every entry point the argtypes / restype of its declaration.  tools/gen_rust_ffi.py writes the Rust
-shim's ffi.rs from the same parse, and tests/test_abi_cpu.py checks the parse, the struct layouts and the scalar types
+header's entry points in header order, `SETTLEMENT_EXPORTS` those of the settlement header, `VERIFY_JOB_EXPORTS` those of
+the verification-job header, `B200_OK` / `B200_ERR_*` are the core header's `#define`s, `STRUCTS` holds one ctypes
+class per struct of any header (by C name), and `load()` gives every entry point the argtypes / restype of its
+declaration.  tools/gen_rust_ffi.py writes the Rust shim's ffi*.rs modules from the same parse, and tests/test_abi_cpu.py checks the parse, the struct layouts and the scalar types
 against a C compiler.
 
 The library is built in-tree by `__graft_entry__.build()` / `make -C renegade_b200/csrc`.
@@ -20,6 +21,7 @@ import re
 _HERE = os.path.dirname(os.path.abspath(__file__))
 HEADER = os.path.join(os.path.dirname(_HERE), "include", "b200prover.h")
 SETTLEMENT_HEADER = os.path.join(os.path.dirname(_HERE), "include", "b200settlement.h")
+VERIFY_JOB_HEADER = os.path.join(os.path.dirname(_HERE), "include", "b200verifyjobs.h")
 # B200_LIB_PATH: developer knob to load an alternative build of the same library (tuning experiments)
 LIB_PATH = os.environ.get("B200_LIB_PATH") or os.path.join(_HERE, "libb200prover.so")
 
@@ -92,16 +94,19 @@ def _struct(name: str, fields) -> type:
     return type(name, (C.Structure,), {"_fields_": members})
 
 
-for _h in (HEADER, SETTLEMENT_HEADER):
+for _h in (HEADER, SETTLEMENT_HEADER, VERIFY_JOB_HEADER):
     if not os.path.exists(_h):
         raise ImportError(f"{_h} is missing: the binding of libb200prover is derived from it")
 _, _structs, _funcs, _codes = parse_header()
 _, _s_structs, _s_funcs, _ = parse_header(SETTLEMENT_HEADER)
+_, _v_structs, _v_funcs, _ = parse_header(VERIFY_JOB_HEADER)
 globals().update(_codes)  # B200_OK, B200_ERR_INVALID, ..., B200_ERR_UNSATISFIED
 EXPORTS = [name for name, _, _ in _funcs]
 SETTLEMENT_EXPORTS = [name for name, _, _ in _s_funcs]
-STRUCTS = {name: _struct(name, fields) for name, fields in {**_structs, **_s_structs}.items()}
-_SIGNATURES = {name: ([_ctype(t) for _, t in args], _ctype(ret, ret=True)) for name, ret, args in _funcs + _s_funcs}
+VERIFY_JOB_EXPORTS = [name for name, _, _ in _v_funcs]
+STRUCTS = {name: _struct(name, fields) for name, fields in {**_structs, **_s_structs, **_v_structs}.items()}
+_SIGNATURES = {name: ([_ctype(t) for _, t in args], _ctype(ret, ret=True))
+               for name, ret, args in _funcs + _s_funcs + _v_funcs}
 
 
 class B200Error(RuntimeError):

@@ -1123,6 +1123,36 @@ def _bundle_table_arrays(proofs, links, resolve, where: str):
 
 
 @dataclass
+class _PoolVerify:
+    """What a queued verification job writes into: the verdicts, and the combined answer in combined mode."""
+    batch: "_VerifyBatch"
+    verdicts: Any
+    ok: Any  # c_int in combined mode, else None
+
+
+def _submit_verify(submit, vks, pub_inputs, proofs, links, combined: bool, g2):
+    """One verification job through `submit` (`b200_pool_submit_verify` or `b200_box_submit_verify` with its handle
+    bound): -> (ticket, _PoolVerify).  The C call copies every input, so only the outputs have to live until the wait."""
+    b = _VerifyBatch(vks, pub_inputs, proofs, links, g2)
+    if not hasattr(b, "args"):  # no items and no G2 pair: a job still checks its G2 records
+        raise ValueError("a verification job without items needs g2=(g2_h, g2_tau_h)")
+    verdicts = (C.c_uint8 * max(1, b.n_c))()
+    ok = C.c_int(0) if combined else None
+    ticket = C.c_uint64()
+    _lib.check(submit(int(combined), *b.args, C.byref(ok) if combined else None, verdicts, C.byref(ticket)))
+    return ticket.value, _PoolVerify(b, verdicts, ok)
+
+
+def _verify_results(v: _PoolVerify, rc: int):
+    """What `verify_each` (a verdict list) or `batch_verify` ((all_ok, verdicts)) returns for the same items."""
+    _lib.check(rc)
+    verdicts = v.batch.verdicts(v.verdicts)
+    if v.ok is None:
+        return verdicts
+    return bool(v.ok.value) and len(v.batch.c_proofs) == v.batch.n_proofs, verdicts
+
+
+@dataclass
 class _PoolBatch:
     """What a queued batch job writes into: its items' arrays and outputs, and the statuses."""
     held: list
@@ -1339,12 +1369,24 @@ class ProverPool:
         self._keep[ticket.value] = (_PoolSettlement(proof, out, st, pub, [wit, bl, arr, held, keep]), None, None, (pk, srs))
         return ticket.value
 
+    def submit_verify(self, vks, pub_inputs, proofs, links=(), combined: bool = False, g2=None) -> int:
+        """Queue one verification job on some worker (`b200_pool_submit_verify`); returns the ticket.  Arguments as
+        `PlonkKzgSnark.verify_each` / `.batch_verify` take them; every input is copied at submit.  `wait(ticket)` returns
+        what `verify_each` returns (the verdict list), or with `combined` what `batch_verify` returns ((all_ok,
+        verdicts): one combined pairing, the failing items found by bisection inside the job)."""
+        ticket, job = _submit_verify(lambda *a: self._lib.b200_pool_submit_verify(self._h, *a), vks, pub_inputs, proofs,
+                                     links, combined, g2)
+        self._keep[ticket] = (job, None, None, None)
+        return ticket
+
     def wait(self, ticket: int):
         """Blocks until the job is done; returns its B200Proof (or (B200Proof, link_poly) when the job was
         submitted with `with_link_poly`, or the B200LinkProof of a link job); raises B200Error with the
         job's own status and message if it failed."""
         rc = self._lib.b200_pool_wait(self._h, ticket)
         proof, link, _, _ = self._keep.pop(ticket, (None, None, None, None))
+        if isinstance(proof, _PoolVerify):
+            return _verify_results(proof, rc)
         if isinstance(proof, _PoolSettlement):  # a settlement: refused links and an unsatisfied proof are in its statuses
             return _settlement_results(proof, rc)
         if isinstance(proof, (_PoolBatch, _PoolLinkBatch)):  # a batch job: refused items are reported in its statuses
@@ -1524,6 +1566,14 @@ class ProverBox:
         self._keep[ticket.value] = (_PoolSettlement(proof, out, st, pub, [wit, bl, arr, held, keep]), None)
         return ticket.value
 
+    def submit_verify(self, vks, pub_inputs, proofs, links=(), combined: bool = False, g2=None) -> int:
+        """`ProverPool.submit_verify` on the least-loaded device (`b200_box_submit_verify`).  `wait(ticket)` returns the
+        verdict list, or (all_ok, verdicts) with `combined`."""
+        ticket, job = _submit_verify(lambda *a: self._lib.b200_box_submit_verify(self._h, *a), vks, pub_inputs, proofs,
+                                     links, combined, g2)
+        self._keep[ticket] = (job, None)
+        return ticket
+
     def verifying_key(self, pk):
         sel, sig = np.zeros((13, 8), dtype=np.uint64), np.zeros((5, 8), dtype=np.uint64)
         _lib.check(self._lib.b200_box_pk_verifying_key(pk, _ptr(sel), _ptr(sig)))
@@ -1544,6 +1594,8 @@ class ProverBox:
     def wait(self, ticket: int):
         rc = self._lib.b200_box_wait(self._h, ticket)
         proof, link, *_ = self._keep.pop(ticket, (None, None))
+        if isinstance(proof, _PoolVerify):
+            return _verify_results(proof, rc)
         if isinstance(proof, _PoolSettlement):
             return _settlement_results(proof, rc)
         _lib.check(rc)

@@ -385,18 +385,25 @@ def verify_singleprover_proof(circuit: type, statement, proof: PlonkProof) -> No
     circuit.verify(statement, proof)
 
 
-def batch_verify_singleprover_proofs(items) -> None:
+def batch_verify_singleprover_proofs(items, pool=None, box=None) -> None:
     """`verify_singleprover_proof` for many (circuit, statement, proof) triples at once: one batch check with ONE
-    pairing on the `SYSTEM_SRS` context's device (`PlonkKzgSnark.batch_verify`).  Raises VerifierError naming the
-    indices of the proofs that fail."""
+    pairing on the `SYSTEM_SRS` context's device (`PlonkKzgSnark.batch_verify`), or, given a `ProverPool` as `pool` or a
+    `ProverBox` as `box`, the same check as one verification job on it (`submit_verify(..., combined=True)`), beside the
+    proofs it is making.  Raises VerifierError naming the indices of the proofs that fail."""
     items = list(items)
     if not items:
         return
-    srs = system_srs()
+    if pool is not None and box is not None:
+        raise ValueError("batch_verify_singleprover_proofs: pass a pool or a box, not both")
     vks = [c.verifying_key() for c, _, _ in items]
     pis = [c.statement_scalars(s) for c, s, _ in items]
+    proofs = [p for _, _, p in items]
     try:
-        _, verdicts = PlonkKzgSnark.batch_verify(srs.ctx, vks, pis, [p for _, _, p in items])
+        if pool is not None or box is not None:
+            jobs = pool if pool is not None else box
+            _, verdicts = jobs.wait(jobs.submit_verify(vks, pis, proofs, combined=True))
+        else:
+            _, verdicts = PlonkKzgSnark.batch_verify(system_srs().ctx, vks, pis, proofs)
     except _lib.B200Error as e:
         raise VerifierError(f"Plonk({e})") from e
     bad = [i for i, ok in enumerate(verdicts) if not ok]

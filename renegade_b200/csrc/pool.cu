@@ -4,7 +4,8 @@
 // 138-201: a rayon pool fed with `spawn_fifo` from the job queue, one proof per worker): proving
 // keys and SRS tables are shared read-only by all workers, so several proofs are in flight on one
 // GPU and the latency-bound kernels of one proof (bucket reductions, scans, the host transcript)
-// overlap the throughput-bound kernels of the others.
+// overlap the throughput-bound kernels of the others.  Verification jobs (b200verifyjobs.h) run the device verifiers
+// on a worker's context in the same queue, so a caller that checks proofs on a proving GPU needs no context of its own.
 //
 // Host-only code (std::thread) above the same C ABI the single-context entry points use.
 #include <algorithm>
@@ -19,14 +20,76 @@
 
 #include "b200prover.h"
 #include "b200settlement.h"
+#include "b200verifyjobs.h"
 #include "device_ctx.h"
 
 namespace {
 
 struct Bundle;
 
+// The inputs of a verification job, copied at submit: the arrays with every pointer into the copies below, so the
+// caller may free or reuse its own as soon as the submit returns.
+struct VerifyCopy {
+    int mode = 0;  // 0: b200_plonk_verify_each, 1: b200_plonk_batch_verify
+    std::vector<b200_verifying_key> vks;
+    std::vector<b200_batch_proof> proofs;
+    std::vector<b200_batch_link> links;
+    std::vector<uint64_t> limbs;  // each key's k / selector / sigma, each proof's public inputs, each link's comm1 / comm2
+    std::vector<b200_proof> proof_bodies;
+    std::vector<b200_link_proof> link_bodies;
+    uint64_t g2_h[16], g2_tau_h[16];
+    int* all_accepted = nullptr;  // the caller's outputs
+    uint8_t* verdicts = nullptr;
+
+    VerifyCopy(int m, const b200_verifying_key* v, size_t n_v, const b200_batch_proof* p, size_t n_p, const b200_batch_link* l,
+               size_t n_l, const uint64_t* h, const uint64_t* tau_h)
+        : mode(m), vks(v, v + n_v), proofs(p, p + n_p), links(l, l + n_l), proof_bodies(n_p), link_bodies(n_l) {
+        size_t total = (20 + 104 + 40) * n_v + 16 * n_l;
+        for (size_t i = 0; i < n_p; ++i) total += 4 * v[p[i].vk].num_inputs;
+        limbs.resize(total);  // sized once: the pointers below stay valid
+        uint64_t* at = limbs.data();
+        auto take = [&at](const uint64_t* src, size_t n) {
+            std::memcpy(at, src, 8 * n);
+            const uint64_t* out = at;
+            at += n;
+            return out;
+        };
+        for (b200_verifying_key& vk : vks) {
+            vk.k = take(vk.k, 20);
+            vk.selector_comms = take(vk.selector_comms, 104);
+            vk.sigma_comms = take(vk.sigma_comms, 40);
+        }
+        for (size_t i = 0; i < n_p; ++i) {
+            const size_t ni = vks[proofs[i].vk].num_inputs;
+            proofs[i].pub_inputs = ni ? take(proofs[i].pub_inputs, 4 * ni) : nullptr;
+            proof_bodies[i] = *proofs[i].proof;
+            proofs[i].proof = &proof_bodies[i];
+        }
+        for (size_t i = 0; i < n_l; ++i) {
+            links[i].comm1 = take(links[i].comm1, 8);
+            links[i].comm2 = take(links[i].comm2, 8);
+            link_bodies[i] = *links[i].proof;
+            links[i].proof = &link_bodies[i];
+        }
+        std::memcpy(g2_h, h, 128);
+        std::memcpy(g2_tau_h, tau_h, 128);
+    }
+
+    int run(b200_ctx* ctx) const {
+        if (mode == 0)
+            return b200_plonk_verify_each(ctx, vks.data(), vks.size(), proofs.data(), proofs.size(), links.data(), links.size(),
+                                          g2_h, g2_tau_h, verdicts);
+        int all = 0;
+        const int rc = b200_plonk_batch_verify(ctx, vks.data(), vks.size(), proofs.data(), proofs.size(), links.data(),
+                                               links.size(), g2_h, g2_tau_h, &all, verdicts);
+        if (all_accepted) *all_accepted = all;
+        return rc;
+    }
+};
+
 struct Job {
-    enum Kind { kProve, kProveWitness, kProveBatch, kProveWitnessBatch, kLink, kLinkBatch, kSettlement, kSettlementWitness } kind = kProve;
+    enum Kind { kProve, kProveWitness, kProveBatch, kProveWitnessBatch, kLink, kLinkBatch, kSettlement, kSettlementWitness,
+                kVerify } kind = kProve;
     uint64_t ticket = 0;
     // prove (wires: the table) and prove witness (wires: the witness vector)
     const b200_pk* pk = nullptr;
@@ -49,6 +112,8 @@ struct Job {
     // settlement (pk, wires, pub_inputs, blinders, proof, link_poly, pub_inputs_out, srs, statuses as above): the links
     // with hint_comm pointing into the copies in `link_comms` (8 limbs per link)
     std::vector<b200_settlement_link> settlement_links;
+    // verify: everything the verifier reads, owned by the job
+    std::unique_ptr<VerifyCopy> verify;
 
     void set_settlement_links(const b200_settlement_link* ls, size_t k) {  // the worker reads the copies
         settlement_links.assign(ls, ls + k);
@@ -160,6 +225,8 @@ struct b200_pool {
                                                                job->proof, job->link_poly, job->pub_inputs_out,
                                                                job->settlement_links.data(), job->settlement_links.size(),
                                                                job->statuses);
+            } else if (job->kind == Job::kVerify) {
+                d.status = job->verify->run(ctxs[w]);
             } else if (job->kind == Job::kLinkBatch) {
                 d.status = b200_plonk_link_batch(ctxs[w], job->srs, job->link_items.data(), job->link_items.size(), job->statuses);
             } else {  // a single link stays on b200_plonk_link, which replays its CUDA graphs
@@ -567,6 +634,37 @@ int b200_pool_submit_settlement_witness(b200_pool* pool, const b200_bases* srs, 
     B200_CATCH
 }
 
+int b200_pool_submit_verify(b200_pool* pool, int mode, const b200_verifying_key* vks, size_t n_vks, const b200_batch_proof* proofs,
+                            size_t n_proofs, const b200_batch_link* links, size_t n_links, const uint64_t g2_h[16],
+                            const uint64_t g2_tau_h[16], int* all_accepted, uint8_t* verdicts, uint64_t* ticket) {
+    B200_TRY
+    const char* who = "pool_submit_verify";
+    // what the verifiers' own checks (b200::verify_check) do not cover, then theirs: nothing is copied before both pass
+    const char* bad = !pool                                                      ? "null pool"
+                      : !ticket                                                  ? "null ticket"
+                      : mode != 0 && mode != 1                                   ? "mode must be 0 or 1"
+                      : n_vks && !vks                                            ? "null vks with n_vks > 0"
+                      : n_proofs && !proofs                                      ? "null proofs with n_proofs > 0"
+                      : n_links && !links                                        ? "null links with n_links > 0"
+                      : !g2_h || !g2_tau_h                                       ? "null G2 record"
+                      : n_proofs + n_links && !verdicts                          ? "null verdicts with items to verify"
+                      : n_vks > 0xffffffffu || n_proofs + n_links > 0xffffffffu ? "more than 2^32 - 1 keys or items"
+                                                                                 : nullptr;
+    if (bad) {
+        b200::set_error(std::string(who) + ": " + bad);
+        return B200_ERR_INVALID;
+    }
+    const int rc = b200::verify_check(who, vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h);
+    if (rc != B200_OK) return rc;
+    std::unique_ptr<Job> j(new Job());
+    j->kind = Job::kVerify;
+    j->verify.reset(new VerifyCopy(mode, vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h));
+    j->verify->all_accepted = all_accepted;
+    j->verify->verdicts = verdicts;
+    return pool_push(pool, std::move(j), ticket);
+    B200_CATCH
+}
+
 int b200_pool_wait(b200_pool* pool, uint64_t ticket) {
     B200_TRY
     if (!pool || ticket == 0) {
@@ -955,6 +1053,24 @@ int b200_box_submit_settlement_witness(b200_box* box, const b200_box_srs* srs, c
     local.pk = pk->per_dev[d];
     uint64_t t = 0;
     rc = b200_pool_submit_settlement_witness(box->pools[d], srs->per_dev[d], &local, links, n_links, statuses, &t);
+    if (rc != B200_OK) return rc;
+    *ticket = ((uint64_t)d << kBoxTicketShift) | t;
+    return B200_OK;
+    B200_CATCH
+}
+
+int b200_box_submit_verify(b200_box* box, int mode, const b200_verifying_key* vks, size_t n_vks, const b200_batch_proof* proofs,
+                           size_t n_proofs, const b200_batch_link* links, size_t n_links, const uint64_t g2_h[16],
+                           const uint64_t g2_tau_h[16], int* all_accepted, uint8_t* verdicts, uint64_t* ticket) {
+    B200_TRY
+    if (!box || !ticket) {
+        b200::set_error("box_submit_verify: null box or ticket");
+        return B200_ERR_INVALID;
+    }
+    const int d = box_least_loaded(box);  // the job reads only its host copies: any device will do
+    uint64_t t = 0;
+    const int rc = b200_pool_submit_verify(box->pools[d], mode, vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h,
+                                           all_accepted, verdicts, &t);
     if (rc != B200_OK) return rc;
     *ticket = ((uint64_t)d << kBoxTicketShift) | t;
     return B200_OK;

@@ -386,7 +386,7 @@ struct Batch {
     }
 
     // Staging, uploads, k_prepare and the inversion of the denominators, for k >= 1 items whose arguments passed
-    // check_items: what both entry points run first.
+    // verify_check: what both entry points run first.
     int stage(const b200_verifying_key* in_vks, size_t n_vks, const b200_batch_proof* in_proofs, size_t n_proofs,
               const b200_batch_link* in_links, size_t n_links) {
         cudaStream_t st = c->stream;
@@ -507,24 +507,27 @@ bool args_present(const b200_ctx* ctx, const b200_verifying_key* vks, size_t n_v
            n_vks <= 0xffffffffu && n_proofs + n_links <= 0xffffffffu;
 }
 
-// The entries' argument checks of both entry points; b200_last_error() names `who`
-int check_items(const char* who, const b200_verifying_key* vks, size_t n_vks, const b200_batch_proof* proofs,
-                size_t n_proofs, const b200_batch_link* links, size_t n_links, const uint64_t g2_h[16],
-                const uint64_t g2_tau_h[16]) {
+}  // namespace
+
+// The entries' argument checks of both entry points and of a verification job at submit; b200_last_error() names `who`
+// and the entry
+int verify_check(const char* who, const b200_verifying_key* vks, size_t n_vks, const b200_batch_proof* proofs,
+                 size_t n_proofs, const b200_batch_link* links, size_t n_links, const uint64_t g2_h[16],
+                 const uint64_t g2_tau_h[16]) {
     const std::string w(who);
     for (size_t v = 0; v < n_vks; ++v)
         if (vks[v].log_n > kMaxAlign || !vks[v].k || !vks[v].selector_comms || !vks[v].sigma_comms) {
-            set_error(w + ": bad verifying key");
+            set_error(w + ": bad verifying key " + std::to_string(v) + " (log_n above 28 or a NULL pointer)");
             return B200_ERR_INVALID;
         }
     for (size_t p = 0; p < n_proofs; ++p)
         if (proofs[p].vk >= n_vks || !proofs[p].proof || (vks[proofs[p].vk].num_inputs && !proofs[p].pub_inputs)) {
-            set_error(w + ": bad proof entry (vk index, proof or public inputs)");
+            set_error(w + ": bad proof entry " + std::to_string(p) + " (vk index, proof or public inputs)");
             return B200_ERR_INVALID;
         }
     for (size_t l = 0; l < n_links; ++l)
         if (!links[l].comm1 || !links[l].comm2 || !links[l].proof || links[l].alignment > kMaxAlign || links[l].size == 0) {
-            set_error(w + ": bad link entry");
+            set_error(w + ": bad link entry " + std::to_string(l) + " (alignment above 28, size 0 or a NULL pointer)");
             return B200_ERR_INVALID;
         }
     if (!g2_records_on_curve(g2_tau_h, g2_h)) {
@@ -533,8 +536,6 @@ int check_items(const char* who, const b200_verifying_key* vks, size_t n_vks, co
     }
     return B200_OK;
 }
-
-}  // namespace
 
 }  // namespace b200
 
@@ -547,7 +548,7 @@ extern "C" int b200_plonk_batch_verify(b200_ctx* ctx, const b200_verifying_key* 
     if (!args_present(ctx, vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h) || !all_accepted)
         return B200_ERR_INVALID;
     *all_accepted = 0;
-    int rc = check_items("batch_verify", vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h);
+    int rc = verify_check("batch_verify", vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h);
     if (rc != B200_OK) return rc;
     const size_t k = n_proofs + n_links;
     if (k == 0) {
@@ -611,9 +612,9 @@ extern "C" int b200_plonk_verify_each(b200_ctx* ctx, const b200_verifying_key* v
     const size_t k = n_proofs + n_links;
     if (!args_present(ctx, vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h) || (k && !verdicts))
         return B200_ERR_INVALID;
-    int rc = check_items("verify_each", vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h);
+    int rc = verify_check("verify_each", vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h);
     if (rc != B200_OK || k == 0) return rc;
-    // Q = ([tau]_2, [1]_2), prepared on the host (both are on the curve: check_items)
+    // Q = ([tau]_2, [1]_2), prepared on the host (both are on the curve: verify_check)
     std::vector<G2Prepared> q(2);
     g2_prepare_record(g2_tau_h, &q[0]);
     g2_prepare_record(g2_h, &q[1]);

@@ -11,6 +11,7 @@
 //! | `proof_linking/intent_only.rs:42-47` | `PlonkKzgSnark::link_proofs::<SolidityTranscript>(a, b, &layout, &ck)` | [`GpuProver::link_proofs`] |
 //! | `native_proof_manager.rs:726-782` | the four `link_proofs` calls of `compute_private_settlement_link_proofs` | [`GpuProver::link_proofs_batch`] |
 //! | `native_proof_manager.rs:514-660` | a settlement arm: `singleprover_prove_with_hint`, then `link_proofs` against each stored hint | [`GpuProver::prove_settlement`], [`GpuProver::prove_settlement_from_witness`] |
+//! | `gossip-server/src/orderbook.rs:180-229` | the order check: two proofs and one link proof per order (`todo!` upstream) | [`GpuProver::submit_verify`], [`GpuProver::submit_verify_combined`] |
 //! | `primitives/srs.rs:63-71` | `parse_ptau_file` + `powers_of_g` | [`GpuProver::load_srs`] |
 //!
 //! Marshalling rules (SURVEY.md §7 "Rust ABI hazards"): `Fr`/`Fq` are `Fp(BigInt<4>, PhantomData)` holding the
@@ -25,6 +26,7 @@
 #![allow(unsafe_code)]
 pub mod ffi;
 pub mod ffi_settlement;
+pub mod ffi_verifyjobs;
 
 use ark_bn254::{Bn254, Fq, Fr, G1Affine};
 use ark_ff::{BigInt, UniformRand};
@@ -413,6 +415,52 @@ impl GpuProver {
         Ok(verdicts.into_iter().map(|v| v == 1).collect())
     }
 
+    /// `verify_each` as ONE job on this GPU's pool (`b200_pool_submit_verify`, mode 0): a worker runs it on its own
+    /// context next to the proofs, so a caller that verifies while the pool proves needs no context of its own.  Every
+    /// input is copied at submit; the ticket owns the verdict buffer.  `wait_verify` returns the verdicts.
+    #[allow(clippy::type_complexity)]
+    pub fn submit_verify(&self, vks: &[BatchVerifyingKey], proofs: &[(usize, &[Fr], &Proof<Bn254>)],
+                         links: &[(&G1Affine, &G1Affine, &mpc_plonk::proof_system::structs::LinkingProof<Bn254>, &GroupLayout)],
+                         g2_h: &[u64; 16], g2_tau_h: &[u64; 16]) -> Result<VerifyTicket<'_>, PlonkError> {
+        self.submit_verify_mode(0, vks, proofs, links, g2_h, g2_tau_h)
+    }
+
+    /// `batch_verify` as ONE pool job (`b200_pool_submit_verify`, mode 1): one combined pairing, the failing items found
+    /// by bisection inside the job.  `wait_verify` returns the verdicts and whether every item was accepted.
+    #[allow(clippy::type_complexity)]
+    pub fn submit_verify_combined(&self, vks: &[BatchVerifyingKey], proofs: &[(usize, &[Fr], &Proof<Bn254>)],
+                                  links: &[(&G1Affine, &G1Affine, &mpc_plonk::proof_system::structs::LinkingProof<Bn254>, &GroupLayout)],
+                                  g2_h: &[u64; 16], g2_tau_h: &[u64; 16]) -> Result<VerifyTicket<'_>, PlonkError> {
+        self.submit_verify_mode(1, vks, proofs, links, g2_h, g2_tau_h)
+    }
+
+    #[allow(clippy::type_complexity)]
+    fn submit_verify_mode(&self, mode: c_int, vks: &[BatchVerifyingKey], proofs: &[(usize, &[Fr], &Proof<Bn254>)],
+                          links: &[(&G1Affine, &G1Affine, &mpc_plonk::proof_system::structs::LinkingProof<Bn254>, &GroupLayout)],
+                          g2_h: &[u64; 16], g2_tau_h: &[u64; 16]) -> Result<VerifyTicket<'_>, PlonkError> {
+        let mut t = VerifyTicket { pool: self.pool, ticket: 0, waited: true, combined: mode == 1, all: Box::new(0),
+                                   verdicts: vec![0u8; proofs.len() + links.len()].into_boxed_slice(),
+                                   _prover: std::marker::PhantomData };
+        let (all, verdicts): (*mut c_int, *mut u8) = (&mut *t.all, t.verdicts.as_mut_ptr());
+        with_batch(vks, proofs, links, |c_vks, c_proofs, c_links| check(unsafe {
+            ffi_verifyjobs::b200_pool_submit_verify(self.pool, mode, c_vks.as_ptr(), c_vks.len(), c_proofs.as_ptr(),
+                                                    c_proofs.len(), c_links.as_ptr(), c_links.len(), g2_h.as_ptr(),
+                                                    g2_tau_h.as_ptr(), all, verdicts, &mut t.ticket)
+        }))?;
+        t.waited = false;
+        Ok(t)
+    }
+
+    /// Waits for a verification job: (every item accepted, verdicts proofs first, then links).  The first value is
+    /// the combined check's answer for `submit_verify_combined`, and whether every verdict is true for `submit_verify`.
+    pub fn wait_verify(&self, mut t: VerifyTicket<'_>) -> Result<(bool, Vec<bool>), PlonkError> {
+        t.waited = true;
+        check(unsafe { ffi::b200_pool_wait(self.pool, t.ticket) })?;
+        let verdicts: Vec<bool> = t.verdicts.iter().map(|v| *v == 1).collect();
+        let all = if t.combined { *t.all == 1 } else { verdicts.iter().all(|v| *v) };
+        Ok((all, verdicts))
+    }
+
     /// Checks the first `n` powers of the loaded SRS against `(g2_h, g2_tau_h)` on this GPU (`b200_srs_check`): one
     /// batch-2 MSM and one pairing, with weights drawn from `seed`, which must be unknown to whoever made the file.
     /// With `locate`, a failed check also names the failing pairs (P_i, P_{i+1}).  Valid exactly when
@@ -462,6 +510,27 @@ fn with_batch<R>(vks: &[BatchVerifyingKey], proofs: &[(usize, &[Fr], &Proof<Bn25
         comm1: a.as_ptr(), comm2: b.as_ptr(), alignment: lay.alignment as c_uint, offset: lay.offset, size: lay.size, proof: lp,
     }).collect();
     f(&c_vks, &c_proofs, &c_links)
+}
+
+/// A queued verification job: it owns the buffers the worker writes (the verdicts, the combined answer), so it waits
+/// for its job when dropped unwaited; it cannot outlive the `GpuProver` whose pool runs the job.
+pub struct VerifyTicket<'a> {
+    pool: *mut ffi::b200_pool,
+    ticket: u64,
+    waited: bool,
+    combined: bool,
+    all: Box<c_int>,
+    verdicts: Box<[u8]>,
+    _prover: std::marker::PhantomData<&'a GpuProver>,
+}
+unsafe impl Send for VerifyTicket<'_> {}
+
+impl Drop for VerifyTicket<'_> {
+    fn drop(&mut self) {
+        if !self.waited {
+            unsafe { ffi::b200_pool_wait(self.pool, self.ticket) };
+        }
+    }
 }
 
 /// The flat verifying key of one circuit, as `verify` takes it.

@@ -657,6 +657,8 @@ int b200_fr_poly_eval_device(b200_ctx* ctx, const void* d_coeffs, size_t len, co
 int b200_fr_poly_div_linear_device(b200_ctx* ctx, const void* d_p, size_t len, const uint64_t z[4], void* d_q);
 
 /* ---- witness-side batch hashing (SURVEY.md §8(f) f4) ------------------------------------- */
+/* Every field element these four calls read (states, inputs, leaf hashes, sisters, seeds) must be a canonical
+ * Montgomery residue, i.e. < r as a 256-bit integer: the kernels' reductions assume it and do not check it. */
 /* `batch` independent Poseidon2 sponge hashes of `len` scalars each (inputs: batch x len x 4
  * limbs, Montgomery; out: batch x 4 limbs; host or device pointers).  Each equals the reference's
  * `compute_poseidon_hash(&values)` / `Poseidon2Sponge::new().hash(&values)`

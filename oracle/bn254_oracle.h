@@ -66,6 +66,14 @@ int orc_msm_window_bits(size_t n);
 void orc_ntt(uint64_t* data, unsigned log_n, int inverse, int coset);
 void orc_domain_generator(unsigned log_n, uint64_t out_mont[4]);
 
+/* --- Poseidon2, t = 3 (crates/crypto/src/hash/poseidon2.rs:25-209; poseidon2_oracle.c) ----------------- */
+/* full_rc: 24 x 4 limbs, partial_rc: 56 x 4 limbs, both Montgomery; states / inputs / out Montgomery. */
+/* `batch` permutations of 3-element states, in place */
+void orc_poseidon2_permute_batch(uint64_t* states, size_t batch, const uint64_t* full_rc, const uint64_t* partial_rc);
+/* out[i] = sponge hash of inputs[i * len .. (i + 1) * len) (absorb at rate 2, one squeeze) */
+void orc_poseidon2_hash_batch(const uint64_t* inputs, size_t batch, size_t len, const uint64_t* full_rc,
+                              const uint64_t* partial_rc, uint64_t* out);
+
 int orc_num_threads(void);
 void orc_set_num_threads(int n);
 

@@ -191,6 +191,71 @@ def autotune_threads(candidates=None) -> int:
 
 
 # ---------------------------------------------------------------------------------------------
+# Poseidon2, t = 3 (poseidon2_oracle.c).  Arrays are Montgomery limbs, like the device calls'.
+# ---------------------------------------------------------------------------------------------
+POSEIDON2_FIXTURE = os.path.join(os.path.dirname(_HERE), "tests", "golden", "poseidon2.json")
+_p2_rc = None
+
+
+def poseidon2_round_constants():
+    """(full (24, 4), partial (56, 4)) Montgomery round constants, read from the fixture (not from the product)."""
+    global _p2_rc
+    if _p2_rc is None:
+        import json
+        with open(POSEIDON2_FIXTURE) as f:
+            d = json.load(f)
+        full = ints_to_array([int(v, 16) for v in d["full_round_constants"]])
+        partial = ints_to_array([int(v, 16) for v in d["partial_round_constants"]])
+        assert full.shape == (24, 4) and partial.shape == (56, 4)
+        _p2_rc = (array_to_mont(FR, full), array_to_mont(FR, partial))
+    return _p2_rc
+
+
+def poseidon2_permute_batch(states: np.ndarray) -> np.ndarray:
+    """(batch, 3, 4) states -> permuted copy."""
+    out = np.array(states, dtype=np.uint64, copy=True, order="C").reshape(-1, 3, 4)
+    full, partial = poseidon2_round_constants()
+    lib().orc_poseidon2_permute_batch(_p(out), C.c_size_t(out.shape[0]), _p(full), _p(partial))
+    return out
+
+
+def poseidon2_hash_batch(values: np.ndarray) -> np.ndarray:
+    """(batch, len, 4) -> (batch, 4): one sponge hash per row (len may be 0)."""
+    v = np.ascontiguousarray(values, dtype=np.uint64)
+    batch, ln = v.shape[0], v.shape[1]
+    out = np.zeros((batch, 4), dtype=np.uint64)
+    if batch == 0:
+        return out
+    full, partial = poseidon2_round_constants()
+    lib().orc_poseidon2_hash_batch(_p(v) if v.size else None, C.c_size_t(batch), C.c_size_t(ln), _p(full), _p(partial),
+                                   _p(out))
+    return out
+
+
+def poseidon2_merkle_roots(leaves: np.ndarray, sisters: np.ndarray, is_right: np.ndarray) -> np.ndarray:
+    """leaves (batch, 4), sisters (batch, height, 4), is_right (batch, height) -> (batch, 4): per level one batched
+    two-to-one hash, H(sister, cur) where is_right != 0, else H(cur, sister)."""
+    cur = np.ascontiguousarray(leaves, dtype=np.uint64).reshape(-1, 4)
+    sis = np.asarray(sisters, dtype=np.uint64).reshape(cur.shape[0], -1, 4)
+    right = np.asarray(is_right).reshape(cur.shape[0], sis.shape[1]) != 0
+    for lvl in range(sis.shape[1]):
+        r = right[:, lvl, None]
+        cur = poseidon2_hash_batch(np.stack([np.where(r, sis[:, lvl], cur), np.where(r, cur, sis[:, lvl])], axis=1))
+    return cur
+
+
+def poseidon2_csprng(seeds: np.ndarray, first_index, count: int) -> np.ndarray:
+    """seeds (batch, 4), first_index (batch,) -> (batch, count, 4): value j of stream s is H(seed_s, first_s + j)."""
+    sd = np.ascontiguousarray(seeds, dtype=np.uint64).reshape(-1, 4)
+    first = [int(f) for f in first_index]
+    assert len(first) == sd.shape[0] and all(0 <= f and f + count <= 1 << 64 for f in first)
+    idx = np.zeros((sd.shape[0], count, 4), dtype=np.uint64)
+    idx[:, :, 0] = np.array(first, dtype=np.uint64)[:, None] + np.arange(count, dtype=np.uint64)[None, :]
+    pairs = np.stack([np.repeat(sd[:, None], count, axis=1), array_to_mont(FR, idx)], axis=2)
+    return poseidon2_hash_batch(pairs.reshape(-1, 2, 4)).reshape(sd.shape[0], count, 4)
+
+
+# ---------------------------------------------------------------------------------------------
 # TurboPlonk prover / verifier restatement (plonk_oracle.c)
 # ---------------------------------------------------------------------------------------------
 class PlonkProof(C.Structure):

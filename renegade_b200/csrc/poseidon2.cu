@@ -140,26 +140,30 @@ __global__ void __launch_bounds__(128) k_csprng(const fe* __restrict__ seeds, co
     fe_store(out + t, hash2(fe_load_ro(seeds + sidx), fe_to_mont<Fr>(i_canon)));
 }
 
-std::once_flag g_constants_once[64];  // one upload per device, whatever context gets there first
+// one upload per device, whatever context gets there first; a failed upload leaves the flag clear and the next call
+// on that device tries again
+std::mutex g_constants_mu[64];
+bool g_constants_loaded[64];  // guarded by g_constants_mu[device]
 
 }  // namespace
 
-static int upload_constants() {
-    B200_CUDA(cudaMemcpyToSymbol(c_full_rc, kPoseidon2FullRc, sizeof(kPoseidon2FullRc)));
-    B200_CUDA(cudaMemcpyToSymbol(c_partial_rc, kPoseidon2PartialRc, sizeof(kPoseidon2PartialRc)));
+// The upload runs on the caller's stream and is waited for before the device is marked loaded: a pageable
+// cudaMemcpyToSymbol on the legacy stream may return before its DMA lands, and the legacy stream does not order the
+// non-blocking context streams the kernels run on (this one's, or another context's that waited on the lock).
+static int upload_constants(cudaStream_t st) {
+    B200_CUDA(cudaMemcpyToSymbolAsync(c_full_rc, kPoseidon2FullRc, sizeof(kPoseidon2FullRc), 0, cudaMemcpyHostToDevice, st));
+    B200_CUDA(cudaMemcpyToSymbolAsync(c_partial_rc, kPoseidon2PartialRc, sizeof(kPoseidon2PartialRc), 0,
+                                      cudaMemcpyHostToDevice, st));
+    B200_CUDA(cudaStreamSynchronize(st));
     return B200_OK;
 }
-static int load_constants(int device) {
-    if (device < 0 || device >= 64) return upload_constants();
-    int rc = B200_OK;
-    bool ran = false;
-    std::call_once(g_constants_once[device], [&] {
-        ran = true;
-        rc = upload_constants();
-    });
-    // a failed first upload leaves the flag set: retry directly (the context mutex does not cover other contexts)
-    if (!ran || rc == B200_OK) return rc;
-    return upload_constants();
+static int load_constants(int device, cudaStream_t st) {
+    if (device < 0 || device >= 64) return upload_constants(st);
+    std::lock_guard<std::mutex> lk(g_constants_mu[device]);  // the context mutex does not cover other contexts
+    if (g_constants_loaded[device]) return B200_OK;
+    const int rc = upload_constants(st);
+    if (rc == B200_OK) g_constants_loaded[device] = true;
+    return rc;
 }
 
 }  // namespace b200
@@ -174,9 +178,9 @@ int b200_poseidon2_permute_batch(b200_ctx* ctx, uint64_t* states, size_t batch) 
     if (batch == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
     B200_CUDA(cudaSetDevice(ctx->c.device));
-    int rc = load_constants(ctx->c.device);
-    if (rc != B200_OK) return rc;
     cudaStream_t st = ctx->c.stream;
+    int rc = load_constants(ctx->c.device, st);
+    if (rc != B200_OK) return rc;
     if ((rc = ctx->c.plonk_ws.reserve(batch * 3 * sizeof(fe))) != B200_OK) return rc;
     fe* d = reinterpret_cast<fe*>(ctx->c.plonk_ws.p);
     B200_CUDA(cudaMemcpyAsync(d, states, batch * 3 * sizeof(fe), cudaMemcpyDefault, st));
@@ -193,9 +197,9 @@ int b200_poseidon2_hash_batch(b200_ctx* ctx, const uint64_t* inputs, size_t batc
     if (batch == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
     B200_CUDA(cudaSetDevice(ctx->c.device));
-    int rc = load_constants(ctx->c.device);
-    if (rc != B200_OK) return rc;
     cudaStream_t st = ctx->c.stream;
+    int rc = load_constants(ctx->c.device, st);
+    if (rc != B200_OK) return rc;
     if ((rc = ctx->c.plonk_ws.reserve((batch * len + batch + 1) * sizeof(fe))) != B200_OK) return rc;
     fe* d_in = reinterpret_cast<fe*>(ctx->c.plonk_ws.p);
     fe* d_out = d_in + batch * len;
@@ -214,9 +218,9 @@ int b200_poseidon2_merkle_root_batch(b200_ctx* ctx, const uint64_t* leaf_hashes,
     if (batch == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
     B200_CUDA(cudaSetDevice(ctx->c.device));
-    int rc = load_constants(ctx->c.device);
-    if (rc != B200_OK) return rc;
     cudaStream_t st = ctx->c.stream;
+    int rc = load_constants(ctx->c.device, st);
+    if (rc != B200_OK) return rc;
     const size_t n_sis = batch * height;
     if ((rc = ctx->c.plonk_ws.reserve((2 * batch + n_sis + 1) * sizeof(fe) + n_sis + 64)) != B200_OK) return rc;
     fe* d_leaf = reinterpret_cast<fe*>(ctx->c.plonk_ws.p);
@@ -242,9 +246,9 @@ int b200_poseidon2_csprng_batch(b200_ctx* ctx, const uint64_t* seeds, const uint
     if (batch == 0 || count == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
     B200_CUDA(cudaSetDevice(ctx->c.device));
-    int rc = load_constants(ctx->c.device);
-    if (rc != B200_OK) return rc;
     cudaStream_t st = ctx->c.stream;
+    int rc = load_constants(ctx->c.device, st);
+    if (rc != B200_OK) return rc;
     const size_t total = batch * count;
     if ((rc = ctx->c.plonk_ws.reserve((batch + total + 1) * sizeof(fe) + batch * 8 + 64)) != B200_OK) return rc;
     fe* d_seeds = reinterpret_cast<fe*>(ctx->c.plonk_ws.p);

@@ -32,9 +32,10 @@ def test_generated_header_matches_fixture(pyoracle):
 
 @pytest.mark.gpu
 def test_gpu_permutation_and_hash(ctx, oracle, pyoracle):
+    """The published known answer through the device permutation; then every output of 300 random permutations and of
+    130 sponge hashes per length 0..7 against the C oracle (itself pinned by tests/test_poseidon2_oracle_cpu.py)."""
     from renegade_b200.backend import compute_poseidon_hash_batch, poseidon2_permute_batch
     py = pyoracle
-    full, partial = py.poseidon2_load_constants(FIX)
     to_m = lambda vals: oracle.ints_to_array([py.to_mont(v, py.R) for v in vals])
     from_m = lambda arr: [py.from_mont(v, py.R) for v in oracle.array_to_ints(arr)]
     # the published known answer through the device permutation
@@ -44,47 +45,33 @@ def test_gpu_permutation_and_hash(ctx, oracle, pyoracle):
     # random states
     import random
     rnd = random.Random(5)
-    states = [[rnd.randrange(py.R) for _ in range(3)] for _ in range(300)]
-    got = poseidon2_permute_batch(ctx, to_m([v for s in states for v in s]).reshape(-1, 3, 4))
-    for i, s in enumerate(states[:40]):
-        assert from_m(got[i]) == py.poseidon2_permute(s, full, partial)
+    states = to_m([rnd.randrange(py.R) for _ in range(3 * 300)]).reshape(-1, 3, 4)
+    assert np.array_equal(poseidon2_permute_batch(ctx, states), oracle.poseidon2_permute_batch(states))
     # sponge hashes of every length 0..7 (odd lengths leave the rate half full; 0 = hash of nothing)
     for ln in range(0, 8):
-        vals = [[rnd.randrange(py.R) for _ in range(ln)] for _ in range(130)]
-        arr = to_m([v for row in vals for v in row]).reshape(130, ln, 4) if ln else np.zeros((130, 0, 4), dtype=np.uint64)
-        out = compute_poseidon_hash_batch(ctx, arr)
-        exp = [py.poseidon2_hash(row, full, partial) for row in vals[:25]]
-        assert from_m(out[:25]) == exp, ln
+        arr = to_m([rnd.randrange(py.R) for _ in range(130 * ln)]).reshape(130, ln, 4)
+        assert np.array_equal(compute_poseidon_hash_batch(ctx, arr), oracle.poseidon2_hash_batch(arr)), ln
 
 
 @pytest.mark.gpu
 def test_gpu_merkle_roots_and_csprng_streams(ctx, oracle, pyoracle):
     """The batch callers of the witness side (SURVEY §8(f) f4): Merkle roots of openings of height 10 (`MERKLE_HEIGHT`,
-    constants/src/lib.rs:50) and Poseidon CSPRNG stream values H(seed, i) (darkpool-types/src/csprng.rs:30-75), device
-    vs the oracle's Poseidon2 on Python integers."""
+    constants/src/lib.rs:50) and Poseidon CSPRNG stream values H(seed, i) (darkpool-types/src/csprng.rs:30-75), every
+    output against the C oracle's Poseidon2 (one batched two-to-one hash per level, H(seed, first + j))."""
     import random
     from renegade_b200.backend import csprng_batch, merkle_root_batch
     py = pyoracle
-    full, partial = py.poseidon2_load_constants(FIX)
-    H = lambda vals: py.poseidon2_hash(vals, full, partial)
     to_m = lambda vals: oracle.ints_to_array([py.to_mont(v, py.R) for v in vals])
-    from_m = lambda arr: [py.from_mont(v, py.R) for v in oracle.array_to_ints(arr)]
     rnd = random.Random(11)
     batch, height = 67, 10
-    leaves = [rnd.randrange(py.R) for _ in range(batch)]
-    sisters = [[rnd.randrange(py.R) for _ in range(height)] for _ in range(batch)]
-    bits = [[rnd.random() < 0.5 for _ in range(height)] for _ in range(batch)]
-    got = from_m(merkle_root_batch(ctx, to_m(leaves), to_m([v for row in sisters for v in row]).reshape(batch, height, 4),
-                                   np.array(bits, dtype=np.uint8)))
-    for i in range(0, batch, 7):
-        cur = leaves[i]
-        for sis, right in zip(sisters[i], bits[i]):
-            cur = H([sis, cur] if right else [cur, sis])
-        assert got[i] == cur, i
+    leaves = to_m([rnd.randrange(py.R) for _ in range(batch)])
+    sisters = to_m([rnd.randrange(py.R) for _ in range(batch * height)]).reshape(batch, height, 4)
+    bits = np.array([[rnd.random() < 0.5 for _ in range(height)] for _ in range(batch)], dtype=np.uint8)
+    got = merkle_root_batch(ctx, leaves, sisters, bits)
+    assert np.array_equal(got, oracle.poseidon2_merkle_roots(leaves, sisters, bits))
     # height 0: the root is the leaf hash itself
-    assert from_m(merkle_root_batch(ctx, to_m(leaves[:3]), np.zeros((3, 0, 4), dtype=np.uint64), np.zeros((3, 0), dtype=np.uint8))) == leaves[:3]
-    seeds = [rnd.randrange(py.R) for _ in range(9)]
+    assert np.array_equal(merkle_root_batch(ctx, leaves[:3], np.zeros((3, 0, 4), dtype=np.uint64),
+                                            np.zeros((3, 0), dtype=np.uint8)), leaves[:3])
+    seeds = to_m([rnd.randrange(py.R) for _ in range(9)])
     first = [rnd.randrange(0, 1 << 40) for _ in range(9)]
-    out = csprng_batch(ctx, to_m(seeds), first, 5)
-    for s in (0, 4, 8):
-        assert from_m(out[s]) == [H([seeds[s], first[s] + j]) for j in range(5)]
+    assert np.array_equal(csprng_batch(ctx, seeds, first, 5), oracle.poseidon2_csprng(seeds, first, 5))

@@ -550,7 +550,8 @@ int b200_pool_stats(b200_pool* pool, uint64_t out[4]);
  * `b200_box` holds one prover pool per device, `b200_box_srs_load` / `b200_box_preprocess` replicate the SRS tables and a
  * proving key on every device (identical results), and every job goes to the device with the fewest unfinished jobs.
  * What ONE host process — the relayer's `NativeProofManager` (native_proof_manager.rs:140-201) — needs to use the
- * whole box.  A ticket encodes its device; tickets are waited for with b200_box_wait. */
+ * whole box.  A ticket encodes its device; tickets are waited for with b200_box_wait.  Every box entry that takes a key
+ * or an SRS returns B200_ERR_INVALID for one made by another box, even one over the same number of devices. */
 typedef struct b200_box b200_box;
 typedef struct b200_box_srs b200_box_srs;
 typedef struct b200_box_pk b200_box_pk;

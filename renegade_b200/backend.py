@@ -16,7 +16,6 @@ from __future__ import annotations
 
 import ctypes as C
 from dataclasses import dataclass
-from typing import Any
 
 import numpy as np
 
@@ -980,23 +979,6 @@ def _settlement_links(links, srs_len, n: int, where: str):
     return arr, held, out
 
 
-@dataclass
-class _PoolSettlement:
-    """What a queued settlement job writes into, and what it reads until the wait."""
-    proof: Any
-    links: list
-    statuses: Any
-    pub_inputs: Any  # None for a wire-table settlement
-    held: list
-
-
-def _settlement_results(s: "_PoolSettlement", rc: int):
-    if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
-        _lib.check(rc)
-    st = [int(s.statuses[i]) for i in range(len(s.links) + 1)]
-    return (s.proof, s.links, st) if s.pub_inputs is None else (s.proof, s.links, st, s.pub_inputs)
-
-
 def compute_poseidon_hash_batch(ctx: Context, values: np.ndarray) -> np.ndarray:
     """`batch` x `crypto::hash::compute_poseidon_hash(&values[i])` (crates/crypto/src/hash/mod.rs:12-18):
     values has shape (batch, len, 4) Montgomery; returns (batch, 4)."""
@@ -1122,65 +1104,121 @@ def _bundle_table_arrays(proofs, links, resolve, where: str):
     return arr_p, arr_l, keep, (out_proofs, out_polys, out_links)
 
 
-@dataclass
-class _PoolVerify:
-    """What a queued verification job writes into: the verdicts, and the combined answer in combined mode."""
-    batch: "_VerifyBatch"
-    verdicts: Any
-    ok: Any  # c_int in combined mode, else None
 
 
-def _submit_verify(submit, vks, pub_inputs, proofs, links, combined: bool, g2):
-    """One verification job through `submit` (`b200_pool_submit_verify` or `b200_box_submit_verify` with its handle
-    bound): -> (ticket, _PoolVerify).  The C call copies every input, so only the outputs have to live until the wait."""
+# ---- queued jobs of a pool or a box --------------------------------------------------------------------------------
+# Each builder checks one job kind's arguments (ProverError or ValueError, before any library call) and returns
+# (args, finish, held): the C arguments after the pool or box handle and, where the entry takes them, the SRS and the key
+# handle; finish(rc), which turns the job's status into what `wait` returns; and the objects the job reads until then.  A
+# pool and a box submit the same job through their own entry point.
+
+def _finish(results, batch: bool = False):
+    """finish(rc) of a job: raises for a failed job, else returns results().  A batch job (`batch`) reports an unsatisfied
+    or refused item in its statuses, so only its other failures raise."""
+    def finish(rc):
+        if not (batch and rc == _lib.B200_ERR_UNSATISFIED):
+            _lib.check(rc)
+        return results()
+    return finish
+
+
+def _prove_job(shape, wires_ptr: int, pub_inputs, blinders, with_link_poly: bool, where: str):
+    """One proof of a wire table at `wires_ptr`; `wait` returns the proof, or (proof, link_poly) with `with_link_poly`."""
+    pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64)
+    bl = np.ascontiguousarray(blinders, dtype=np.uint64)
+    if pi.size != 4 * shape.num_inputs:
+        raise ProverError(_lib.B200_ERR_INVALID, f"{where}: {pi.size // 4} public inputs for a key with {shape.num_inputs}")
+    if bl.size != 4 * 17:
+        raise ProverError(_lib.B200_ERR_INVALID, f"{where}: blinders must be 17 Fr elements")
+    proof = B200Proof()
+    link = np.zeros((shape.domain_size + 2, 4), dtype=np.uint64) if with_link_poly else None
+    args = (C.c_void_p(wires_ptr), _ptr(pi) if pi.size else None, pi.size // 4, _ptr(bl), C.byref(proof),
+            _ptr(link) if link is not None else None)
+    return args, _finish(lambda: proof if link is None else (proof, link)), ()
+
+
+def _prove_witness_job(shape, witness, blinders, with_link_poly: bool, where: str):
+    """One proof of a witness vector; `wait` returns (proof, pub_inputs), or (proof, link_poly, pub_inputs) with
+    `with_link_poly`."""
+    try:
+        wit, wit_ptr = _witness_arg(shape, witness, where)
+    except ValueError as e:
+        raise ProverError(_lib.B200_ERR_INVALID, str(e))
+    bl = np.ascontiguousarray(blinders, dtype=np.uint64)
+    if bl.size != 4 * 17:
+        raise ProverError(_lib.B200_ERR_INVALID, f"{where}: blinders must be 17 Fr elements")
+    proof = B200Proof()
+    pub = np.zeros((shape.num_inputs, 4), dtype=np.uint64)
+    link = np.zeros((shape.domain_size + 2, 4), dtype=np.uint64) if with_link_poly else None
+    args = (wit_ptr, _ptr(bl), C.byref(proof), _ptr(link) if link is not None else None, _ptr(pub) if pub.size else None)
+    return args, _finish(lambda: (proof, pub) if link is None else (proof, link, pub)), wit
+
+
+def _settlement_job(h, shape, srs_len, wires, pub_inputs, blinders, links, where: str):
+    """A settlement of a wire table, the key's handle `h` in its proof entry; args start at the proof entry.  `wait`
+    returns (proof, link_proofs, statuses) like `PlonkKzgSnark.prove_settlement`."""
+    w, w_ptr = _wires_arg(shape.domain_size, wires, where)
+    pi, bl = _settlement_inputs(shape.num_inputs, pub_inputs, blinders, where)
+    arr, held, out = _settlement_links(links, srs_len, shape.domain_size, where)
+    proof = B200Proof()
+    item = BundleProof(h, w_ptr, _ptr(pi) if pi.size else None, pi.shape[0], _ptr(bl), C.cast(C.pointer(proof), C.c_void_p),
+                       None)
+    st = (C.c_int * (len(out) + 1))()
+    return (C.byref(item), arr, len(out), st), _finish(lambda: (proof, out, list(st)), batch=True), (w, held)
+
+
+def _settlement_witness_job(h, shape, srs_len, witness, blinders, links, where: str):
+    """`_settlement_job` from the settlement's witness vector; `wait` returns (proof, link_proofs, statuses,
+    pub_inputs) like `PlonkKzgSnark.prove_settlement_witness`."""
+    if shape.num_vars == 0:
+        raise ProverError(_lib.B200_ERR_INVALID, f"{where}: the key holds no wiring (made by preprocess)")
+    try:
+        wit, wit_ptr = _witness_arg(shape, witness, where)
+    except ValueError as e:
+        raise ProverError(_lib.B200_ERR_INVALID, str(e))
+    _, bl = _settlement_inputs(0, (), blinders, where)
+    arr, held, out = _settlement_links(links, srs_len, shape.domain_size, where)
+    proof = B200Proof()
+    pub = np.zeros((shape.num_inputs, 4), dtype=np.uint64)
+    item = BundleWitness(h, wit_ptr, _ptr(bl), C.cast(C.pointer(proof), C.c_void_p), None, _ptr(pub) if pub.size else None)
+    st = (C.c_int * (len(out) + 1))()
+    return (C.byref(item), arr, len(out), st), _finish(lambda: (proof, out, list(st), pub), batch=True), (wit, held)
+
+
+def _verify_job(vks, pub_inputs, proofs, links, combined: bool, g2):
+    """One verification job.  The C call copies every input, so only the outputs have to live until the wait, which
+    returns what `verify_each` (a verdict list) or, `combined`, `batch_verify` ((all_ok, verdicts)) returns."""
     b = _VerifyBatch(vks, pub_inputs, proofs, links, g2)
     if not hasattr(b, "args"):  # no items and no G2 pair: a job still checks its G2 records
         raise ValueError("a verification job without items needs g2=(g2_h, g2_tau_h)")
     verdicts = (C.c_uint8 * max(1, b.n_c))()
     ok = C.c_int(0) if combined else None
-    ticket = C.c_uint64()
-    _lib.check(submit(int(combined), *b.args, C.byref(ok) if combined else None, verdicts, C.byref(ticket)))
-    return ticket.value, _PoolVerify(b, verdicts, ok)
+
+    def results():
+        v = b.verdicts(verdicts)
+        return v if ok is None else (bool(ok.value) and len(b.c_proofs) == b.n_proofs, v)
+    return (int(combined), *b.args, C.byref(ok) if combined else None, verdicts), _finish(results), ()
 
 
-def _verify_results(v: _PoolVerify, rc: int):
-    """What `verify_each` (a verdict list) or `batch_verify` ((all_ok, verdicts)) returns for the same items."""
-    _lib.check(rc)
-    verdicts = v.batch.verdicts(v.verdicts)
-    if v.ok is None:
-        return verdicts
-    return bool(v.ok.value) and len(v.batch.c_proofs) == v.batch.n_proofs, verdicts
+class _Tickets:
+    """The tickets a pool or a box handed out and nobody has waited for yet: `_jobs` maps ticket -> (finish, held)."""
+
+    def _submit(self, c_submit, args, finish, held) -> int:
+        ticket = C.c_uint64()
+        _lib.check(c_submit(self._h, *args, C.byref(ticket)))
+        self._jobs[ticket.value] = (finish, held)
+        return ticket.value
+
+    def _wait(self, c_wait, ticket: int):
+        rc = c_wait(self._h, ticket)
+        finish, _ = self._jobs.pop(ticket, (None, None))
+        if finish is None:  # not a ticket of this object
+            _lib.check(rc)
+            return None
+        return finish(rc)
 
 
-@dataclass
-class _PoolBatch:
-    """What a queued batch job writes into: its items' arrays and outputs, and the statuses."""
-    held: list
-    statuses: Any
-    link_hints: bool
-
-
-@dataclass
-class _PoolWitness:
-    """What a queued witness job writes into."""
-    proof: Any
-    pub_inputs: np.ndarray
-
-
-@dataclass
-class _PoolWitnessBatch(_PoolBatch):
-    """What a queued witness batch job writes into: as a batch job, and each item's public inputs."""
-    pub_inputs: list = None
-
-
-@dataclass
-class _PoolLinkBatch:
-    """What a queued link batch job writes into: its items' arrays and outputs, and the statuses."""
-    held: list
-    statuses: Any
-
-
-class ProverPool:
+class ProverPool(_Tickets):
     """b200_pool: the device-side counterpart of the reference's `NativeProofManager` thread pool
     (crates/workers/proof-manager/src/implementations/native_proof_manager.rs:138-201, `spawn_fifo`
     per job).  `workers` proofs are in flight on one GPU; keys and SRS tables are shared.
@@ -1193,7 +1231,7 @@ class ProverPool:
         _lib.check(self._lib.b200_pool_create(device, workers, C.byref(h)))
         self._h = h
         self.device = device
-        self._keep = {}  # ticket -> objects the job reads or writes
+        self._jobs = {}
         self._borrowed = []
 
     @property
@@ -1211,47 +1249,25 @@ class ProverPool:
         self._borrowed.append(ctx)
         return ctx
 
+    @staticmethod
+    def _resolve(pk):
+        return pk._h, pk
+
     def submit_prove(self, pk: "ProvingKey", wires_ptr: int, pub_inputs: np.ndarray, blinders: np.ndarray,
                      with_link_poly: bool = False, keep=None) -> int:
         """Queue one proof; returns the ticket.  `wires_ptr`: address of the 5 x n wire table (pinned host
         or device memory), which the caller keeps valid until `wait(ticket)` returns (pass the owning
         object as `keep` to let the pool hold a reference)."""
-        proof = B200Proof()
-        pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64)
-        bl = np.ascontiguousarray(blinders, dtype=np.uint64)
-        if pi.size != 4 * pk.num_inputs:
-            raise ProverError(_lib.B200_ERR_INVALID, f"submit_prove: {pi.size // 4} public inputs for a key with {pk.num_inputs}")
-        if bl.size != 4 * 17:
-            raise ProverError(_lib.B200_ERR_INVALID, "submit_prove: blinders must be 17 Fr elements")
-        link = np.zeros((pk.domain_size + 2, 4), dtype=np.uint64) if with_link_poly else None
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_pool_submit_prove(self._h, pk._h, C.c_void_p(wires_ptr), _ptr(pi) if pi.size else None,
-                                                    pi.size // 4, _ptr(bl), C.byref(proof),
-                                                    _ptr(link) if link is not None else None, C.byref(ticket)))
-        self._keep[ticket.value] = (proof, link, keep, pk)
-        return ticket.value
+        args, finish, held = _prove_job(pk, wires_ptr, pub_inputs, blinders, with_link_poly, "submit_prove")
+        return self._submit(self._lib.b200_pool_submit_prove, (pk._h, *args), finish, (held, keep, pk))
 
     def submit_prove_witness(self, pk: "ProvingKey", witness, blinders: np.ndarray, with_link_poly: bool = False,
                              keep=None) -> int:
         """Queue one proof from a witness vector (array, or address in pinned host or device memory kept valid until
         `wait(ticket)` returns) of a key made by `preprocess_wiring`; returns the ticket.  `wait(ticket)` returns
         (proof, pub_inputs), or (proof, link_poly, pub_inputs) with `with_link_poly`."""
-        try:
-            wit, wit_ptr = _witness_arg(pk, witness, "submit_prove_witness")
-        except ValueError as e:
-            raise ProverError(_lib.B200_ERR_INVALID, str(e))
-        bl = np.ascontiguousarray(blinders, dtype=np.uint64)
-        if bl.size != 4 * 17:
-            raise ProverError(_lib.B200_ERR_INVALID, "submit_prove_witness: blinders must be 17 Fr elements")
-        proof = B200Proof()
-        pub = np.zeros((pk.num_inputs, 4), dtype=np.uint64)
-        link = np.zeros((pk.domain_size + 2, 4), dtype=np.uint64) if with_link_poly else None
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_pool_submit_prove_witness(self._h, pk._h, wit_ptr, _ptr(bl), C.byref(proof),
-                                                            _ptr(link) if link is not None else None,
-                                                            _ptr(pub) if pub.size else None, C.byref(ticket)))
-        self._keep[ticket.value] = (_PoolWitness(proof, pub), link, (wit, keep), pk)
-        return ticket.value
+        args, finish, held = _prove_witness_job(pk, witness, blinders, with_link_poly, "submit_prove_witness")
+        return self._submit(self._lib.b200_pool_submit_prove_witness, (pk._h, *args), finish, (held, keep, pk))
 
     def submit_prove_batch(self, pk: "ProvingKey", wires_list, pub_inputs_list, blinders_list, link_hints: bool = False,
                            keep=None) -> int:
@@ -1260,10 +1276,9 @@ class ProverPool:
         (pass their owners as `keep`).  `wait(ticket)` returns (proofs, hints, statuses) like `prove_batch`."""
         items, held = _prove_items(pk, wires_list, pub_inputs_list, blinders_list, link_hints, False)
         statuses = (C.c_int * max(1, len(held)))()
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_pool_submit_prove_batch(self._h, pk._h, items, len(held), statuses, C.byref(ticket)))
-        self._keep[ticket.value] = (_PoolBatch(held, statuses, link_hints), None, (items, keep), pk)
-        return ticket.value
+        finish = _finish(lambda: _batch_results(held, statuses, link_hints, False), batch=True)
+        return self._submit(self._lib.b200_pool_submit_prove_batch, (pk._h, items, len(held), statuses), finish,
+                            (held, keep, pk))
 
     def submit_link(self, srs: "Bases", hint_a: "LinkingHint", hint_b: "LinkingHint", layout: "GroupLayout") -> int:
         a1 = np.ascontiguousarray(hint_a.linking_wire_poly, dtype=np.uint64).reshape(-1, 4)
@@ -1271,12 +1286,9 @@ class ProverPool:
         c1 = np.ascontiguousarray(hint_a.linking_wire_comm, dtype=np.uint64)
         c2 = np.ascontiguousarray(hint_b.linking_wire_comm, dtype=np.uint64)
         proof = B200LinkProof()
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_pool_submit_link(self._h, srs._h, _ptr(a1), a1.shape[0], _ptr(a2), a2.shape[0],
-                                                   _ptr(c1), _ptr(c2), layout.alignment, layout.offset, layout.size,
-                                                   C.byref(proof), C.byref(ticket)))
-        self._keep[ticket.value] = (proof, None, (a1, a2, c1, c2), srs)
-        return ticket.value
+        args = (srs._h, _ptr(a1), a1.shape[0], _ptr(a2), a2.shape[0], _ptr(c1), _ptr(c2), layout.alignment, layout.offset,
+                layout.size, C.byref(proof))
+        return self._submit(self._lib.b200_pool_submit_link, args, _finish(lambda: proof), (a1, a2, srs))
 
     def submit_link_batch(self, srs: "Bases", triples, keep=None) -> int:
         """Queue one `b200_plonk_link_batch` as a single job on one worker; returns the ticket.  Arguments as for
@@ -1284,33 +1296,27 @@ class ProverPool:
         their owners as `keep`).  `wait(ticket)` returns (proofs, etas, statuses) like `link_proofs_batch`."""
         items, held = _link_items(srs, triples)
         statuses = (C.c_int * max(1, len(held)))()
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_pool_submit_link_batch(self._h, srs._h, items, len(held), statuses, C.byref(ticket)))
-        self._keep[ticket.value] = (_PoolLinkBatch(held, statuses), None, (items, keep), srs)
-        return ticket.value
+        finish = _finish(lambda: _link_batch_results(held, statuses), batch=True)
+        return self._submit(self._lib.b200_pool_submit_link_batch, (srs._h, items, len(held), statuses), finish,
+                            (held, keep, srs))
 
     def submit_bundle(self, srs: "Bases", proofs, links) -> int:
         """One ticket for a whole proof bundle (`b200_pool_submit_bundle`): `proofs` = [(pk, wires_ptr, pub_inputs,
         blinders)], `links` = [(a, b, GroupLayout)] — link proof between the hints of proofs a and b, forked inside the
         pool once every proof is in (native_proof_manager.rs:526-584, 726-782).  `wait(ticket)` returns
         ([B200Proof], [link polys], [B200LinkProof])."""
-        arr_p, arr_l, keep, out = _bundle_table_arrays(proofs, links, lambda pk: (pk._h, pk), "submit_bundle")
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_pool_submit_bundle(self._h, srs._h, arr_p, len(proofs), arr_l, len(links), C.byref(ticket)))
-        self._keep[ticket.value] = (out, None, keep, srs)
-        return ticket.value
+        arr_p, arr_l, keep, out = _bundle_table_arrays(proofs, links, self._resolve, "submit_bundle")
+        return self._submit(self._lib.b200_pool_submit_bundle, (srs._h, arr_p, len(proofs), arr_l, len(links)),
+                            _finish(lambda: out), (keep, srs))
 
     def submit_bundle_witness(self, srs: "Bases", proofs, links) -> int:
         """`submit_bundle` with every proof given as a witness vector (`b200_pool_submit_bundle_witness`): `proofs` =
         [(pk, witness, blinders)], pk a key made by `preprocess_wiring`, witness an array or an address (pinned host or
         device memory, kept valid until `wait(ticket)` returns) as `submit_prove_witness` takes.  `wait(ticket)` returns
         ([B200Proof], [link polys], [B200LinkProof], [pub_inputs])."""
-        arr_p, arr_l, keep, out = _bundle_witness_arrays(proofs, links, lambda pk: (pk._h, pk), "submit_bundle_witness")
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_pool_submit_bundle_witness(self._h, srs._h if srs is not None else None, arr_p, len(proofs),
-                                                             arr_l, len(links), C.byref(ticket)))
-        self._keep[ticket.value] = (out, None, keep, srs)
-        return ticket.value
+        arr_p, arr_l, keep, out = _bundle_witness_arrays(proofs, links, self._resolve, "submit_bundle_witness")
+        args = (srs._h if srs is not None else None, arr_p, len(proofs), arr_l, len(links))
+        return self._submit(self._lib.b200_pool_submit_bundle_witness, args, _finish(lambda: out), (keep, srs))
 
     def submit_prove_witness_batch(self, pk: "ProvingKey", witnesses, blinders_list, link_hints: bool = False,
                                    keep=None) -> int:
@@ -1325,86 +1331,42 @@ class ProverPool:
         except ValueError as e:
             raise ProverError(_lib.B200_ERR_INVALID, str(e))
         statuses = (C.c_int * max(1, len(held)))()
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_pool_submit_prove_witness_batch(self._h, pk._h, items, len(held), statuses, C.byref(ticket)))
-        self._keep[ticket.value] = (_PoolWitnessBatch(held, statuses, link_hints, pubs), None, (items, keep), pk)
-        return ticket.value
+        finish = _finish(lambda: _batch_results(held, statuses, link_hints, False) + (pubs,), batch=True)
+        return self._submit(self._lib.b200_pool_submit_prove_witness_batch, (pk._h, items, len(held), statuses), finish,
+                            (held, keep, pk))
 
     def submit_settlement(self, srs: "Bases", pk: "ProvingKey", wires, pub_inputs, blinders, links, keep=None) -> int:
         """Queue one `PlonkKzgSnark.prove_settlement` as ONE job on one worker (`b200_pool_submit_settlement`); returns the
         ticket.  Arguments as `prove_settlement` takes them; a wire table or hint given by address stays owned by the
         caller until `wait(ticket)` returns (pass its owner as `keep`).  `wait(ticket)` returns (proof, link_proofs,
         statuses) like `prove_settlement`."""
-        w, w_ptr = _wires_arg(pk.domain_size, wires, "submit_settlement")
-        pi, bl = _settlement_inputs(pk.num_inputs, pub_inputs, blinders, "submit_settlement")
-        arr, held, out = _settlement_links(links, len(srs), pk.domain_size, "submit_settlement")
-        proof = B200Proof()
-        item = BundleProof(pk._h, w_ptr, _ptr(pi) if pi.size else None, pi.shape[0], _ptr(bl),
-                           C.cast(C.pointer(proof), C.c_void_p), None)
-        st = (C.c_int * (len(out) + 1))()
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_pool_submit_settlement(self._h, srs._h, C.byref(item), arr, len(out), st, C.byref(ticket)))
-        self._keep[ticket.value] = (_PoolSettlement(proof, out, st, None, [w, pi, bl, arr, held, keep]), None, None, (pk, srs))
-        return ticket.value
+        args, finish, held = _settlement_job(pk._h, pk, len(srs), wires, pub_inputs, blinders, links, "submit_settlement")
+        return self._submit(self._lib.b200_pool_submit_settlement, (srs._h, *args), finish, (held, keep, pk, srs))
 
     def submit_settlement_witness(self, srs: "Bases", pk: "ProvingKey", witness, blinders, links, keep=None) -> int:
         """`submit_settlement` from the settlement's witness vector (`b200_pool_submit_settlement_witness`), arguments as
         `PlonkKzgSnark.prove_settlement_witness` takes them.  `wait(ticket)` returns (proof, link_proofs, statuses,
         pub_inputs)."""
-        if pk.num_vars == 0:
-            raise ProverError(_lib.B200_ERR_INVALID, "submit_settlement_witness: the key holds no wiring (made by preprocess)")
-        try:
-            wit, wit_ptr = _witness_arg(pk, witness, "submit_settlement_witness")
-        except ValueError as e:
-            raise ProverError(_lib.B200_ERR_INVALID, str(e))
-        _, bl = _settlement_inputs(0, (), blinders, "submit_settlement_witness")
-        arr, held, out = _settlement_links(links, len(srs), pk.domain_size, "submit_settlement_witness")
-        proof = B200Proof()
-        pub = np.zeros((pk.num_inputs, 4), dtype=np.uint64)
-        item = BundleWitness(pk._h, wit_ptr, _ptr(bl), C.cast(C.pointer(proof), C.c_void_p), None, _ptr(pub) if pub.size else None)
-        st = (C.c_int * (len(out) + 1))()
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_pool_submit_settlement_witness(self._h, srs._h, C.byref(item), arr, len(out), st,
-                                                                 C.byref(ticket)))
-        self._keep[ticket.value] = (_PoolSettlement(proof, out, st, pub, [wit, bl, arr, held, keep]), None, None, (pk, srs))
-        return ticket.value
+        args, finish, held = _settlement_witness_job(pk._h, pk, len(srs), witness, blinders, links, "submit_settlement_witness")
+        return self._submit(self._lib.b200_pool_submit_settlement_witness, (srs._h, *args), finish, (held, keep, pk, srs))
 
     def submit_verify(self, vks, pub_inputs, proofs, links=(), combined: bool = False, g2=None) -> int:
         """Queue one verification job on some worker (`b200_pool_submit_verify`); returns the ticket.  Arguments as
         `PlonkKzgSnark.verify_each` / `.batch_verify` take them; every input is copied at submit.  `wait(ticket)` returns
         what `verify_each` returns (the verdict list), or with `combined` what `batch_verify` returns ((all_ok,
         verdicts): one combined pairing, the failing items found by bisection inside the job)."""
-        ticket, job = _submit_verify(lambda *a: self._lib.b200_pool_submit_verify(self._h, *a), vks, pub_inputs, proofs,
-                                     links, combined, g2)
-        self._keep[ticket] = (job, None, None, None)
-        return ticket
+        job = _verify_job(vks, pub_inputs, proofs, links, combined, g2)
+        return self._submit(self._lib.b200_pool_submit_verify, *job)
 
     def wait(self, ticket: int):
         """Blocks until the job is done; returns its B200Proof (or (B200Proof, link_poly) when the job was
         submitted with `with_link_poly`, or the B200LinkProof of a link job); raises B200Error with the
         job's own status and message if it failed."""
-        rc = self._lib.b200_pool_wait(self._h, ticket)
-        proof, link, _, _ = self._keep.pop(ticket, (None, None, None, None))
-        if isinstance(proof, _PoolVerify):
-            return _verify_results(proof, rc)
-        if isinstance(proof, _PoolSettlement):  # a settlement: refused links and an unsatisfied proof are in its statuses
-            return _settlement_results(proof, rc)
-        if isinstance(proof, (_PoolBatch, _PoolLinkBatch)):  # a batch job: refused items are reported in its statuses
-            if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
-                _lib.check(rc)
-            if isinstance(proof, _PoolLinkBatch):
-                return _link_batch_results(proof.held, proof.statuses)
-            if isinstance(proof, _PoolWitnessBatch):
-                return _batch_results(proof.held, proof.statuses, proof.link_hints, False) + (proof.pub_inputs,)
-            return _batch_results(proof.held, proof.statuses, proof.link_hints, False)
-        _lib.check(rc)
-        if isinstance(proof, _PoolWitness):
-            return (proof.proof, proof.pub_inputs) if link is None else (proof.proof, link, proof.pub_inputs)
-        return (proof, link) if link is not None else proof
+        return self._wait(self._lib.b200_pool_wait, ticket)
 
     def wait_all(self) -> None:
         rc = self._lib.b200_pool_wait_all(self._h)
-        self._keep.clear()
+        self._jobs.clear()
         _lib.check(rc)
 
     def stats(self) -> dict:
@@ -1416,7 +1378,7 @@ class ProverPool:
         if getattr(self, "_h", None):
             self._lib.b200_pool_destroy(self._h)
             self._h = None
-            self._keep.clear()
+            self._jobs.clear()
             for ctx in self._borrowed:  # their handles died with the pool
                 ctx._h = None
 
@@ -1435,7 +1397,7 @@ class _BoxKeyShape:
     num_vars: int
 
 
-class ProverBox:
+class ProverBox(_Tickets):
     """`b200_box`: every GPU of the box behind one object — one prover pool per device, the SRS tables and the proving
     keys replicated on each, jobs routed to the least-loaded device.  The single-process counterpart of running one
     `ProverPool` per rank under torchrun."""
@@ -1445,7 +1407,7 @@ class ProverBox:
         arr = (C.c_int * len(devices))(*devices)
         h = C.c_void_p()
         _lib.check(self._lib.b200_box_create(arr, len(devices), workers_per_device, C.byref(h)))
-        self._h, self._keep, self.devices = h, {}, list(devices)
+        self._h, self._jobs, self.devices = h, {}, list(devices)
         self._shapes = {}  # key handle -> _BoxKeyShape, for the keys this box made
 
     def load_srs(self, points: np.ndarray, window_bits: int = 0, check_on_curve: bool = False):
@@ -1483,37 +1445,29 @@ class ProverBox:
             raise ProverError(_lib.B200_ERR_INVALID, "box: the key was not made by this box")
         return pk, shape
 
+    def submit_prove(self, pk, wires_ptr: int, pub_inputs: np.ndarray, blinders: np.ndarray, with_link_poly: bool = False,
+                     keep=None) -> int:
+        """`ProverPool.submit_prove` on the least-loaded device (`b200_box_submit_prove`).  `wait(ticket)` returns the
+        proof, or (proof, link_poly) with `with_link_poly`."""
+        h, shape = self._resolve(pk)
+        args, finish, held = _prove_job(shape, wires_ptr, pub_inputs, blinders, with_link_poly, "box.submit_prove")
+        return self._submit(self._lib.b200_box_submit_prove, (h, *args), finish, (held, keep))
+
     def submit_prove_witness(self, pk, witness, blinders: np.ndarray, with_link_poly: bool = False, keep=None) -> int:
         """`ProverPool.submit_prove_witness` on the box (`b200_box_submit_prove_witness`): a witness in device memory runs
         on its own device, any other on the least-loaded one.  `wait(ticket)` returns (proof, pub_inputs), or (proof,
         link_poly, pub_inputs) with `with_link_poly`."""
-        _, shape = self._resolve(pk)
-        try:
-            wit, wit_ptr = _witness_arg(shape, witness, "box.submit_prove_witness")
-        except ValueError as e:
-            raise ProverError(_lib.B200_ERR_INVALID, str(e))
-        bl = np.ascontiguousarray(blinders, dtype=np.uint64)
-        if bl.size != 4 * 17:
-            raise ProverError(_lib.B200_ERR_INVALID, "box.submit_prove_witness: blinders must be 17 Fr elements")
-        proof = B200Proof()
-        pub = np.zeros((shape.num_inputs, 4), dtype=np.uint64)
-        link = np.zeros((shape.domain_size + 2, 4), dtype=np.uint64) if with_link_poly else None
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_box_submit_prove_witness(self._h, pk, wit_ptr, _ptr(bl), C.byref(proof),
-                                                           _ptr(link) if link is not None else None,
-                                                           _ptr(pub) if pub.size else None, C.byref(ticket)))
-        self._keep[ticket.value] = (_PoolWitness(proof, pub), link, (wit, keep), bl)
-        return ticket.value
+        h, shape = self._resolve(pk)
+        args, finish, held = _prove_witness_job(shape, witness, blinders, with_link_poly, "box.submit_prove_witness")
+        return self._submit(self._lib.b200_box_submit_prove_witness, (h, *args), finish, (held, keep))
 
     def submit_bundle(self, srs, proofs, links) -> int:
         """`ProverPool.submit_bundle` on the least-loaded device (`b200_box_submit_bundle`): `proofs` = [(box key,
         wires_ptr, pub_inputs, blinders)].  `wait(ticket)` returns ([B200Proof], [link polys], [B200LinkProof])."""
         arr_p, arr_l, keep, out = _bundle_table_arrays(proofs, links, self._resolve, "box.submit_bundle")
         pks = (C.c_void_p * max(len(proofs), 1))(*[p[0] for p in proofs])
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_box_submit_bundle(self._h, srs, pks, arr_p, len(proofs), arr_l, len(links), C.byref(ticket)))
-        self._keep[ticket.value] = (out, None, (keep, pks))
-        return ticket.value
+        return self._submit(self._lib.b200_box_submit_bundle, (srs, pks, arr_p, len(proofs), arr_l, len(links)),
+                            _finish(lambda: out), keep)
 
     def submit_bundle_witness(self, srs, proofs, links) -> int:
         """`ProverPool.submit_bundle_witness` on one device of the box (`b200_box_submit_bundle_witness`): `proofs` = [(box
@@ -1521,87 +1475,37 @@ class ProverBox:
         returns ([B200Proof], [link polys], [B200LinkProof], [pub_inputs])."""
         arr_p, arr_l, keep, out = _bundle_witness_arrays(proofs, links, self._resolve, "box.submit_bundle_witness")
         pks = (C.c_void_p * max(len(proofs), 1))(*[p[0] for p in proofs])
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_box_submit_bundle_witness(self._h, srs, pks, arr_p, len(proofs), arr_l, len(links),
-                                                            C.byref(ticket)))
-        self._keep[ticket.value] = (out, None, (keep, pks))
-        return ticket.value
+        return self._submit(self._lib.b200_box_submit_bundle_witness, (srs, pks, arr_p, len(proofs), arr_l, len(links)),
+                            _finish(lambda: out), keep)
 
     def submit_settlement(self, srs, pk, wires, pub_inputs, blinders, links, keep=None) -> int:
         """`ProverPool.submit_settlement` on one device of the box (`b200_box_submit_settlement`): pk a box key, srs a box
         SRS.  A wire table or hint polynomial in device memory pins the job to its device (all of them on one); otherwise
         the job goes to the least-loaded device.  `wait(ticket)` returns (proof, link_proofs, statuses)."""
-        _, shape = self._resolve(pk)
-        w, w_ptr = _wires_arg(shape.domain_size, wires, "box.submit_settlement")
-        pi, bl = _settlement_inputs(shape.num_inputs, pub_inputs, blinders, "box.submit_settlement")
-        arr, held, out = _settlement_links(links, None, shape.domain_size, "box.submit_settlement")
-        proof = B200Proof()
-        item = BundleProof(None, w_ptr, _ptr(pi) if pi.size else None, pi.shape[0], _ptr(bl),
-                           C.cast(C.pointer(proof), C.c_void_p), None)
-        st = (C.c_int * (len(out) + 1))()
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_box_submit_settlement(self._h, srs, pk, C.byref(item), arr, len(out), st, C.byref(ticket)))
-        self._keep[ticket.value] = (_PoolSettlement(proof, out, st, None, [w, pi, bl, arr, held, keep]), None)
-        return ticket.value
+        h, shape = self._resolve(pk)
+        args, finish, held = _settlement_job(h, shape, None, wires, pub_inputs, blinders, links, "box.submit_settlement")
+        return self._submit(self._lib.b200_box_submit_settlement, (srs, h, *args), finish, (held, keep))
 
     def submit_settlement_witness(self, srs, pk, witness, blinders, links, keep=None) -> int:
         """`submit_settlement` from a witness vector (`b200_box_submit_settlement_witness`); the witness counts among the
         job's device pointers.  `wait(ticket)` returns (proof, link_proofs, statuses, pub_inputs)."""
-        _, shape = self._resolve(pk)
-        if shape.num_vars == 0:
-            raise ProverError(_lib.B200_ERR_INVALID, "box.submit_settlement_witness: the key holds no wiring (made by preprocess)")
-        try:
-            wit, wit_ptr = _witness_arg(shape, witness, "box.submit_settlement_witness")
-        except ValueError as e:
-            raise ProverError(_lib.B200_ERR_INVALID, str(e))
-        _, bl = _settlement_inputs(0, (), blinders, "box.submit_settlement_witness")
-        arr, held, out = _settlement_links(links, None, shape.domain_size, "box.submit_settlement_witness")
-        proof = B200Proof()
-        pub = np.zeros((shape.num_inputs, 4), dtype=np.uint64)
-        item = BundleWitness(None, wit_ptr, _ptr(bl), C.cast(C.pointer(proof), C.c_void_p), None, _ptr(pub) if pub.size else None)
-        st = (C.c_int * (len(out) + 1))()
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_box_submit_settlement_witness(self._h, srs, pk, C.byref(item), arr, len(out), st,
-                                                                C.byref(ticket)))
-        self._keep[ticket.value] = (_PoolSettlement(proof, out, st, pub, [wit, bl, arr, held, keep]), None)
-        return ticket.value
+        h, shape = self._resolve(pk)
+        args, finish, held = _settlement_witness_job(h, shape, None, witness, blinders, links, "box.submit_settlement_witness")
+        return self._submit(self._lib.b200_box_submit_settlement_witness, (srs, h, *args), finish, (held, keep))
 
     def submit_verify(self, vks, pub_inputs, proofs, links=(), combined: bool = False, g2=None) -> int:
         """`ProverPool.submit_verify` on the least-loaded device (`b200_box_submit_verify`).  `wait(ticket)` returns the
         verdict list, or (all_ok, verdicts) with `combined`."""
-        ticket, job = _submit_verify(lambda *a: self._lib.b200_box_submit_verify(self._h, *a), vks, pub_inputs, proofs,
-                                     links, combined, g2)
-        self._keep[ticket] = (job, None)
-        return ticket
+        job = _verify_job(vks, pub_inputs, proofs, links, combined, g2)
+        return self._submit(self._lib.b200_box_submit_verify, *job)
 
     def verifying_key(self, pk):
         sel, sig = np.zeros((13, 8), dtype=np.uint64), np.zeros((5, 8), dtype=np.uint64)
         _lib.check(self._lib.b200_box_pk_verifying_key(pk, _ptr(sel), _ptr(sig)))
         return sel, sig
 
-    def submit_prove(self, pk, wires_ptr: int, pub_inputs: np.ndarray, blinders: np.ndarray, log_n: int = 0, keep=None) -> int:
-        proof = B200Proof()
-        pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64)
-        bl = np.ascontiguousarray(blinders, dtype=np.uint64)
-        link = np.zeros(((1 << log_n) + 2, 4), dtype=np.uint64) if log_n else None
-        ticket = C.c_uint64()
-        _lib.check(self._lib.b200_box_submit_prove(self._h, pk, C.c_void_p(wires_ptr), _ptr(pi) if pi.size else None, pi.size // 4,
-                                                   _ptr(bl), C.byref(proof), _ptr(link) if link is not None else None,
-                                                   C.byref(ticket)))
-        self._keep[ticket.value] = (proof, link, keep, pi, bl)
-        return ticket.value
-
     def wait(self, ticket: int):
-        rc = self._lib.b200_box_wait(self._h, ticket)
-        proof, link, *_ = self._keep.pop(ticket, (None, None))
-        if isinstance(proof, _PoolVerify):
-            return _verify_results(proof, rc)
-        if isinstance(proof, _PoolSettlement):
-            return _settlement_results(proof, rc)
-        _lib.check(rc)
-        if isinstance(proof, _PoolWitness):
-            return (proof.proof, proof.pub_inputs) if link is None else (proof.proof, link, proof.pub_inputs)
-        return (proof, link) if link is not None else proof
+        return self._wait(self._lib.b200_box_wait, ticket)
 
     def ticket_device(self, ticket: int) -> int:
         return self._lib.b200_box_ticket_device(self._h, ticket)

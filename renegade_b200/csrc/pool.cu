@@ -10,8 +10,8 @@
 // Host-only code (std::thread) above the same C ABI the single-context entry points use.
 #include <algorithm>
 #include <condition_variable>
-#include <cstring>
 #include <deque>
+#include <functional>
 #include <map>
 #include <memory>
 #include <set>
@@ -27,114 +27,81 @@ namespace {
 
 struct Bundle;
 
-// The inputs of a verification job, copied at submit: the arrays with every pointer into the copies below, so the
-// caller may free or reuse its own as soon as the submit returns.
-struct VerifyCopy {
-    int mode = 0;  // 0: b200_plonk_verify_each, 1: b200_plonk_batch_verify
-    std::vector<b200_verifying_key> vks;
-    std::vector<b200_batch_proof> proofs;
-    std::vector<b200_batch_link> links;
-    std::vector<uint64_t> limbs;  // each key's k / selector / sigma, each proof's public inputs, each link's comm1 / comm2
-    std::vector<b200_proof> proof_bodies;
-    std::vector<b200_link_proof> link_bodies;
-    uint64_t g2_h[16], g2_tau_h[16];
-    int* all_accepted = nullptr;  // the caller's outputs
-    uint8_t* verdicts = nullptr;
+// The inputs a job copies at submit, so that the caller may free or reuse its own as soon as the submit returns.  Every
+// copy is an allocation of its own: a pointer into one stays valid while more are taken, for as long as the job lives.
+struct Held {
+    std::vector<std::shared_ptr<void>> blocks;
 
-    VerifyCopy(int m, const b200_verifying_key* v, size_t n_v, const b200_batch_proof* p, size_t n_p, const b200_batch_link* l,
-               size_t n_l, const uint64_t* h, const uint64_t* tau_h)
-        : mode(m), vks(v, v + n_v), proofs(p, p + n_p), links(l, l + n_l), proof_bodies(n_p), link_bodies(n_l) {
-        size_t total = (20 + 104 + 40) * n_v + 16 * n_l;
-        for (size_t i = 0; i < n_p; ++i) total += 4 * v[p[i].vk].num_inputs;
-        limbs.resize(total);  // sized once: the pointers below stay valid
-        uint64_t* at = limbs.data();
-        auto take = [&at](const uint64_t* src, size_t n) {
-            std::memcpy(at, src, 8 * n);
-            const uint64_t* out = at;
-            at += n;
-            return out;
-        };
-        for (b200_verifying_key& vk : vks) {
-            vk.k = take(vk.k, 20);
-            vk.selector_comms = take(vk.selector_comms, 104);
-            vk.sigma_comms = take(vk.sigma_comms, 40);
-        }
-        for (size_t i = 0; i < n_p; ++i) {
-            const size_t ni = vks[proofs[i].vk].num_inputs;
-            proofs[i].pub_inputs = ni ? take(proofs[i].pub_inputs, 4 * ni) : nullptr;
-            proof_bodies[i] = *proofs[i].proof;
-            proofs[i].proof = &proof_bodies[i];
-        }
-        for (size_t i = 0; i < n_l; ++i) {
-            links[i].comm1 = take(links[i].comm1, 8);
-            links[i].comm2 = take(links[i].comm2, 8);
-            link_bodies[i] = *links[i].proof;
-            links[i].proof = &link_bodies[i];
-        }
-        std::memcpy(g2_h, h, 128);
-        std::memcpy(g2_tau_h, tau_h, 128);
+    template <class T>
+    T* copy(const T* src, size_t n) {  // nullptr for n == 0
+        if (n == 0) return nullptr;
+        std::shared_ptr<T> p(new T[n], std::default_delete<T[]>());
+        std::copy(src, src + n, p.get());
+        blocks.push_back(p);
+        return p.get();
     }
 
-    int run(b200_ctx* ctx) const {
-        if (mode == 0)
-            return b200_plonk_verify_each(ctx, vks.data(), vks.size(), proofs.data(), proofs.size(), links.data(), links.size(),
-                                          g2_h, g2_tau_h, verdicts);
-        int all = 0;
-        const int rc = b200_plonk_batch_verify(ctx, vks.data(), vks.size(), proofs.data(), proofs.size(), links.data(),
-                                               links.size(), g2_h, g2_tau_h, &all, verdicts);
-        if (all_accepted) *all_accepted = all;
-        return rc;
+    // A proof's inputs: public inputs (the key's num_inputs) and blinders
+    b200_bundle_proof proof(b200_bundle_proof p) {
+        p.pub_inputs = copy(p.pub_inputs, 4 * p.num_inputs);
+        p.blinders = copy(p.blinders, 4 * 17);
+        return p;
+    }
+    b200_bundle_witness proof(b200_bundle_witness p) {
+        p.blinders = copy(p.blinders, 4 * 17);
+        return p;
+    }
+    b200_link_item* link_items(const b200_link_item* its, size_t k) {
+        b200_link_item* out = copy(its, k);
+        for (size_t i = 0; i < k; ++i) {
+            out[i].comm1 = copy(its[i].comm1, 8);
+            out[i].comm2 = copy(its[i].comm2, 8);
+        }
+        return out;
+    }
+    b200_settlement_link* settlement_links(const b200_settlement_link* ls, size_t k) {
+        b200_settlement_link* out = copy(ls, k);
+        for (size_t i = 0; i < k; ++i) out[i].hint_comm = copy(ls[i].hint_comm, 8);
+        return out;
     }
 };
 
+// A queued job: the context call it makes, on the copies it owns.  The call's captures point into `held`.
 struct Job {
-    enum Kind { kProve, kProveWitness, kProveBatch, kProveWitnessBatch, kLink, kLinkBatch, kSettlement, kSettlementWitness,
-                kVerify } kind = kProve;
     uint64_t ticket = 0;
-    // prove (wires: the table) and prove witness (wires: the witness vector)
-    const b200_pk* pk = nullptr;
-    const uint64_t* wires = nullptr;
-    std::vector<uint64_t> pub_inputs, blinders;
-    b200_proof* proof = nullptr;
-    uint64_t* link_poly = nullptr;
-    uint64_t* pub_inputs_out = nullptr;
-    // prove batch: the items with pub_inputs / blinders pointing into the copies below (pub_inputs, blinders: k each)
-    std::vector<b200_prove_item> items;
-    // prove witness batch: the items with blinders pointing into the copies in `blinders` (k of them)
-    std::vector<b200_witness_item> witness_items;
-    int* statuses = nullptr;
-    // link (one item) and link batch: the items with comm1 / comm2 pointing into the copies below (8 limbs each, two per
-    // item)
-    const b200_bases* srs = nullptr;
-    std::vector<b200_link_item> link_items;
-    std::vector<uint64_t> link_comms;
-    std::shared_ptr<Bundle> bundle;  // set for the sub-jobs of a bundle (they carry no ticket of their own)
-    // settlement (pk, wires, pub_inputs, blinders, proof, link_poly, pub_inputs_out, srs, statuses as above): the links
-    // with hint_comm pointing into the copies in `link_comms` (8 limbs per link)
-    std::vector<b200_settlement_link> settlement_links;
-    // verify: everything the verifier reads, owned by the job
-    std::unique_ptr<VerifyCopy> verify;
-
-    void set_settlement_links(const b200_settlement_link* ls, size_t k) {  // the worker reads the copies
-        settlement_links.assign(ls, ls + k);
-        link_comms.resize(8 * k);
-        for (size_t i = 0; i < k; ++i) {
-            std::memcpy(&link_comms[8 * i], ls[i].hint_comm, 64);
-            settlement_links[i].hint_comm = &link_comms[8 * i];
-        }
-    }
-
-    void set_link_items(const b200_link_item* its, size_t k) {  // the worker reads the copies
-        link_items.assign(its, its + k);
-        link_comms.resize(16 * k);
-        for (size_t i = 0; i < k; ++i) {
-            std::memcpy(&link_comms[16 * i], its[i].comm1, 64);
-            std::memcpy(&link_comms[16 * i + 8], its[i].comm2, 64);
-            link_items[i].comm1 = &link_comms[16 * i];
-            link_items[i].comm2 = &link_comms[16 * i + 8];
-        }
-    }
+    std::shared_ptr<Bundle> bundle;  // set for the sub-jobs of a bundle (the bundle holds their ticket)
+    Held held;
+    std::function<int(b200_ctx*)> call;
 };
+
+std::unique_ptr<Job> proof_job(const b200_bundle_proof& in) {
+    std::unique_ptr<Job> j(new Job());
+    const b200_bundle_proof p = j->held.proof(in);
+    j->call = [p](b200_ctx* ctx) {
+        return b200_plonk_prove(ctx, p.pk, p.wires, p.pub_inputs, p.blinders, p.proof, p.link_poly, nullptr);
+    };
+    return j;
+}
+
+std::unique_ptr<Job> proof_job(const b200_bundle_witness& in) {
+    std::unique_ptr<Job> j(new Job());
+    const b200_bundle_witness p = j->held.proof(in);
+    j->call = [p](b200_ctx* ctx) {
+        return b200_plonk_prove_witness(ctx, p.pk, p.witness, p.blinders, p.proof, p.link_poly, nullptr, p.pub_inputs_out);
+    };
+    return j;
+}
+
+// A single link stays on b200_plonk_link, which replays its CUDA graphs
+std::unique_ptr<Job> link_job(const b200_bases* srs, const b200_link_item& it) {
+    std::unique_ptr<Job> j(new Job());
+    const b200_link_item x = *j->held.link_items(&it, 1);
+    j->call = [srs, x](b200_ctx* ctx) {
+        return b200_plonk_link(ctx, srs, x.a1, x.len1, x.a2, x.len2, x.comm1, x.comm2, x.alignment, x.offset, x.size, x.proof,
+                               x.eta);
+    };
+    return j;
+}
 
 struct Done {
     int status = B200_OK;
@@ -144,7 +111,7 @@ struct Done {
 // A bundle: proofs first, then — once all of them are in — the link proofs between their wire-0 polynomials; one
 // ticket for the whole thing.  Its links name proofs of the same bundle only; a settlement linked against hints kept from
 // earlier proofs (the settlement arms of `NativeProofManager::handle_proof_job`, native_proof_manager.rs:514-660) is a
-// settlement job (kSettlement), one call of b200_plonk_prove_settlement.
+// settlement job, one call of b200_plonk_prove_settlement.
 // Both bundle entry points (wire tables and witness vectors) share it: a link job needs only each proof's key, proof and
 // link polynomial.
 struct BundleHint {
@@ -179,15 +146,11 @@ struct b200_pool {
     static std::unique_ptr<Job> make_link_job(const std::shared_ptr<Bundle>& b, const b200_bundle_link& l) {
         const BundleHint& pa = b->proofs[l.a];
         const BundleHint& pb = b->proofs[l.b];
-        std::unique_ptr<Job> j(new Job());
-        j->kind = Job::kLink;
-        j->bundle = b;
-        j->srs = b->srs;
         // comm1 / comm2: the `linking_wire_comm` of each hint
-        const b200_link_item it{pa.link_poly, ((size_t)1 << b200_pk_log_n(pa.pk)) + 2, pb.link_poly,
-                                ((size_t)1 << b200_pk_log_n(pb.pk)) + 2, pa.proof->wires_poly_comms[0], pb.proof->wires_poly_comms[0],
-                                l.alignment, l.offset, l.size, l.proof, nullptr};
-        j->set_link_items(&it, 1);
+        std::unique_ptr<Job> j = link_job(b->srs, {pa.link_poly, ((size_t)1 << b200_pk_log_n(pa.pk)) + 2, pb.link_poly,
+                                                   ((size_t)1 << b200_pk_log_n(pb.pk)) + 2, pa.proof->wires_poly_comms[0],
+                                                   pb.proof->wires_poly_comms[0], l.alignment, l.offset, l.size, l.proof, nullptr});
+        j->bundle = b;
         return j;
     }
 
@@ -203,37 +166,7 @@ struct b200_pool {
                 ++n_running;
             }
             Done d;
-            if (job->kind == Job::kProve) {
-                d.status = b200_plonk_prove(ctxs[w], job->pk, job->wires,
-                                            job->pub_inputs.empty() ? nullptr : job->pub_inputs.data(),
-                                            job->blinders.data(), job->proof, job->link_poly, nullptr);
-            } else if (job->kind == Job::kProveWitness) {
-                d.status = b200_plonk_prove_witness(ctxs[w], job->pk, job->wires, job->blinders.data(), job->proof, job->link_poly,
-                                                    nullptr, job->pub_inputs_out);
-            } else if (job->kind == Job::kProveBatch) {
-                d.status = b200_plonk_prove_batch(ctxs[w], job->pk, job->items.data(), job->items.size(), job->statuses);
-            } else if (job->kind == Job::kProveWitnessBatch) {
-                d.status = b200_plonk_prove_witness_batch(ctxs[w], job->pk, job->witness_items.data(), job->witness_items.size(),
-                                                          job->statuses);
-            } else if (job->kind == Job::kSettlement) {
-                d.status = b200_plonk_prove_settlement(ctxs[w], job->srs, job->pk, job->wires,
-                                                       job->pub_inputs.empty() ? nullptr : job->pub_inputs.data(),
-                                                       job->blinders.data(), job->proof, job->link_poly,
-                                                       job->settlement_links.data(), job->settlement_links.size(), job->statuses);
-            } else if (job->kind == Job::kSettlementWitness) {
-                d.status = b200_plonk_prove_settlement_witness(ctxs[w], job->srs, job->pk, job->wires, job->blinders.data(),
-                                                               job->proof, job->link_poly, job->pub_inputs_out,
-                                                               job->settlement_links.data(), job->settlement_links.size(),
-                                                               job->statuses);
-            } else if (job->kind == Job::kVerify) {
-                d.status = job->verify->run(ctxs[w]);
-            } else if (job->kind == Job::kLinkBatch) {
-                d.status = b200_plonk_link_batch(ctxs[w], job->srs, job->link_items.data(), job->link_items.size(), job->statuses);
-            } else {  // a single link stays on b200_plonk_link, which replays its CUDA graphs
-                const b200_link_item& x = job->link_items[0];
-                d.status = b200_plonk_link(ctxs[w], job->srs, x.a1, x.len1, x.a2, x.len2, x.comm1, x.comm2, x.alignment,
-                                           x.offset, x.size, x.proof, x.eta);
-            }
+            d.status = job->call(ctxs[w]);
             if (d.status != B200_OK) d.message = b200_last_error();  // this worker's thread-local message
             bool new_jobs = false;
             {
@@ -266,6 +199,63 @@ struct b200_pool {
         }
     }
 };
+
+// Queues jobs[0..n) under one new ticket: a single job, or the proof jobs of `bundle`.  Nothing is queued on a refusal.
+static int pool_push(b200_pool* pool, std::unique_ptr<Job>* jobs, size_t n, const std::shared_ptr<Bundle>& bundle,
+                     uint64_t* ticket) {
+    {
+        std::lock_guard<std::mutex> lk(pool->mu);
+        if (pool->stopping) {
+            b200::set_error("pool: shutting down");
+            return B200_ERR_INVALID;
+        }
+        const uint64_t t = pool->next_ticket++;
+        *ticket = t;
+        if (bundle) {
+            bundle->ticket = t;
+            bundle->pending = n;
+        }
+        pool->n_submitted += n;
+        pool->inflight.insert(t);
+        for (size_t i = 0; i < n; ++i) {
+            jobs[i]->ticket = t;
+            jobs[i]->bundle = bundle;
+            pool->queue.push_back(std::move(jobs[i]));
+        }
+    }
+    if (n == 1)
+        pool->cv_job.notify_one();
+    else
+        pool->cv_job.notify_all();
+    return B200_OK;
+}
+
+static int push_one(b200_pool* pool, std::unique_ptr<Job> job, uint64_t* ticket) {
+    return pool_push(pool, &job, 1, nullptr, ticket);
+}
+
+// The part of a bundle submission both entry points share, once each proof entry is checked: check the links against the
+// proofs, then queue one proof job per entry under one ticket.  Nothing is queued on a refusal.
+template <class P>
+static int bundle_push(b200_pool* pool, const char* who, const b200_bases* srs, const P* proofs, size_t n_proofs,
+                       const b200_bundle_link* links, size_t n_links, uint64_t* ticket) {
+    for (size_t i = 0; i < n_links; ++i) {
+        const b200_bundle_link& l = links[i];
+        if (l.a >= n_proofs || l.b >= n_proofs || !l.proof || !proofs[l.a].link_poly || !proofs[l.b].link_poly) {
+            b200::set_error(std::string(who) + ": a link names a proof that is missing or has no link_poly buffer");
+            return B200_ERR_INVALID;
+        }
+    }
+    std::shared_ptr<Bundle> b(new Bundle());
+    b->srs = srs;
+    b->links.assign(links, links + n_links);
+    std::vector<std::unique_ptr<Job>> jobs;
+    for (size_t i = 0; i < n_proofs; ++i) {
+        b->proofs.push_back({proofs[i].pk, proofs[i].proof, proofs[i].link_poly});
+        jobs.push_back(proof_job(proofs[i]));
+    }
+    return pool_push(pool, jobs.data(), jobs.size(), b, ticket);
+}
 
 extern "C" {
 
@@ -311,23 +301,6 @@ b200_ctx* b200_pool_ctx(b200_pool* pool, unsigned worker) {
     return pool->ctxs[worker];
 }
 
-static int pool_push(b200_pool* pool, std::unique_ptr<Job> job, uint64_t* ticket) {
-    {
-        std::lock_guard<std::mutex> lk(pool->mu);
-        if (pool->stopping) {
-            b200::set_error("pool: shutting down");
-            return B200_ERR_INVALID;
-        }
-        job->ticket = pool->next_ticket++;
-        *ticket = job->ticket;
-        ++pool->n_submitted;
-        pool->inflight.insert(job->ticket);
-        pool->queue.push_back(std::move(job));
-    }
-    pool->cv_job.notify_one();
-    return B200_OK;
-}
-
 int b200_pool_submit_prove(b200_pool* pool, const b200_pk* pk, const uint64_t* wires,
                            const uint64_t* pub_inputs, size_t num_inputs, const uint64_t* blinders,
                            b200_proof* proof, uint64_t* link_poly, uint64_t* ticket) {
@@ -340,15 +313,7 @@ int b200_pool_submit_prove(b200_pool* pool, const b200_pk* pk, const uint64_t* w
         b200::set_error("pool_submit_prove: num_inputs does not match the proving key");
         return B200_ERR_INVALID;
     }
-    std::unique_ptr<Job> j(new Job());
-    j->kind = Job::kProve;
-    j->pk = pk;
-    j->wires = wires;
-    j->pub_inputs.assign(pub_inputs, pub_inputs + 4 * num_inputs);
-    j->blinders.assign(blinders, blinders + 4 * 17);
-    j->proof = proof;
-    j->link_poly = link_poly;
-    return pool_push(pool, std::move(j), ticket);
+    return push_one(pool, proof_job(b200_bundle_proof{pk, wires, pub_inputs, num_inputs, blinders, proof, link_poly}), ticket);
     B200_CATCH
 }
 
@@ -363,15 +328,7 @@ int b200_pool_submit_prove_witness(b200_pool* pool, const b200_pk* pk, const uin
         b200::set_error("pool_submit_prove_witness: the key holds no wiring (made by b200_plonk_preprocess)");
         return B200_ERR_INVALID;
     }
-    std::unique_ptr<Job> j(new Job());
-    j->kind = Job::kProveWitness;
-    j->pk = pk;
-    j->wires = witness;
-    j->blinders.assign(blinders, blinders + 4 * 17);
-    j->proof = proof;
-    j->link_poly = link_poly;
-    j->pub_inputs_out = pub_inputs_out;
-    return pool_push(pool, std::move(j), ticket);
+    return push_one(pool, proof_job(b200_bundle_witness{pk, witness, blinders, proof, link_poly, pub_inputs_out}), ticket);
     B200_CATCH
 }
 
@@ -389,19 +346,13 @@ int b200_pool_submit_prove_batch(b200_pool* pool, const b200_pk* pk, const b200_
             return B200_ERR_INVALID;
         }
     std::unique_ptr<Job> j(new Job());
-    j->kind = Job::kProveBatch;
-    j->pk = pk;
-    j->statuses = statuses;
-    j->pub_inputs.resize(4 * ni * k);
-    j->blinders.resize(4 * 17 * k);
-    j->items.assign(items, items + k);
-    for (size_t i = 0; i < k; ++i) {  // the worker reads the copies
-        if (ni) std::memcpy(&j->pub_inputs[4 * ni * i], items[i].pub_inputs, 32 * ni);
-        std::memcpy(&j->blinders[4 * 17 * i], items[i].blinders, 32 * 17);
-        j->items[i].pub_inputs = ni ? &j->pub_inputs[4 * ni * i] : nullptr;
-        j->items[i].blinders = &j->blinders[4 * 17 * i];
+    b200_prove_item* its = j->held.copy(items, k);
+    for (size_t i = 0; i < k; ++i) {
+        its[i].pub_inputs = j->held.copy(items[i].pub_inputs, 4 * ni);
+        its[i].blinders = j->held.copy(items[i].blinders, 4 * 17);
     }
-    return pool_push(pool, std::move(j), ticket);
+    j->call = [pk, its, k, statuses](b200_ctx* ctx) { return b200_plonk_prove_batch(ctx, pk, its, k, statuses); };
+    return push_one(pool, std::move(j), ticket);
     B200_CATCH
 }
 
@@ -422,16 +373,10 @@ int b200_pool_submit_prove_witness_batch(b200_pool* pool, const b200_pk* pk, con
             return B200_ERR_INVALID;
         }
     std::unique_ptr<Job> j(new Job());
-    j->kind = Job::kProveWitnessBatch;
-    j->pk = pk;
-    j->statuses = statuses;
-    j->blinders.resize(4 * 17 * k);
-    j->witness_items.assign(items, items + k);
-    for (size_t i = 0; i < k; ++i) {  // the worker reads the copies
-        std::memcpy(&j->blinders[4 * 17 * i], items[i].blinders, 32 * 17);
-        j->witness_items[i].blinders = &j->blinders[4 * 17 * i];
-    }
-    return pool_push(pool, std::move(j), ticket);
+    b200_witness_item* its = j->held.copy(items, k);
+    for (size_t i = 0; i < k; ++i) its[i].blinders = j->held.copy(items[i].blinders, 4 * 17);
+    j->call = [pk, its, k, statuses](b200_ctx* ctx) { return b200_plonk_prove_witness_batch(ctx, pk, its, k, statuses); };
+    return push_one(pool, std::move(j), ticket);
     B200_CATCH
 }
 
@@ -444,12 +389,7 @@ int b200_pool_submit_link(b200_pool* pool, const b200_bases* srs, const uint64_t
         b200::set_error("pool_submit_link: null argument");
         return B200_ERR_INVALID;
     }
-    std::unique_ptr<Job> j(new Job());
-    j->kind = Job::kLink;
-    j->srs = srs;
-    const b200_link_item it{a1, len1, a2, len2, comm1, comm2, alignment, offset, size, proof, nullptr};
-    j->set_link_items(&it, 1);
-    return pool_push(pool, std::move(j), ticket);
+    return push_one(pool, link_job(srs, {a1, len1, a2, len2, comm1, comm2, alignment, offset, size, proof, nullptr}), ticket);
     B200_CATCH
 }
 
@@ -466,45 +406,10 @@ int b200_pool_submit_link_batch(b200_pool* pool, const b200_bases* srs, const b2
             return B200_ERR_INVALID;
         }
     std::unique_ptr<Job> j(new Job());
-    j->kind = Job::kLinkBatch;
-    j->srs = srs;
-    j->statuses = statuses;
-    j->set_link_items(items, k);
-    return pool_push(pool, std::move(j), ticket);
+    const b200_link_item* its = j->held.link_items(items, k);
+    j->call = [srs, its, k, statuses](b200_ctx* ctx) { return b200_plonk_link_batch(ctx, srs, its, k, statuses); };
+    return push_one(pool, std::move(j), ticket);
     B200_CATCH
-}
-
-// The part of a bundle submission both entry points share: check the links against the proofs' hints, then queue the
-// proof jobs (each already filled in but for its `bundle`) under one ticket.  Nothing is queued on a refusal.
-static int bundle_push(b200_pool* pool, const char* who, const b200_bases* srs, std::vector<BundleHint> hints,
-                       const b200_bundle_link* links, size_t n_links, std::vector<std::unique_ptr<Job>> jobs, uint64_t* ticket) {
-    for (size_t i = 0; i < n_links; ++i) {
-        const b200_bundle_link& l = links[i];
-        if (l.a >= hints.size() || l.b >= hints.size() || !l.proof || !hints[l.a].link_poly || !hints[l.b].link_poly) {
-            b200::set_error(std::string(who) + ": a link names a proof that is missing or has no link_poly buffer");
-            return B200_ERR_INVALID;
-        }
-    }
-    std::shared_ptr<Bundle> b(new Bundle());
-    b->srs = srs;
-    b->proofs = std::move(hints);
-    b->links.assign(links, links + n_links);
-    b->pending = jobs.size();
-    for (auto& j : jobs) j->bundle = b;
-    {
-        std::lock_guard<std::mutex> lk(pool->mu);
-        if (pool->stopping) {
-            b200::set_error("pool: shutting down");
-            return B200_ERR_INVALID;
-        }
-        b->ticket = pool->next_ticket++;
-        *ticket = b->ticket;
-        pool->n_submitted += jobs.size();
-        pool->inflight.insert(b->ticket);
-        for (auto& j : jobs) pool->queue.push_back(std::move(j));
-    }
-    pool->cv_job.notify_all();
-    return B200_OK;
 }
 
 int b200_pool_submit_bundle(b200_pool* pool, const b200_bases* srs, const b200_bundle_proof* proofs, size_t n_proofs,
@@ -522,22 +427,7 @@ int b200_pool_submit_bundle(b200_pool* pool, const b200_bases* srs, const b200_b
             return B200_ERR_INVALID;
         }
     }
-    std::vector<BundleHint> hints;
-    std::vector<std::unique_ptr<Job>> jobs;
-    for (size_t i = 0; i < n_proofs; ++i) {
-        const b200_bundle_proof& p = proofs[i];
-        hints.push_back({p.pk, p.proof, p.link_poly});
-        std::unique_ptr<Job> j(new Job());
-        j->kind = Job::kProve;
-        j->pk = p.pk;
-        j->wires = p.wires;
-        j->pub_inputs.assign(p.pub_inputs, p.pub_inputs + 4 * p.num_inputs);
-        j->blinders.assign(p.blinders, p.blinders + 4 * 17);
-        j->proof = p.proof;
-        j->link_poly = p.link_poly;
-        jobs.push_back(std::move(j));
-    }
-    return bundle_push(pool, "pool_submit_bundle", srs, std::move(hints), links, n_links, std::move(jobs), ticket);
+    return bundle_push(pool, "pool_submit_bundle", srs, proofs, n_proofs, links, n_links, ticket);
     B200_CATCH
 }
 
@@ -560,22 +450,7 @@ int b200_pool_submit_bundle_witness(b200_pool* pool, const b200_bases* srs, cons
             return B200_ERR_INVALID;
         }
     }
-    std::vector<BundleHint> hints;
-    std::vector<std::unique_ptr<Job>> jobs;
-    for (size_t i = 0; i < n_proofs; ++i) {
-        const b200_bundle_witness& p = proofs[i];
-        hints.push_back({p.pk, p.proof, p.link_poly});
-        std::unique_ptr<Job> j(new Job());
-        j->kind = Job::kProveWitness;
-        j->pk = p.pk;
-        j->wires = p.witness;
-        j->blinders.assign(p.blinders, p.blinders + 4 * 17);
-        j->proof = p.proof;
-        j->link_poly = p.link_poly;
-        j->pub_inputs_out = p.pub_inputs_out;
-        jobs.push_back(std::move(j));
-    }
-    return bundle_push(pool, "pool_submit_bundle_witness", srs, std::move(hints), links, n_links, std::move(jobs), ticket);
+    return bundle_push(pool, "pool_submit_bundle_witness", srs, proofs, n_proofs, links, n_links, ticket);
     B200_CATCH
 }
 
@@ -595,17 +470,13 @@ int b200_pool_submit_settlement(b200_pool* pool, const b200_bases* srs, const b2
     const int rc = b200::settlement_check(srs, proof->pk, /*witness=*/false, links, n_links, who);
     if (rc != B200_OK) return rc;
     std::unique_ptr<Job> j(new Job());
-    j->kind = Job::kSettlement;
-    j->srs = srs;
-    j->pk = proof->pk;
-    j->wires = proof->wires;
-    j->pub_inputs.assign(proof->pub_inputs, proof->pub_inputs + 4 * proof->num_inputs);
-    j->blinders.assign(proof->blinders, proof->blinders + 4 * 17);
-    j->proof = proof->proof;
-    j->link_poly = proof->link_poly;
-    j->statuses = statuses;
-    j->set_settlement_links(links, n_links);
-    return pool_push(pool, std::move(j), ticket);
+    const b200_bundle_proof p = j->held.proof(*proof);
+    const b200_settlement_link* ls = j->held.settlement_links(links, n_links);
+    j->call = [srs, p, ls, n_links, statuses](b200_ctx* ctx) {
+        return b200_plonk_prove_settlement(ctx, srs, p.pk, p.wires, p.pub_inputs, p.blinders, p.proof, p.link_poly, ls, n_links,
+                                           statuses);
+    };
+    return push_one(pool, std::move(j), ticket);
     B200_CATCH
 }
 
@@ -620,17 +491,13 @@ int b200_pool_submit_settlement_witness(b200_pool* pool, const b200_bases* srs, 
     const int rc = b200::settlement_check(srs, proof->pk, /*witness=*/true, links, n_links, who);
     if (rc != B200_OK) return rc;
     std::unique_ptr<Job> j(new Job());
-    j->kind = Job::kSettlementWitness;
-    j->srs = srs;
-    j->pk = proof->pk;
-    j->wires = proof->witness;
-    j->blinders.assign(proof->blinders, proof->blinders + 4 * 17);
-    j->proof = proof->proof;
-    j->link_poly = proof->link_poly;
-    j->pub_inputs_out = proof->pub_inputs_out;
-    j->statuses = statuses;
-    j->set_settlement_links(links, n_links);
-    return pool_push(pool, std::move(j), ticket);
+    const b200_bundle_witness p = j->held.proof(*proof);
+    const b200_settlement_link* ls = j->held.settlement_links(links, n_links);
+    j->call = [srs, p, ls, n_links, statuses](b200_ctx* ctx) {
+        return b200_plonk_prove_settlement_witness(ctx, srs, p.pk, p.witness, p.blinders, p.proof, p.link_poly, p.pub_inputs_out,
+                                                   ls, n_links, statuses);
+    };
+    return push_one(pool, std::move(j), ticket);
     B200_CATCH
 }
 
@@ -654,14 +521,38 @@ int b200_pool_submit_verify(b200_pool* pool, int mode, const b200_verifying_key*
         b200::set_error(std::string(who) + ": " + bad);
         return B200_ERR_INVALID;
     }
+    // before any copy: the copy of a proof's public inputs reads vks[proofs[i].vk]
     const int rc = b200::verify_check(who, vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h);
     if (rc != B200_OK) return rc;
     std::unique_ptr<Job> j(new Job());
-    j->kind = Job::kVerify;
-    j->verify.reset(new VerifyCopy(mode, vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h));
-    j->verify->all_accepted = all_accepted;
-    j->verify->verdicts = verdicts;
-    return pool_push(pool, std::move(j), ticket);
+    Held& h = j->held;
+    b200_verifying_key* v = h.copy(vks, n_vks);
+    for (size_t i = 0; i < n_vks; ++i) {
+        v[i].k = h.copy(vks[i].k, 20);
+        v[i].selector_comms = h.copy(vks[i].selector_comms, 104);
+        v[i].sigma_comms = h.copy(vks[i].sigma_comms, 40);
+    }
+    b200_batch_proof* p = h.copy(proofs, n_proofs);
+    for (size_t i = 0; i < n_proofs; ++i) {
+        p[i].pub_inputs = h.copy(proofs[i].pub_inputs, 4 * vks[proofs[i].vk].num_inputs);
+        p[i].proof = h.copy(proofs[i].proof, 1);
+    }
+    b200_batch_link* l = h.copy(links, n_links);
+    for (size_t i = 0; i < n_links; ++i) {
+        l[i].comm1 = h.copy(links[i].comm1, 8);
+        l[i].comm2 = h.copy(links[i].comm2, 8);
+        l[i].proof = h.copy(links[i].proof, 1);
+    }
+    const uint64_t* g2 = h.copy(g2_h, 16);
+    const uint64_t* g2_tau = h.copy(g2_tau_h, 16);
+    j->call = [=](b200_ctx* ctx) {  // mode 0: b200_plonk_verify_each, 1: b200_plonk_batch_verify
+        if (mode == 0) return b200_plonk_verify_each(ctx, v, n_vks, p, n_proofs, l, n_links, g2, g2_tau, verdicts);
+        int all = 0;
+        const int st = b200_plonk_batch_verify(ctx, v, n_vks, p, n_proofs, l, n_links, g2, g2_tau, &all, verdicts);
+        if (all_accepted) *all_accepted = all;
+        return st;
+    };
+    return push_one(pool, std::move(j), ticket);
     B200_CATCH
 }
 
@@ -743,6 +634,7 @@ struct b200_box {
 };
 struct b200_box_srs {
     std::vector<b200_bases*> per_dev;
+    const b200_box* owner = nullptr;  // the box that made it
 };
 struct b200_box_pk {
     std::vector<b200_pk*> per_dev;
@@ -796,8 +688,56 @@ int box_witness_device(b200_box* box, const char* who, const uint64_t* const* ws
     return B200_OK;
 }
 
-bool box_owns(const b200_box* box, const b200_box_pk* pk) {
-    return pk && pk->owner == box && pk->per_dev.size() == box->pools.size();
+// A key or SRS this box made.  One made by another box holds memory of that box's contexts, even when both boxes have as
+// many devices.
+template <class T>
+bool box_owns(const b200_box* box, const T* x) {
+    return x && x->owner == box && x->per_dev.size() == box->pools.size();
+}
+
+// Runs submit(box->pools[d], &t) and returns the box ticket: d << kBoxTicketShift | t
+template <class Submit>
+int box_submit(b200_box* box, int d, uint64_t* ticket, Submit submit) {
+    uint64_t t = 0;
+    const int rc = submit(box->pools[d], &t);
+    if (rc != B200_OK) return rc;
+    *ticket = ((uint64_t)d << kBoxTicketShift) | t;
+    return B200_OK;
+}
+
+// Every proof of a bundle with its box key: all keys (and the SRS, if any) must be this box's
+int box_bundle_check(const b200_box* box, const char* who, const b200_box_srs* srs, const b200_box_pk* const* pks, size_t n) {
+    if (srs && !box_owns(box, srs)) {
+        b200::set_error(std::string(who) + ": SRS of another box");
+        return B200_ERR_INVALID;
+    }
+    for (size_t i = 0; i < n; ++i)
+        if (!box_owns(box, pks[i])) {
+            b200::set_error(std::string(who) + ": proof " + std::to_string(i) + " has no key or a key of another box");
+            return B200_ERR_INVALID;
+        }
+    return B200_OK;
+}
+
+// One key per device, made by make(device's first context, device's SRS, &key) from the same arguments
+template <class Make>
+int box_replicate(b200_box* box, const char* who, const b200_box_srs* srs, b200_box_pk** out, Make make) {
+    if (!box || !out || !box_owns(box, srs)) {
+        b200::set_error(std::string(who) + ": null argument or SRS of another box");
+        return B200_ERR_INVALID;
+    }
+    std::unique_ptr<b200_box_pk> pk(new b200_box_pk());
+    pk->per_dev.assign(box->pools.size(), nullptr);
+    pk->owner = box;
+    for (size_t i = 0; i < box->pools.size(); ++i) {
+        const int rc = make(b200_pool_ctx(box->pools[i], 0), srs->per_dev[i], &pk->per_dev[i]);
+        if (rc != B200_OK) {
+            b200_box_pk_free(box, pk.release());
+            return rc;
+        }
+    }
+    *out = pk.release();
+    return B200_OK;
 }
 }  // namespace
 
@@ -849,6 +789,7 @@ int b200_box_srs_load(b200_box* box, const uint8_t* points64, size_t n, int wind
     if (!box || !points64 || !out) return B200_ERR_INVALID;
     std::unique_ptr<b200_box_srs> s(new b200_box_srs());
     s->per_dev.assign(box->pools.size(), nullptr);
+    s->owner = box;
     for (size_t i = 0; i < box->pools.size(); ++i) {
         // the on-curve assertion of srs.rs:178-179 once is enough: every device gets the same bytes
         const int rc = b200_bases_load(b200_pool_ctx(box->pools[i], 0), points64, n, window_bits, i == 0 ? check_on_curve : 0, &s->per_dev[i]);
@@ -872,20 +813,9 @@ void b200_box_pk_free(b200_box* box, b200_box_pk* pk) {
 int b200_box_preprocess(b200_box* box, const b200_box_srs* srs, unsigned log_n, size_t num_inputs, const uint64_t* selectors_evals,
                         const uint64_t* perm, const uint64_t* k, b200_box_pk** out) {
     B200_TRY
-    if (!box || !srs || !out || srs->per_dev.size() != box->pools.size()) return B200_ERR_INVALID;
-    std::unique_ptr<b200_box_pk> pk(new b200_box_pk());
-    pk->per_dev.assign(box->pools.size(), nullptr);
-    pk->owner = box;
-    for (size_t i = 0; i < box->pools.size(); ++i) {
-        const int rc = b200_plonk_preprocess(b200_pool_ctx(box->pools[i], 0), srs->per_dev[i], log_n, num_inputs, selectors_evals, perm, k,
-                                             &pk->per_dev[i]);
-        if (rc != B200_OK) {
-            b200_box_pk_free(box, pk.release());
-            return rc;
-        }
-    }
-    *out = pk.release();
-    return B200_OK;
+    return box_replicate(box, "box_preprocess", srs, out, [&](b200_ctx* ctx, const b200_bases* s, b200_pk** pk) {
+        return b200_plonk_preprocess(ctx, s, log_n, num_inputs, selectors_evals, perm, k, pk);
+    });
     B200_CATCH
 }
 
@@ -897,16 +827,14 @@ int b200_box_pk_verifying_key(const b200_box_pk* pk, uint64_t* selector_comms, u
 int b200_box_submit_prove(b200_box* box, const b200_box_pk* pk, const uint64_t* wires, const uint64_t* pub_inputs, size_t num_inputs,
                           const uint64_t* blinders, b200_proof* proof, uint64_t* link_poly, uint64_t* ticket) {
     B200_TRY
-    if (!box || !pk || !ticket || pk->per_dev.size() != box->pools.size()) {
+    if (!box || !ticket || !box_owns(box, pk)) {
         b200::set_error("box_submit_prove: null argument or key of another box");
         return B200_ERR_INVALID;
     }
     const int d = box_least_loaded(box);
-    uint64_t t = 0;
-    const int rc = b200_pool_submit_prove(box->pools[d], pk->per_dev[d], wires, pub_inputs, num_inputs, blinders, proof, link_poly, &t);
-    if (rc != B200_OK) return rc;
-    *ticket = ((uint64_t)d << kBoxTicketShift) | t;
-    return B200_OK;
+    return box_submit(box, d, ticket, [&](b200_pool* p, uint64_t* t) {
+        return b200_pool_submit_prove(p, pk->per_dev[d], wires, pub_inputs, num_inputs, blinders, proof, link_poly, t);
+    });
     B200_CATCH
 }
 
@@ -917,20 +845,14 @@ int b200_box_submit_bundle(b200_box* box, const b200_box_srs* srs, const b200_bo
         b200::set_error("box_submit_bundle: null argument");
         return B200_ERR_INVALID;
     }
+    const int rc = box_bundle_check(box, "box_submit_bundle", srs, pks, n_proofs);
+    if (rc != B200_OK) return rc;
     const int d = box_least_loaded(box);  // a bundle stays on one device: its link proofs need its proofs' polynomials
     std::vector<b200_bundle_proof> local(proofs, proofs + n_proofs);
-    for (size_t i = 0; i < n_proofs; ++i) {
-        if (!pks[i] || pks[i]->per_dev.size() != box->pools.size()) {
-            b200::set_error("box_submit_bundle: missing key");
-            return B200_ERR_INVALID;
-        }
-        local[i].pk = pks[i]->per_dev[d];
-    }
-    uint64_t t = 0;
-    const int rc = b200_pool_submit_bundle(box->pools[d], srs ? srs->per_dev[d] : nullptr, local.data(), n_proofs, links, n_links, &t);
-    if (rc != B200_OK) return rc;
-    *ticket = ((uint64_t)d << kBoxTicketShift) | t;
-    return B200_OK;
+    for (size_t i = 0; i < n_proofs; ++i) local[i].pk = pks[i]->per_dev[d];
+    return box_submit(box, d, ticket, [&](b200_pool* p, uint64_t* t) {
+        return b200_pool_submit_bundle(p, srs ? srs->per_dev[d] : nullptr, local.data(), n_proofs, links, n_links, t);
+    });
     B200_CATCH
 }
 
@@ -938,23 +860,9 @@ int b200_box_preprocess_wiring(b200_box* box, const b200_box_srs* srs, unsigned 
                                const uint64_t* selectors_evals, const unsigned* wire_vars, size_t num_vars, const uint64_t* k,
                                b200_box_pk** out) {
     B200_TRY
-    if (!box || !srs || !out || srs->per_dev.size() != box->pools.size()) {
-        b200::set_error("box_preprocess_wiring: null argument or SRS of another box");
-        return B200_ERR_INVALID;
-    }
-    std::unique_ptr<b200_box_pk> pk(new b200_box_pk());
-    pk->per_dev.assign(box->pools.size(), nullptr);
-    pk->owner = box;
-    for (size_t i = 0; i < box->pools.size(); ++i) {
-        const int rc = b200_plonk_preprocess_wiring(b200_pool_ctx(box->pools[i], 0), srs->per_dev[i], log_n, num_inputs,
-                                                    selectors_evals, wire_vars, num_vars, k, &pk->per_dev[i]);
-        if (rc != B200_OK) {
-            b200_box_pk_free(box, pk.release());
-            return rc;
-        }
-    }
-    *out = pk.release();
-    return B200_OK;
+    return box_replicate(box, "box_preprocess_wiring", srs, out, [&](b200_ctx* ctx, const b200_bases* s, b200_pk** pk) {
+        return b200_plonk_preprocess_wiring(ctx, s, log_n, num_inputs, selectors_evals, wire_vars, num_vars, k, pk);
+    });
     B200_CATCH
 }
 
@@ -966,13 +874,11 @@ int b200_box_submit_prove_witness(b200_box* box, const b200_box_pk* pk, const ui
         return B200_ERR_INVALID;
     }
     int d = 0;
-    int rc = box_witness_device(box, "box_submit_prove_witness", &witness, 1, &d);
+    const int rc = box_witness_device(box, "box_submit_prove_witness", &witness, 1, &d);
     if (rc != B200_OK) return rc;
-    uint64_t t = 0;
-    rc = b200_pool_submit_prove_witness(box->pools[d], pk->per_dev[d], witness, blinders, proof, link_poly, pub_inputs_out, &t);
-    if (rc != B200_OK) return rc;
-    *ticket = ((uint64_t)d << kBoxTicketShift) | t;
-    return B200_OK;
+    return box_submit(box, d, ticket, [&](b200_pool* p, uint64_t* t) {
+        return b200_pool_submit_prove_witness(p, pk->per_dev[d], witness, blinders, proof, link_poly, pub_inputs_out, t);
+    });
     B200_CATCH
 }
 
@@ -980,35 +886,36 @@ int b200_box_submit_bundle_witness(b200_box* box, const b200_box_srs* srs, const
                                    const b200_bundle_witness* proofs, size_t n_proofs, const b200_bundle_link* links,
                                    size_t n_links, uint64_t* ticket) {
     B200_TRY
-    if (!box || !pks || !proofs || n_proofs == 0 || !ticket || (n_links && (!srs || srs->per_dev.size() != box->pools.size()))) {
-        b200::set_error("box_submit_bundle_witness: null argument");
+    const char* who = "box_submit_bundle_witness";
+    if (!box || !pks || !proofs || n_proofs == 0 || !ticket || (n_links && !srs)) {
+        b200::set_error(std::string(who) + ": null argument");
         return B200_ERR_INVALID;
     }
+    int rc = box_bundle_check(box, who, srs, pks, n_proofs);
+    if (rc != B200_OK) return rc;
     std::vector<const uint64_t*> ws(n_proofs);
     for (size_t i = 0; i < n_proofs; ++i) {
-        if (!box_owns(box, pks[i]) || !proofs[i].witness) {
-            b200::set_error("box_submit_bundle_witness: proof " + std::to_string(i) + " has no witness or a key of another box");
+        if (!proofs[i].witness) {
+            b200::set_error(std::string(who) + ": proof " + std::to_string(i) + " has no witness");
             return B200_ERR_INVALID;
         }
         ws[i] = proofs[i].witness;
     }
     int d = 0;  // a bundle stays on one device: its link proofs need its proofs' polynomials
-    int rc = box_witness_device(box, "box_submit_bundle_witness", ws.data(), n_proofs, &d);
+    rc = box_witness_device(box, who, ws.data(), n_proofs, &d);
     if (rc != B200_OK) return rc;
     std::vector<b200_bundle_witness> local(proofs, proofs + n_proofs);
     for (size_t i = 0; i < n_proofs; ++i) local[i].pk = pks[i]->per_dev[d];
-    uint64_t t = 0;
-    rc = b200_pool_submit_bundle_witness(box->pools[d], srs ? srs->per_dev[d] : nullptr, local.data(), n_proofs, links, n_links, &t);
-    if (rc != B200_OK) return rc;
-    *ticket = ((uint64_t)d << kBoxTicketShift) | t;
-    return B200_OK;
+    return box_submit(box, d, ticket, [&](b200_pool* p, uint64_t* t) {
+        return b200_pool_submit_bundle_witness(p, srs ? srs->per_dev[d] : nullptr, local.data(), n_proofs, links, n_links, t);
+    });
     B200_CATCH
 }
 
 // The device a box settlement runs on: its input (wire table or witness) and every hint polynomial count
 static int box_settlement_device(b200_box* box, const char* who, const b200_box_srs* srs, const b200_box_pk* pk,
                                  const uint64_t* input, const b200_settlement_link* links, size_t n_links, int* out) {
-    if (!box_owns(box, pk) || !srs || srs->per_dev.size() != box->pools.size() || !input || (n_links && !links)) {
+    if (!box_owns(box, pk) || !box_owns(box, srs) || !input || (n_links && !links)) {
         b200::set_error(std::string(who) + ": null argument, or a key or SRS of another box");
         return B200_ERR_INVALID;
     }
@@ -1026,15 +933,13 @@ int b200_box_submit_settlement(b200_box* box, const b200_box_srs* srs, const b20
         return B200_ERR_INVALID;
     }
     int d = 0;
-    int rc = box_settlement_device(box, "box_submit_settlement", srs, pk, proof->wires, links, n_links, &d);
+    const int rc = box_settlement_device(box, "box_submit_settlement", srs, pk, proof->wires, links, n_links, &d);
     if (rc != B200_OK) return rc;
     b200_bundle_proof local = *proof;
     local.pk = pk->per_dev[d];
-    uint64_t t = 0;
-    rc = b200_pool_submit_settlement(box->pools[d], srs->per_dev[d], &local, links, n_links, statuses, &t);
-    if (rc != B200_OK) return rc;
-    *ticket = ((uint64_t)d << kBoxTicketShift) | t;
-    return B200_OK;
+    return box_submit(box, d, ticket, [&](b200_pool* p, uint64_t* t) {
+        return b200_pool_submit_settlement(p, srs->per_dev[d], &local, links, n_links, statuses, t);
+    });
     B200_CATCH
 }
 
@@ -1047,15 +952,13 @@ int b200_box_submit_settlement_witness(b200_box* box, const b200_box_srs* srs, c
         return B200_ERR_INVALID;
     }
     int d = 0;
-    int rc = box_settlement_device(box, "box_submit_settlement_witness", srs, pk, proof->witness, links, n_links, &d);
+    const int rc = box_settlement_device(box, "box_submit_settlement_witness", srs, pk, proof->witness, links, n_links, &d);
     if (rc != B200_OK) return rc;
     b200_bundle_witness local = *proof;
     local.pk = pk->per_dev[d];
-    uint64_t t = 0;
-    rc = b200_pool_submit_settlement_witness(box->pools[d], srs->per_dev[d], &local, links, n_links, statuses, &t);
-    if (rc != B200_OK) return rc;
-    *ticket = ((uint64_t)d << kBoxTicketShift) | t;
-    return B200_OK;
+    return box_submit(box, d, ticket, [&](b200_pool* p, uint64_t* t) {
+        return b200_pool_submit_settlement_witness(p, srs->per_dev[d], &local, links, n_links, statuses, t);
+    });
     B200_CATCH
 }
 
@@ -1067,13 +970,11 @@ int b200_box_submit_verify(b200_box* box, int mode, const b200_verifying_key* vk
         b200::set_error("box_submit_verify: null box or ticket");
         return B200_ERR_INVALID;
     }
-    const int d = box_least_loaded(box);  // the job reads only its host copies: any device will do
-    uint64_t t = 0;
-    const int rc = b200_pool_submit_verify(box->pools[d], mode, vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h,
-                                           all_accepted, verdicts, &t);
-    if (rc != B200_OK) return rc;
-    *ticket = ((uint64_t)d << kBoxTicketShift) | t;
-    return B200_OK;
+    // the job reads only its host copies: any device will do
+    return box_submit(box, box_least_loaded(box), ticket, [&](b200_pool* p, uint64_t* t) {
+        return b200_pool_submit_verify(p, mode, vks, n_vks, proofs, n_proofs, links, n_links, g2_h, g2_tau_h, all_accepted,
+                                       verdicts, t);
+    });
     B200_CATCH
 }
 

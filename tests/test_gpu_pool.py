@@ -4,6 +4,7 @@ the single-context call with the same witness and blinders (hence to the oracle'
 test_gpu_plonk pins), whatever worker ran them and in whatever order they finished; a failing job
 reports ITS status and message to the thread that waits for it and leaves the pool usable; link
 jobs match the direct call."""
+import ctypes as C
 import threading
 
 import numpy as np
@@ -11,7 +12,7 @@ import pytest
 
 from renegade_b200 import synth
 from renegade_b200._lib import B200Error
-from renegade_b200.backend import GroupLayout, PlonkKzgSnark, ProverPool, link_proofs
+from renegade_b200.backend import B200Proof, GroupLayout, PlonkKzgSnark, ProverPool, link_proofs
 
 pytestmark = pytest.mark.gpu
 
@@ -97,24 +98,29 @@ def test_pool_failed_job_reports_its_error_and_pool_survives(ctx, oracle, pyorac
         pool.close()
 
 
-def test_pool_destroy_drains_the_queue(ctx, oracle, pyoracle):
+def test_pool_destroy_drains_the_queue_into_caller_buffers(ctx, oracle, pyoracle):
     """`b200_pool_destroy` finishes what is queued (the reference's proof manager answers every job it took off
-    the queue): results land in the caller's buffers although nobody waited."""
+    the queue): results land in the caller's buffers although nobody waited.  The jobs go through the C entry point,
+    so the caller owns the proof structs and reads them after the destroy."""
     log_n = 9
     circ, tau, srs = make(ctx, oracle, pyoracle, log_n, seed=23)
     bases = ctx.load_bases(srs)  # keys made on another context of the device are usable by the workers
     pk = PlonkKzgSnark.preprocess(ctx, bases, log_n, circ.num_inputs, circ.selectors, circ.perm, circ.k)
     wires = np.ascontiguousarray(circ.wires, dtype=np.uint64)
+    pub = np.ascontiguousarray(circ.pub_inputs, dtype=np.uint64)
     bl = synth.splitmix_blinders(77)
     ref, _ = PlonkKzgSnark.prove_with_link_hint(ctx, pk, circ.wires, circ.pub_inputs, bl)
     pool = ProverPool(0, workers=2)
-    tickets = [pool.submit_prove(pk, wires.ctypes.data, circ.pub_inputs, bl, keep=wires) for _ in range(8)]
-    proofs = [pool._keep[t][0] for t in tickets]  # the output structs the jobs write into
-    held = dict(pool._keep)  # keep the buffers alive across close()
+    proofs = [B200Proof() for _ in range(8)]
+    ticket = C.c_uint64()
+    ptr = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+    for p in proofs:
+        assert pool._lib.b200_pool_submit_prove(pool._h, pk._h, ptr(wires), ptr(pub), circ.num_inputs, ptr(bl),
+                                                C.byref(p), None, C.byref(ticket)) == 0
+    assert pool.stats()["submitted"] == 8
     pool.close()
     for p in proofs:
         assert bytes(p) == bytes(ref)
-    del held
     pk.free()
 
 

@@ -165,16 +165,16 @@ def test_context_checks_run_before_the_library(parts):
 
 def test_pool_checks_run_before_the_library(parts):
     pool = ProverPool.__new__(ProverPool)
-    pool._lib, pool._h, pool._keep, pool._borrowed = _NoLibrary(), None, {}, []
+    pool._lib, pool._h, pool._jobs, pool._borrowed = _NoLibrary(), None, {}, []
     srs, pk = _Srs(), _key()
     _checks(lambda *a: pool.submit_settlement(srs, pk, *a), lambda k, *a: pool.submit_settlement_witness(srs, k, *a), srs, pk,
             parts)
-    assert pool._keep == {}
+    assert pool._jobs == {}
 
 
 def test_box_checks_run_before_the_library(parts):
     box = ProverBox.__new__(ProverBox)
-    box._lib, box._h, box._keep, box.devices = _NoLibrary(), None, {}, [0]
+    box._lib, box._h, box._jobs, box.devices = _NoLibrary(), None, {}, [0]
     wired, tables, stranger = C.c_void_p(0x10), C.c_void_p(0x20), C.c_void_p(0x30)
     box._shapes = {0x10: _key(), 0x20: _key(num_vars=0)}
     _checks(lambda *a: box.submit_settlement(None, wired, *a),
@@ -182,4 +182,4 @@ def test_box_checks_run_before_the_library(parts):
     wit, wires, pub, bl, hint, lay = parts
     _refused(box.submit_settlement, None, stranger, wires, pub, bl, [(hint, lay)], match="not made by this box")
     _refused(box.submit_settlement_witness, None, stranger, wit, bl, [(hint, lay)], match="not made by this box")
-    assert box._keep == {}
+    assert box._jobs == {}

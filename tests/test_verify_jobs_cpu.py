@@ -108,9 +108,9 @@ def _checks(submit):
 
 def test_pool_and_box_checks_run_before_the_library():
     pool = ProverPool.__new__(ProverPool)
-    pool._lib, pool._h, pool._keep, pool._borrowed = _NoLibrary(), None, {}, []
+    pool._lib, pool._h, pool._jobs, pool._borrowed = _NoLibrary(), None, {}, []
     box = ProverBox.__new__(ProverBox)
-    box._lib, box._h, box._keep, box.devices, box._shapes = _NoLibrary(), None, {}, [0], {}
+    box._lib, box._h, box._jobs, box.devices, box._shapes = _NoLibrary(), None, {}, [0], {}
     for jobs in (pool, box):
         _checks(jobs.submit_verify)
-        assert jobs._keep == {}
+        assert jobs._jobs == {}

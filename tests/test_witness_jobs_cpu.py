@@ -68,13 +68,13 @@ class _NoLibrary:
 
 def _pool():
     pool = ProverPool.__new__(ProverPool)
-    pool._lib, pool._h, pool._keep, pool._borrowed = _NoLibrary(), None, {}, []
+    pool._lib, pool._h, pool._jobs, pool._borrowed = _NoLibrary(), None, {}, []
     return pool
 
 
 def _box(shapes):
     box = ProverBox.__new__(ProverBox)
-    box._lib, box._h, box._keep, box.devices = _NoLibrary(), None, {}, [0]
+    box._lib, box._h, box._jobs, box.devices = _NoLibrary(), None, {}, [0]
     box._shapes = shapes
     return box
 
@@ -128,3 +128,15 @@ def test_box_checks_run_before_the_library(parts):
     _refused(box.submit_bundle_witness, None, [(stranger, wit, bl)], [], match="not made by this box")
     _refused(box.submit_bundle, None, [(wired, 0, np.zeros((1, 4), dtype=np.uint64), bl)], [],
              match="public inputs / blinders do not match")
+
+
+def test_box_and_pool_prove_checks_run_before_the_library():
+    """A wire-table proof reads 17 blinders and the key's public inputs: the box refuses short arrays as the pool does."""
+    bl, pub = synth.splitmix_blinders(1), np.zeros((2, 4), dtype=np.uint64)
+    box, pool = _box({0x10: _key()}), _pool()
+    for submit, pk in ((box.submit_prove, C.c_void_p(0x10)), (pool.submit_prove, _key())):
+        _refused(submit, pk, 0x1000, pub, bl[:16], match="blinders must be 17 Fr elements")
+        _refused(submit, pk, 0x1000, pub[:1], bl, match="1 public inputs for a key with 2")
+        _refused(submit, pk, 0x1000, np.zeros((3, 4), dtype=np.uint64), bl, match="3 public inputs for a key with 2")
+    _refused(box.submit_prove, C.c_void_p(0x30), 0x1000, pub, bl, match="not made by this box")
+    assert box._jobs == {} and pool._jobs == {}

@@ -428,7 +428,8 @@ int b200_pairing_check_many(b200_ctx* ctx, const uint64_t* g2_points, size_t m, 
                             size_t n_checks, uint8_t* is_one);
 
 /* Wall-clock milliseconds of the last proof's phases on this context: round 1, round 2, round 3
- * (coset NTTs + quotient + split), round 3 commitments, round 4, round 5, then two spare slots. */
+ * (coset NTTs + quotient + split), round 3 commitments, round 4, round 5, then the host part of the self-check at zeta
+ * (inside round 5's time, under its commitments), then one spare slot. */
 int b200_plonk_last_timings(b200_ctx* ctx, float out_ms[8]);
 
 /* ---- prover pool --------------------------------------------------------------------------

@@ -814,7 +814,9 @@ static int preprocess(Context* c, const Bases* srs, unsigned log_n, size_t num_i
                       const uint64_t* h_perm, const uint32_t* h_wire_vars, size_t num_vars, const fe* h_k, ProvingKey** out) {
     const size_t n = (size_t)1 << log_n;
     // 6 cosets (6n > 5n + 7 points) from n = 16 on; all 8 for the tiny domains, where 6n would not exceed
-    // the quotient's degree by enough to keep the degree check meaningful
+    // the quotient's degree by enough to keep the degree check meaningful.  Six cosets determine t for a satisfied
+    // witness but do not decide satisfaction: the degree check misses violations of degree <= 7 on H, which prove()'s
+    // self-check at zeta refuses (DESIGN §4)
     const int nc = log_n >= 4 ? 6 : 8;
     const size_t m = (size_t)nc * n;
     if (log_n < 2 || log_n + 3 > 28) {
@@ -1117,6 +1119,46 @@ struct InGraphReset {
     ~InGraphReset() { s.in_graph = false; }
 };
 
+// The value at zeta that the verifier expects of the batched polynomial opened at zeta (lin + sum v^i w_i + sum
+// v^(5+i) sigma_i): E = -r0 + sum v^i w_i(zeta) + sum v^(5+i) sigma_i(zeta), read from vt::plonk_terms (with u = 0 the
+// generator's B scalar is -E).  The proof verifies only if the polynomial takes this value at zeta; for a witness that
+// satisfies the circuit it does.  The 1 / (n (zeta - w^j)) of the public inputs come from one batch inversion.
+static fe expected_opening(const ProvingKey* pk, const fe* pub, const ProofOut& proof, const fe ch[5]) {
+    const size_t cnt = std::max<size_t>(pk->num_inputs, 1);  // j = 0 also gives L_1's denominator
+    std::vector<fe> wpow(cnt), inv(cnt);
+    const fe nfr = host_from_u64(pk->n);
+    fe acc = fe_one<Fr>(), wj = fe_one<Fr>();
+    for (size_t j = 0; j < cnt; ++j) {  // inv[j]: the product of the denominators before j
+        wpow[j] = wj;
+        inv[j] = acc;
+        acc = FMUL(acc, FMUL(FSUB(ch[3], wj), nfr));
+        wj = FMUL(wj, pk->group_gen);
+    }
+    acc = fe_inv<Fr>(acc);
+    for (size_t j = cnt; j-- > 0;) {
+        const fe d = FMUL(FSUB(ch[3], wpow[j]), nfr);
+        inv[j] = FMUL(inv[j], acc);
+        acc = FMUL(acc, d);
+    }
+    struct Den {
+        const fe *inv, *wpow;
+        void get(size_t j, fe* i, fe* w) const {
+            *i = inv[j];
+            *w = wpow[j];
+        }
+    } den{inv.data(), wpow.data()};
+    struct Sink {
+        fe g = fe_zero();
+        void operator()(int slot, int side, const fe& s) {
+            if (slot == vt::kSlotG && side == vt::kSideB) g = s;
+        }
+    } sink;
+    const vt::PlonkChallenges pc{ch[0], ch[1], ch[2], ch[3], ch[4], fe_zero()};
+    vt::plonk_terms(pk->log_n, pk->num_inputs, pk->k.v, pub, *reinterpret_cast<const vt::ProofIn*>(&proof), pc,
+                    pk->group_gen, den, sink);
+    return fe_neg<Fr>(sink.g);
+}
+
 // The five prover rounds for k proofs of one key.  Every launch covers all k proofs (see Workspace and the kernels'
 // batch index); every commitment round is ONE batched MSM over the k proofs' polynomials; the host runs the k
 // Fiat–Shamir transcripts between rounds, so a batch makes the five host round trips once.
@@ -1129,13 +1171,14 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
     const unsigned log_n = pk->log_n;
     cudaStream_t st = c->stream;
     int rc;
-    const size_t flags_bytes = ((size_t)k * 4 + 63) / 64 * 64;  // h_small: the k degree flags, then k x 2 NW evaluations
+    // h_small: the k degree flags, then k x 2 NW evaluations, then the k batched polynomials' values at zeta
+    const size_t flags_bytes = ((size_t)k * 4 + 63) / 64 * 64;
     if ((rc = bf.ws->reserve(workspace_elems(n, k) * sizeof(fe))) != B200_OK) return rc;
     const bool from_witness = items[0].witness != nullptr;  // every item of a call has the same kind of input
     // the NTT scratch doubles as the staging area of the witness vectors: the gather has read them before round 1 uses it
     if ((rc = bf.nscr->reserve((size_t)k * std::max(7 * m, from_witness ? pk->num_vars : 0) * sizeof(fe))) != B200_OK) return rc;
     if ((rc = bf.nscr2->reserve((size_t)k * 6 * m * sizeof(fe))) != B200_OK) return rc;
-    if ((rc = bf.h_small->reserve(std::max<size_t>(4096, flags_bytes + (size_t)k * 2 * NW * sizeof(fe)))) != B200_OK) return rc;
+    if ((rc = bf.h_small->reserve(std::max<size_t>(4096, flags_bytes + (size_t)k * (2 * NW + 1) * sizeof(fe)))) != B200_OK) return rc;
     if ((rc = bf.h_params->reserve(k * sizeof(ProofParams))) != B200_OK) return rc;
     if ((rc = bf.d_params->reserve(k * sizeof(ProofParams))) != B200_OK) return rc;
     if (!c->stream2) {
@@ -1403,6 +1446,7 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
         zeta_w[p] = FMUL(zeta[p], pk->group_gen);
     }
     fe* h_evals = reinterpret_cast<fe*>(reinterpret_cast<char*>(bf.h_small->p) + flags_bytes);  // pinned, [proof][2 NW]
+    fe* h_bz = h_evals + (size_t)k * 2 * NW;                                                      // pinned, [proof]
     {
         // proof 0's polynomials; proof p's are `pstrides` further (the key's sigmas are shared)
         const fe* polys[kMaxEval];
@@ -1514,9 +1558,24 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
         hs.dyn = D;
         horner_suffix(w.lin, n + 3, zeta[0], w.sdiv, w.evals + 16, w.hscr, st, &dp->open[0], hs);
         horner_suffix(w.zpoly, n + 3, zeta_w[0], w.sdiv + (S + 8), w.evals + 17, w.hscr, st, &dp->open[1], hs);
+        B200_CUDA(cudaMemcpy2DAsync(h_bz, sizeof(fe), w.evals + 16, kEvalSlots * sizeof(fe), sizeof(fe), k,
+                                    cudaMemcpyDeviceToHost, st));
         return B200_OK;
     });
     if (rc != B200_OK) return rc;
+    // Self-check at zeta, on the host while the opening commitments run: the batched polynomial must take the value the
+    // verifier expects.  Round 3's degree check reads a quotient interpolated from 6 cosets, which misses every witness
+    // whose per-row violations are the values on H of a polynomial of degree <= 7 (DESIGN §4); this check refuses those,
+    // except with probability at most (6n + 8) / r.
+    std::vector<fe> want_bz(k);
+    {
+        const auto t0 = clk::now();
+        for (unsigned p = 0; p < k; ++p) {
+            const fe ch[5] = {beta[p], gamma[p], alpha[p], zeta[p], v[p]};
+            if (items[p].status == B200_OK) want_bz[p] = expected_opening(pk, items[p].pub_inputs, *items[p].proof, ch);
+        }
+        c->plonk_ms[6] = std::chrono::duration<float, std::milli>(clk::now() - t0).count();
+    }
     comms.resize(2 * k);
     if ((rc = commit_collect(bf.msm, 2 * k, comms.data())) != B200_OK) return rc;
     for (unsigned p = 0; p < k; ++p) {
@@ -1525,6 +1584,15 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
     }
     mark();  // [5] round 5
     if (gset && !gs) gset->proofs_seen = 1;  // this key has now run eagerly on this context: later proofs replay graphs
+    satisfied = 0;
+    for (unsigned p = 0; p < k; ++p) {  // h_bz was copied before the opening commitments on the same stream
+        if (items[p].status == B200_OK && !fe_eq(h_bz[p], want_bz[p])) items[p].status = B200_ERR_UNSATISFIED;
+        if (items[p].status == B200_OK) ++satisfied;
+    }
+    if (!satisfied) {
+        set_error("WrongQuotientPolyDegree: the witness does not satisfy the circuit");
+        return B200_ERR_UNSATISFIED;
+    }
     for (unsigned p = 0; p < k; ++p) {
         if (!items[p].challenges || items[p].status != B200_OK) continue;
         SolidityTranscript& tr = trs[p];

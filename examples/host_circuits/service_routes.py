@@ -3,7 +3,9 @@ the request decoders (`{statement, witness[, link hints]}`, api_types.rs:141-264
 statements.py.  The other four paths of prover_service_client.rs:101-147 are not registered here (their circuits verify Schnorr
 signatures / ElGamal ciphertexts on BabyJubJub in-circuit and are not restated); the service answers 501 for them.
 
-    python -m host_circuits.service_routes --port 3000 --password PW --srs /path/to/ptau [--device 0 --workers 6]
+    python -m host_circuits.service_routes --port 3000 --password PW --srs /path/to/ptau [--device 0 --workers 6 --express 0]
+
+`--express N` adds N express workers to the pool and expedites every settlement route's job onto them (b200express.h).
 """
 from __future__ import annotations
 
@@ -105,8 +107,10 @@ def main():
                          "device, and refuse to start on an SRS that fails")
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--workers", type=int, default=6)
+    ap.add_argument("--express", type=int, default=0,
+                    help="express workers; > 0 also expedites the settlement routes' jobs (DESIGN.md §6, express lane)")
     args = ap.parse_args()
-    pool = ProverPool(args.device, workers=args.workers)
+    pool = ProverPool(args.device, workers=args.workers, express=args.express)
     ctx = pool.context(0)
     data = open(args.srs, "rb").read()
     params = rb.parse_ptau_file(ctx, data, count=(1 << 14) + 3)
@@ -126,7 +130,7 @@ def main():
     ct.set_system_srs(ctx, params.powers_of_g, g2[:16], g2[16:32], pool=pool)
     for c in st.REGISTERED:  # `NativeProofManager::preprocess_circuits` (native_proof_manager.rs:305-331)
         c.proving_key()
-    server = ProverService(routes(), args.password, pool=pool).make_server(args.host, args.port)
+    server = ProverService(routes(), args.password, pool=pool, expedite_settlements=args.express > 0).make_server(args.host, args.port)
     print(f"prover service on {args.host}:{server.server_address[1]} ({len(routes())} circuits)", flush=True)
     server.serve_forever()
 

@@ -444,6 +444,7 @@ int b200_plonk_last_timings(b200_ctx* ctx, float out_ms[8]);
  * been waited for.  Any thread may submit or wait. */
 typedef struct b200_pool b200_pool;
 int b200_pool_create(int device, unsigned n_workers, b200_pool** out);
+/* (b200express.h: pools and boxes with express workers, and moving a queued job to them by ticket) */
 /* Finishes the queued jobs, joins the workers, frees the contexts. */
 void b200_pool_destroy(b200_pool* pool);
 unsigned b200_pool_workers(const b200_pool* pool);
@@ -543,7 +544,7 @@ int b200_pool_wait(b200_pool* pool, uint64_t ticket);
 /* Blocks until the queue is empty and no job is running; returns the oldest failure among the
  * jobs not individually waited for (their tickets are consumed), else B200_OK. */
 int b200_pool_wait_all(b200_pool* pool);
-/* out = { submitted, completed, failed, queued } */
+/* out = { submitted, completed, failed, queued }; queued counts the express queue too (b200express.h) */
 int b200_pool_stats(b200_pool* pool, uint64_t out[4]);
 
 /* ---- all GPUs of a box behind one object: prover pools + replicated keys -----------------------

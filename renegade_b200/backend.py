@@ -1209,13 +1209,29 @@ class _Tickets:
         self._jobs[ticket.value] = (finish, held)
         return ticket.value
 
-    def _wait(self, c_wait, ticket: int):
-        rc = c_wait(self._h, ticket)
+    def _wait(self, c_wait, ticket: int, *info):
+        rc = c_wait(self._h, ticket, *info)
         finish, _ = self._jobs.pop(ticket, (None, None))
         if finish is None:  # not a ticket of this object
             _lib.check(rc)
             return None
         return finish(rc)
+
+    def _expedite(self, c_expedite, ticket: int) -> int:
+        moved = C.c_size_t()
+        _lib.check(c_expedite(self._h, ticket, C.byref(moved)))
+        return moved.value
+
+    def _wait_info(self, c_wait_info, ticket: int):
+        info = (C.c_uint64 * 2)()
+        result = self._wait(c_wait_info, ticket, info)
+        return result, int(info[0]), int(info[1])
+
+
+def _express_count(express, who: str) -> int:
+    if isinstance(express, bool) or not isinstance(express, int) or express < 0:
+        raise ValueError(f"{who}: the express worker count must be an int >= 0, not {express!r}")
+    return express
 
 
 class ProverPool(_Tickets):
@@ -1223,12 +1239,17 @@ class ProverPool(_Tickets):
     (crates/workers/proof-manager/src/implementations/native_proof_manager.rs:138-201, `spawn_fifo`
     per job).  `workers` proofs are in flight on one GPU; keys and SRS tables are shared.
 
-    Buffers passed to `submit_*` are kept alive by the pool object until the ticket is waited for."""
+    Buffers passed to `submit_*` are kept alive by the pool object until the ticket is waited for.
 
-    def __init__(self, device: int = 0, workers: int = 6):
+    `express` workers (b200express.h) take only jobs moved to the express queue by `expedite(ticket)`; their contexts'
+    streams rank above the normal workers'.  Any pool can expedite: with no express workers the express queue is the
+    front of the line."""
+
+    def __init__(self, device: int = 0, workers: int = 6, express: int = 0):
+        express = _express_count(express, "ProverPool")
         self._lib = _lib.load()
         h = C.c_void_p()
-        _lib.check(self._lib.b200_pool_create(device, workers, C.byref(h)))
+        _lib.check(self._lib.b200_pool_create_express(device, workers, express, C.byref(h)))
         self._h = h
         self.device = device
         self._jobs = {}
@@ -1364,6 +1385,17 @@ class ProverPool(_Tickets):
         job's own status and message if it failed."""
         return self._wait(self._lib.b200_pool_wait, ticket)
 
+    def expedite(self, ticket: int) -> int:
+        """Move the ticket's queued jobs to the express queue (`b200_pool_expedite`); returns how many moved (0 once they
+        have all started or finished, or when already expedited)."""
+        return self._expedite(self._lib.b200_pool_expedite, ticket)
+
+    def wait_info(self, ticket: int):
+        """`wait` that also returns where and when the job finished (`b200_pool_wait_info`): (result, the pool's completed
+        count right after the ticket's last job, the index of the worker that ran it — express workers after the normal
+        ones)."""
+        return self._wait_info(self._lib.b200_pool_wait_info, ticket)
+
     def wait_all(self) -> None:
         rc = self._lib.b200_pool_wait_all(self._h)
         self._jobs.clear()
@@ -1400,13 +1432,14 @@ class _BoxKeyShape:
 class ProverBox(_Tickets):
     """`b200_box`: every GPU of the box behind one object — one prover pool per device, the SRS tables and the proving
     keys replicated on each, jobs routed to the least-loaded device.  The single-process counterpart of running one
-    `ProverPool` per rank under torchrun."""
+    `ProverPool` per rank under torchrun.  `express_per_device` express workers per device as in `ProverPool`."""
 
-    def __init__(self, devices, workers_per_device: int = 6):
+    def __init__(self, devices, workers_per_device: int = 6, express_per_device: int = 0):
+        express_per_device = _express_count(express_per_device, "ProverBox")
         self._lib = _lib.load()
         arr = (C.c_int * len(devices))(*devices)
         h = C.c_void_p()
-        _lib.check(self._lib.b200_box_create(arr, len(devices), workers_per_device, C.byref(h)))
+        _lib.check(self._lib.b200_box_create_express(arr, len(devices), workers_per_device, express_per_device, C.byref(h)))
         self._h, self._jobs, self.devices = h, {}, list(devices)
         self._shapes = {}  # key handle -> _BoxKeyShape, for the keys this box made
 
@@ -1506,6 +1539,14 @@ class ProverBox(_Tickets):
 
     def wait(self, ticket: int):
         return self._wait(self._lib.b200_box_wait, ticket)
+
+    def expedite(self, ticket: int) -> int:
+        """`ProverPool.expedite` on the pool of the ticket's device (`b200_box_expedite`)."""
+        return self._expedite(self._lib.b200_box_expedite, ticket)
+
+    def wait_info(self, ticket: int):
+        """`ProverPool.wait_info` on the pool of the ticket's device (`b200_box_wait_info`)."""
+        return self._wait_info(self._lib.b200_box_wait_info, ticket)
 
     def ticket_device(self, ticket: int) -> int:
         return self._lib.b200_box_ticket_device(self._h, ticket)

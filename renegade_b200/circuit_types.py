@@ -244,18 +244,21 @@ class SingleProverCircuit:
             raise ProverError("Plonk", e) from e
 
     @classmethod
-    def prove_settlement(cls, witness, statement, hints, rng=None, pool=None, srs_bases=None):
+    def prove_settlement(cls, witness, statement, hints, rng=None, pool=None, srs_bases=None, urgent=False):
         """A settlement arm of `NativeProofManager::handle_proof_job` (native_proof_manager.rs:514-660) in ONE call:
         `singleprover_prove_with_hint` of this statement, then `link_proofs(hint, &settlement_hint, &layout)` for every
         (stored hint, link group id) in `hints` (validity hint first, intent_and_balance.rs:57-72), the group layouts
         taken from `get_circuit_layout()`.  One settlement job on `pool` (default: the system SRS's pool), else one call
         on the SRS context; `srs_bases` defaults to the system SRS.  The proof and link proofs equal
         `prove_with_link_hint` + `link_proofs` with the same rng.  Returns (proof, [link proofs]); an unsatisfied witness
-        or a hint that differs from the statement on its group (a stale hint) raises ProverError("Plonk") naming it."""
-        return settlement_result(hints, *cls.prove_settlement_statuses(witness, statement, hints, rng, pool, srs_bases))
+        or a hint that differs from the statement on its group (a stale hint) raises ProverError("Plonk") naming it.
+        `urgent`: on a pool, expedite the job right after submit (`ProverPool.expedite`), so that it overtakes the
+        queued proofs and runs on an express worker when the pool has one; the bytes do not change."""
+        return settlement_result(hints, *cls.prove_settlement_statuses(witness, statement, hints, rng, pool, srs_bases,
+                                                                       urgent))
 
     @classmethod
-    def prove_settlement_statuses(cls, witness, statement, hints, rng=None, pool=None, srs_bases=None):
+    def prove_settlement_statuses(cls, witness, statement, hints, rng=None, pool=None, srs_bases=None, urgent=False):
         """`prove_settlement` without the raising: (proof, link proofs, statuses), statuses[0] the proof's and
         statuses[1 + i] hint i's (0, or B200_ERR_UNSATISFIED)."""
         pk, circ = cls._arithmetize(witness, statement)
@@ -266,13 +269,14 @@ class SingleProverCircuit:
         bases = srs_bases or srs.powers_of_g
         blinders = draw_blinders(rng)
         try:
-            if cls.prove_from_witness:
-                res = (pool.wait(pool.submit_settlement_witness(bases, pk, circ.witness, blinders, links)) if pool is not None
-                       else PlonkKzgSnark.prove_settlement_witness(srs.ctx, bases, pk, circ.witness, blinders, links))
+            if pool is not None:
+                tk = (pool.submit_settlement_witness(bases, pk, circ.witness, blinders, links) if cls.prove_from_witness
+                      else pool.submit_settlement(bases, pk, circ.wires, circ.pub_inputs, blinders, links))
+                res = pool.wait(_expedited(pool, tk, urgent))
+            elif cls.prove_from_witness:
+                res = PlonkKzgSnark.prove_settlement_witness(srs.ctx, bases, pk, circ.witness, blinders, links)
             else:
-                res = (pool.wait(pool.submit_settlement(bases, pk, circ.wires, circ.pub_inputs, blinders, links))
-                       if pool is not None
-                       else PlonkKzgSnark.prove_settlement(srs.ctx, bases, pk, circ.wires, circ.pub_inputs, blinders, links))
+                res = PlonkKzgSnark.prove_settlement(srs.ctx, bases, pk, circ.wires, circ.pub_inputs, blinders, links)
         except _lib.B200Error as e:
             raise ProverError("Plonk", e) from e
         return res[:3]
@@ -385,11 +389,19 @@ def verify_singleprover_proof(circuit: type, statement, proof: PlonkProof) -> No
     circuit.verify(statement, proof)
 
 
-def batch_verify_singleprover_proofs(items, pool=None, box=None) -> None:
+def _expedited(jobs, ticket: int, urgent: bool) -> int:
+    """The ticket, expedited on its pool or box first when `urgent` (the job overtakes the queued ones)."""
+    if urgent:
+        jobs.expedite(ticket)
+    return ticket
+
+
+def batch_verify_singleprover_proofs(items, pool=None, box=None, urgent=False) -> None:
     """`verify_singleprover_proof` for many (circuit, statement, proof) triples at once: one batch check with ONE
     pairing on the `SYSTEM_SRS` context's device (`PlonkKzgSnark.batch_verify`), or, given a `ProverPool` as `pool` or a
     `ProverBox` as `box`, the same check as one verification job on it (`submit_verify(..., combined=True)`), beside the
-    proofs it is making.  Raises VerifierError naming the indices of the proofs that fail."""
+    proofs it is making; `urgent` expedites that job right after submit.  Raises VerifierError naming the indices of the
+    proofs that fail."""
     items = list(items)
     if not items:
         return
@@ -401,7 +413,7 @@ def batch_verify_singleprover_proofs(items, pool=None, box=None) -> None:
     try:
         if pool is not None or box is not None:
             jobs = pool if pool is not None else box
-            _, verdicts = jobs.wait(jobs.submit_verify(vks, pis, proofs, combined=True))
+            _, verdicts = jobs.wait(_expedited(jobs, jobs.submit_verify(vks, pis, proofs, combined=True), urgent))
         else:
             _, verdicts = PlonkKzgSnark.batch_verify(system_srs().ctx, vks, pis, proofs)
     except _lib.B200Error as e:

@@ -152,7 +152,11 @@ int b200_ctx_use_graphs(b200_ctx* ctx, int on) {
 
 void b200_keccak256(const uint8_t* data, size_t len, uint8_t out[32]) { Keccak256::hash(data, len, out); }
 
-int b200_init(int device, b200_ctx** out) {
+int b200_init(int device, b200_ctx** out) { return b200::context_create(device, /*express=*/false, out); }
+
+}  // extern "C"
+
+int b200::context_create(int device, bool express, b200_ctx** out) {
     B200_TRY
     if (!out) return B200_ERR_INVALID;
     int count = 0;
@@ -174,13 +178,20 @@ int b200_init(int device, b200_ctx** out) {
     // accumulation, the side-stream coset NTTs) go to a lowest-priority companion stream.  With several
     // contexts proving on one GPU the block scheduler then slots a proof's short kernels in as soon as
     // SM resources free up instead of queueing them behind another proof's big grid.
+    // An express context (a pool's express worker) ranks each stream role above a normal context's where the device has
+    // the levels: the companion one level above the least priority, and with priorities off its one stream at the
+    // greatest instead of 0.  The main stream is at the greatest for both.  Lower numbers are higher priorities.
     int prio_least = 0, prio_greatest = 0;
     cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest);
     const char* pe = std::getenv("B200_STREAM_PRIORITIES");
     const bool prio = !(pe && pe[0] == '0');
-    e = cudaStreamCreateWithPriority(&ctx->c.stream, cudaStreamNonBlocking, prio ? prio_greatest : 0);
+    const bool lift = express && prio_least - prio_greatest >= 1;  // at least two levels
+    const int main_prio = prio ? prio_greatest : (lift ? prio_greatest : 0);
+    const int heavy_prio = lift ? prio_least - 1 : prio_least;
+    ctx->c.stream2_prio = prio ? heavy_prio : main_prio;
+    e = cudaStreamCreateWithPriority(&ctx->c.stream, cudaStreamNonBlocking, main_prio);
     if (e == cudaSuccess && prio) {
-        e = cudaStreamCreateWithPriority(&ctx->c.heavy, cudaStreamNonBlocking, prio_least);
+        e = cudaStreamCreateWithPriority(&ctx->c.heavy, cudaStreamNonBlocking, heavy_prio);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->c.hv_fork, cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->c.hv_join, cudaEventDisableTiming);
     }
@@ -199,6 +210,8 @@ int b200_init(int device, b200_ctx** out) {
     return B200_OK;
     B200_CATCH
 }
+
+extern "C" {
 
 void b200_shutdown(b200_ctx* ctx) {
     if (!ctx) return;

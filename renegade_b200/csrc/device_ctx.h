@@ -226,6 +226,7 @@ struct Context {
     cudaStream_t heavy = nullptr;
     cudaEvent_t hv_fork = nullptr, hv_join = nullptr;
     bool heavy_plonk = false;  // also route the prover's NTT passes and quotient kernel there
+    int stream2_prio = 0;      // priority `stream2` is created with: the companion's, or the main stream's with priorities off
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     DevBuf ntt_scratch2;
     HostPinned h_small;  // pinned landing zone of the prover's small read-backs (degree flag, evaluations)
@@ -246,6 +247,10 @@ struct Context {
 };
 
 int get_domain(Context* c, unsigned log_n, Domain** out);
+
+// b200_init (express = false), or a context for a pool's express worker (pool.cu), whose streams rank above a normal
+// context's of the same role where the device has two priority levels or more (api.cu).
+int context_create(int device, bool express, b200_ctx** out);
 
 // a 128-byte G2 record x0 || x1 || y0 || y1 (Montgomery) is on the twist, every coordinate below q (verify.cu)
 bool g2_record_on_curve(const uint64_t rec[16]);

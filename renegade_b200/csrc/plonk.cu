@@ -1182,9 +1182,7 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
     if ((rc = bf.h_params->reserve(k * sizeof(ProofParams))) != B200_OK) return rc;
     if ((rc = bf.d_params->reserve(k * sizeof(ProofParams))) != B200_OK) return rc;
     if (!c->stream2) {
-        int prio_least = 0, prio_greatest = 0;
-        cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest);
-        B200_CUDA(cudaStreamCreateWithPriority(&c->stream2, cudaStreamNonBlocking, c->heavy ? prio_least : 0));
+        B200_CUDA(cudaStreamCreateWithPriority(&c->stream2, cudaStreamNonBlocking, c->stream2_prio));
         B200_CUDA(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
         B200_CUDA(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
     }

@@ -6,6 +6,8 @@
 // GPU and the latency-bound kernels of one proof (bucket reductions, scans, the host transcript)
 // overlap the throughput-bound kernels of the others.  Verification jobs (b200verifyjobs.h) run the device verifiers
 // on a worker's context in the same queue, so a caller that checks proofs on a proving GPU needs no context of its own.
+// The express lane (b200express.h): a second queue that b200_pool_expedite moves a ticket's queued jobs to, drained by
+// express workers whose contexts' streams outrank the normal workers' (and by normal workers when it backs up).
 //
 // Host-only code (std::thread) above the same C ABI the single-context entry points use.
 #include <algorithm>
@@ -18,6 +20,7 @@
 #include <thread>
 #include <vector>
 
+#include "b200express.h"
 #include "b200prover.h"
 #include "b200settlement.h"
 #include "b200verifyjobs.h"
@@ -106,6 +109,8 @@ std::unique_ptr<Job> link_job(const b200_bases* srs, const b200_link_item& it) {
 struct Done {
     int status = B200_OK;
     std::string message;
+    uint64_t completed = 0;  // the pool's completed count right after the ticket's last job
+    unsigned worker = 0;     // the worker that ran that job (express workers after the normal ones)
 };
 
 // A bundle: proofs first, then — once all of them are in — the link proofs between their wire-0 polynomials; one
@@ -126,19 +131,26 @@ struct Bundle {
     std::vector<b200_bundle_link> links;
     size_t pending = 0;     // sub-jobs of the current phase still queued or running
     bool linking = false;   // false: proof phase, true: link phase
+    bool expedited = false; // its link jobs are forked onto the express queue
     Done result;            // first failure wins
 };
 
 }  // namespace
 
+// Two queues: the normal one, FIFO in submit order, and the express queue, FIFO in the order jobs were expedited.  Workers
+// 0..n_normal-1 take from the express queue when it holds more jobs than there are idle express workers, else from the
+// normal queue; the express workers (n_normal and up, each with an express context) take from the express queue only.
 struct b200_pool {
-    std::vector<b200_ctx*> ctxs;
+    std::vector<b200_ctx*> ctxs;     // the normal workers' contexts, then the express workers'
+    unsigned n_normal = 0;
     std::vector<std::thread> workers;
     std::mutex mu;
-    std::condition_variable cv_job, cv_done;
-    std::deque<std::unique_ptr<Job>> queue;
+    std::condition_variable cv_job, cv_express, cv_done;  // cv_job: normal workers, cv_express: express workers
+    std::deque<std::unique_ptr<Job>> queue, express;
+    unsigned idle_express = 0;       // express workers running no job (and not yet gone at shutdown)
     std::map<uint64_t, Done> done;   // finished, not yet waited for
     std::set<uint64_t> inflight;     // queued or running
+    std::map<uint64_t, Bundle*> bundles;  // unfinished bundles by ticket, so that expediting one marks it
     uint64_t next_ticket = 1;
     uint64_t n_submitted = 0, n_completed = 0, n_failed = 0, n_running = 0;
     bool stopping = false;
@@ -150,30 +162,57 @@ struct b200_pool {
         std::unique_ptr<Job> j = link_job(b->srs, {pa.link_poly, ((size_t)1 << b200_pk_log_n(pa.pk)) + 2, pb.link_poly,
                                                    ((size_t)1 << b200_pk_log_n(pb.pk)) + 2, pa.proof->wires_poly_comms[0],
                                                    pb.proof->wires_poly_comms[0], l.alignment, l.offset, l.size, l.proof, nullptr});
+        j->ticket = b->ticket;
         j->bundle = b;
         return j;
     }
 
+    // The queue worker w takes its next job from: &express, &queue, or nullptr (none for it now)
+    std::deque<std::unique_ptr<Job>>* source(unsigned w) {
+        if (w >= n_normal) return express.empty() ? nullptr : &express;
+        if (express.size() > idle_express) return &express;
+        return queue.empty() ? nullptr : &queue;
+    }
+
+    void notify_jobs(bool to_express) {
+        if (to_express) cv_express.notify_all();
+        cv_job.notify_all();  // a normal worker takes an express job no idle express worker will
+    }
+
     void run(unsigned w) {
+        const bool is_express = w >= n_normal;
+        std::condition_variable& cv = is_express ? cv_express : cv_job;
         for (;;) {
             std::unique_ptr<Job> job;
             {
                 std::unique_lock<std::mutex> lk(mu);
-                cv_job.wait(lk, [&] { return stopping || !queue.empty(); });
-                if (queue.empty()) return;  // stopping and drained
-                job = std::move(queue.front());
-                queue.pop_front();
+                std::deque<std::unique_ptr<Job>>* q = nullptr;
+                cv.wait(lk, [&] { return (q = source(w)) != nullptr || stopping; });
+                if (!q) {  // stopping and drained
+                    if (is_express) {
+                        --idle_express;  // gone: a normal worker takes what a bundle forks onto the express queue from now
+                        lk.unlock();
+                        cv_job.notify_all();
+                    }
+                    return;
+                }
+                job = std::move(q->front());
+                q->pop_front();
                 ++n_running;
+                if (is_express) --idle_express;
             }
             Done d;
             d.status = job->call(ctxs[w]);
             if (d.status != B200_OK) d.message = b200_last_error();  // this worker's thread-local message
-            bool new_jobs = false;
+            bool new_jobs = false, new_express = false;
             {
                 std::lock_guard<std::mutex> lk(mu);
                 --n_running;
+                if (is_express) ++idle_express;
                 ++n_completed;
                 if (d.status != B200_OK) ++n_failed;
+                d.completed = n_completed;
+                d.worker = w;
                 if (!job->bundle) {
                     inflight.erase(job->ticket);
                     done.emplace(job->ticket, std::move(d));
@@ -183,18 +222,23 @@ struct b200_pool {
                     if (--b.pending == 0) {
                         if (!b.linking && b.result.status == B200_OK && !b.links.empty()) {
                             b.linking = true;  // every proof is in: fork the link proofs
-                            for (const b200_bundle_link& l : b.links) queue.push_back(make_link_job(job->bundle, l));
+                            std::deque<std::unique_ptr<Job>>& q = b.expedited ? express : queue;
+                            for (const b200_bundle_link& l : b.links) q.push_back(make_link_job(job->bundle, l));
                             b.pending = b.links.size();
                             n_submitted += b.links.size();
                             new_jobs = true;
+                            new_express = b.expedited;
                         } else {
+                            b.result.completed = d.completed;
+                            b.result.worker = d.worker;
+                            bundles.erase(b.ticket);
                             inflight.erase(b.ticket);
                             done.emplace(b.ticket, b.result);
                         }
                     }
                 }
             }
-            if (new_jobs) cv_job.notify_all();
+            if (new_jobs) notify_jobs(new_express);
             cv_done.notify_all();
         }
     }
@@ -214,6 +258,7 @@ static int pool_push(b200_pool* pool, std::unique_ptr<Job>* jobs, size_t n, cons
         if (bundle) {
             bundle->ticket = t;
             bundle->pending = n;
+            pool->bundles.emplace(t, bundle.get());
         }
         pool->n_submitted += n;
         pool->inflight.insert(t);
@@ -259,24 +304,28 @@ static int bundle_push(b200_pool* pool, const char* who, const b200_bases* srs, 
 
 extern "C" {
 
-int b200_pool_create(int device, unsigned n_workers, b200_pool** out) {
+int b200_pool_create(int device, unsigned n_workers, b200_pool** out) { return b200_pool_create_express(device, n_workers, 0, out); }
+
+int b200_pool_create_express(int device, unsigned n_workers, unsigned n_express, b200_pool** out) {
     B200_TRY
-    if (!out || n_workers == 0 || n_workers > 64) {
-        b200::set_error("pool: n_workers must be in [1, 64]");
+    if (!out || n_workers == 0 || n_workers > 64 || n_express > 64) {
+        b200::set_error("pool: n_workers must be in [1, 64] and n_express in [0, 64]");
         return B200_ERR_INVALID;
     }
     std::unique_ptr<b200_pool> p(new b200_pool());
-    for (unsigned i = 0; i < n_workers; ++i) {
+    for (unsigned i = 0; i < n_workers + n_express; ++i) {
         b200_ctx* c = nullptr;
-        const int rc = b200_init(device, &c);
+        const int rc = b200::context_create(device, /*express=*/i >= n_workers, &c);
         if (rc != B200_OK) {
             for (b200_ctx* q : p->ctxs) b200_shutdown(q);
             return rc;
         }
         p->ctxs.push_back(c);
     }
+    p->n_normal = n_workers;
+    p->idle_express = n_express;
     b200_pool* raw = p.release();
-    for (unsigned i = 0; i < n_workers; ++i) raw->workers.emplace_back([raw, i] { raw->run(i); });
+    for (unsigned i = 0; i < n_workers + n_express; ++i) raw->workers.emplace_back([raw, i] { raw->run(i); });
     *out = raw;
     return B200_OK;
     B200_CATCH
@@ -289,15 +338,16 @@ void b200_pool_destroy(b200_pool* pool) {
         pool->stopping = true;  // workers drain what is queued, then leave
     }
     pool->cv_job.notify_all();
+    pool->cv_express.notify_all();
     for (std::thread& t : pool->workers) t.join();
     for (b200_ctx* c : pool->ctxs) b200_shutdown(c);
     delete pool;
 }
 
-unsigned b200_pool_workers(const b200_pool* pool) { return pool ? (unsigned)pool->ctxs.size() : 0u; }
+unsigned b200_pool_workers(const b200_pool* pool) { return pool ? pool->n_normal : 0u; }
 
 b200_ctx* b200_pool_ctx(b200_pool* pool, unsigned worker) {
-    if (!pool || worker >= pool->ctxs.size()) return nullptr;
+    if (!pool || worker >= pool->n_normal) return nullptr;  // express contexts are the pool's own
     return pool->ctxs[worker];
 }
 
@@ -556,15 +606,51 @@ int b200_pool_submit_verify(b200_pool* pool, int mode, const b200_verifying_key*
     B200_CATCH
 }
 
-int b200_pool_wait(b200_pool* pool, uint64_t ticket) {
+int b200_pool_expedite(b200_pool* pool, uint64_t ticket, size_t* moved) {
     B200_TRY
+    if (!pool || !moved || ticket == 0) {
+        b200::set_error("pool_expedite: null pool or moved, or ticket 0");
+        return B200_ERR_INVALID;
+    }
+    size_t n = 0;
+    {
+        std::lock_guard<std::mutex> lk(pool->mu);
+        if (ticket >= pool->next_ticket) {
+            b200::set_error("pool_expedite: unknown ticket");
+            return B200_ERR_INVALID;
+        }
+        if (!pool->inflight.count(ticket) && !pool->done.count(ticket)) {
+            b200::set_error("pool_expedite: ticket already waited for");
+            return B200_ERR_INVALID;
+        }
+        auto b = pool->bundles.find(ticket);
+        if (b != pool->bundles.end()) b->second->expedited = true;  // the links it forks later go to the express queue
+        std::deque<std::unique_ptr<Job>> rest;
+        for (std::unique_ptr<Job>& j : pool->queue) {
+            if (j->ticket == ticket) {
+                pool->express.push_back(std::move(j));
+                ++n;
+            } else {
+                rest.push_back(std::move(j));
+            }
+        }
+        pool->queue.swap(rest);
+    }
+    *moved = n;
+    if (n) pool->notify_jobs(true);
+    return B200_OK;
+    B200_CATCH
+}
+
+// b200_pool_wait, and with info != nullptr the ticket's completion index and worker
+static int pool_wait(b200_pool* pool, uint64_t ticket, uint64_t* info, const char* who) {
     if (!pool || ticket == 0) {
-        b200::set_error("pool_wait: bad ticket");
+        b200::set_error(std::string(who) + ": bad ticket");
         return B200_ERR_INVALID;
     }
     std::unique_lock<std::mutex> lk(pool->mu);
     if (ticket >= pool->next_ticket) {
-        b200::set_error("pool_wait: unknown ticket");
+        b200::set_error(std::string(who) + ": unknown ticket");
         return B200_ERR_INVALID;
     }
     for (;;) {
@@ -573,15 +659,34 @@ int b200_pool_wait(b200_pool* pool, uint64_t ticket) {
             const Done d = std::move(it->second);
             pool->done.erase(it);
             lk.unlock();
+            if (info) {
+                info[0] = d.completed;
+                info[1] = d.worker;
+            }
             if (d.status != B200_OK) b200::set_error(d.message);
             return d.status;
         }
         if (!pool->inflight.count(ticket)) {
-            b200::set_error("pool_wait: ticket already waited for");
+            b200::set_error(std::string(who) + ": ticket already waited for");
             return B200_ERR_INVALID;
         }
         pool->cv_done.wait(lk);
     }
+}
+
+int b200_pool_wait(b200_pool* pool, uint64_t ticket) {
+    B200_TRY
+    return pool_wait(pool, ticket, nullptr, "pool_wait");
+    B200_CATCH
+}
+
+int b200_pool_wait_info(b200_pool* pool, uint64_t ticket, uint64_t info[2]) {
+    B200_TRY
+    if (!info) {
+        b200::set_error("pool_wait_info: null info");
+        return B200_ERR_INVALID;
+    }
+    return pool_wait(pool, ticket, info, "pool_wait_info");
     B200_CATCH
 }
 
@@ -592,7 +697,7 @@ int b200_pool_wait_all(b200_pool* pool) {
         return B200_ERR_INVALID;
     }
     std::unique_lock<std::mutex> lk(pool->mu);
-    pool->cv_done.wait(lk, [&] { return pool->queue.empty() && pool->n_running == 0; });
+    pool->cv_done.wait(lk, [&] { return pool->queue.empty() && pool->express.empty() && pool->n_running == 0; });
     int status = B200_OK;
     std::string message;
     for (auto& kv : pool->done)  // tickets are increasing: report the oldest failure
@@ -616,7 +721,7 @@ int b200_pool_stats(b200_pool* pool, uint64_t out[4]) {
     out[0] = pool->n_submitted;
     out[1] = pool->n_completed;
     out[2] = pool->n_failed;
-    out[3] = pool->queue.size();
+    out[3] = pool->queue.size() + pool->express.size();
     return B200_OK;
 }
 
@@ -750,6 +855,11 @@ void b200_box_destroy(b200_box* box) {
 }
 
 int b200_box_create(const int* devices, int n_dev, unsigned workers_per_device, b200_box** out) {
+    return b200_box_create_express(devices, n_dev, workers_per_device, 0, out);
+}
+
+int b200_box_create_express(const int* devices, int n_dev, unsigned workers_per_device, unsigned express_per_device,
+                            b200_box** out) {
     B200_TRY
     if (!devices || n_dev <= 0 || n_dev > 64 || !out) {
         b200::set_error("box_create: need 1..64 device ordinals");
@@ -758,7 +868,7 @@ int b200_box_create(const int* devices, int n_dev, unsigned workers_per_device, 
     std::unique_ptr<b200_box> box(new b200_box());
     for (int i = 0; i < n_dev; ++i) {
         b200_pool* p = nullptr;
-        const int rc = b200_pool_create(devices[i], workers_per_device, &p);
+        const int rc = b200_pool_create_express(devices[i], workers_per_device, express_per_device, &p);
         if (rc != B200_OK) {
             b200_box_destroy(box.release());
             return rc;
@@ -978,14 +1088,38 @@ int b200_box_submit_verify(b200_box* box, int mode, const b200_verifying_key* vk
     B200_CATCH
 }
 
-int b200_box_wait(b200_box* box, uint64_t ticket) {
-    B200_TRY
+// The pool of a box ticket's device and the ticket in that pool; nullptr for a NULL box or a device index out of range
+static b200_pool* box_ticket_pool(b200_box* box, uint64_t ticket, const char* who, uint64_t* local) {
     const uint64_t d = ticket >> kBoxTicketShift;
     if (!box || d >= box->pools.size()) {
-        b200::set_error("box_wait: bad ticket");
-        return B200_ERR_INVALID;
+        b200::set_error(std::string(who) + ": bad ticket");
+        return nullptr;
     }
-    return b200_pool_wait(box->pools[d], ticket & (((uint64_t)1 << kBoxTicketShift) - 1));
+    *local = ticket & (((uint64_t)1 << kBoxTicketShift) - 1);
+    return box->pools[d];
+}
+
+int b200_box_wait(b200_box* box, uint64_t ticket) {
+    B200_TRY
+    uint64_t t = 0;
+    b200_pool* p = box_ticket_pool(box, ticket, "box_wait", &t);
+    return p ? b200_pool_wait(p, t) : B200_ERR_INVALID;
+    B200_CATCH
+}
+
+int b200_box_expedite(b200_box* box, uint64_t ticket, size_t* moved) {
+    B200_TRY
+    uint64_t t = 0;
+    b200_pool* p = box_ticket_pool(box, ticket, "box_expedite", &t);
+    return p ? b200_pool_expedite(p, t, moved) : B200_ERR_INVALID;
+    B200_CATCH
+}
+
+int b200_box_wait_info(b200_box* box, uint64_t ticket, uint64_t info[2]) {
+    B200_TRY
+    uint64_t t = 0;
+    b200_pool* p = box_ticket_pool(box, ticket, "box_wait_info", &t);
+    return p ? b200_pool_wait_info(p, t, info) : B200_ERR_INVALID;
     B200_CATCH
 }
 

@@ -199,8 +199,11 @@ class Route:
 
 
 class ProverService:
-    def __init__(self, routes: Dict[str, Route], password: str, srs_bases=None, pool=None):
+    def __init__(self, routes: Dict[str, Route], password: str, srs_bases=None, pool=None, expedite_settlements=False):
+        """`expedite_settlements`: the settlement routes' jobs are expedited on `pool` right after submit — they sit on
+        a trade's critical path, so they overtake queued validity proofs and run on the pool's express workers."""
         self.routes, self.password, self.pool, self.srs_bases = routes, password, pool, srs_bases
+        self.expedite_settlements = expedite_settlements
         self.stats = {"requests": 0, "proofs": 0, "link_proofs": 0, "errors": 0}
         self._lock = threading.Lock()
 
@@ -247,7 +250,8 @@ class ProverService:
         """A settlement route on the pool: ONE settlement job proves the statement and links every hint of the request
         (`SingleProverCircuit.prove_settlement`), with no host round trip between the proof and its links."""
         hints = [(decode_link_hint(body[req_field]), group) for req_field, _, group in route.links]
-        res = route.circuit.prove_settlement_statuses(witness, statement, hints, pool=self.pool, srs_bases=self.srs_bases)
+        res = route.circuit.prove_settlement_statuses(witness, statement, hints, pool=self.pool, srs_bases=self.srs_bases,
+                                                      urgent=self.expedite_settlements)
         with self._lock:  # counted as on the two-step path: the proof once made, the link proofs once all are made
             self.stats["proofs"] += res[2][0] == _lib.B200_OK
         proof, link_proofs = ct.settlement_result(hints, *res)

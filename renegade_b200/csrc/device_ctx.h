@@ -135,25 +135,16 @@ struct MsmScratch {
     DevBuf scan_state;  // ScanState header + tile status words of the single-pass scan (msm.cu)
     DevBuf tree;        // partial sums of the row / column reduction trees
     DevBuf bit_sums;    // per window, the c - 1 bit sums T_b of the weighted tail
-    HostPinned h_sums;  // window sums land here (pinned), read by the host epilogue
-    cudaEvent_t done_ev = nullptr;  // recorded after the D2H of the window sums
-    // the MSM batch queued by msm_launch_batch and not yet collected by msm_finish_batch
-    MsmPlan pending_plan;
-    size_t pending_n = 0;
-    unsigned pending_batch = 0;
-    // optional per-phase device timing (CUDA events on the launching stream)
+    HostPinned h_sums;  // window sums, or their bit sums, land here (pinned), read by the host epilogue
+    // recorded after the D2H of the sums; inside a stream capture the caller records it after launching the graph
+    cudaEvent_t done_ev = nullptr;
+    // optional per-phase device timing (CUDA events on the launching stream; graph nodes inside a stream capture)
     bool timing = false;
     bool ev_init = false;
     cudaEvent_t ev[5] = {};
     float ms[4] = {0, 0, 0, 0};  // total, sort (count+scan+scatter), accumulate, reduce
     // running totals since timing was switched on: accumulate ms, (point, scalar) pairs, launches
     double tot_acc_ms = 0, tot_pairs = 0, tot_launches = 0;
-    // the final weighted sum of each window's bit sums runs on the host (msm_finish_batch); false: msm_horner_kernel leaves the
-    // window sums on the device (the multi-GPU path adds them there)
-    bool host_horner = true;
-    // set by a caller that captures / replays the launches as a CUDA graph: timing events become graph nodes, and the
-    // caller records done_ev itself
-    bool in_graph = false;
     // borrowed from the context: low-priority stream for the accumulation kernel (null: same stream)
     cudaStream_t hv_stream = nullptr;
     cudaEvent_t hv_fork = nullptr, hv_join = nullptr;
@@ -172,18 +163,36 @@ int bases_create(const g1_affine* h_points, size_t n, int c_override, int check_
 constexpr size_t kTablesAuto = ~(size_t)0;
 int bases_create_device(const g1_affine* d_points, size_t n, int c_override, cudaStream_t st,
                         Bases** out, size_t table_budget_bytes = kTablesAuto);
-// scalars on device (n x 32 B); result: XYZZ sums of the n_phys windows copied to host and
-// combined there (Horner + one inversion).
+// scalars on device (n x 32 B); result: the c - 1 bit sums of every window copied to the host and
+// combined there (Horner + one inversion per batch).
 int msm_device(const Bases* b, size_t base_off, const fe* d_scalars, size_t n, int montgomery,
                MsmScratch* s, cudaStream_t st, g1_affine* out, int* out_inf);
 int msm_device_batch(const Bases* b, size_t base_off, const fe* d_scalars, size_t n, size_t stride,
                      unsigned batch, int montgomery, MsmScratch* s, cudaStream_t st, g1_affine* out,
                      int* out_inf);
-// the two halves of msm_device_batch: enqueue only / wait + host epilogue (one batch pending per scratch)
-int msm_launch_batch(const Bases* b, size_t base_off, const fe* d_scalars, size_t n, size_t stride,
-                     unsigned batch, int montgomery, MsmScratch* s, cudaStream_t st);
-int msm_finish_batch(MsmScratch* s, g1_affine* out, int* out_inf);
-void msm_mark_pending(const Bases* b, size_t n, unsigned batch, MsmScratch* s);
+// How an MSM launch ends: where the last step of every window sum, sum_b 2^b T_b, runs and what stays where.
+enum class MsmEpilogue {
+    HostBits,     // the c - 1 bit sums of every window go to the host (B200_HOST_HORNER=0 makes this HostWindows)
+    HostWindows,  // msm_horner_kernel makes the window sums on the device; they go to the host
+    DevicePoint,  // one XYZZ point per MSM (batch 1) stays on the device, at the launch's d_point
+};
+// A launched batch that msm_finish_batch collects.  `epilogue` is the effective one.
+struct MsmPending {
+    MsmPlan plan;
+    size_t n = 0;
+    unsigned batch = 0;
+    MsmEpilogue epilogue = MsmEpilogue::HostBits;
+};
+// What msm_launch_batch returns for these arguments: a caller that replays the captured launches finishes with it.
+MsmPending msm_pending(const Bases* b, size_t n, unsigned batch, MsmEpilogue e);
+// the two halves of msm_device_batch: enqueue only / wait + host epilogue (one batch in flight per scratch).  Inside a stream
+// capture of `st` the caller records s->done_ev after launching the graph.
+int msm_launch_batch(const Bases* b, size_t base_off, const fe* d_scalars, size_t n, size_t stride, unsigned batch,
+                     int montgomery, MsmEpilogue e, MsmScratch* s, cudaStream_t st, MsmPending* pending,
+                     g1_xyzz* d_point = nullptr);
+int msm_finish_batch(MsmScratch* s, const MsmPending& p, g1_affine* out, int* out_inf);
+// the identity as the device point of an MSM without points, in one launch
+int msm_identity_point(g1_xyzz* d_point, cudaStream_t st);
 void msm_collect_timing(MsmScratch* s, size_t n, unsigned batch);
 // synthetic known-discrete-log bases P_i = a_i * G, a_i = SplitMix64-derived (SURVEY §8(d))
 int g1_known_dlog_bases_device(uint64_t seed, size_t first, size_t n, g1_affine* d_out,

@@ -1107,10 +1107,10 @@ static void tree_shape(int c, int latency, size_t n_buckets, int* l_log, int* r_
 // digit sort, the bucket folding and the reduction each run once over batch * buckets buckets,
 // which is what fills the GPU's SMs at the prover's 2^16-point sizes.
 //
-// msm_launch_batch only ENQUEUES (kernels + one D2H of the window sums into pinned memory);
-// msm_finish_batch waits for that copy and runs the host epilogue.  The prover queues further
-// work between the two.
-// B200_HOST_HORNER=0 keeps the last step of the reduction on the device (A/B measurements)
+// msm_launch_batch only ENQUEUES (kernels + one D2H of the bit or window sums into pinned memory,
+// as its MsmEpilogue says); msm_finish_batch waits for that copy and runs the host epilogue.  The
+// prover queues further work between the two.
+// B200_HOST_HORNER=0 keeps the last step of the reduction on the device (A/B measurements; read by msm_pending)
 // B200_QUAD_ADD: 0 = one lane per addition everywhere (the round-1/2 kernels, kept for A/B measurements), 1 = four lanes per
 // addition (xyzz_add_quad) in the two tail kernels, 2 (default) = and in the serial tree level of a latency plan with few outputs
 static int quad_mode() {
@@ -1121,12 +1121,46 @@ static int quad_mode() {
     return mode;
 }
 
-static bool use_host_horner(const MsmScratch* s) {
-    static const bool env_on = [] {
-        const char* e = std::getenv("B200_HOST_HORNER");
-        return !(e && e[0] == '0');
+MsmPending msm_pending(const Bases* b, size_t n, unsigned batch, MsmEpilogue e) {
+    static const bool host_bits = [] {
+        const char* v = std::getenv("B200_HOST_HORNER");
+        return !(v && v[0] == '0');
     }();
-    return s->host_horner && env_on;
+    if (e == MsmEpilogue::HostBits && !host_bits) e = MsmEpilogue::HostWindows;
+    return {b->plan, n, batch, e};
+}
+
+// sum_i t[i] 2^(shift i) over the n >= 1 terms, highest term first (Horner's rule)
+static FF_HD g1_xyzz g1_horner_pow2(const g1_xyzz* t, int n, int shift) {
+#ifdef __CUDA_ARCH__
+    auto at = [&](int i) { return g1_xyzz_load(t + i); };  // 16-byte loads
+#else
+    auto at = [&](int i) { return t[i]; };
+#endif
+    g1_xyzz acc = at(n - 1);
+    for (int i = n - 2; i >= 0; --i) {
+        for (int k = 0; k < shift; ++k) acc = g1_dbl(acc);
+        acc = g1_add(acc, at(i));
+    }
+    return acc;
+}
+
+// one MSM's window sums -> a single group element: Horner over the physical windows (a single window, the
+// usual fully precomputed plan, passes through).  `empty`: the identity.
+static __global__ void k_windows_to_point(const g1_xyzz* __restrict__ window_sums, int n_phys, int c, int empty,
+                                          g1_xyzz* __restrict__ out) {
+    if (threadIdx.x || blockIdx.x) return;
+    if (empty) {
+        g1_xyzz_store(out, g1_xyzz_inf());
+        return;
+    }
+    g1_xyzz_store(out, g1_horner_pow2(window_sums, n_phys, c));
+}
+
+int msm_identity_point(g1_xyzz* d_point, cudaStream_t st) {
+    B200_LAUNCH(k_windows_to_point, 1, 32, 0, st)(nullptr, 1, 1, 1, d_point);
+    B200_CUDA(cudaGetLastError());
+    return B200_OK;
 }
 
 // SMs of the current device: the grid-stride heavy-bucket combine runs 4 blocks per SM (132 on an H100 SXM)
@@ -1138,18 +1172,15 @@ static size_t sm_count() {
     return (size_t)sms;
 }
 
-int msm_launch_batch(const Bases* b, size_t base_off, const fe* d_scalars, size_t n, size_t stride,
-                     unsigned batch, int montgomery, MsmScratch* s, cudaStream_t st) {
+int msm_launch_batch(const Bases* b, size_t base_off, const fe* d_scalars, size_t n, size_t stride, unsigned batch,
+                     int montgomery, MsmEpilogue epilogue, MsmScratch* s, cudaStream_t st, MsmPending* pending,
+                     g1_xyzz* d_point) {
     if (base_off + n > b->n) {
         set_error("msm: base_off + n exceeds the loaded bases");
         return B200_ERR_INVALID;
     }
-    s->pending_batch = 0;
-    if (batch == 0) return B200_OK;
-    s->pending_plan = b->plan;
-    s->pending_n = n;
-    s->pending_batch = batch;
-    if (n == 0) return B200_OK;
+    *pending = msm_pending(b, n, batch, epilogue);
+    if (batch == 0 || n == 0) return B200_OK;
     const MsmPlan& pl = b->plan;
     const uint32_t half = 1u << (pl.c - 1);
     const size_t buckets_per_msm = (size_t)pl.n_phys * half;
@@ -1212,6 +1243,9 @@ int msm_launch_batch(const Bases* b, size_t base_off, const fe* d_scalars, size_
     uint32_t* heavy_list = (uint32_t*)s->heavy.p;
     uint32_t* seg_order = (uint32_t*)s->seg_order.p;
 
+    cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+    B200_CUDA(cudaStreamIsCapturing(st, &capture));
+    const bool capturing = capture != cudaStreamCaptureStatusNone;
     const bool timing = s->timing;
     if (timing && !s->ev_init) {
         for (auto& e : s->ev) B200_CUDA(cudaEventCreate(&e));
@@ -1220,7 +1254,7 @@ int msm_launch_batch(const Bases* b, size_t base_off, const fe* d_scalars, size_
     // inside a stream capture a timing event has to become a node of the graph (external record), or a replay would not record it
     auto stamp = [&](int i) {
         if (!timing) return;
-        if (s->in_graph) cudaEventRecordWithFlags(s->ev[i], st, cudaEventRecordExternal);
+        if (capturing) cudaEventRecordWithFlags(s->ev[i], st, cudaEventRecordExternal);
         else cudaEventRecord(s->ev[i], st);
     };
     stamp(0);
@@ -1330,24 +1364,19 @@ int msm_launch_batch(const Bases* b, size_t base_off, const fe* d_scalars, size_
                                                                                                       (uint32_t)r_log, bit_sums);
     }
     // The last step, sum_b 2^b T_b, is a chain of c - 2 dependent doublings whoever runs it, and a host core runs it an
-    // order of magnitude faster than a lone warp.  The host takes it (msm_finish_batch) unless the sums are consumed on the device.
-    if (!use_host_horner(s)) B200_LAUNCH(msm_horner_kernel, (unsigned)n_windows, 32, 0, st)(bit_sums, n_bits, window_sums);
+    // order of magnitude faster than a lone warp.  The host takes it (msm_finish_batch) unless the epilogue says otherwise.
+    const MsmEpilogue e = pending->epilogue;
+    if (e != MsmEpilogue::HostBits) B200_LAUNCH(msm_horner_kernel, (unsigned)n_windows, 32, 0, st)(bit_sums, n_bits, window_sums);
+    if (e == MsmEpilogue::DevicePoint) B200_LAUNCH(k_windows_to_point, 1, 32, 0, st)(window_sums, pl.n_phys, pl.c, 0, d_point);
     B200_CUDA(cudaGetLastError());
     stamp(3);
-    if (use_host_horner(s))
+    if (e == MsmEpilogue::HostBits)
         B200_CUDA(cudaMemcpyAsync(s->h_sums.p, s->bit_sums.p, n_windows * (size_t)(pl.c - 1) * sizeof(g1_xyzz), cudaMemcpyDeviceToHost, st));
-    else
+    else if (e == MsmEpilogue::HostWindows)
         B200_CUDA(cudaMemcpyAsync(s->h_sums.p, window_sums, n_windows * sizeof(g1_xyzz), cudaMemcpyDeviceToHost, st));
     stamp(4);
-    if (!s->in_graph) B200_CUDA(cudaEventRecord(s->done_ev, st));  // a replaying caller records it after the graph launch
+    if (!capturing) B200_CUDA(cudaEventRecord(s->done_ev, st));  // a replaying caller records it after the graph launch
     return B200_OK;
-}
-
-// What msm_launch_batch leaves for msm_finish_batch, for a caller that replays the launches from a captured graph.
-void msm_mark_pending(const Bases* b, size_t n, unsigned batch, MsmScratch* s) {
-    s->pending_plan = b->plan;
-    s->pending_n = n;
-    s->pending_batch = batch;
 }
 
 // phase times of the MSM whose events have completed (the caller has waited for the stream / done_ev)
@@ -1362,11 +1391,10 @@ void msm_collect_timing(MsmScratch* s, size_t n, unsigned batch) {
     s->tot_launches += 1;
 }
 
-int msm_finish_batch(MsmScratch* s, g1_affine* out, int* out_inf) {
-    const unsigned batch = s->pending_batch;
-    s->pending_batch = 0;
+int msm_finish_batch(MsmScratch* s, const MsmPending& p, g1_affine* out, int* out_inf) {
+    const unsigned batch = p.batch;
     if (batch == 0) return B200_OK;
-    if (s->pending_n == 0) {
+    if (p.n == 0) {
         for (unsigned i = 0; i < batch; ++i) {
             out[i].x = fe_zero();
             out[i].y = fe_zero();
@@ -1374,36 +1402,25 @@ int msm_finish_batch(MsmScratch* s, g1_affine* out, int* out_inf) {
         }
         return B200_OK;
     }
-    const MsmPlan& pl = s->pending_plan;
+    const MsmPlan& pl = p.plan;
     B200_CUDA(cudaEventSynchronize(s->done_ev));
-    msm_collect_timing(s, s->pending_n, batch);
+    msm_collect_timing(s, p.n, batch);
     // host epilogue: per MSM a Horner over the physical windows (none when fully precomputed), then
     // ONE field inversion for the whole batch (Montgomery's trick over the ZZZ coordinates) — a few
     // hundred bytes of work, read straight from the pinned copy of the window sums.
     const g1_xyzz* h_sums = reinterpret_cast<const g1_xyzz*>(s->h_sums.p);
     std::vector<g1_xyzz> wsum;
-    if (use_host_horner(s)) {  // window sum = sum_b 2^b T_b from the c - 1 bit sums of each window
+    if (p.epilogue == MsmEpilogue::HostBits) {  // window sum = sum_b 2^b T_b from the c - 1 bit sums of each window
         const int n_bits = pl.c - 1;
-        const size_t n_windows = (size_t)batch * pl.n_phys;
-        wsum.resize(n_windows);
-        for (size_t w = 0; w < n_windows; ++w) {
-            const g1_xyzz* T = h_sums + w * (size_t)n_bits;
-            g1_xyzz acc = T[n_bits - 1];
-            for (int b = n_bits - 2; b >= 0; --b) acc = g1_add(g1_dbl(acc), T[b]);
-            wsum[w] = acc;
-        }
+        wsum.resize((size_t)batch * pl.n_phys);
+        for (size_t w = 0; w < wsum.size(); ++w) wsum[w] = g1_horner_pow2(h_sums + w * (size_t)n_bits, n_bits, 1);
         h_sums = wsum.data();
     }
     std::vector<g1_xyzz> totals(batch);
     std::vector<fe> prefix(batch);
     fe run = fe_one<FqCfg>();
     for (unsigned i = 0; i < batch; ++i) {
-        const g1_xyzz* hs = h_sums + (size_t)i * pl.n_phys;
-        g1_xyzz total = hs[pl.n_phys - 1];
-        for (int p = pl.n_phys - 2; p >= 0; --p) {
-            for (int k = 0; k < pl.c; ++k) total = g1_dbl(total);
-            total = g1_add(total, hs[p]);
-        }
+        const g1_xyzz total = g1_horner_pow2(h_sums + (size_t)i * pl.n_phys, pl.n_phys, pl.c);
         totals[i] = total;
         prefix[i] = run;
         if (!g1_xyzz_is_inf(total)) run = fe_mul<FqCfg>(run, total.zzz);
@@ -1430,9 +1447,10 @@ int msm_finish_batch(MsmScratch* s, g1_affine* out, int* out_inf) {
 int msm_device_batch(const Bases* b, size_t base_off, const fe* d_scalars, size_t n, size_t stride,
                      unsigned batch, int montgomery, MsmScratch* s, cudaStream_t st, g1_affine* out,
                      int* out_inf) {
-    int rc = msm_launch_batch(b, base_off, d_scalars, n, stride, batch, montgomery, s, st);
+    MsmPending p;
+    const int rc = msm_launch_batch(b, base_off, d_scalars, n, stride, batch, montgomery, MsmEpilogue::HostBits, s, st, &p);
     if (rc != B200_OK) return rc;
-    return msm_finish_batch(s, out, out_inf);
+    return msm_finish_batch(s, p, out, out_inf);
 }
 
 int msm_device(const Bases* b, size_t base_off, const fe* d_scalars, size_t n, int montgomery,

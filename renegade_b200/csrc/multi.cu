@@ -94,29 +94,13 @@ __global__ void k_sum_partials(const g1_xyzz* __restrict__ gathered, int world, 
     g1_xyzz_store(total, acc);
 }
 
-// one MSM's window sums -> a single group element: Horner over the physical windows (a single window, the
-// usual fully precomputed plan, passes through).  An empty shard contributes the identity.
-__global__ void k_windows_to_point(const g1_xyzz* __restrict__ window_sums, int n_phys, int c, int empty,
-                                   g1_xyzz* __restrict__ out) {
-    if (threadIdx.x || blockIdx.x) return;
-    if (empty) {
-        g1_xyzz_store(out, g1_xyzz_inf());
-        return;
-    }
-    g1_xyzz total = g1_xyzz_load(window_sums + (n_phys - 1));
-    for (int p = n_phys - 2; p >= 0; --p) {
-        for (int k = 0; k < c; ++k) total = g1_dbl(total);
-        total = g1_add(total, g1_xyzz_load(window_sums + p));
-    }
-    g1_xyzz_store(out, total);
-}
-
 }  // namespace
 
 struct MultiLocal {
     b200_ctx* ctx = nullptr;
     ncclComm_t comm = nullptr;
     int rank = 0;
+    DevBuf scalars;   // this rank's scalar slice, when the caller's is in host memory
     DevBuf partial;   // this rank's 128-byte record
     DevBuf gathered;  // world records + the total behind them
     HostPinned h_total;
@@ -152,6 +136,31 @@ static int multi_alloc_local(MultiLocal* l, int world) {
     if ((rc = l->gathered.reserve((size_t)(world + 1) * sizeof(g1_xyzz))) != B200_OK) return rc;
     if ((rc = l->h_total.reserve(sizeof(g1_xyzz))) != B200_OK) return rc;
     B200_CUDA(cudaEventCreateWithFlags(&l->done, cudaEventDisableTiming));
+    return B200_OK;
+}
+
+// The shards of n points over this process's devices, each non-empty one made by load(ctx, begin, count, &shard); every
+// shard made so far is freed when one fails.
+template <class Load>
+static int multi_bases_make(b200_multi* m, size_t n, b200_multi_bases** out, Load&& load) {
+    std::lock_guard<std::mutex> lk(m->mu);
+    std::unique_ptr<b200_multi_bases> b(new b200_multi_bases());
+    b->n = n;
+    const size_t nl = m->locals.size();
+    b->shard.assign(nl, nullptr);
+    b->begin.resize(nl);
+    b->end.resize(nl);
+    for (size_t i = 0; i < nl; ++i) {
+        shard_range(n, m->locals[i].rank, m->world, &b->begin[i], &b->end[i]);
+        const size_t cnt = b->end[i] - b->begin[i];
+        if (cnt == 0) continue;  // more ranks than points: this shard is empty
+        const int rc = load(m->locals[i].ctx, b->begin[i], cnt, &b->shard[i]);
+        if (rc != B200_OK) {
+            b200_multi_bases_free(m, b.release());
+            return rc;
+        }
+    }
+    *out = b.release();
     return B200_OK;
 }
 
@@ -280,56 +289,24 @@ int b200_multi_bases_load(b200_multi* m, const uint8_t* points64, size_t n, int 
                           b200_multi_bases** out) {
     B200_TRY
     if (!m || !points64 || !out || n == 0) return B200_ERR_INVALID;
-    std::lock_guard<std::mutex> lk(m->mu);
-    std::unique_ptr<b200_multi_bases> b(new b200_multi_bases());
-    b->n = n;
-    const size_t nl = m->locals.size();
-    b->shard.assign(nl, nullptr);
-    b->begin.resize(nl);
-    b->end.resize(nl);
-    for (size_t i = 0; i < nl; ++i) {
-        shard_range(n, m->locals[i].rank, m->world, &b->begin[i], &b->end[i]);
-        const size_t cnt = b->end[i] - b->begin[i];
-        if (cnt == 0) continue;  // more ranks than points: this shard is empty
-        int rc = b200_bases_load(m->locals[i].ctx, points64 + 64 * b->begin[i], cnt, window_bits, check_on_curve, &b->shard[i]);
-        if (rc != B200_OK) {
-            b200_multi_bases_free(m, b.release());
-            return rc;
-        }
-    }
-    *out = b.release();
-    return B200_OK;
+    return multi_bases_make(m, n, out, [&](b200_ctx* ctx, size_t begin, size_t cnt, b200_bases** shard) {
+        return b200_bases_load(ctx, points64 + 64 * begin, cnt, window_bits, check_on_curve, shard);
+    });
     B200_CATCH
 }
 
 int b200_multi_bases_known_dlog(b200_multi* m, uint64_t seed, size_t n, int window_bits, b200_multi_bases** out) {
     B200_TRY
     if (!m || !out || n == 0) return B200_ERR_INVALID;
-    std::lock_guard<std::mutex> lk(m->mu);
-    std::unique_ptr<b200_multi_bases> b(new b200_multi_bases());
-    b->n = n;
-    const size_t nl = m->locals.size();
-    b->shard.assign(nl, nullptr);
-    b->begin.resize(nl);
-    b->end.resize(nl);
-    for (size_t i = 0; i < nl; ++i) {
-        shard_range(n, m->locals[i].rank, m->world, &b->begin[i], &b->end[i]);
-        const size_t cnt = b->end[i] - b->begin[i];
-        if (cnt == 0) continue;
-        b200_ctx* ctx = m->locals[i].ctx;
+    return multi_bases_make(m, n, out, [&](b200_ctx* ctx, size_t begin, size_t cnt, b200_bases** shard) -> int {
         B200_CUDA(cudaSetDevice(ctx->c.device));
         void* d_pts = nullptr;
         B200_CUDA(cudaMalloc(&d_pts, cnt * 64));
-        int rc = b200_known_dlog_bases_device(ctx, seed, b->begin[i], cnt, d_pts);
-        if (rc == B200_OK) rc = b200_bases_load_device(ctx, d_pts, cnt, window_bits, &b->shard[i]);
+        int rc = b200_known_dlog_bases_device(ctx, seed, begin, cnt, d_pts);
+        if (rc == B200_OK) rc = b200_bases_load_device(ctx, d_pts, cnt, window_bits, shard);
         cudaFree(d_pts);
-        if (rc != B200_OK) {
-            b200_multi_bases_free(m, b.release());
-            return rc;
-        }
-    }
-    *out = b.release();
-    return B200_OK;
+        return rc;
+    });
     B200_CATCH
 }
 
@@ -364,23 +341,16 @@ static int multi_msm(b200_multi* m, const b200_multi_bases* b, const void* const
         B200_CUDA(cudaSetDevice(c.device));
         const fe* d_scalars = reinterpret_cast<const fe*>(scalars_local[i]);
         if (cnt && !scalars_on_device) {
-            if ((rc = c.msm.scalars.reserve(cnt * sizeof(fe) + 32)) != B200_OK) return rc;
-            B200_CUDA(cudaMemcpyAsync(c.msm.scalars.p, scalars_local[i], cnt * sizeof(fe), cudaMemcpyHostToDevice, c.stream));
-            d_scalars = reinterpret_cast<const fe*>(c.msm.scalars.p);
+            if ((rc = l.scalars.reserve(cnt * sizeof(fe) + 32)) != B200_OK) return rc;
+            B200_CUDA(cudaMemcpyAsync(l.scalars.p, scalars_local[i], cnt * sizeof(fe), cudaMemcpyHostToDevice, c.stream));
+            d_scalars = reinterpret_cast<const fe*>(l.scalars.p);
         }
         g1_xyzz* partial = reinterpret_cast<g1_xyzz*>(l.partial.p);
-        if (cnt) {
-            const Bases* bs = b->shard[i]->b;
-            c.msm.host_horner = false;  // the window sums stay on the device
-            rc = msm_launch_batch(bs, 0, d_scalars, cnt, cnt, 1, montgomery, &c.msm, c.stream);
-            c.msm.host_horner = true;
-            if (rc != B200_OK) return rc;
-            c.msm.pending_batch = 0;  // the window sums are consumed on the device, not by msm_finish_batch
-            B200_LAUNCH(k_windows_to_point, 1, 32, 0, c.stream)(reinterpret_cast<const g1_xyzz*>(c.msm.window_sums.p), bs->plan.n_phys,
-                                                      bs->plan.c, 0, partial);
-        } else {
-            B200_LAUNCH(k_windows_to_point, 1, 32, 0, c.stream)(nullptr, 1, 1, 1, partial);
-        }
+        MsmPending launched;  // nothing for msm_finish_batch: the point stays on the device
+        rc = cnt ? msm_launch_batch(b->shard[i]->b, 0, d_scalars, cnt, cnt, 1, montgomery, MsmEpilogue::DevicePoint, &c.msm, c.stream,
+                                    &launched, partial)
+                 : msm_identity_point(partial, c.stream);  // an empty shard contributes the identity
+        if (rc != B200_OK) return rc;
     }
     // 2. the exchange: all_gather of the 128-byte records (grouped when this process drives several devices)
     if (m->world > 1) {

@@ -1031,29 +1031,37 @@ static int run_segment(ProofGraphSet* gs, int idx, cudaStream_t st, F&& fn) {
     return B200_OK;
 }
 
-// Enqueue `count` commitments as segment `idx` (after `before`'s launches), leaving the batch pending for commit_collect.
+// Commitment epilogue of a batch: from this many commitments in one MSM on, the last step of every window sum (sum_b 2^b
+// T_b) runs on the device (msm_horner_kernel, one warp per window, all windows at once) instead of on the host
+// (msm_finish_batch, serial in the number of commitments).  Measured with tools/prove_batch_bench.py on an H100 80GB HBM3
+// at 700 W (DESIGN §6): even at 5 commitments of 2^12-2^14 points, the device ahead from 10 on (2^13: 0.64 vs 0.71 ms
+// at 10, 2.85 vs 3.86 ms at 64).
+constexpr unsigned kDeviceHornerFrom = 10;
+
+// Enqueue `count` commitments as segment `idx` (after `before`'s launches); `*pending` is the batch for commit_collect.
 template <class F>
-static int commit_enqueue(Context* c, MsmScratch* msm, const Bases* srs, ProofGraphSet* gs, int idx, const fe* d_coeffs, size_t len,
-                          size_t stride, unsigned count, F&& before) {
+static int commit_enqueue(Context* c, MsmScratch* msm, const Bases* srs, ProofGraphSet* gs, bool single, int idx, const fe* d_coeffs,
+                          size_t len, size_t stride, unsigned count, MsmPending* pending, F&& before) {
     cudaStream_t st = c->stream;
+    const MsmEpilogue e = single || count < kDeviceHornerFrom ? MsmEpilogue::HostBits : MsmEpilogue::HostWindows;
     const int r = run_segment(gs, idx, st, [&]() -> int {
         const int r2 = before();
         if (r2 != B200_OK) return r2;
-        return msm_launch_batch(srs, 0, d_coeffs, len, stride, count, /*montgomery=*/1, msm, st);
+        return msm_launch_batch(srs, 0, d_coeffs, len, stride, count, /*montgomery=*/1, e, msm, st, pending);
     });
     if (r != B200_OK) return r;
-    if (gs) {  // what msm_launch_batch leaves behind when it runs outside a capture
-        msm_mark_pending(srs, len, count, msm);
+    if (gs) {  // a graph launch: the batch the captured launch describes, and the event it leaves to its caller
+        *pending = msm_pending(srs, len, count, e);
         B200_CUDA(cudaEventRecord(msm->done_ev, st));
     }
     return B200_OK;
 }
 
-static int commit_collect(MsmScratch* msm, unsigned count, g1_affine* out) {
-    std::vector<int> inf(count);
-    const int rc = msm_finish_batch(msm, out, inf.data());
+static int commit_collect(MsmScratch* msm, const MsmPending& pending, g1_affine* out) {
+    std::vector<int> inf(pending.batch);
+    const int rc = msm_finish_batch(msm, pending, out, inf.data());
     if (rc != B200_OK) return rc;
-    for (unsigned i = 0; i < count; ++i)
+    for (unsigned i = 0; i < pending.batch; ++i)
         if (inf[i]) std::memset(&out[i], 0, sizeof(out[i]));
     return B200_OK;
 }
@@ -1105,19 +1113,6 @@ static ProverBufs batch_bufs(Context* c) {
     Context::BatchBufs& b = c->batch;
     return {&b.ws, &b.nscr, &b.nscr2, &b.d_params, &b.h_small, &b.h_params, &b.msm};
 }
-
-// Commitment epilogue of a batch: from this many commitments in one MSM on, the last step of every window sum (sum_b 2^b
-// T_b) runs on the device (msm_horner_kernel, one warp per window, all windows at once) instead of on the host
-// (msm_finish_batch, serial in the number of commitments).  Measured with tools/prove_batch_bench.py on an H100 80GB HBM3
-// at 700 W (DESIGN §6): even at 5 commitments of 2^12-2^14 points, the device ahead from 10 on (2^13: 0.64 vs 0.71 ms
-// at 10, 2.85 vs 3.86 ms at 64).
-constexpr unsigned kDeviceHornerFrom = 10;
-
-// MsmScratch::in_graph holds only while a prover call runs: cleared on every way out of it
-struct InGraphReset {
-    MsmScratch& s;
-    ~InGraphReset() { s.in_graph = false; }
-};
 
 // The value at zeta that the verifier expects of the batched polynomial opened at zeta (lin + sum v^i w_i + sum
 // v^(5+i) sigma_i): E = -r0 + sum v^i w_i(zeta) + sum v^(5+i) sigma_i(zeta), read from vt::plonk_terms (with u = 0 the
@@ -1196,8 +1191,6 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
     // graphs: only once a proof of this key has run eagerly on this context (every buffer has its final size then)
     ProofGraphSet* gset = single ? graph_set_for(c, pk->id) : nullptr;
     ProofGraphSet* gs = gset && gset->proofs_seen > 0 ? gset : nullptr;
-    bf.msm->in_graph = gs != nullptr;
-    InGraphReset in_graph_reset{*bf.msm};
     ProofParams* hp = reinterpret_cast<ProofParams*>(bf.h_params->p);  // pinned staging copy, one block per proof
     ProofParams* dp = reinterpret_cast<ProofParams*>(bf.d_params->p);  // what the kernels read
     static_assert(sizeof(ProofParams) % sizeof(fe) == 0, "ProofParams is an array of field elements");
@@ -1207,9 +1200,9 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
         B200_CUDA(cudaMemcpyAsync(dp, hp, k * sizeof(ProofParams), cudaMemcpyHostToDevice, st));
         return B200_OK;
     };
+    MsmPending pending;  // the commitments between commit_enqueue and commit_collect
     auto commit_enqueue = [&](int idx, const fe* d_coeffs, size_t len, size_t stride, unsigned count, auto&& before) -> int {
-        if (!single) bf.msm->host_horner = count < kDeviceHornerFrom;
-        return b200::commit_enqueue(c, bf.msm, pk->srs, gs, idx, d_coeffs, len, stride, count, before);
+        return b200::commit_enqueue(c, bf.msm, pk->srs, gs, single, idx, d_coeffs, len, stride, count, &pending, before);
     };
     auto nothing = []() -> int { return B200_OK; };
     std::vector<g1_affine> comms((size_t)NW * k);  // the commitments of the current round, [proof][i]
@@ -1328,7 +1321,7 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
         B200_CUDA(cudaEventRecord(c->ev_join, s2));
     }
     if ((rc = commit_enqueue(2, w.wpoly, n + 2, S, NW * k, nothing)) != B200_OK) return rc;
-    if ((rc = commit_collect(bf.msm, NW * k, comms.data())) != B200_OK) return rc;
+    if ((rc = commit_collect(bf.msm, pending, comms.data())) != B200_OK) return rc;
     for (unsigned p = 0; p < k; ++p) {
         ProofOut* proof = items[p].proof;
         std::memcpy(proof->wires_poly_comms, &comms[(size_t)p * NW], sizeof(proof->wires_poly_comms));
@@ -1364,7 +1357,7 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
         return B200_OK;
     });
     if (rc != B200_OK) return rc;
-    if ((rc = commit_collect(bf.msm, k, comms.data())) != B200_OK) return rc;
+    if ((rc = commit_collect(bf.msm, pending, comms.data())) != B200_OK) return rc;
     for (unsigned p = 0; p < k; ++p) {
         items[p].proof->prod_perm_poly_comm = comms[p];
         trs[p].append_commitment(comms[p]);
@@ -1421,7 +1414,7 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
         return B200_OK;
     });
     if (rc != B200_OK) return rc;
-    if ((rc = commit_collect(bf.msm, NW * k, comms.data())) != B200_OK) return rc;
+    if ((rc = commit_collect(bf.msm, pending, comms.data())) != B200_OK) return rc;
     unsigned satisfied = 0;
     for (unsigned p = 0; p < k; ++p) {  // the flags were copied before the commitments' window sums on the same stream
         if (h_flag[p]) items[p].status = B200_ERR_UNSATISFIED;
@@ -1575,7 +1568,7 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
         c->plonk_ms[6] = std::chrono::duration<float, std::milli>(clk::now() - t0).count();
     }
     comms.resize(2 * k);
-    if ((rc = commit_collect(bf.msm, 2 * k, comms.data())) != B200_OK) return rc;
+    if ((rc = commit_collect(bf.msm, pending, comms.data())) != B200_OK) return rc;
     for (unsigned p = 0; p < k; ++p) {
         items[p].proof->opening_proof = comms[2 * p];
         items[p].proof->shifted_opening_proof = comms[2 * p + 1];
@@ -1765,9 +1758,7 @@ static int link_chunk(Context* c, const ProverBufs& bf, const Bases* srs, LinkIt
                              (uint64_t)i0.size};
     ProofGraphSet* gset = single ? graph_set_for(c, ~(uint64_t)0, sub) : nullptr;
     ProofGraphSet* gs = gset && gset->proofs_seen > 0 ? gset : nullptr;
-    msm->in_graph = gs != nullptr;
-    InGraphReset in_graph_reset{*msm};
-    if (!single) msm->host_horner = k < kDeviceHornerFrom;
+    MsmPending pending;  // the commitments between commit_enqueue and commit_collect
 
     size_t at = 0;
     for (unsigned y = 0; y < k; ++y) {
@@ -1787,7 +1778,7 @@ static int link_chunk(Context* c, const ProverBufs& bf, const Bases* srs, LinkIt
         B200_CUDA(cudaMemcpyAsync(d_a1 + (size_t)y * L, items[y]->a1, items[y]->len1 * sizeof(fe), cudaMemcpyDefault, st));
         B200_CUDA(cudaMemcpyAsync(d_a2 + (size_t)y * L, items[y]->a2, items[y]->len2 * sizeof(fe), cudaMemcpyDefault, st));
     }
-    rc = commit_enqueue(c, msm, srs, gs, 0, d_quot, Q, Q, k, [&]() -> int {
+    rc = commit_enqueue(c, msm, srs, gs, single, 0, d_quot, Q, Q, k, &pending, [&]() -> int {
         int r;
         B200_CUDA(cudaMemcpyAsync(d_desc, h_desc, desc_bytes, cudaMemcpyHostToDevice, st));
         B200_CUDA(cudaMemsetAsync(d_flag, 0, (size_t)k * 4, st));
@@ -1827,7 +1818,7 @@ static int link_chunk(Context* c, const ProverBufs& bf, const Bases* srs, LinkIt
     });
     if (rc != B200_OK) return rc;
     std::vector<g1_affine> comms(k);
-    if ((rc = commit_collect(msm, k, comms.data())) != B200_OK) return rc;
+    if ((rc = commit_collect(msm, pending, comms.data())) != B200_OK) return rc;
     unsigned proved = 0;
     for (unsigned y = 0; y < k; ++y) {  // the flags were copied before the commitments' window sums on the same stream
         LinkItem& it = *items[y];
@@ -1849,7 +1840,7 @@ static int link_chunk(Context* c, const ProverBufs& bf, const Bases* srs, LinkIt
         fill_open_params(&p.open, eta);
     }
     if (!proved) return B200_OK;  // see the statuses
-    rc = commit_enqueue(c, msm, srs, gs, 1, d_open + 1, L - 1, L, k, [&]() -> int {
+    rc = commit_enqueue(c, msm, srs, gs, single, 1, d_open + 1, L - 1, L, k, &pending, [&]() -> int {
         B200_CUDA(cudaMemcpyAsync(dp, hp, k * sizeof(LinkParams), cudaMemcpyHostToDevice, st));
         LinArgs a{};
         a.count = 2;
@@ -1867,7 +1858,7 @@ static int link_chunk(Context* c, const ProverBufs& bf, const Bases* srs, LinkIt
         return B200_OK;
     });
     if (rc != B200_OK) return rc;
-    if ((rc = commit_collect(msm, k, comms.data())) != B200_OK) return rc;
+    if ((rc = commit_collect(msm, pending, comms.data())) != B200_OK) return rc;
     for (unsigned y = 0; y < k; ++y)
         if (items[y]->status == B200_OK) items[y]->out->opening_proof = comms[y];
     if (gset && !gs) gset->proofs_seen = 1;  // both segments have run eagerly: the next call with this key captures them

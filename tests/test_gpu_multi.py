@@ -8,10 +8,10 @@ result: the window plan of every shard (`b200_multi_bases_plan`, the window rest
 ranges, and which windows hold digits (`msm_digits.py`).
 
 What the layer adds to the single-context MSM and is pinned here: both entry points (`b200_multi_init` and the
-per-rank `b200_multi_init_rank`), every window plan with the window sums kept on the device (`host_horner` off),
-`k_windows_to_point`'s Horner over split physical windows, `k_sum_partials` on cancelling and equal partials and next to
-an empty shard, the context's own MSMs and replayed proofs around multi MSMs (the `host_horner` restore), the timing
-`bench.py` reads, and the refusals."""
+per-rank `b200_multi_init_rank`), every window plan through the MSM's device-point epilogue (one point per shard left on
+the device), `k_windows_to_point`'s Horner over split physical windows, `k_sum_partials` on cancelling and equal partials
+and next to an empty shard, the context's own MSMs and replayed proofs around multi MSMs (each launch names its own
+epilogue), the timing `bench.py` reads, and the refusals."""
 import ast
 import ctypes as C
 import math
@@ -322,10 +322,10 @@ def _batch_device(c, bases, d_scalars, n, stride, batch, montgomery):
 
 
 def test_context_msms_around_multi_msms(oracle, pyoracle):
-    """multi_msm turns the context's host Horner off for its own launch and back on.  On multi.ctx(0) of a fresh
-    handle: first a proof whose graphs are captured BEFORE the context's first multi MSM and replayed after each of
-    several (a replay finishes its commitments by whatever host_horner says then, so a flag left off reads bit sums as
-    window sums); then the context's MSMs on another base set (host and device scalars, batches through
+    """multi_msm launches on the context's MSM scratch with the device-point epilogue, the context's own calls with theirs.
+    On multi.ctx(0) of a fresh handle: first a proof whose graphs are captured BEFORE the context's first multi MSM and
+    replayed after each of several (a replay must finish its commitments by the epilogue it captured, or it reads bit
+    sums as window sums); then the context's MSMs on another base set (host and device scalars, batches through
     b200_msm_batch_device, canonical and Montgomery) interleaved with multi MSMs from host and device slices; then
     another proof.  Every result = oracle."""
     from renegade_b200.sharded import MultiGpu
@@ -554,7 +554,7 @@ def test_multi_partials_cancel_and_double(multi_w, oracle):
 
 def test_multi_one_point_next_to_an_empty_shard(multi_w, oracle):
     """n = 1: at world 2 shard 1 is empty (plan all zeros, no scalar slice needed) and contributes the identity
-    record of k_windows_to_point(…, empty = 1)."""
+    record of msm_identity_point (k_windows_to_point(…, empty = 1))."""
     m = multi_w
     pts = oracle.known_dlog_bases(0x1, 1)
     mb = m.load_bases(pts, check_on_curve=True)

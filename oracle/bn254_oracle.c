@@ -116,6 +116,30 @@ void orc_splitmix_fr(u64 seed, size_t first, size_t n, int montgomery, u64* out)
     }
 }
 
+/* sum_i a_i b_i mod r over i < n, a_i = splitmix_fr(seed_a)[first_a + i], b_i = splitmix_fr(seed_b)[first_b + i]: the
+ * discrete log of an MSM of n known-dlog bases with SplitMix scalars, without holding either vector.  Montgomery
+ * products of canonical operands carry one factor R^-1, which the final to_mont removes. */
+void orc_fr_dot(u64 seed_a, size_t first_a, u64 seed_b, size_t first_b, size_t n, u64 out_canon[4]) {
+    const size_t chunk = (size_t)1 << 14, n_chunks = (n + chunk - 1) / chunk;
+    u64* part = (u64*)calloc(n_chunks ? n_chunks * 4 : 4, sizeof(u64));
+#pragma omp parallel for schedule(static)
+    for (size_t c = 0; c < n_chunks; ++c) {
+        const size_t end = (c + 1) * chunk < n ? (c + 1) * chunk : n;
+        u64 acc[4] = {0, 0, 0, 0}, a[4], b[4], t[4];
+        for (size_t i = c * chunk; i < end; ++i) {
+            splitmix_fr_one(seed_a, first_a + i, a);
+            splitmix_fr_one(seed_b, first_b + i, b);
+            fp_mul(&FR, t, a, b);
+            fp_add(&FR, acc, acc, t);
+        }
+        memcpy(part + 4 * c, acc, 32);
+    }
+    u64 sum[4] = {0, 0, 0, 0};
+    for (size_t c = 0; c < n_chunks; ++c) fp_add(&FR, sum, sum, part + 4 * c);
+    free(part);
+    fp_to_mont(&FR, out_canon, sum);
+}
+
 void orc_g1_known_dlog_bases(u64 seed, size_t first, size_t n, u64* out_xy) {
     /* table T[b] = 2^b * G (affine) so each base costs popcount(a_i) mixed adds */
     aff* T = (aff*)malloc(256 * sizeof(aff));

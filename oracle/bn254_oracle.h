@@ -50,6 +50,10 @@ void orc_splitmix_fr(uint64_t seed, size_t first, size_t n, int montgomery, uint
 /* known-dlog bases P_i = a_i * G, a_i = splitmix_fr(seed)[first + i]; out n x 8 limbs (Montgomery) */
 void orc_g1_known_dlog_bases(uint64_t seed, size_t first, size_t n, uint64_t* out_xy);
 
+/* sum_i a_i b_i mod r (canonical) over i < n, a_i = splitmix_fr(seed_a)[first_a + i], b_i = splitmix_fr(seed_b)[first_b + i]
+ * (OpenMP): the discrete log of an MSM of known-dlog bases with SplitMix scalars */
+void orc_fr_dot(uint64_t seed_a, size_t first_a, uint64_t seed_b, size_t first_b, size_t n, uint64_t out_canon[4]);
+
 /* --- MSM: restates ark-ec 0.4.2 VariableBaseMSM::msm_bigint (SURVEY.md App. B) ------------ */
 /* scalars canonical (BigInt<4>), bases affine Montgomery; threads across windows (OpenMP,
  * like arkworks' rayon cfg_into_iter over windows). */

@@ -106,6 +106,15 @@ def known_dlog_bases(seed: int, n: int, first: int = 0) -> np.ndarray:
     return out
 
 
+def fr_dot(seed_a: int, seed_b: int, n: int, first_a: int = 0, first_b: int = 0) -> int:
+    """sum_i a_i b_i mod r over i < n, a = splitmix_fr(seed_a, first=first_a), b = splitmix_fr(seed_b, first=first_b):
+    the discrete log of an MSM of known-dlog bases with SplitMix scalars, computed without materialising either vector."""
+    out = np.zeros(4, dtype=np.uint64)
+    lib().orc_fr_dot(C.c_uint64(seed_a), C.c_size_t(first_a), C.c_uint64(seed_b), C.c_size_t(first_b), C.c_size_t(n),
+                     _p(out))
+    return limbs_to_int(out)
+
+
 def g1_on_curve(xy: np.ndarray) -> bool:
     return bool(lib().orc_g1_on_curve(_p(np.ascontiguousarray(xy, dtype=np.uint64))))
 

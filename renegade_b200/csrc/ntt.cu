@@ -319,12 +319,13 @@ int domain_create(unsigned log_n, cudaStream_t st, Domain** out) {
     return B200_OK;
 }
 
-// data: batch transforms of n elements, `stride` elements apart, transformed in place.
-// scratch: at least (batch-1)*stride + n elements when log_n > kTileLog.
-int ntt_device(const Domain* d, fe* data, fe* scratch, int inverse, int coset, unsigned batch,
-               size_t stride, cudaStream_t st) {
+// CUDA caps gridDim.y at 65535: a larger batch is launched in chunks of at most this many transforms
+constexpr unsigned kMaxBatchPerLaunch = 65535;
+
+// the passes of `batch` <= kMaxBatchPerLaunch transforms, one grid row per transform
+static int ntt_launch(const Domain* d, fe* data, fe* scratch, int inverse, int coset, unsigned batch, size_t stride,
+                      cudaStream_t st) {
     const int L = (int)d->log_n;
-    if (L == 0 || batch == 0) return B200_OK;  // size-1 transform is the identity (n^-1 = 1)
     const int P = (L + kTileLog - 1) / kTileLog;
     const int e_log = L < kTileLog ? L : kTileLog;
     const int base = L / P, extra = L % P;
@@ -365,6 +366,20 @@ int ntt_device(const Domain* d, fe* data, fe* scratch, int inverse, int coset, u
         hi -= w;
     }
     return cudaGetLastError() == cudaSuccess ? B200_OK : B200_ERR_CUDA;
+}
+
+// data: batch transforms of n elements, `stride` elements apart, transformed in place.
+// scratch: at least (batch-1)*stride + n elements when log_n > kTileLog.
+int ntt_device(const Domain* d, fe* data, fe* scratch, int inverse, int coset, unsigned batch,
+               size_t stride, cudaStream_t st) {
+    if (d->log_n == 0 || batch == 0) return B200_OK;  // size-1 transform is the identity (n^-1 = 1)
+    for (unsigned first = 0; first < batch; first += kMaxBatchPerLaunch) {
+        const unsigned rows = batch - first < kMaxBatchPerLaunch ? batch - first : kMaxBatchPerLaunch;
+        const size_t off = (size_t)first * stride;
+        const int rc = ntt_launch(d, data + off, scratch + off, inverse, coset, rows, stride, st);
+        if (rc != B200_OK) return rc;
+    }
+    return B200_OK;
 }
 
 }  // namespace b200

@@ -37,6 +37,12 @@ SEG_LEN = _constant(r"#define B200_SEG_LEN (\d+)")
 COMBINE_SEQ = _constant(r"constexpr int kCombineSeq = (\d+);")
 HEAVY_MIN = SEG_LEN * COMBINE_SEQ + 1  # fewest entries of a heavy bucket
 SCAN_TILE = _constant(r"constexpr int kScanThreads = (\d+);") * _constant(r"constexpr int kScanItems = (\d+);")  # buckets per scan tile
+IDX_BITS = _constant(r"constexpr uint32_t kIdxBits = (\d+);")  # bits of the point index in a bucket entry
+# msm_launch_batch refuses a launch whose worst-case entries, buckets or segments reach these powers of two
+_GUARD = re.search(r"max_entries >= \(\(size_t\)1 << (\d+)\) \|\| n_buckets >= \(\(size_t\)1 << (\d+)\) \|\| "
+                   r"max_segs >= \(\(size_t\)1 << (\d+)\)", _msm_source())
+assert _GUARD, "msm.cu no longer states the launch guard of msm_launch_batch"
+ENTRIES_LOG, BUCKETS_LOG, SEGMENTS_LOG = (int(g) for g in _GUARD.groups())
 
 R = 0x30644E72E131A029B85045B68181585D2833E84879B97091_43E1F593F0000001  # the scalar field
 
@@ -44,6 +50,74 @@ R = 0x30644E72E131A029B85045B68181585D2833E84879B97091_43E1F593F0000001  # the s
 def num_windows(c: int) -> int:
     """W of msm_choose_plan: enough c-bit windows for 255 bits."""
     return (255 + c - 1) // c
+
+
+def choose_window(n: int, window_bits: int) -> int:
+    """The window c of msm_choose_plan (msm.cu) restated: a fixed window as given, else the c in 6 … 23 with at most 32
+    windows that minimises the throughput model (window_bits 0) or the latency model (1).  Where the two models pick
+    different windows (31 and 4099 points: 8 / 10 and 13 / 15; 110 000 points: 17 / 16) the plan's window shows which
+    model ran."""
+    if window_bits > 1:
+        return window_bits
+    best, best_cost = 0, 1e300
+    for c in range(6, 24):
+        W = num_windows(c)
+        if W > 32:
+            continue
+        t = 254 - c * (W - 1)
+        nw = float(n) * W
+        shrt = 0 if t >= c - 6 else c - 6 - t
+        if window_bits == 0:
+            buckets = float(1 << (c - 1))
+            extra = max(0.0, nw / 32.0 - 0.55 * buckets)
+            cost = (nw * (9.5 + 1.6 * (1.0 + 0.3 * shrt)) + buckets * 25.0 + extra * 12.5) / 66.7e6
+        else:
+            load = nw / float(1 << (c - 1))
+            acc = max(nw / 6.6e6, 0.055 + 0.006 * min(load, 32.0) + 0.004 * min(load / 32.0, 64.0))
+            top = float(n) / float(1 << t) / 32.0 if t < c - 1 else 0.0
+            cost = (0.042 + nw * (1.0 + 0.1 * shrt) / 54e6 + acc + 0.13 + 0.0075 * c + float(1 << c) / 4.9e6
+                    + 0.008 * min(top, 64.0))
+        if cost < best_cost:
+            best, best_cost = c, cost
+    return best
+
+
+def physical_windows(n: int, W: int, budget_bytes: int, forced: int = 1) -> int:
+    """n_phys of msm_choose_plan: from the forced split (B200_MSM_PHYS_WINDOWS, ignored outside 1 … W), one more physical
+    window at a time until the ceil(W / n_phys) tables of n 64-byte points fit the budget, or every window is physical."""
+    phys = forced if 1 <= forced <= W else 1
+    while -(-W // phys) * n * 64 > budget_bytes and phys < W:
+        phys += 1
+    return phys
+
+
+def expected_plan(n: int, window_bits: int, phys: int = 1) -> dict:
+    c = choose_window(n, window_bits)
+    W = num_windows(c)
+    return {"window_bits": c, "digits": W, "physical_windows": phys, "tables": -(-W // phys)}
+
+
+def index_space(n: int, c: int, n_phys: int, batch: int) -> dict:
+    """What msm_launch_batch sizes a launch of `batch` MSMs of n points by, before it allocates anything: the worst-case
+    bucket entries (every digit non-zero), the buckets, and the worst-case segments (full ones plus one partial per
+    bucket); and whether the launch is refused because one of them leaves its index space (32-bit entry offsets, bucket
+    indices below 2^31, 30-bit segment counts in the scan's status word)."""
+    entries = n * num_windows(c) * batch
+    buckets = n_phys * (1 << (c - 1)) * batch
+    segments = entries // SEG_LEN + buckets
+    refused = entries >= 1 << ENTRIES_LOG or buckets >= 1 << BUCKETS_LOG or segments >= 1 << SEGMENTS_LOG
+    return {"entries": entries, "buckets": buckets, "segments": segments, "refused": refused}
+
+
+# One launch shape (n, c, n_phys, batch) per guard of msm_launch_batch, each the first batch past its limit (the
+# b200_msm_batch_device cap of 64 for the entries): worst-case entries exactly 2^32; buckets past 2^31; segments past 2^30
+# with entries and buckets inside theirs.  The guards run before anything is allocated, so the last two cost a
+# one-point base set; the first needs 2^21 points at c = 8, split into one table.
+GUARD_SHAPES = {
+    "entries": (1 << 21, 8, 32, 64),
+    "buckets": (1, 23, 12, 43),
+    "segments": (1, 23, 12, 22),
+}
 
 
 def edge_scalars(c: int) -> list[int]:

@@ -64,42 +64,6 @@ def bench_multi_plan():
     return ns["multi_plan"]
 
 
-def choose_window(n: int, window_bits: int) -> int:
-    """The window c of msm_choose_plan (msm.cu) restated: a fixed window as given, else the c in 6 … 23 with at most 32
-    windows that minimises the throughput model (window_bits 0) or the latency model (1).  Where the two models pick
-    different windows (31 and 4099 points: 8 / 10 and 13 / 15; 110 000 points: 17 / 16) the plan's window shows which
-    model ran."""
-    if window_bits > 1:
-        return window_bits
-    best, best_cost = 0, 1e300
-    for c in range(6, 24):
-        W = md.num_windows(c)
-        if W > 32:
-            continue
-        t = 254 - c * (W - 1)
-        nw = float(n) * W
-        shrt = 0 if t >= c - 6 else c - 6 - t
-        if window_bits == 0:
-            buckets = float(1 << (c - 1))
-            extra = max(0.0, nw / 32.0 - 0.55 * buckets)
-            cost = (nw * (9.5 + 1.6 * (1.0 + 0.3 * shrt)) + buckets * 25.0 + extra * 12.5) / 66.7e6
-        else:
-            load = nw / float(1 << (c - 1))
-            acc = max(nw / 6.6e6, 0.055 + 0.006 * min(load, 32.0) + 0.004 * min(load / 32.0, 64.0))
-            top = float(n) / float(1 << t) / 32.0 if t < c - 1 else 0.0
-            cost = (0.042 + nw * (1.0 + 0.1 * shrt) / 54e6 + acc + 0.13 + 0.0075 * c + float(1 << c) / 4.9e6
-                    + 0.008 * min(top, 64.0))
-        if cost < best_cost:
-            best, best_cost = c, cost
-    return best
-
-
-def expected_plan(n: int, window_bits: int, phys: int = 1) -> dict:
-    c = choose_window(n, window_bits)
-    W = md.num_windows(c)
-    return {"window_bits": c, "digits": W, "physical_windows": phys, "tables": -(-W // phys)}
-
-
 def assert_point(got, exp, what=""):
     (out, inf), (eout, einf) = got, exp
     assert inf == einf and (out == eout).all(), what
@@ -183,9 +147,9 @@ PLAN_SIZES = [1, 31, 4099, 110_000]  # 110 000 > 2^16: the throughput and latenc
 def test_window_model_restatement_separates_the_plans():
     """The sizes above are where the plan's window tells the two automatic plans apart (n = 1 cannot)."""
     for n in PLAN_SIZES[1:]:
-        assert choose_window(n, 0) != choose_window(n, 1), n
-    assert (choose_window(1, 0), choose_window(31, 0), choose_window(4099, 0), choose_window(110_000, 0)) == (8, 8, 13, 17)
-    assert (choose_window(1, 1), choose_window(31, 1), choose_window(4099, 1), choose_window(110_000, 1)) == (8, 10, 15, 16)
+        assert md.choose_window(n, 0) != md.choose_window(n, 1), n
+    assert [md.choose_window(n, 0) for n in (1, 31, 4099, 110_000)] == [8, 8, 13, 17]
+    assert [md.choose_window(n, 1) for n in (1, 31, 4099, 110_000)] == [8, 10, 15, 16]
 
 
 @pytest.mark.parametrize("entry", ["single_process", "for_rank"])
@@ -204,7 +168,7 @@ def test_multi_plans_match_oracle(request, ctx, inputs, entry, source, n, window
     try:
         assert len(mb) == n and mb.shard(0) == (0, n)
         plan = plan_of(m, mb)
-        assert plan == single.plan == expected_plan(n, window_bits), (plan, single.plan)
+        assert plan == single.plan == md.expected_plan(n, window_bits), (plan, single.plan)
         assert_point(m.msm(mb, s), exp, "canonical")
         assert_point(m.msm(mb, s_mont, montgomery=True), exp, "montgomery")
         assert_point(ctx.msm(single, s), exp, "single context")
@@ -271,7 +235,7 @@ def test_multi_physical_windows(multi1, ctx, oracle, monkeypatch, c, phys):
         for key, p in (("pts", pts), ("one", one)):
             mb, single = multi1.load_bases(p, window_bits=c), ctx.load_bases(p, window_bits=c)
             loaded[key] = (mb, single)
-            assert plan_of(multi1, mb) == single.plan == expected_plan(n, c, n_phys)
+            assert plan_of(multi1, mb) == single.plan == md.expected_plan(n, c, n_phys)
         for p, name, vals in cases:
             mb, single = loaded["pts" if p is pts else "one"]
             s = oracle.ints_to_array(vals)
@@ -467,7 +431,7 @@ def test_multi_msm_2_20_per_gpu_closed_form(oracle, pyoracle, world):
     m = MultiGpu.single_process(list(range(world)))
     try:
         mb = m.known_dlog_bases(0xB200, n)
-        assert bench_multi_plan()(m, mb) == plan_of(m, mb, 0) == expected_plan(per, 0)
+        assert bench_multi_plan()(m, mb) == plan_of(m, mb, 0) == md.expected_plan(per, 0)
         ctxs = [m.ctx(i) for i in range(world)]
         for c in ctxs:
             c.msm_timing(True)
@@ -561,7 +525,7 @@ def test_multi_one_point_next_to_an_empty_shard(multi_w, oracle):
     try:
         cuts = [mb.shard(i) for i in range(m.world)]
         assert cuts == [(0, 1)] + [(1, 1)] * (m.world - 1)
-        assert plan_of(m, mb, 0) == expected_plan(1, 0)
+        assert plan_of(m, mb, 0) == md.expected_plan(1, 0)
         for i in range(1, m.world):
             assert plan_of(m, mb, i) == dict.fromkeys(PLAN_KEYS, 0)
         for v in (1, 2, R - 1, 0xDEADBEEF, (R - 1) // 2):
@@ -583,7 +547,7 @@ def test_multi_physical_windows_sharded(multi_w, oracle, monkeypatch):
     try:
         for i in range(m.world):
             b, e = mb.shard(i)
-            assert plan_of(m, mb, i) == expected_plan(e - b, c, n_phys)
+            assert plan_of(m, mb, i) == md.expected_plan(e - b, c, n_phys)
         rng = random.Random(77)
         for name, vals in phys_scalar_sets(c, n_phys, n, rng):
             s = oracle.ints_to_array(vals)

@@ -17,6 +17,55 @@ edge_scalars = md.edge_scalars
 
 def test_constants_read_from_the_kernel():
     assert md.SEG_LEN == 32 and md.COMBINE_SEQ == 64 and md.HEAVY_MIN == 2049 and md.SCAN_TILE == 4096
+    assert md.IDX_BITS == 26 and (md.ENTRIES_LOG, md.BUCKETS_LOG, md.SEGMENTS_LOG) == (32, 31, 30)
+
+
+def test_guard_shapes_land_on_their_guard():
+    """Each shape of GUARD_SHAPES trips the guard it is named for, with one MSM fewer in the batch inside that limit: the
+    GPU test that runs them checks each guard at its boundary.  The entries and segments shapes trip nothing else and
+    one MSM fewer is not refused at all."""
+    limit = {"entries": 1 << md.ENTRIES_LOG, "buckets": 1 << md.BUCKETS_LOG, "segments": 1 << md.SEGMENTS_LOG}
+    for name, (n, c, n_phys, batch) in md.GUARD_SHAPES.items():
+        assert 1 <= n_phys <= md.num_windows(c) and batch <= 64, name
+        at = md.index_space(n, c, n_phys, batch)
+        below = md.index_space(n, c, n_phys, batch - 1)
+        assert at["refused"] and at[name] >= limit[name] > below[name], name
+        assert name == "buckets" or not below["refused"], name
+        assert [k for k in limit if at[k] >= limit[k]] == (["buckets", "segments"] if name == "buckets" else [name])
+    assert md.index_space(*md.GUARD_SHAPES["entries"])["entries"] == 1 << 32
+    # the buckets guard cannot trip alone: every bucket is at least one worst-case segment
+    for c in range(8, 24):
+        for n_phys in (1, md.num_windows(c)):
+            batch = -(-(1 << md.BUCKETS_LOG) // (n_phys << (c - 1)))
+            assert md.index_space(1, c, n_phys, batch)["segments"] >= 1 << md.SEGMENTS_LOG
+
+
+def test_large_launches_inside_the_index_space():
+    """The GPU runs of 2^22 points at c = 16: 40 MSMs put the worst-case entry offsets past 2^31 (bit 31 set in real
+    offsets, as at most one digit in 2^15 is zero), 63 just below 2^32; 64 would be refused.  One MSM of 2^26 points
+    at any automatic window stays inside every limit."""
+    big = md.index_space(1 << 22, 16, 1, 40)
+    assert big["entries"] >= (1 << 31) + (1 << 28) and not big["refused"]
+    top = md.index_space(1 << 22, 16, 1, 63)
+    assert (1 << 32) - top["entries"] == 1 << 26 and not top["refused"]
+    assert md.index_space(1 << 22, 16, 1, 64)["refused"]
+    for wb in (0, 1):
+        c = md.choose_window(1 << 26, wb)
+        assert not md.index_space(1 << 26, c, md.num_windows(c), 1)["refused"]
+
+
+def test_physical_windows_restatement():
+    """The budget split of msm_choose_plan: 2^26 points at c = 20 (13 windows) need 52 GiB unsplit, so half of an
+    idle 80 GB GPU's memory takes two physical windows (7 tables); a forced split is a floor, not a ceiling."""
+    assert md.choose_window(1 << 26, 0) == 20 and md.num_windows(20) == 13
+    gib = 1 << 30
+    assert md.physical_windows(1 << 26, 13, 52 * gib) == 1
+    assert md.physical_windows(1 << 26, 13, 52 * gib - 1) == 2
+    assert md.physical_windows(1 << 26, 13, 39 * gib) == 2
+    assert md.physical_windows(1 << 26, 13, 0) == 13
+    assert md.physical_windows(1 << 26, 13, 39 * gib, forced=13) == 13
+    assert md.physical_windows(1 << 26, 13, 39 * gib, forced=14) == 2  # out of range: ignored
+    assert md.expected_plan(1 << 26, 0, 2) == {"window_bits": 20, "digits": 13, "physical_windows": 2, "tables": 7}
 
 
 @pytest.mark.parametrize("c", WIDTHS)

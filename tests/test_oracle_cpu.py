@@ -158,6 +158,16 @@ def test_splitmix_and_bases_match_python(oracle, pyoracle):
         assert py.decode_g1_mont(B.tobytes(), i) == py.g1_mul(py.G1_GEN, a[i])
 
 
+@pytest.mark.parametrize("n, first_a, first_b", [(0, 0, 0), (1, 0, 0), (5, (1 << 26) - 5, (1 << 26) - 5),
+                                                  ((1 << 14) - 1, 0, 7), ((1 << 14) + 1, 3, 0), (1 << 16, 0, 1 << 22)])
+def test_fr_dot_matches_python(oracle, pyoracle, n, first_a, first_b):
+    """orc_fr_dot, the closed form of the large known-dlog MSMs, against Python integers: across its chunk edges
+    (2^14 terms) and at the offsets the GPU tests use (the top 5 of 2^26 bases, batch members 2^22 scalars apart)."""
+    a = oracle.array_to_ints(oracle.splitmix_fr(0xB200, n, False, first=first_a))
+    b = oracle.array_to_ints(oracle.splitmix_fr(0x5CA1A8, n, False, first=first_b))
+    assert oracle.fr_dot(0xB200, 0x5CA1A8, n, first_a, first_b) == sum(x * y for x, y in zip(a, b)) % pyoracle.R
+
+
 def test_quotient_domain_of_six_cosets_matches_the_8n_coset(pyoracle):
     """The algebra behind the device prover's quotient domain (DESIGN.md §4), pinned with the Python oracle's own
     transforms: a polynomial t of degree <= 5n + 7 is recovered from its values on 6 of the 8 cosets s_j * H_n of

@@ -21,6 +21,10 @@
 namespace b200 {
 
 void set_error(const std::string& msg);
+inline int refuse(const std::string& msg) {  // records the message, returns B200_ERR_INVALID
+    set_error(msg);
+    return B200_ERR_INVALID;
+}
 int cuda_fail(cudaError_t e, const char* what);  // records the message, returns B200_ERR_CUDA
 
 #define B200_CUDA(expr)                                            \
@@ -269,9 +273,25 @@ bool g2_record_on_curve(const uint64_t rec[16]);
 // B200_ERR_INVALID, naming the first position, for a variable index >= num_vars.
 int wiring_permutation(const uint32_t* d_wire_vars, size_t count, size_t num_vars, uint64_t* d_perm, cudaStream_t st);
 
-// The link and key checks of b200_plonk_prove_settlement[_witness] (witness: the key must hold wiring), for a pool to make
-// at submit: B200_OK, or B200_ERR_INVALID with a message that starts with `who` and names the link.
-int settlement_check(const b200_bases* srs, const b200_pk* pk, bool witness, const b200_settlement_link* links, size_t n_links,
+// The argument checks of the proof and link entry points (plonk.cu), which a pool also makes at submit: B200_OK, or
+// B200_ERR_INVALID with a message that starts with `where` (the entry point, and ": item i" / ": proof i" for an entry of
+// a batch / bundle) and names the field.
+// A proof from a wire table: non-NULL pk, wires, blinders and proof, and pub_inputs for a key with public inputs.
+int check_prove_item(const b200_pk* pk, const b200_prove_item& x, const std::string& where);
+// A proof from a witness vector: non-NULL pk, witness, blinders and proof, and a key that holds wiring (check_wiring).
+int check_witness_item(const b200_pk* pk, const b200_witness_item& x, const std::string& where);
+int check_wiring(const b200_pk* pk, const std::string& where);  // pk non-NULL
+// A pool's proof entry: its item's check, and for a wire table num_inputs equal to the key's (the job copies that many).
+int check_entry(const b200_bundle_proof& p, const std::string& where);
+int check_entry(const b200_bundle_witness& p, const std::string& where);
+// A link item's pointers: a1, a2, comm1, comm2 and proof.  Its layout and lengths are checked where the proof is made.
+int check_link_ptrs(const b200_link_item& x, const std::string& where);
+
+// The checks of b200_plonk_prove_settlement[_witness] for a pool to make at submit: check_entry of the proof, then the
+// SRS and the links; the message starts with `who` and names the link.
+int settlement_check(const b200_bases* srs, const b200_bundle_proof& proof, const b200_settlement_link* links, size_t n_links,
+                     const char* who);
+int settlement_check(const b200_bases* srs, const b200_bundle_witness& proof, const b200_settlement_link* links, size_t n_links,
                      const char* who);
 
 // The item checks of b200_plonk_batch_verify / b200_plonk_verify_each (verify_batch.cu), which a pool also makes at submit:

@@ -1922,44 +1922,96 @@ struct b200_pk {
 namespace b200 {
 
 // ---------------------------------------------------------------------------------------------
+// argument checks of the proof and link entry points, which the prover pool (pool.cu) also makes at submit
+// ---------------------------------------------------------------------------------------------
+
+// B200_OK, or B200_ERR_INVALID with "<where> has a NULL <name>" for the first NULL pointer
+static int refuse_null(const std::string& where, std::initializer_list<std::pair<const void*, const char*>> ptrs) {
+    for (const auto& p : ptrs)
+        if (!p.first) return refuse(where + " has a NULL " + p.second);
+    return B200_OK;
+}
+
+int check_wiring(const b200_pk* pk, const std::string& where) {
+    if (pk->pk->wire_vars) return B200_OK;
+    return refuse(where + ": the key holds no wiring (made by b200_plonk_preprocess, not b200_plonk_preprocess_wiring)");
+}
+
+int check_prove_item(const b200_pk* pk, const b200_prove_item& x, const std::string& where) {
+    const int rc = refuse_null(where, {{pk, "pk"}, {x.wires, "wires"}, {x.blinders, "blinders"}, {x.proof, "proof"}});
+    if (rc != B200_OK || x.pub_inputs || pk->pk->num_inputs == 0) return rc;
+    return refuse(where + " has a NULL pub_inputs for a key with " + std::to_string(pk->pk->num_inputs) + " public inputs");
+}
+
+int check_witness_item(const b200_pk* pk, const b200_witness_item& x, const std::string& where) {
+    const int rc = refuse_null(where, {{pk, "pk"}, {x.witness, "witness"}, {x.blinders, "blinders"}, {x.proof, "proof"}});
+    return rc != B200_OK ? rc : check_wiring(pk, where);
+}
+
+int check_entry(const b200_bundle_proof& p, const std::string& where) {
+    const int rc = check_prove_item(p.pk, {p.wires, p.pub_inputs, p.blinders, p.proof, p.link_poly, nullptr}, where);
+    if (rc != B200_OK || p.num_inputs == p.pk->pk->num_inputs) return rc;
+    return refuse(where + ": num_inputs " + std::to_string(p.num_inputs) + " does not match the proving key's " +
+                  std::to_string(p.pk->pk->num_inputs));
+}
+
+int check_entry(const b200_bundle_witness& p, const std::string& where) {
+    return check_witness_item(p.pk, {p.witness, p.blinders, p.proof, p.link_poly, nullptr, p.pub_inputs_out}, where);
+}
+
+int check_link_ptrs(const b200_link_item& x, const std::string& where) {
+    return refuse_null(where, {{x.a1, "a1"}, {x.a2, "a2"}, {x.comm1, "comm1"}, {x.comm2, "comm2"}, {x.proof, "proof"}});
+}
+
+static ProveItem prove_item(const b200_prove_item& x) {
+    return ProveItem{reinterpret_cast<const fe*>(x.wires),    reinterpret_cast<const fe*>(x.pub_inputs),
+                     reinterpret_cast<const fe*>(x.blinders), reinterpret_cast<ProofOut*>(x.proof),
+                     reinterpret_cast<fe*>(x.link_poly),      reinterpret_cast<fe*>(x.challenges), B200_OK};
+}
+
+static ProveItem prove_item(const b200_witness_item& x) {
+    return ProveItem{nullptr, nullptr, reinterpret_cast<const fe*>(x.blinders), reinterpret_cast<ProofOut*>(x.proof),
+                     reinterpret_cast<fe*>(x.link_poly), reinterpret_cast<fe*>(x.challenges), B200_OK,
+                     reinterpret_cast<const fe*>(x.witness), reinterpret_cast<fe*>(x.pub_inputs_out)};
+}
+
+// ---------------------------------------------------------------------------------------------
 // settlements — the settlement arms of `NativeProofManager::handle_proof_job` (native_proof_manager.rs:514-660): prove
 // the statement, then link each hint the job brings (validity first, settlement second) to the statement's hint
 // ---------------------------------------------------------------------------------------------
 
-// The link items of a settlement of the key `pk`: each caller hint first, the settlement's n + 2 coefficients second
-// (a2 and comm2 are filled in once the proof is made).  Every argument check of the settlement entry points but the
-// proof's own pointers: B200_ERR_INVALID, with a message that starts with `who`, before any device work.
-static int settlement_items(const b200_bases* srs, const b200_pk* pk, bool witness, const b200_settlement_link* links,
-                            size_t n_links, const std::string& who, std::vector<LinkItem>* its) {
-    if (!srs || !pk || (n_links && !links)) {
-        set_error(who + ": NULL srs, key or links");
-        return B200_ERR_INVALID;
-    }
-    if (witness && !pk->pk->wire_vars) {
-        set_error(who + ": the key holds no wiring (made by b200_plonk_preprocess, not b200_plonk_preprocess_wiring)");
-        return B200_ERR_INVALID;
-    }
+// The link items of a settlement of the (checked) key `pk`: each caller hint first, the settlement's n + 2 coefficients
+// second (a2 and comm2 are filled in once the proof is made).  The checks of the SRS and the links: B200_ERR_INVALID,
+// with a message that starts with `who`, before any device work.
+static int settlement_items(const b200_bases* srs, const b200_pk* pk, const b200_settlement_link* links, size_t n_links,
+                            const std::string& who, std::vector<LinkItem>* its) {
+    if (!srs || (n_links && !links)) return refuse(who + ": null argument");
     static const uint64_t kNoComm[8] = {};
     its->resize(n_links);
     for (size_t i = 0; i < n_links; ++i) {
         const b200_settlement_link& l = links[i];
         const std::string where = who + ": link " + std::to_string(i);
-        if (!l.hint_poly || !l.hint_comm || !l.proof) {
-            set_error(where + " has a NULL hint_poly, hint_comm or proof");
-            return B200_ERR_INVALID;
-        }
+        int rc = refuse_null(where, {{l.hint_poly, "hint_poly"}, {l.hint_comm, "hint_comm"}, {l.proof, "proof"}});
         const b200_link_item x{l.hint_poly, l.hint_len, nullptr, pk->pk->n + 2, l.hint_comm, kNoComm,
                                l.alignment, l.offset, l.size, l.proof, l.eta};
-        const int rc = link_item(srs->b, x, where, &(*its)[i]);
+        if (rc == B200_OK) rc = link_item(srs->b, x, where, &(*its)[i]);
         if (rc != B200_OK) return rc;
     }
     return B200_OK;
 }
 
-int settlement_check(const b200_bases* srs, const b200_pk* pk, bool witness, const b200_settlement_link* links, size_t n_links,
+int settlement_check(const b200_bases* srs, const b200_bundle_proof& proof, const b200_settlement_link* links, size_t n_links,
                      const char* who) {
     std::vector<LinkItem> its;
-    return settlement_items(srs, pk, witness, links, n_links, who, &its);
+    const int rc = check_entry(proof, who);
+    return rc != B200_OK ? rc : settlement_items(srs, proof.pk, links, n_links, who, &its);
+}
+
+int settlement_check(const b200_bases* srs, const b200_bundle_witness& proof, const b200_settlement_link* links, size_t n_links,
+                     const char* who) {
+    std::vector<LinkItem> its;
+    const int rc = check_entry(proof, who);
+    return rc != B200_OK ? rc : settlement_items(srs, proof.pk, links, n_links, who, &its);
 }
 
 // Both settlement entry points once their arguments are checked: the proof (b200_plonk_prove's path, graphs included),
@@ -2057,9 +2109,11 @@ int b200_plonk_link(b200_ctx* ctx, const b200_bases* srs, const uint64_t* a1, si
                     size_t len2, const uint64_t* comm1, const uint64_t* comm2, unsigned alignment, size_t offset,
                     size_t size, b200_link_proof* proof, uint64_t* eta) {
     B200_TRY
-    if (!ctx || !srs || !a1 || !a2 || !comm1 || !comm2 || !proof) return B200_ERR_INVALID;
+    if (!ctx || !srs) return refuse("link: null argument");
+    const b200_link_item x{a1, len1, a2, len2, comm1, comm2, alignment, offset, size, proof, eta};
     LinkItem it;
-    int rc = link_item(srs->b, b200_link_item{a1, len1, a2, len2, comm1, comm2, alignment, offset, size, proof, eta}, "link", &it);
+    int rc = check_link_ptrs(x, "link");
+    if (rc == B200_OK) rc = link_item(srs->b, x, "link", &it);
     if (rc != B200_OK) return rc;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
     B200_CUDA(cudaSetDevice(ctx->c.device));
@@ -2076,20 +2130,13 @@ int b200_plonk_link(b200_ctx* ctx, const b200_bases* srs, const uint64_t* a1, si
 
 int b200_plonk_link_batch(b200_ctx* ctx, const b200_bases* srs, const b200_link_item* items, size_t k, int* statuses) {
     B200_TRY
-    if (!ctx || !srs || (k && !items)) {
-        set_error("plonk_link_batch: null argument");
-        return B200_ERR_INVALID;
-    }
+    if (!ctx || !srs || (k && !items)) return refuse("plonk_link_batch: null argument");
     // every argument error fails the call before any device work (b200_plonk_link's B200_ERR_INVALID conditions)
     std::vector<LinkItem> its(k);
     for (size_t i = 0; i < k; ++i) {
-        const b200_link_item& x = items[i];
         const std::string item = "plonk_link_batch: item " + std::to_string(i);
-        if (!x.a1 || !x.a2 || !x.comm1 || !x.comm2 || !x.proof) {
-            set_error(item + " has a NULL pointer");
-            return B200_ERR_INVALID;
-        }
-        const int rc = link_item(srs->b, x, item, &its[i]);
+        int rc = check_link_ptrs(items[i], item);
+        if (rc == B200_OK) rc = link_item(srs->b, items[i], item, &its[i]);
         if (rc != B200_OK) return rc;
     }
     if (k == 0) return B200_OK;
@@ -2136,34 +2183,27 @@ void b200_pk_free(b200_ctx* ctx, b200_pk* pk) {
 int b200_plonk_prove(b200_ctx* ctx, const b200_pk* pk, const uint64_t* wires, const uint64_t* pub_inputs,
                      const uint64_t* blinders, b200_proof* proof, uint64_t* link_poly, uint64_t* challenges) {
     B200_TRY
-    if (!ctx || !pk || !wires || !blinders || !proof || (pk->pk->num_inputs && !pub_inputs)) return B200_ERR_INVALID;
+    if (!ctx || !pk) return refuse("plonk_prove: null argument");
+    const b200_prove_item x{wires, pub_inputs, blinders, proof, link_poly, challenges};
+    const int rc = check_prove_item(pk, x, "plonk_prove");
+    if (rc != B200_OK) return rc;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
     B200_CUDA(cudaSetDevice(ctx->c.device));
-    ProveItem item{reinterpret_cast<const fe*>(wires),     reinterpret_cast<const fe*>(pub_inputs),
-                   reinterpret_cast<const fe*>(blinders),  reinterpret_cast<ProofOut*>(proof),
-                   reinterpret_cast<fe*>(link_poly),       reinterpret_cast<fe*>(challenges), B200_OK};
+    ProveItem item = prove_item(x);
     return prove(&ctx->c, single_bufs(&ctx->c), pk->pk, &item, 1, /*single=*/true);
     B200_CATCH
-}
-
-// A key that proves from witness vectors, or B200_ERR_INVALID
-static int require_wiring(const b200_pk* pk, const char* who) {
-    if (pk->pk->wire_vars) return B200_OK;
-    set_error(std::string(who) + ": the key holds no wiring (made by b200_plonk_preprocess, not b200_plonk_preprocess_wiring)");
-    return B200_ERR_INVALID;
 }
 
 int b200_plonk_prove_witness(b200_ctx* ctx, const b200_pk* pk, const uint64_t* witness, const uint64_t* blinders,
                              b200_proof* proof, uint64_t* link_poly, uint64_t* challenges, uint64_t* pub_inputs_out) {
     B200_TRY
-    if (!ctx || !pk || !witness || !blinders || !proof) return B200_ERR_INVALID;
-    const int ok = require_wiring(pk, "plonk_prove_witness");
-    if (ok != B200_OK) return ok;
+    if (!ctx || !pk) return refuse("plonk_prove_witness: null argument");
+    const b200_witness_item x{witness, blinders, proof, link_poly, challenges, pub_inputs_out};
+    const int rc = check_witness_item(pk, x, "plonk_prove_witness");
+    if (rc != B200_OK) return rc;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
     B200_CUDA(cudaSetDevice(ctx->c.device));
-    ProveItem item{nullptr, nullptr, reinterpret_cast<const fe*>(blinders), reinterpret_cast<ProofOut*>(proof),
-                   reinterpret_cast<fe*>(link_poly), reinterpret_cast<fe*>(challenges), B200_OK,
-                   reinterpret_cast<const fe*>(witness), reinterpret_cast<fe*>(pub_inputs_out)};
+    ProveItem item = prove_item(x);
     return prove(&ctx->c, single_bufs(&ctx->c), pk->pk, &item, 1, /*single=*/true);
     B200_CATCH
 }
@@ -2173,16 +2213,13 @@ int b200_plonk_prove_settlement(b200_ctx* ctx, const b200_bases* srs, const b200
                                 const b200_settlement_link* links, size_t n_links, int* statuses) {
     B200_TRY
     const std::string who = "plonk_prove_settlement";
-    if (!ctx || !pk || !wires || !blinders || !proof || (pk->pk->num_inputs && !pub_inputs)) {
-        set_error(who + ": NULL argument");
-        return B200_ERR_INVALID;
-    }
+    if (!ctx || !pk) return refuse(who + ": null argument");
+    const b200_prove_item x{wires, pub_inputs, blinders, proof, link_poly, nullptr};
     std::vector<LinkItem> its;
-    const int rc = settlement_items(srs, pk, /*witness=*/false, links, n_links, who, &its);
+    int rc = check_prove_item(pk, x, who);
+    if (rc == B200_OK) rc = settlement_items(srs, pk, links, n_links, who, &its);
     if (rc != B200_OK) return rc;
-    ProveItem item{reinterpret_cast<const fe*>(wires),     reinterpret_cast<const fe*>(pub_inputs),
-                   reinterpret_cast<const fe*>(blinders),  reinterpret_cast<ProofOut*>(proof),
-                   reinterpret_cast<fe*>(link_poly),       nullptr, B200_OK};
+    ProveItem item = prove_item(x);
     return prove_settlement(ctx, srs->b, pk->pk, &item, its, statuses, who);
     B200_CATCH
 }
@@ -2193,16 +2230,13 @@ int b200_plonk_prove_settlement_witness(b200_ctx* ctx, const b200_bases* srs, co
                                         int* statuses) {
     B200_TRY
     const std::string who = "plonk_prove_settlement_witness";
-    if (!ctx || !pk || !witness || !blinders || !proof) {
-        set_error(who + ": NULL argument");
-        return B200_ERR_INVALID;
-    }
+    if (!ctx || !pk) return refuse(who + ": null argument");
+    const b200_witness_item x{witness, blinders, proof, link_poly, nullptr, pub_inputs_out};
     std::vector<LinkItem> its;
-    const int rc = settlement_items(srs, pk, /*witness=*/true, links, n_links, who, &its);
+    int rc = check_witness_item(pk, x, who);
+    if (rc == B200_OK) rc = settlement_items(srs, pk, links, n_links, who, &its);
     if (rc != B200_OK) return rc;
-    ProveItem item{nullptr, nullptr, reinterpret_cast<const fe*>(blinders), reinterpret_cast<ProofOut*>(proof),
-                   reinterpret_cast<fe*>(link_poly), nullptr, B200_OK,
-                   reinterpret_cast<const fe*>(witness), reinterpret_cast<fe*>(pub_inputs_out)};
+    ProveItem item = prove_item(x);
     return prove_settlement(ctx, srs->b, pk->pk, &item, its, statuses, who);
     B200_CATCH
 }
@@ -2237,38 +2271,27 @@ static int prove_batch_items(b200_ctx* ctx, const ProvingKey* key, std::vector<P
 
 int b200_plonk_prove_batch(b200_ctx* ctx, const b200_pk* pk, const b200_prove_item* items, size_t k, int* statuses) {
     B200_TRY
-    if (!ctx || !pk || (k && !items)) return B200_ERR_INVALID;
-    const ProvingKey* key = pk->pk;
+    if (!ctx || !pk || (k && !items)) return refuse("plonk_prove_batch: null argument");
     std::vector<ProveItem> its(k);
     for (size_t i = 0; i < k; ++i) {
-        const b200_prove_item& x = items[i];
-        if (!x.wires || !x.blinders || !x.proof || (key->num_inputs && !x.pub_inputs)) {
-            set_error("plonk_prove_batch: item " + std::to_string(i) + " has a NULL pointer");
-            return B200_ERR_INVALID;
-        }
-        its[i] = ProveItem{reinterpret_cast<const fe*>(x.wires), reinterpret_cast<const fe*>(x.pub_inputs),
-                           reinterpret_cast<const fe*>(x.blinders), reinterpret_cast<ProofOut*>(x.proof),
-                           reinterpret_cast<fe*>(x.link_poly), reinterpret_cast<fe*>(x.challenges), B200_OK};
+        const int rc = check_prove_item(pk, items[i], "plonk_prove_batch: item " + std::to_string(i));
+        if (rc != B200_OK) return rc;
+        its[i] = prove_item(items[i]);
     }
-    return prove_batch_items(ctx, key, its, statuses);
+    return prove_batch_items(ctx, pk->pk, its, statuses);
     B200_CATCH
 }
 
 int b200_plonk_prove_witness_batch(b200_ctx* ctx, const b200_pk* pk, const b200_witness_item* items, size_t k, int* statuses) {
     B200_TRY
-    if (!ctx || !pk || (k && !items)) return B200_ERR_INVALID;
-    const int ok = require_wiring(pk, "plonk_prove_witness_batch");
-    if (ok != B200_OK) return ok;
+    const std::string who = "plonk_prove_witness_batch";
+    if (!ctx || !pk || (k && !items)) return refuse(who + ": null argument");
+    int rc = check_wiring(pk, who);  // a batch of no items is refused too
+    if (rc != B200_OK) return rc;
     std::vector<ProveItem> its(k);
     for (size_t i = 0; i < k; ++i) {
-        const b200_witness_item& x = items[i];
-        if (!x.witness || !x.blinders || !x.proof) {
-            set_error("plonk_prove_witness_batch: item " + std::to_string(i) + " has a NULL pointer");
-            return B200_ERR_INVALID;
-        }
-        its[i] = ProveItem{nullptr, nullptr, reinterpret_cast<const fe*>(x.blinders), reinterpret_cast<ProofOut*>(x.proof),
-                           reinterpret_cast<fe*>(x.link_poly), reinterpret_cast<fe*>(x.challenges), B200_OK,
-                           reinterpret_cast<const fe*>(x.witness), reinterpret_cast<fe*>(x.pub_inputs_out)};
+        if ((rc = check_witness_item(pk, items[i], who + ": item " + std::to_string(i))) != B200_OK) return rc;
+        its[i] = prove_item(items[i]);
     }
     return prove_batch_items(ctx, pk->pk, its, statuses);
     B200_CATCH

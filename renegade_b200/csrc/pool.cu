@@ -279,17 +279,19 @@ static int push_one(b200_pool* pool, std::unique_ptr<Job> job, uint64_t* ticket)
     return pool_push(pool, &job, 1, nullptr, ticket);
 }
 
-// The part of a bundle submission both entry points share, once each proof entry is checked: check the links against the
+// A bundle submission after its NULL-handle checks, for both entry points: check each proof entry and the links against the
 // proofs, then queue one proof job per entry under one ticket.  Nothing is queued on a refusal.
 template <class P>
 static int bundle_push(b200_pool* pool, const char* who, const b200_bases* srs, const P* proofs, size_t n_proofs,
                        const b200_bundle_link* links, size_t n_links, uint64_t* ticket) {
+    for (size_t i = 0; i < n_proofs; ++i) {
+        const int rc = b200::check_entry(proofs[i], std::string(who) + ": proof " + std::to_string(i));
+        if (rc != B200_OK) return rc;
+    }
     for (size_t i = 0; i < n_links; ++i) {
         const b200_bundle_link& l = links[i];
-        if (l.a >= n_proofs || l.b >= n_proofs || !l.proof || !proofs[l.a].link_poly || !proofs[l.b].link_poly) {
-            b200::set_error(std::string(who) + ": a link names a proof that is missing or has no link_poly buffer");
-            return B200_ERR_INVALID;
-        }
+        if (l.a >= n_proofs || l.b >= n_proofs || !l.proof || !proofs[l.a].link_poly || !proofs[l.b].link_poly)
+            return b200::refuse(std::string(who) + ": a link names a proof that is missing or has no link_poly buffer");
     }
     std::shared_ptr<Bundle> b(new Bundle());
     b->srs = srs;
@@ -355,46 +357,32 @@ int b200_pool_submit_prove(b200_pool* pool, const b200_pk* pk, const uint64_t* w
                            const uint64_t* pub_inputs, size_t num_inputs, const uint64_t* blinders,
                            b200_proof* proof, uint64_t* link_poly, uint64_t* ticket) {
     B200_TRY
-    if (!pool || !pk || !wires || !blinders || !proof || !ticket || (num_inputs && !pub_inputs)) {
-        b200::set_error("pool_submit_prove: null argument");
-        return B200_ERR_INVALID;
-    }
-    if (num_inputs != b200_pk_num_inputs(pk)) {  // the worker reads exactly pk.num_inputs elements
-        b200::set_error("pool_submit_prove: num_inputs does not match the proving key");
-        return B200_ERR_INVALID;
-    }
-    return push_one(pool, proof_job(b200_bundle_proof{pk, wires, pub_inputs, num_inputs, blinders, proof, link_poly}), ticket);
+    if (!pool || !pk || !ticket) return b200::refuse("pool_submit_prove: null argument");
+    const b200_bundle_proof p{pk, wires, pub_inputs, num_inputs, blinders, proof, link_poly};
+    const int rc = b200::check_entry(p, "pool_submit_prove");
+    return rc != B200_OK ? rc : push_one(pool, proof_job(p), ticket);
     B200_CATCH
 }
 
 int b200_pool_submit_prove_witness(b200_pool* pool, const b200_pk* pk, const uint64_t* witness, const uint64_t* blinders,
                                    b200_proof* proof, uint64_t* link_poly, uint64_t* pub_inputs_out, uint64_t* ticket) {
     B200_TRY
-    if (!pool || !pk || !witness || !blinders || !proof || !ticket) {
-        b200::set_error("pool_submit_prove_witness: null argument");
-        return B200_ERR_INVALID;
-    }
-    if (b200_pk_num_vars(pk) == 0) {
-        b200::set_error("pool_submit_prove_witness: the key holds no wiring (made by b200_plonk_preprocess)");
-        return B200_ERR_INVALID;
-    }
-    return push_one(pool, proof_job(b200_bundle_witness{pk, witness, blinders, proof, link_poly, pub_inputs_out}), ticket);
+    if (!pool || !pk || !ticket) return b200::refuse("pool_submit_prove_witness: null argument");
+    const b200_bundle_witness p{pk, witness, blinders, proof, link_poly, pub_inputs_out};
+    const int rc = b200::check_entry(p, "pool_submit_prove_witness");
+    return rc != B200_OK ? rc : push_one(pool, proof_job(p), ticket);
     B200_CATCH
 }
 
 int b200_pool_submit_prove_batch(b200_pool* pool, const b200_pk* pk, const b200_prove_item* items, size_t k, int* statuses,
                                  uint64_t* ticket) {
     B200_TRY
-    if (!pool || !pk || (k && !items) || !ticket) {
-        b200::set_error("pool_submit_prove_batch: null argument");
-        return B200_ERR_INVALID;
+    if (!pool || !pk || (k && !items) || !ticket) return b200::refuse("pool_submit_prove_batch: null argument");
+    for (size_t i = 0; i < k; ++i) {
+        const int rc = b200::check_prove_item(pk, items[i], "pool_submit_prove_batch: item " + std::to_string(i));
+        if (rc != B200_OK) return rc;
     }
     const size_t ni = b200_pk_num_inputs(pk);
-    for (size_t i = 0; i < k; ++i)
-        if (!items[i].wires || !items[i].blinders || !items[i].proof || (ni && !items[i].pub_inputs)) {
-            b200::set_error("pool_submit_prove_batch: item " + std::to_string(i) + " has a NULL pointer");
-            return B200_ERR_INVALID;
-        }
     std::unique_ptr<Job> j(new Job());
     b200_prove_item* its = j->held.copy(items, k);
     for (size_t i = 0; i < k; ++i) {
@@ -409,19 +397,12 @@ int b200_pool_submit_prove_batch(b200_pool* pool, const b200_pk* pk, const b200_
 int b200_pool_submit_prove_witness_batch(b200_pool* pool, const b200_pk* pk, const b200_witness_item* items, size_t k,
                                          int* statuses, uint64_t* ticket) {
     B200_TRY
-    if (!pool || !pk || (k && !items) || !ticket) {
-        b200::set_error("pool_submit_prove_witness_batch: null argument");
-        return B200_ERR_INVALID;
-    }
-    if (b200_pk_num_vars(pk) == 0) {
-        b200::set_error("pool_submit_prove_witness_batch: the key holds no wiring (made by b200_plonk_preprocess)");
-        return B200_ERR_INVALID;
-    }
+    if (!pool || !pk || (k && !items) || !ticket) return b200::refuse("pool_submit_prove_witness_batch: null argument");
+    int rc = b200::check_wiring(pk, "pool_submit_prove_witness_batch");  // a batch of no items is refused too
+    if (rc != B200_OK) return rc;
     for (size_t i = 0; i < k; ++i)
-        if (!items[i].witness || !items[i].blinders || !items[i].proof) {
-            b200::set_error("pool_submit_prove_witness_batch: item " + std::to_string(i) + " has a NULL pointer");
-            return B200_ERR_INVALID;
-        }
+        if ((rc = b200::check_witness_item(pk, items[i], "pool_submit_prove_witness_batch: item " + std::to_string(i))) != B200_OK)
+            return rc;
     std::unique_ptr<Job> j(new Job());
     b200_witness_item* its = j->held.copy(items, k);
     for (size_t i = 0; i < k; ++i) its[i].blinders = j->held.copy(items[i].blinders, 4 * 17);
@@ -435,26 +416,21 @@ int b200_pool_submit_link(b200_pool* pool, const b200_bases* srs, const uint64_t
                           unsigned alignment, size_t offset, size_t size, b200_link_proof* proof,
                           uint64_t* ticket) {
     B200_TRY
-    if (!pool || !srs || !a1 || !a2 || !comm1 || !comm2 || !proof || !ticket) {
-        b200::set_error("pool_submit_link: null argument");
-        return B200_ERR_INVALID;
-    }
-    return push_one(pool, link_job(srs, {a1, len1, a2, len2, comm1, comm2, alignment, offset, size, proof, nullptr}), ticket);
+    if (!pool || !srs || !ticket) return b200::refuse("pool_submit_link: null argument");
+    const b200_link_item x{a1, len1, a2, len2, comm1, comm2, alignment, offset, size, proof, nullptr};
+    const int rc = b200::check_link_ptrs(x, "pool_submit_link");
+    return rc != B200_OK ? rc : push_one(pool, link_job(srs, x), ticket);
     B200_CATCH
 }
 
 int b200_pool_submit_link_batch(b200_pool* pool, const b200_bases* srs, const b200_link_item* items, size_t k,
                                 int* statuses, uint64_t* ticket) {
     B200_TRY
-    if (!pool || !srs || (k && !items) || !ticket) {
-        b200::set_error("pool_submit_link_batch: null argument");
-        return B200_ERR_INVALID;
+    if (!pool || !srs || (k && !items) || !ticket) return b200::refuse("pool_submit_link_batch: null argument");
+    for (size_t i = 0; i < k; ++i) {
+        const int rc = b200::check_link_ptrs(items[i], "pool_submit_link_batch: item " + std::to_string(i));
+        if (rc != B200_OK) return rc;
     }
-    for (size_t i = 0; i < k; ++i)
-        if (!items[i].a1 || !items[i].a2 || !items[i].comm1 || !items[i].comm2 || !items[i].proof) {
-            b200::set_error("pool_submit_link_batch: item " + std::to_string(i) + " has a NULL pointer");
-            return B200_ERR_INVALID;
-        }
     std::unique_ptr<Job> j(new Job());
     const b200_link_item* its = j->held.link_items(items, k);
     j->call = [srs, its, k, statuses](b200_ctx* ctx) { return b200_plonk_link_batch(ctx, srs, its, k, statuses); };
@@ -465,18 +441,8 @@ int b200_pool_submit_link_batch(b200_pool* pool, const b200_bases* srs, const b2
 int b200_pool_submit_bundle(b200_pool* pool, const b200_bases* srs, const b200_bundle_proof* proofs, size_t n_proofs,
                             const b200_bundle_link* links, size_t n_links, uint64_t* ticket) {
     B200_TRY
-    if (!pool || !proofs || n_proofs == 0 || (n_links && (!links || !srs)) || !ticket) {
-        b200::set_error("pool_submit_bundle: null argument");
-        return B200_ERR_INVALID;
-    }
-    for (size_t i = 0; i < n_proofs; ++i) {
-        const b200_bundle_proof& p = proofs[i];
-        if (!p.pk || !p.wires || !p.blinders || !p.proof || (p.num_inputs && !p.pub_inputs) ||
-            p.num_inputs != b200_pk_num_inputs(p.pk)) {
-            b200::set_error("pool_submit_bundle: bad proof entry (null pointer or num_inputs does not match the key)");
-            return B200_ERR_INVALID;
-        }
-    }
+    if (!pool || !proofs || n_proofs == 0 || (n_links && (!links || !srs)) || !ticket)
+        return b200::refuse("pool_submit_bundle: null argument");
     return bundle_push(pool, "pool_submit_bundle", srs, proofs, n_proofs, links, n_links, ticket);
     B200_CATCH
 }
@@ -484,22 +450,8 @@ int b200_pool_submit_bundle(b200_pool* pool, const b200_bases* srs, const b200_b
 int b200_pool_submit_bundle_witness(b200_pool* pool, const b200_bases* srs, const b200_bundle_witness* proofs,
                                     size_t n_proofs, const b200_bundle_link* links, size_t n_links, uint64_t* ticket) {
     B200_TRY
-    if (!pool || !proofs || n_proofs == 0 || (n_links && (!links || !srs)) || !ticket) {
-        b200::set_error("pool_submit_bundle_witness: null argument");
-        return B200_ERR_INVALID;
-    }
-    for (size_t i = 0; i < n_proofs; ++i) {
-        const b200_bundle_witness& p = proofs[i];
-        if (!p.pk || !p.witness || !p.blinders || !p.proof) {
-            b200::set_error("pool_submit_bundle_witness: proof " + std::to_string(i) + " has a NULL pointer");
-            return B200_ERR_INVALID;
-        }
-        if (b200_pk_num_vars(p.pk) == 0) {
-            b200::set_error("pool_submit_bundle_witness: the key of proof " + std::to_string(i) +
-                            " holds no wiring (made by b200_plonk_preprocess)");
-            return B200_ERR_INVALID;
-        }
-    }
+    if (!pool || !proofs || n_proofs == 0 || (n_links && (!links || !srs)) || !ticket)
+        return b200::refuse("pool_submit_bundle_witness: null argument");
     return bundle_push(pool, "pool_submit_bundle_witness", srs, proofs, n_proofs, links, n_links, ticket);
     B200_CATCH
 }
@@ -508,16 +460,8 @@ int b200_pool_submit_settlement(b200_pool* pool, const b200_bases* srs, const b2
                                 const b200_settlement_link* links, size_t n_links, int* statuses, uint64_t* ticket) {
     B200_TRY
     const char* who = "pool_submit_settlement";
-    if (!pool || !proof || !ticket || !proof->pk || !proof->wires || !proof->blinders || !proof->proof ||
-        (proof->num_inputs && !proof->pub_inputs)) {
-        b200::set_error(std::string(who) + ": null argument");
-        return B200_ERR_INVALID;
-    }
-    if (proof->num_inputs != b200_pk_num_inputs(proof->pk)) {  // the worker reads exactly pk.num_inputs elements
-        b200::set_error(std::string(who) + ": num_inputs does not match the proving key");
-        return B200_ERR_INVALID;
-    }
-    const int rc = b200::settlement_check(srs, proof->pk, /*witness=*/false, links, n_links, who);
+    if (!pool || !proof || !ticket) return b200::refuse(std::string(who) + ": null argument");
+    const int rc = b200::settlement_check(srs, *proof, links, n_links, who);
     if (rc != B200_OK) return rc;
     std::unique_ptr<Job> j(new Job());
     const b200_bundle_proof p = j->held.proof(*proof);
@@ -534,11 +478,8 @@ int b200_pool_submit_settlement_witness(b200_pool* pool, const b200_bases* srs, 
                                         const b200_settlement_link* links, size_t n_links, int* statuses, uint64_t* ticket) {
     B200_TRY
     const char* who = "pool_submit_settlement_witness";
-    if (!pool || !proof || !ticket || !proof->pk || !proof->witness || !proof->blinders || !proof->proof) {
-        b200::set_error(std::string(who) + ": null argument");
-        return B200_ERR_INVALID;
-    }
-    const int rc = b200::settlement_check(srs, proof->pk, /*witness=*/true, links, n_links, who);
+    if (!pool || !proof || !ticket) return b200::refuse(std::string(who) + ": null argument");
+    const int rc = b200::settlement_check(srs, *proof, links, n_links, who);
     if (rc != B200_OK) return rc;
     std::unique_ptr<Job> j(new Job());
     const b200_bundle_witness p = j->held.proof(*proof);

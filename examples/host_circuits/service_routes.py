@@ -3,9 +3,11 @@ the request decoders (`{statement, witness[, link hints]}`, api_types.rs:141-264
 statements.py.  The other four paths of prover_service_client.rs:101-147 are not registered here (their circuits verify Schnorr
 signatures / ElGamal ciphertexts on BabyJubJub in-circuit and are not restated); the service answers 501 for them.
 
-    python -m host_circuits.service_routes --port 3000 --password PW --srs /path/to/ptau [--device 0 --workers 6 --express 0]
+    python -m host_circuits.service_routes --port 3000 --password PW --srs /path/to/ptau [--device 0 --workers 6 --express 0 --express-sms 0]
 
 `--express N` adds N express workers to the pool and expedites every settlement route's job onto them (b200express.h).
+`--express-sms R` (with `--express N`, N >= 1) runs those workers on R reserved SMs, a multiple of 8, and the normal workers
+on the rest (b200reserved.h).
 """
 from __future__ import annotations
 
@@ -109,8 +111,12 @@ def main():
     ap.add_argument("--workers", type=int, default=6)
     ap.add_argument("--express", type=int, default=0,
                     help="express workers; > 0 also expedites the settlement routes' jobs (DESIGN.md §6, express lane)")
+    ap.add_argument("--express-sms", type=int, default=0,
+                    help="SMs reserved for the express workers, a multiple of 8; needs --express (DESIGN.md §6, reserved SMs)")
     args = ap.parse_args()
-    pool = ProverPool(args.device, workers=args.workers, express=args.express)
+    if args.express_sms and args.express < 1:
+        ap.error("--express-sms reserves SMs for express workers: it requires --express N with N >= 1")
+    pool = ProverPool(args.device, workers=args.workers, express=args.express, express_sms=args.express_sms)
     ctx = pool.context(0)
     data = open(args.srs, "rb").read()
     params = rb.parse_ptau_file(ctx, data, count=(1 << 14) + 3)

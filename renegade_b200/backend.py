@@ -1234,6 +1234,21 @@ def _express_count(express, who: str) -> int:
     return express
 
 
+def _express_sms(express_sms, express: int, who: str) -> int:
+    """The reserved SM count of b200reserved.h, checked as the library checks it (0: no partition)."""
+    if isinstance(express_sms, bool) or not isinstance(express_sms, int) or express_sms < 0:
+        raise ValueError(f"{who}: express_sms must be an int >= 0, not {express_sms!r}")
+    if express_sms and (express_sms % 8 or express_sms > 248):
+        raise ValueError(f"{who}: express_sms must be a multiple of 8 in [8, 248], not {express_sms}")
+    if express_sms and express == 0:
+        raise ValueError(f"{who}: express_sms reserves SMs for express workers: it needs express >= 1")
+    return express_sms
+
+
+def _mask_sms(mask) -> set:
+    return {64 * i + b for i, word in enumerate(mask) for b in range(64) if (int(word) >> b) & 1}
+
+
 class ProverPool(_Tickets):
     """b200_pool: the device-side counterpart of the reference's `NativeProofManager` thread pool
     (crates/workers/proof-manager/src/implementations/native_proof_manager.rs:138-201, `spawn_fifo`
@@ -1243,13 +1258,21 @@ class ProverPool(_Tickets):
 
     `express` workers (b200express.h) take only jobs moved to the express queue by `expedite(ticket)`; their contexts'
     streams rank above the normal workers'.  Any pool can expedite: with no express workers the express queue is the
-    front of the line."""
+    front of the line.
 
-    def __init__(self, device: int = 0, workers: int = 6, express: int = 0):
+    `express_sms` > 0 (b200reserved.h) also splits the device's SMs: the express workers run on a group of at least that
+    many SMs (a multiple of 8), the normal workers on the rest, so that an expedited job's kernels never wait for the
+    load's running blocks; `partition()` gives the two groups' sizes as the split rounded them."""
+
+    def __init__(self, device: int = 0, workers: int = 6, express: int = 0, express_sms: int = 0):
         express = _express_count(express, "ProverPool")
+        express_sms = _express_sms(express_sms, express, "ProverPool")
         self._lib = _lib.load()
         h = C.c_void_p()
-        _lib.check(self._lib.b200_pool_create_express(device, workers, express, C.byref(h)))
+        if express_sms:
+            _lib.check(self._lib.b200_pool_create_reserved(device, workers, express, express_sms, C.byref(h)))
+        else:
+            _lib.check(self._lib.b200_pool_create_express(device, workers, express, C.byref(h)))
         self._h = h
         self.device = device
         self._jobs = {}
@@ -1258,6 +1281,19 @@ class ProverPool(_Tickets):
     @property
     def workers(self) -> int:
         return int(self._lib.b200_pool_workers(self._h))
+
+    def partition(self):
+        """(normal SMs, express SMs) of a pool made with `express_sms` (`b200_pool_partition`); (0, 0) without one."""
+        out = (C.c_uint * 2)()
+        _lib.check(self._lib.b200_pool_partition(self._h, out))
+        return int(out[0]), int(out[1])
+
+    def probe_sms(self, worker: int) -> set:
+        """The SM ids a small kernel reached on each stream of worker `worker`'s context, eagerly and under graph replay
+        (`b200_pool_probe_sms`; express workers after the normal ones)."""
+        mask = (C.c_uint64 * 4)()
+        _lib.check(self._lib.b200_pool_probe_sms(self._h, worker, mask))
+        return _mask_sms(mask)
 
     def context(self, worker: int = 0) -> Context:
         """Worker `worker`'s context (borrowed: the pool frees it), for set-up calls."""
@@ -1432,14 +1468,20 @@ class _BoxKeyShape:
 class ProverBox(_Tickets):
     """`b200_box`: every GPU of the box behind one object — one prover pool per device, the SRS tables and the proving
     keys replicated on each, jobs routed to the least-loaded device.  The single-process counterpart of running one
-    `ProverPool` per rank under torchrun.  `express_per_device` express workers per device as in `ProverPool`."""
+    `ProverPool` per rank under torchrun.  `express_per_device` express workers per device, and `express_sms` SMs
+    reserved for them on every device, as in `ProverPool`."""
 
-    def __init__(self, devices, workers_per_device: int = 6, express_per_device: int = 0):
+    def __init__(self, devices, workers_per_device: int = 6, express_per_device: int = 0, express_sms: int = 0):
         express_per_device = _express_count(express_per_device, "ProverBox")
+        express_sms = _express_sms(express_sms, express_per_device, "ProverBox")
         self._lib = _lib.load()
         arr = (C.c_int * len(devices))(*devices)
         h = C.c_void_p()
-        _lib.check(self._lib.b200_box_create_express(arr, len(devices), workers_per_device, express_per_device, C.byref(h)))
+        if express_sms:
+            _lib.check(self._lib.b200_box_create_reserved(arr, len(devices), workers_per_device, express_per_device, express_sms,
+                                                          C.byref(h)))
+        else:
+            _lib.check(self._lib.b200_box_create_express(arr, len(devices), workers_per_device, express_per_device, C.byref(h)))
         self._h, self._jobs, self.devices = h, {}, list(devices)
         self._shapes = {}  # key handle -> _BoxKeyShape, for the keys this box made
 

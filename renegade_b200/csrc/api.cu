@@ -1,6 +1,8 @@
 // C ABI of libb200prover (declared in include/b200prover.h).  Every entry point catches C++
 // exceptions, records a thread-local message and returns an error code: nothing unwinds across
 // the boundary into the Rust host.
+#include <cudaTypedefs.h>
+
 #include <cstring>
 #include <new>
 #include <string>
@@ -152,13 +154,80 @@ int b200_ctx_use_graphs(b200_ctx* ctx, int on) {
 
 void b200_keccak256(const uint8_t* data, size_t len, uint8_t out[32]) { Keccak256::hash(data, len, out); }
 
-int b200_init(int device, b200_ctx** out) { return b200::context_create(device, /*express=*/false, out); }
+int b200_init(int device, b200_ctx** out) { return b200::context_create(device, /*express=*/false, nullptr, out); }
 
 }  // extern "C"
 
-int b200::context_create(int device, bool express, b200_ctx** out) {
-    B200_TRY
-    if (!out) return B200_ERR_INVALID;
+// ---- SM partitions ----------------------------------------------------------------------------------
+// The green-context calls of the driver API are looked up through the runtime (cudaGetDriverEntryPointByVersion) rather
+// than linked from libcuda: the library then loads, and refuses arguments, on a machine without a driver, and takes the
+// driver the runtime has already loaded.
+namespace {
+struct Driver {
+    PFN_cuDeviceGet_v2000 device_get = nullptr;
+    PFN_cuCtxGetCurrent_v4000 ctx_get_current = nullptr;
+    PFN_cuCtxSetCurrent_v4000 ctx_set_current = nullptr;
+    PFN_cuGetErrorString_v6000 error_string = nullptr;
+    PFN_cuDeviceGetDevResource_v12040 device_get_resource = nullptr;
+    PFN_cuDevSmResourceSplitByCount_v12040 sm_split_by_count = nullptr;
+    PFN_cuDevResourceGenerateDesc_v12040 generate_desc = nullptr;
+    PFN_cuGreenCtxCreate_v12040 green_create = nullptr;
+    PFN_cuGreenCtxDestroy_v12040 green_destroy = nullptr;
+    PFN_cuCtxFromGreenCtx_v12040 ctx_from_green = nullptr;
+    PFN_cuGreenCtxGetDevResource_v12040 green_get_resource = nullptr;
+    PFN_cuGreenCtxStreamCreate_v12050 green_stream_create = nullptr;
+    std::string missing;  // the first entry point the driver did not give; empty when all are there
+};
+
+template <class F>
+void lookup(Driver& d, const char* name, unsigned version, F* f) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
+    if (cudaGetDriverEntryPointByVersion(name, &p, version, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess || !p) {
+        cudaGetLastError();
+        if (d.missing.empty()) d.missing = name;
+        return;
+    }
+    *f = reinterpret_cast<F>(p);
+}
+
+const Driver& driver() {
+    static const Driver d = [] {
+        Driver x;
+        lookup(x, "cuDeviceGet", 2000, &x.device_get);
+        lookup(x, "cuCtxGetCurrent", 4000, &x.ctx_get_current);
+        lookup(x, "cuCtxSetCurrent", 4000, &x.ctx_set_current);
+        lookup(x, "cuGetErrorString", 6000, &x.error_string);
+        lookup(x, "cuDeviceGetDevResource", 12040, &x.device_get_resource);
+        lookup(x, "cuDevSmResourceSplitByCount", 12040, &x.sm_split_by_count);
+        lookup(x, "cuDevResourceGenerateDesc", 12040, &x.generate_desc);
+        lookup(x, "cuGreenCtxCreate", 12040, &x.green_create);
+        lookup(x, "cuGreenCtxDestroy", 12040, &x.green_destroy);
+        lookup(x, "cuCtxFromGreenCtx", 12040, &x.ctx_from_green);
+        lookup(x, "cuGreenCtxGetDevResource", 12040, &x.green_get_resource);
+        lookup(x, "cuGreenCtxStreamCreate", 12050, &x.green_stream_create);
+        return x;
+    }();
+    return d;
+}
+
+int driver_ready(const char* who) {
+    const Driver& d = driver();
+    if (d.missing.empty()) return B200_OK;
+    set_error(std::string(who) + ": the CUDA driver has no " + d.missing + " (green contexts need CUDA 12.5 or later)");
+    return B200_ERR_CUDA;
+}
+
+int cu_fail(CUresult r, const char* what) {
+    const char* s = nullptr;
+    if (driver().error_string) driver().error_string(r, &s);
+    set_error(std::string(what) + ": " + (s ? s : "CUresult " + std::to_string((int)r)));
+    return B200_ERR_CUDA;
+}
+
+// cudaGetDeviceCount and the ordinal's range, with the messages of b200_init
+int check_device(int device) {
     int count = 0;
     cudaError_t e = cudaGetDeviceCount(&count);
     if (e != cudaSuccess || count == 0) {
@@ -170,9 +239,159 @@ int b200::context_create(int device, bool express, b200_ctx** out) {
         set_error("device ordinal out of range");
         return B200_ERR_INVALID;
     }
+    return B200_OK;
+}
+
+// A context's teardown: its streams, events and buffers inside its partition, then the green context itself
+void context_destroy(b200_ctx* ctx) {
+    CUgreenCtx g = ctx->c.green;
+    {
+        Enter in(ctx->c);
+        cudaStreamSynchronize(ctx->c.stream);
+        delete ctx;
+    }
+    if (g) driver().green_destroy(g);
+}
+
+// One block's SM into a 256-bit mask; every block then holds its SM a few microseconds so that the grid spreads over
+// every SM the launch may use
+__global__ void probe_sms_kernel(unsigned long long* mask) {
+    if (threadIdx.x == 0) {
+        unsigned smid;
+        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+        atomicOr(mask + ((smid >> 6) & 3), 1ull << (smid & 63));
+    }
+    const long long t0 = clock64();
+    while (clock64() - t0 < 20000) {
+    }
+}
+}  // namespace
+
+b200::Enter::Enter(const Context& c) {
+    if (!c.green) {
+        const cudaError_t e = cudaSetDevice(c.device);
+        if (e != cudaSuccess) rc = cuda_fail(e, "cudaSetDevice");
+        return;
+    }
+    const Driver& d = driver();  // complete: the context was made through it
+    if (d.ctx_get_current(&prev) != CUDA_SUCCESS) prev = nullptr;
+    const CUresult r = d.ctx_set_current(c.green_cu);
+    if (r != CUDA_SUCCESS) {
+        rc = cu_fail(r, "cuCtxSetCurrent(green context)");
+        return;
+    }
+    restore = true;
+}
+
+b200::Enter::~Enter() {
+    if (restore) driver().ctx_set_current(prev);
+}
+
+int b200::stream_create(const Context& c, int prio, cudaStream_t* out) {
+    if (!c.green) B200_CUDA(cudaStreamCreateWithPriority(out, cudaStreamNonBlocking, prio));
+    else {
+        CUstream s = nullptr;
+        const CUresult r = driver().green_stream_create(&s, c.green, CU_STREAM_NON_BLOCKING, prio);
+        if (r != CUDA_SUCCESS) return cu_fail(r, "cuGreenCtxStreamCreate");
+        *out = s;
+    }
+    return B200_OK;
+}
+
+int b200::sm_split(int device, unsigned first_sms, SmGroup groups[2]) {
+    int rc = check_device(device);
+    if (rc != B200_OK || (rc = driver_ready("sm_split")) != B200_OK) return rc;
+    B200_CUDA(cudaSetDevice(device));  // the primary context, which the green contexts retain, is up before them
+    B200_CUDA(cudaFree(nullptr));
+    const Driver& d = driver();
+    CUdevice dev = 0;
+    CUresult r = d.device_get(&dev, device);
+    CUdevResource all{}, split[2]{};
+    if (r == CUDA_SUCCESS) r = d.device_get_resource(dev, &all, CU_DEV_RESOURCE_TYPE_SM);
+    if (r != CUDA_SUCCESS) return cu_fail(r, "cuDeviceGetDevResource");
+    if (first_sms + 8 > all.sm.smCount) {
+        set_error("express_sms must leave at least 8 SMs for the normal group: the device has " + std::to_string(all.sm.smCount));
+        return B200_ERR_INVALID;
+    }
+    unsigned n_groups = 1;
+    r = d.sm_split_by_count(&split[0], &n_groups, &all, &split[1], 0, first_sms);
+    if (r != CUDA_SUCCESS || n_groups != 1) return cu_fail(r, "cuDevSmResourceSplitByCount");
+    if (split[1].sm.smCount < 8) {
+        set_error("express_sms must leave at least 8 SMs for the normal group: the split of " + std::to_string(all.sm.smCount) +
+                  " SMs gave " + std::to_string(split[0].sm.smCount) + " and " + std::to_string(split[1].sm.smCount));
+        return B200_ERR_INVALID;
+    }
+    for (int i = 0; i < 2; ++i) {
+        if ((r = d.generate_desc(&groups[i].desc, &split[i], 1)) != CUDA_SUCCESS) return cu_fail(r, "cuDevResourceGenerateDesc");
+        groups[i].sms = split[i].sm.smCount;
+    }
+    return B200_OK;
+}
+
+int b200::probe_sms(Context* c, uint64_t mask[4]) {
+    B200_ENTER(*c);
+    int sms = (int)c->sms;
+    if (!sms) B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
+    unsigned long long* d_mask = nullptr;
+    B200_CUDA(cudaMalloc(&d_mask, 32));
+    cudaError_t e = cudaMemsetAsync(d_mask, 0, 32, c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    const cudaStream_t streams[3] = {c->stream, c->heavy, c->stream2};
+    for (cudaStream_t st : streams) {
+        if (!st || e != cudaSuccess) continue;
+        B200_LAUNCH(probe_sms_kernel, 8 * (unsigned)sms, 128, 0, st)(d_mask);  // eagerly
+        cudaGraph_t g = nullptr;
+        cudaGraphExec_t x = nullptr;
+        e = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal);
+        if (e == cudaSuccess) {
+            B200_LAUNCH(probe_sms_kernel, 8 * (unsigned)sms, 128, 0, st)(d_mask);  // captured, then replayed
+            e = cudaStreamEndCapture(st, &g);
+        }
+        if (e == cudaSuccess) e = cudaGraphInstantiate(&x, g, 0);
+        if (e == cudaSuccess) {
+            e = cudaGraphLaunch(x, st);
+            g_graph_launches.fetch_add(1, std::memory_order_relaxed);
+        }
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (x) cudaGraphExecDestroy(x);
+        if (g) cudaGraphDestroy(g);
+    }
+    unsigned long long h[4] = {};
+    if (e == cudaSuccess) e = cudaMemcpy(h, d_mask, 32, cudaMemcpyDeviceToHost);
+    cudaFree(d_mask);
+    if (e != cudaSuccess) return cuda_fail(e, "probe_sms");
+    for (int i = 0; i < 4; ++i) mask[i] |= h[i];
+    return B200_OK;
+}
+
+int b200::context_create(int device, bool express, const SmGroup* group, b200_ctx** out) {
+    B200_TRY
+    if (!out) return B200_ERR_INVALID;
+    int rc = check_device(device);
+    if (rc != B200_OK) return rc;
     B200_CUDA(cudaSetDevice(device));
     b200_ctx* ctx = new b200_ctx();
     ctx->c.device = device;
+    if (group) {
+        const Driver& d = driver();
+        CUdevice dev = 0;
+        CUdevResource res{};
+        CUresult r = d.device_get(&dev, device);
+        if (r == CUDA_SUCCESS) r = d.green_create(&ctx->c.green, group->desc, dev, CU_GREEN_CTX_DEFAULT_STREAM);
+        if (r == CUDA_SUCCESS) r = d.ctx_from_green(&ctx->c.green_cu, ctx->c.green);
+        if (r == CUDA_SUCCESS) r = d.green_get_resource(ctx->c.green, &res, CU_DEV_RESOURCE_TYPE_SM);
+        if (r != CUDA_SUCCESS) {
+            rc = cu_fail(r, "green context");
+            context_destroy(ctx);
+            return rc;
+        }
+        ctx->c.sms = res.sm.smCount;
+    }
+    Enter in(ctx->c);
+    if (in.rc != B200_OK) {
+        context_destroy(ctx);
+        return in.rc;
+    }
     // The context's own stream runs at the highest priority and carries the short, latency-bound kernels
     // (sorts, scans, bucket reduction, transcript-driven glue); the long throughput-bound kernels (bucket
     // accumulation, the side-stream coset NTTs) go to a lowest-priority companion stream.  With several
@@ -189,15 +408,17 @@ int b200::context_create(int device, bool express, b200_ctx** out) {
     const int main_prio = prio ? prio_greatest : (lift ? prio_greatest : 0);
     const int heavy_prio = lift ? prio_least - 1 : prio_least;
     ctx->c.stream2_prio = prio ? heavy_prio : main_prio;
-    e = cudaStreamCreateWithPriority(&ctx->c.stream, cudaStreamNonBlocking, main_prio);
-    if (e == cudaSuccess && prio) {
-        e = cudaStreamCreateWithPriority(&ctx->c.heavy, cudaStreamNonBlocking, heavy_prio);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->c.hv_fork, cudaEventDisableTiming);
+    rc = stream_create(ctx->c, main_prio, &ctx->c.stream);
+    if (rc == B200_OK && prio) {
+        rc = stream_create(ctx->c, heavy_prio, &ctx->c.heavy);
+        cudaError_t e = cudaSuccess;
+        if (rc == B200_OK) e = cudaEventCreateWithFlags(&ctx->c.hv_fork, cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->c.hv_join, cudaEventDisableTiming);
+        if (e != cudaSuccess) rc = cuda_fail(e, "cudaEventCreate");
     }
-    if (e != cudaSuccess) {
-        delete ctx;
-        return cuda_fail(e, "cudaStreamCreate");
+    if (rc != B200_OK) {
+        context_destroy(ctx);
+        return rc;
     }
     ctx->c.msm.hv_stream = ctx->c.heavy;
     ctx->c.heavy_plonk = prio && !(pe && pe[0] == '1');  // B200_STREAM_PRIORITIES=1: accumulation only
@@ -206,6 +427,7 @@ int b200::context_create(int device, bool express, b200_ctx** out) {
     ctx->c.batch.msm.hv_stream = ctx->c.heavy;
     ctx->c.batch.msm.hv_fork = ctx->c.hv_fork;
     ctx->c.batch.msm.hv_join = ctx->c.hv_join;
+    ctx->c.msm.sms = ctx->c.batch.msm.sms = ctx->c.sms;
     *out = ctx;
     return B200_OK;
     B200_CATCH
@@ -214,10 +436,7 @@ int b200::context_create(int device, bool express, b200_ctx** out) {
 extern "C" {
 
 void b200_shutdown(b200_ctx* ctx) {
-    if (!ctx) return;
-    cudaSetDevice(ctx->c.device);
-    cudaStreamSynchronize(ctx->c.stream);
-    delete ctx;
+    if (ctx) context_destroy(ctx);
 }
 
 // ---- SRS ------------------------------------------------------------------------------------
@@ -353,7 +572,7 @@ int b200_bases_load(b200_ctx* ctx, const uint8_t* points64, size_t n, int window
         return B200_ERR_INVALID;
     }
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     Bases* b = nullptr;
     int rc = bases_create(reinterpret_cast<const g1_affine*>(points64), n, window_bits, check_on_curve,
                           ctx->c.stream, &b);
@@ -371,7 +590,7 @@ int b200_bases_load_device(b200_ctx* ctx, const void* d_points64, size_t n, int 
         return B200_ERR_INVALID;
     }
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     Bases* b = nullptr;
     int rc = bases_create_device(reinterpret_cast<const g1_affine*>(d_points64), n, window_bits, ctx->c.stream, &b);
     if (rc != B200_OK) return rc;
@@ -384,7 +603,7 @@ void b200_bases_free(b200_ctx* ctx, b200_bases* bases) {
     if (!bases) return;
     if (ctx) {
         std::lock_guard<std::mutex> lk(ctx->c.mu);
-        cudaSetDevice(ctx->c.device);
+        Enter in(ctx->c);
         cudaStreamSynchronize(ctx->c.stream);
         delete bases->b;
     } else {
@@ -411,7 +630,7 @@ int b200_msm_device(b200_ctx* ctx, const b200_bases* bases, size_t base_off, con
     B200_TRY
     if (!ctx || !bases || !out_xy || (n && !d_scalars)) return B200_ERR_INVALID;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     g1_affine r;
     int inf = 0;
     int rc = msm_device(bases->b, base_off, reinterpret_cast<const fe*>(d_scalars), n, scalars_montgomery,
@@ -428,7 +647,7 @@ int b200_msm(b200_ctx* ctx, const b200_bases* bases, size_t base_off, const uint
     B200_TRY
     if (!ctx || !bases || !out_xy || (n && !scalars)) return B200_ERR_INVALID;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     int rc = ctx->c.msm.scalars.reserve(n * sizeof(fe) + 32);
     if (rc != B200_OK) return rc;
     if (n) B200_CUDA(cudaMemcpyAsync(ctx->c.msm.scalars.p, scalars, n * sizeof(fe), cudaMemcpyHostToDevice, ctx->c.stream));
@@ -467,7 +686,7 @@ int b200_msm_batch_device(b200_ctx* ctx, const b200_bases* bases, size_t base_of
     B200_TRY
     if (!ctx || !bases || !out_xy || (n && !d_scalars) || batch == 0 || batch > 64 || stride < n) return B200_ERR_INVALID;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     std::vector<g1_affine> r(batch);
     std::vector<int> inf(batch, 0);
     int rc = msm_device_batch(bases->b, base_off, reinterpret_cast<const fe*>(d_scalars), n, stride, batch,
@@ -526,7 +745,7 @@ int b200_msm_timing(b200_ctx* ctx, int enable, float out_ms[4]) {
 static int ntt_device_locked(b200_ctx* ctx, void* d_data, unsigned log_n, int inverse, int coset, unsigned batch,
                              size_t stride) {
     const size_t n = (size_t)1 << log_n;
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     Domain* d = nullptr;
     int rc = get_domain(&ctx->c, log_n, &d);
     if (rc != B200_OK) return rc;
@@ -570,7 +789,7 @@ int b200_ntt(b200_ctx* ctx, uint64_t* data, unsigned log_n, int inverse, int cos
     // one critical section: upload, transform and download cannot interleave with another caller's
     // (whose reserve() could otherwise free the staging buffer under this call)
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     int rc = ctx->c.ntt_data.reserve(n * sizeof(fe));
     if (rc != B200_OK) return rc;
     B200_CUDA(cudaMemcpyAsync(ctx->c.ntt_data.p, data, n * sizeof(fe), cudaMemcpyHostToDevice, ctx->c.stream));
@@ -592,7 +811,7 @@ int b200_domain_generator(b200_ctx* ctx, unsigned log_n, uint64_t out[4]) {
     B200_TRY
     if (!ctx || !out || log_n > 28) return B200_ERR_INVALID;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     Domain* d = nullptr;
     int rc = get_domain(&ctx->c, log_n, &d);
     if (rc != B200_OK) return rc;
@@ -606,7 +825,7 @@ int b200_splitmix_fr_device(b200_ctx* ctx, uint64_t seed, size_t first, size_t n
     B200_TRY
     if (!ctx || (n && !d_out)) return B200_ERR_INVALID;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     int rc = splitmix_fr_device(seed, first, n, montgomery, reinterpret_cast<fe*>(d_out), ctx->c.stream);
     if (rc != B200_OK) return rc;
     B200_CUDA(cudaStreamSynchronize(ctx->c.stream));
@@ -618,7 +837,7 @@ int b200_known_dlog_bases_device(b200_ctx* ctx, uint64_t seed, size_t first, siz
     B200_TRY
     if (!ctx || (n && !d_out)) return B200_ERR_INVALID;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     int rc = g1_known_dlog_bases_device(seed, first, n, reinterpret_cast<g1_affine*>(d_out), ctx->c.stream);
     if (rc != B200_OK) return rc;
     B200_CUDA(cudaStreamSynchronize(ctx->c.stream));
@@ -631,7 +850,7 @@ int b200_selftest_field(b200_ctx* ctx, uint64_t seed, size_t iters, uint64_t* mi
     B200_TRY
     if (!ctx || !mismatches) return B200_ERR_INVALID;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     unsigned long long* d_bad = nullptr;
     B200_CUDA(cudaMalloc(&d_bad, 8));
     cudaMemsetAsync(d_bad, 0, 8, ctx->c.stream);
@@ -651,7 +870,7 @@ int b200_field_op(b200_ctx* ctx, int field, int op, const uint64_t* a, const uin
     if (!ctx || !a || !b || !out || field < 0 || field > 1 || op < 0 || op > 6) return B200_ERR_INVALID;
     if (n == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     fe *da = nullptr, *db = nullptr, *dout = nullptr;
     B200_CUDA(cudaMalloc(&da, n * sizeof(fe)));
     B200_CUDA(cudaMalloc(&db, n * sizeof(fe)));

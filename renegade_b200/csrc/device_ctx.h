@@ -1,6 +1,7 @@
 // Internal (C++) declarations shared by the CUDA translation units behind the C ABI in
 // include/b200prover.h.  Nothing here is part of the public boundary.
 #pragma once
+#include <cuda.h>  // green-context types; the driver calls are looked up at run time (api.cu)
 #include <cuda_runtime.h>
 
 #include <atomic>
@@ -152,6 +153,7 @@ struct MsmScratch {
     // borrowed from the context: low-priority stream for the accumulation kernel (null: same stream)
     cudaStream_t hv_stream = nullptr;
     cudaEvent_t hv_fork = nullptr, hv_join = nullptr;
+    unsigned sms = 0;  // from the context: the SMs of its partition, 0 on the whole device (sizes the grid-stride kernels)
     ~MsmScratch() {
         if (ev_init)
             for (auto& e : ev) cudaEventDestroy(e);
@@ -256,14 +258,52 @@ struct Context {
         HostPinned h_small, h_params;
         MsmScratch msm;
     } batch;
+    // A context bound to an SM partition (b200reserved.h): its own green context, which owns its streams and which every
+    // entry point makes current (Enter); null on the whole device.  `sms` is the partition's SM count (0: whole device).
+    CUgreenCtx green = nullptr;
+    CUcontext green_cu = nullptr;  // cuCtxFromGreenCtx(green)
+    unsigned sms = 0;
     ~Context();
 };
 
 int get_domain(Context* c, unsigned log_n, Domain** out);
 
-// b200_init (express = false), or a context for a pool's express worker (pool.cu), whose streams rank above a normal
-// context's of the same role where the device has two priority levels or more (api.cu).
-int context_create(int device, bool express, b200_ctx** out);
+// One group of a device's SMs that contexts can be bound to: the descriptor each bound context's green context is made
+// from, and the group's SM count as the split rounded it (api.cu).
+struct SmGroup {
+    CUdevResourceDesc desc = nullptr;
+    unsigned sms = 0;
+};
+// Splits the device's SMs into groups[0], at least `first_sms` (a multiple of 8), and groups[1], the rest.
+// B200_ERR_INVALID when the rest is fewer than 8 SMs.  Descriptors need no release.
+int sm_split(int device, unsigned first_sms, SmGroup groups[2]);
+
+// b200_init (express = false, group = nullptr), or a context for a pool's worker (pool.cu): `express` ranks its streams
+// above a normal context's of the same role where the device has two priority levels or more, and a non-null `group`
+// binds it to those SMs through a green context of its own, its streams made there at the same priorities (api.cu).
+int context_create(int device, bool express, const SmGroup* group, b200_ctx** out);
+
+// What every entry point does before it touches the device: for a context on the whole device, cudaSetDevice (left
+// set, as always); for a partitioned one, its green context made current for the scope and the caller's context back
+// after, so that allocations, captures, graph instantiation and launches all stay inside the partition.
+struct Enter {
+    int rc = B200_OK;
+    bool restore = false;
+    CUcontext prev = nullptr;
+    explicit Enter(const Context& c);
+    ~Enter();
+    Enter(const Enter&) = delete;
+    Enter& operator=(const Enter&) = delete;
+};
+#define B200_ENTER(c)                                 \
+    ::b200::Enter _b200_enter(c);                     \
+    if (_b200_enter.rc != B200_OK) return _b200_enter.rc
+
+// A non-blocking stream of the context at `prio`: on its green context when it has one (api.cu)
+int stream_create(const Context& c, int prio, cudaStream_t* out);
+// ORs into mask[4] the %smid of every block of a small kernel run, eagerly and as a replayed graph, on each stream the
+// context has; the caller holds c->mu (api.cu)
+int probe_sms(Context* c, uint64_t mask[4]);
 
 // a 128-byte G2 record x0 || x1 || y0 || y1 (Montgomery) is on the twist, every coordinate below q (verify.cu)
 bool g2_record_on_curve(const uint64_t rec[16]);

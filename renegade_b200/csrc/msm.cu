@@ -1163,8 +1163,10 @@ int msm_identity_point(g1_xyzz* d_point, cudaStream_t st) {
     return B200_OK;
 }
 
-// SMs of the current device: the grid-stride heavy-bucket combine runs 4 blocks per SM (132 on an H100 SXM)
-static size_t sm_count() {
+// SMs the scratch's context may use: its partition's, or the current device's (132 on an H100 SXM).  The grid-stride
+// heavy-bucket combine runs 4 blocks per SM.
+static size_t sm_count(const MsmScratch* s) {
+    if (s->sms) return s->sms;
     int dev = 0, sms = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
         sms <= 0)
@@ -1284,7 +1286,7 @@ int msm_launch_batch(const Bases* b, size_t base_off, const fe* d_scalars, size_
     if (pl.latency)
         B200_LAUNCH(msm_bucket_combine_kernel, (unsigned)((n_buckets + 127) / 128), 128, 0, st)(seg_sums, seg_offsets,
                                                                                               (uint32_t)n_buckets, buckets);
-    B200_LAUNCH(msm_heavy_combine_kernel, (unsigned)std::min<size_t>(max_heavy, 4 * sm_count()), kReduceThreads, 0, st)(
+    B200_LAUNCH(msm_heavy_combine_kernel, (unsigned)std::min<size_t>(max_heavy, 4 * sm_count(s)), kReduceThreads, 0, st)(
         seg_sums, seg_offsets, &stt->heavy_count, heavy_list, buckets);
     stamp(2);
     const unsigned n_bits = (unsigned)(pl.c - 1);

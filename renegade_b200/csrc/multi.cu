@@ -299,7 +299,7 @@ int b200_multi_bases_known_dlog(b200_multi* m, uint64_t seed, size_t n, int wind
     B200_TRY
     if (!m || !out || n == 0) return B200_ERR_INVALID;
     return multi_bases_make(m, n, out, [&](b200_ctx* ctx, size_t begin, size_t cnt, b200_bases** shard) -> int {
-        B200_CUDA(cudaSetDevice(ctx->c.device));
+        B200_ENTER(ctx->c);
         void* d_pts = nullptr;
         B200_CUDA(cudaMalloc(&d_pts, cnt * 64));
         int rc = b200_known_dlog_bases_device(ctx, seed, begin, cnt, d_pts);

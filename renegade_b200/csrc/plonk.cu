@@ -1177,7 +1177,7 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
     if ((rc = bf.h_params->reserve(k * sizeof(ProofParams))) != B200_OK) return rc;
     if ((rc = bf.d_params->reserve(k * sizeof(ProofParams))) != B200_OK) return rc;
     if (!c->stream2) {
-        B200_CUDA(cudaStreamCreateWithPriority(&c->stream2, cudaStreamNonBlocking, c->stream2_prio));
+        if ((rc = stream_create(*c, c->stream2_prio, &c->stream2)) != B200_OK) return rc;
         B200_CUDA(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
         B200_CUDA(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
     }
@@ -2020,7 +2020,7 @@ int settlement_check(const b200_bases* srs, const b200_bundle_witness& proof, co
 static int prove_settlement(b200_ctx* ctx, const Bases* srs, const ProvingKey* pk, ProveItem* item, std::vector<LinkItem>& its,
                             int* statuses, const std::string& who) {
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     int rc = prove(&ctx->c, single_bufs(&ctx->c), pk, item, 1, /*single=*/true);
     if (rc == B200_ERR_UNSATISFIED) {
         std::memset(item->proof, 0, sizeof(b200_proof));
@@ -2063,7 +2063,7 @@ int b200_plonk_preprocess(b200_ctx* ctx, const b200_bases* srs, unsigned log_n, 
     B200_TRY
     if (!ctx || !srs || !selectors_evals || !perm || !k || !out) return B200_ERR_INVALID;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     ProvingKey* pk = nullptr;
     int rc = preprocess(&ctx->c, srs->b, log_n, num_inputs, reinterpret_cast<const fe*>(selectors_evals), perm, nullptr, 0,
                         reinterpret_cast<const fe*>(k), &pk);
@@ -2084,7 +2084,7 @@ int b200_plonk_preprocess_wiring(b200_ctx* ctx, const b200_bases* srs, unsigned 
         return B200_ERR_INVALID;
     }
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     ProvingKey* pk = nullptr;
     int rc = preprocess(&ctx->c, srs->b, log_n, num_inputs, reinterpret_cast<const fe*>(selectors_evals), nullptr,
                         reinterpret_cast<const uint32_t*>(wire_vars), num_vars, reinterpret_cast<const fe*>(k), &pk);
@@ -2116,7 +2116,7 @@ int b200_plonk_link(b200_ctx* ctx, const b200_bases* srs, const uint64_t* a1, si
     if (rc == B200_OK) rc = link_item(srs->b, x, "link", &it);
     if (rc != B200_OK) return rc;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     LinkItem* one = &it;
     if ((rc = link_chunk(&ctx->c, single_bufs(&ctx->c), srs->b, &one, 1, /*single=*/true)) != B200_OK) return rc;
     if (it.status != B200_OK) {
@@ -2141,7 +2141,7 @@ int b200_plonk_link_batch(b200_ctx* ctx, const b200_bases* srs, const b200_link_
     }
     if (k == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     const int rc = link_batch_run(&ctx->c, srs->b, its);
     if (rc != B200_OK) return rc;
     size_t bad = 0;
@@ -2171,7 +2171,7 @@ void b200_pk_free(b200_ctx* ctx, b200_pk* pk) {
     if (!pk) return;
     if (ctx) {
         std::lock_guard<std::mutex> lk(ctx->c.mu);
-        cudaSetDevice(ctx->c.device);
+        Enter in(ctx->c);
         cudaStreamSynchronize(ctx->c.stream);
         delete pk->pk;
     } else {
@@ -2188,7 +2188,7 @@ int b200_plonk_prove(b200_ctx* ctx, const b200_pk* pk, const uint64_t* wires, co
     const int rc = check_prove_item(pk, x, "plonk_prove");
     if (rc != B200_OK) return rc;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     ProveItem item = prove_item(x);
     return prove(&ctx->c, single_bufs(&ctx->c), pk->pk, &item, 1, /*single=*/true);
     B200_CATCH
@@ -2202,7 +2202,7 @@ int b200_plonk_prove_witness(b200_ctx* ctx, const b200_pk* pk, const uint64_t* w
     const int rc = check_witness_item(pk, x, "plonk_prove_witness");
     if (rc != B200_OK) return rc;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     ProveItem item = prove_item(x);
     return prove(&ctx->c, single_bufs(&ctx->c), pk->pk, &item, 1, /*single=*/true);
     B200_CATCH
@@ -2246,7 +2246,7 @@ static int prove_batch_items(b200_ctx* ctx, const ProvingKey* key, std::vector<P
     const size_t k = its.size();
     if (k == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     const size_t chunk = prove_batch_chunk(&ctx->c, key, k);
     for (size_t off = 0; off < k; off += chunk) {
         const unsigned cnt = (unsigned)std::min(chunk, k - off);
@@ -2304,7 +2304,7 @@ int b200_fr_vec_op(b200_ctx* ctx, int op, const void* d_a, const void* d_b, int 
     if (!ctx || op < 0 || op > 2 || (n && (!d_a || !d_b || !d_out))) return B200_ERR_INVALID;
     if (n == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     B200_LAUNCH(k_fr_vec_op, grid_for(n, 256), 256, 0, ctx->c.stream)(op, reinterpret_cast<const fe*>(d_a), reinterpret_cast<const fe*>(d_b),
                                                                      b_is_scalar, n, reinterpret_cast<fe*>(d_out));
     B200_CUDA(cudaGetLastError());
@@ -2318,7 +2318,7 @@ int b200_fr_batch_inverse_device(b200_ctx* ctx, void* d_data, size_t n) {
     if (!ctx || (n && !d_data)) return B200_ERR_INVALID;
     if (n == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     int rc = ctx->c.ntt_scratch.reserve(n * sizeof(fe));
     if (rc != B200_OK) return rc;
     batch_inverse_enqueue(nullptr, reinterpret_cast<fe*>(d_data), reinterpret_cast<fe*>(ctx->c.ntt_scratch.p), n, ctx->c.stream);
@@ -2336,7 +2336,7 @@ int b200_fr_poly_eval_device(b200_ctx* ctx, const void* d_coeffs, size_t len, co
         return B200_OK;
     }
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     int rc = ctx->c.plonk_ws.reserve((2 * (len / CH + len / CH / CH) + 4 * CH + 64) * sizeof(fe));
     if (rc != B200_OK) return rc;
     fe* scr = reinterpret_cast<fe*>(ctx->c.plonk_ws.p);
@@ -2355,7 +2355,7 @@ int b200_fr_poly_div_linear_device(b200_ctx* ctx, const void* d_p, size_t len, c
     B200_TRY
     if (!ctx || !z || len < 2 || !d_p || !d_q) return B200_ERR_INVALID;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     const size_t L = len + 8;
     int rc = ctx->c.plonk_ws.reserve((L + 4 * (L / CH + 4 * CH + 64) + 16) * sizeof(fe));
     if (rc != B200_OK) return rc;

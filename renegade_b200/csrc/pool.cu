@@ -8,6 +8,8 @@
 // on a worker's context in the same queue, so a caller that checks proofs on a proving GPU needs no context of its own.
 // The express lane (b200express.h): a second queue that b200_pool_expedite moves a ticket's queued jobs to, drained by
 // express workers whose contexts' streams outrank the normal workers' (and by normal workers when it backs up).
+// Reserved SMs (b200reserved.h): the same pool with the express workers' contexts bound to a group of SMs of their own
+// and the normal workers' to the rest, through green contexts (api.cu).
 //
 // Host-only code (std::thread) above the same C ABI the single-context entry points use.
 #include <algorithm>
@@ -22,6 +24,7 @@
 
 #include "b200express.h"
 #include "b200prover.h"
+#include "b200reserved.h"
 #include "b200settlement.h"
 #include "b200verifyjobs.h"
 #include "device_ctx.h"
@@ -143,6 +146,7 @@ struct Bundle {
 struct b200_pool {
     std::vector<b200_ctx*> ctxs;     // the normal workers' contexts, then the express workers'
     unsigned n_normal = 0;
+    unsigned sms[2] = {0, 0};        // SMs of the normal and the express group (b200_pool_create_reserved); 0, 0: no partition
     std::vector<std::thread> workers;
     std::mutex mu;
     std::condition_variable cv_job, cv_express, cv_done;  // cv_job: normal workers, cv_express: express workers
@@ -304,6 +308,32 @@ static int bundle_push(b200_pool* pool, const char* who, const b200_bases* srs, 
     return pool_push(pool, jobs.data(), jobs.size(), b, ticket);
 }
 
+// A pool of n_workers normal and n_express express workers; with `groups`, the express workers' contexts on groups[0] and
+// the normal workers' on groups[1].  Nothing is left behind on a failure.
+static int pool_create(int device, unsigned n_workers, unsigned n_express, const b200::SmGroup* groups, b200_pool** out) {
+    std::unique_ptr<b200_pool> p(new b200_pool());
+    for (unsigned i = 0; i < n_workers + n_express; ++i) {
+        b200_ctx* c = nullptr;
+        const bool express = i >= n_workers;
+        const int rc = b200::context_create(device, express, groups ? &groups[express ? 0 : 1] : nullptr, &c);
+        if (rc != B200_OK) {
+            for (b200_ctx* q : p->ctxs) b200_shutdown(q);
+            return rc;
+        }
+        p->ctxs.push_back(c);
+    }
+    p->n_normal = n_workers;
+    p->idle_express = n_express;
+    if (groups) {
+        p->sms[0] = groups[1].sms;
+        p->sms[1] = groups[0].sms;
+    }
+    b200_pool* raw = p.release();
+    for (unsigned i = 0; i < n_workers + n_express; ++i) raw->workers.emplace_back([raw, i] { raw->run(i); });
+    *out = raw;
+    return B200_OK;
+}
+
 extern "C" {
 
 int b200_pool_create(int device, unsigned n_workers, b200_pool** out) { return b200_pool_create_express(device, n_workers, 0, out); }
@@ -314,22 +344,52 @@ int b200_pool_create_express(int device, unsigned n_workers, unsigned n_express,
         b200::set_error("pool: n_workers must be in [1, 64] and n_express in [0, 64]");
         return B200_ERR_INVALID;
     }
-    std::unique_ptr<b200_pool> p(new b200_pool());
-    for (unsigned i = 0; i < n_workers + n_express; ++i) {
-        b200_ctx* c = nullptr;
-        const int rc = b200::context_create(device, /*express=*/i >= n_workers, &c);
-        if (rc != B200_OK) {
-            for (b200_ctx* q : p->ctxs) b200_shutdown(q);
-            return rc;
-        }
-        p->ctxs.push_back(c);
+    return pool_create(device, n_workers, n_express, nullptr, out);
+    B200_CATCH
+}
+
+int b200_pool_create_reserved(int device, unsigned n_workers, unsigned n_express, unsigned express_sms, b200_pool** out) {
+    B200_TRY
+    const char* bad = !out                                   ? "null out"
+                      : n_workers == 0 || n_workers > 64     ? "n_workers must be in [1, 64]"
+                      : n_express == 0 || n_express > 64     ? "n_express must be in [1, 64]: the reserved SMs are the express workers'"
+                      : express_sms == 0 || express_sms % 8  ? "express_sms must be a positive multiple of 8 (the SM granularity of a split)"
+                      : express_sms > 248                    ? "express_sms must leave at least 8 SMs for the normal group (at most 248)"
+                                                             : nullptr;
+    if (bad) {
+        b200::set_error(std::string("pool_create_reserved: ") + bad);
+        return B200_ERR_INVALID;
     }
-    p->n_normal = n_workers;
-    p->idle_express = n_express;
-    b200_pool* raw = p.release();
-    for (unsigned i = 0; i < n_workers + n_express; ++i) raw->workers.emplace_back([raw, i] { raw->run(i); });
-    *out = raw;
+    b200::SmGroup groups[2];
+    const int rc = b200::sm_split(device, express_sms, groups);
+    if (rc != B200_OK) {
+        b200::set_error("pool_create_reserved: " + std::string(b200_last_error()));
+        return rc;
+    }
+    return pool_create(device, n_workers, n_express, groups, out);
+    B200_CATCH
+}
+
+int b200_pool_partition(const b200_pool* pool, unsigned out[2]) {
+    if (!pool || !out) {
+        b200::set_error("pool_partition: null argument");
+        return B200_ERR_INVALID;
+    }
+    out[0] = pool->sms[0];
+    out[1] = pool->sms[1];
     return B200_OK;
+}
+
+int b200_pool_probe_sms(b200_pool* pool, unsigned worker, uint64_t mask[4]) {
+    B200_TRY
+    if (!pool || !mask || worker >= pool->ctxs.size()) {
+        b200::set_error("pool_probe_sms: null pool or mask, or a worker index out of range");
+        return B200_ERR_INVALID;
+    }
+    for (int i = 0; i < 4; ++i) mask[i] = 0;
+    b200::Context& c = pool->ctxs[worker]->c;
+    std::lock_guard<std::mutex> lk(c.mu);
+    return b200::probe_sms(&c, mask);
     B200_CATCH
 }
 
@@ -799,9 +859,11 @@ int b200_box_create(const int* devices, int n_dev, unsigned workers_per_device, 
     return b200_box_create_express(devices, n_dev, workers_per_device, 0, out);
 }
 
-int b200_box_create_express(const int* devices, int n_dev, unsigned workers_per_device, unsigned express_per_device,
-                            b200_box** out) {
-    B200_TRY
+}  // extern "C"
+
+// A box of one pool per device, each made by make(device, &pool); nothing is left behind on a failure
+template <class Make>
+static int box_create(const int* devices, int n_dev, b200_box** out, Make make) {
     if (!devices || n_dev <= 0 || n_dev > 64 || !out) {
         b200::set_error("box_create: need 1..64 device ordinals");
         return B200_ERR_INVALID;
@@ -809,7 +871,7 @@ int b200_box_create_express(const int* devices, int n_dev, unsigned workers_per_
     std::unique_ptr<b200_box> box(new b200_box());
     for (int i = 0; i < n_dev; ++i) {
         b200_pool* p = nullptr;
-        const int rc = b200_pool_create_express(devices[i], workers_per_device, express_per_device, &p);
+        const int rc = make(devices[i], &p);
         if (rc != B200_OK) {
             b200_box_destroy(box.release());
             return rc;
@@ -819,6 +881,25 @@ int b200_box_create_express(const int* devices, int n_dev, unsigned workers_per_
     }
     *out = box.release();
     return B200_OK;
+}
+
+extern "C" {
+
+int b200_box_create_express(const int* devices, int n_dev, unsigned workers_per_device, unsigned express_per_device,
+                            b200_box** out) {
+    B200_TRY
+    return box_create(devices, n_dev, out, [&](int device, b200_pool** p) {
+        return b200_pool_create_express(device, workers_per_device, express_per_device, p);
+    });
+    B200_CATCH
+}
+
+int b200_box_create_reserved(const int* devices, int n_dev, unsigned workers_per_device, unsigned express_per_device,
+                             unsigned express_sms, b200_box** out) {
+    B200_TRY
+    return box_create(devices, n_dev, out, [&](int device, b200_pool** p) {
+        return b200_pool_create_reserved(device, workers_per_device, express_per_device, express_sms, p);
+    });
     B200_CATCH
 }
 

@@ -177,7 +177,7 @@ int b200_poseidon2_permute_batch(b200_ctx* ctx, uint64_t* states, size_t batch) 
     if (!ctx || (batch && !states)) return B200_ERR_INVALID;
     if (batch == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     cudaStream_t st = ctx->c.stream;
     int rc = load_constants(ctx->c.device, st);
     if (rc != B200_OK) return rc;
@@ -196,7 +196,7 @@ int b200_poseidon2_hash_batch(b200_ctx* ctx, const uint64_t* inputs, size_t batc
     if (!ctx || !out || (batch && len && !inputs)) return B200_ERR_INVALID;
     if (batch == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     cudaStream_t st = ctx->c.stream;
     int rc = load_constants(ctx->c.device, st);
     if (rc != B200_OK) return rc;
@@ -217,7 +217,7 @@ int b200_poseidon2_merkle_root_batch(b200_ctx* ctx, const uint64_t* leaf_hashes,
     if (!ctx || !roots || (batch && (!leaf_hashes || (height && (!sisters || !is_right)))) || height > 64) return B200_ERR_INVALID;
     if (batch == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     cudaStream_t st = ctx->c.stream;
     int rc = load_constants(ctx->c.device, st);
     if (rc != B200_OK) return rc;
@@ -245,7 +245,7 @@ int b200_poseidon2_csprng_batch(b200_ctx* ctx, const uint64_t* seeds, const uint
     if (!ctx || !out || (batch && (!seeds || !first_index))) return B200_ERR_INVALID;
     if (batch == 0 || count == 0) return B200_OK;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     cudaStream_t st = ctx->c.stream;
     int rc = load_constants(ctx->c.device, st);
     if (rc != B200_OK) return rc;

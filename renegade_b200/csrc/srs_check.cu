@@ -241,7 +241,7 @@ int b200_srs_check(b200_ctx* ctx, const b200_bases* srs, size_t n, const uint64_
     r.g2_subgroup = g2_in_subgroup(h) && g2_in_subgroup(tau_h) ? 1 : 0;
     const fe rho = srs_rho(seed, n, g2_h, g2_tau_h);
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     cudaStream_t st = ctx->c.stream;
     g1_affine p0;
     B200_CUDA(cudaMemcpyAsync(&p0, srs->b->tables, sizeof(p0), cudaMemcpyDeviceToHost, st));

@@ -556,7 +556,7 @@ extern "C" int b200_plonk_batch_verify(b200_ctx* ctx, const b200_verifying_key* 
         return B200_OK;
     }
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     cudaStream_t st = ctx->c.stream;
     Batch bt;
     bt.c = &ctx->c;
@@ -619,7 +619,7 @@ extern "C" int b200_plonk_verify_each(b200_ctx* ctx, const b200_verifying_key* v
     g2_prepare_record(g2_tau_h, &q[0]);
     g2_prepare_record(g2_h, &q[1]);
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     cudaStream_t st = ctx->c.stream;
     Batch bt;
     bt.c = &ctx->c;
@@ -665,7 +665,7 @@ extern "C" int b200_pairing_check_many(b200_ctx* ctx, const uint64_t* g2_points,
     if (n_checks == 0) return B200_OK;
     if (p_bytes) std::memcpy(h.data() + q_bytes, g1_points, p_bytes);
     std::lock_guard<std::mutex> lk(ctx->c.mu);
-    B200_CUDA(cudaSetDevice(ctx->c.device));
+    B200_ENTER(ctx->c);
     cudaStream_t st = ctx->c.stream;
     DevBuf d_in, d_out;
     int rc;

@@ -15,7 +15,9 @@ All arithmetic runs in libb200prover.so on the GPU; nothing here computes on the
 from __future__ import annotations
 
 import ctypes as C
+import functools
 from dataclasses import dataclass
+from typing import NamedTuple
 
 import numpy as np
 
@@ -605,51 +607,33 @@ class PlonkKzgSnark:
         witness is the num_vars x 4 array, or the address of one in device or pinned host memory (int).  Returns
         (proof, LinkingHint, pub_inputs[, challenges]); proof, hint and challenges equal `prove_with_link_hint` on the
         expanded wire table."""
-        n = pk.domain_size
-        wit, wit_ptr = _witness_arg(pk, witness, "prove_witness")
-        bl = np.ascontiguousarray(blinders, dtype=np.uint64).reshape(17, 4)
-        proof = B200Proof()
-        link = np.zeros((n + 2, 4), dtype=np.uint64)
-        ch = np.zeros((6, 4), dtype=np.uint64)
-        pub = np.zeros((pk.num_inputs, 4), dtype=np.uint64)
-        _lib.check(ctx._lib.b200_plonk_prove_witness(ctx._h, pk._h, wit_ptr, _ptr(bl), C.byref(proof), _ptr(link),
-                                                     _ptr(ch) if want_challenges else None, _ptr(pub) if pub.size else None))
-        hint = LinkingHint(linking_wire_poly=link, linking_wire_comm=np.array(proof.wires_poly_comms[0], dtype=np.uint64))
-        return (proof, hint, pub, ch) if want_challenges else (proof, hint, pub)
+        p = _witness_proof(pk, witness, blinders, "prove_witness", link=True, challenges=True)
+        _lib.check(ctx._lib.b200_plonk_prove_witness(ctx._h, pk._h, p.src, _ptr(p.bl), C.byref(p.proof), _ptr(p.link),
+                                                     _ptr(p.challenges) if want_challenges else None, _opt(p.pub)))
+        return (p.proof, p.hint(), p.pub, p.challenges) if want_challenges else (p.proof, p.hint(), p.pub)
 
     @staticmethod
     def prove_witness_batch(ctx: Context, pk: ProvingKey, witness_list, blinders_list, link_hints: bool = False,
                             want_challenges: bool = False):
         """`prove_batch` with the items given as witness vectors (b200_plonk_prove_witness_batch).  Returns
         (proofs, hints, statuses, pub_inputs[, challenges]), item i as `prove_witness` of the same arguments."""
-        items, keep, pubs = _witness_items(pk, witness_list, blinders_list, link_hints, want_challenges, "prove_witness_batch")
-        k = len(keep)
-        statuses = (C.c_int * max(1, k))()
-        rc = ctx._lib.b200_plonk_prove_witness_batch(ctx._h, pk._h, items, k, statuses)
+        items, ps = _witness_items(pk, witness_list, blinders_list, link_hints, want_challenges, "prove_witness_batch")
+        statuses = (C.c_int * max(1, len(ps)))()
+        rc = ctx._lib.b200_plonk_prove_witness_batch(ctx._h, pk._h, items, len(ps), statuses)
         if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
             _lib.check(rc)
-        res = _batch_results(keep, statuses, link_hints, want_challenges)
-        return res[:3] + (pubs,) + res[3:]
+        res = _batch_results(ps, statuses, link_hints, want_challenges)
+        return res[:3] + ([p.pub for p in ps],) + res[3:]
 
     @staticmethod
     def prove_with_link_hint(ctx: Context, pk: ProvingKey, wires: np.ndarray, pub_inputs: np.ndarray,
                              blinders: np.ndarray, want_challenges: bool = False):
         """Returns (proof, LinkingHint[, challenges]).  `blinders` are the 17 field elements the
         reference draws from `thread_rng()` (traits.rs:994), in draw order."""
-        n = pk.domain_size
-        w = np.ascontiguousarray(wires, dtype=np.uint64).reshape(5, n, 4)
-        pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64).reshape(-1, 4)
-        if pi.shape[0] != pk.num_inputs:
-            raise ValueError("wrong number of public inputs")
-        bl = np.ascontiguousarray(blinders, dtype=np.uint64).reshape(17, 4)
-        proof = B200Proof()
-        link = np.zeros((n + 2, 4), dtype=np.uint64)
-        ch = np.zeros((6, 4), dtype=np.uint64)
-        _lib.check(ctx._lib.b200_plonk_prove(ctx._h, pk._h, _ptr(w), _ptr(pi) if pi.size else None, _ptr(bl),
-                                             C.byref(proof), _ptr(link), _ptr(ch) if want_challenges else None))
-        hint = LinkingHint(linking_wire_poly=link, linking_wire_comm=np.array(proof.wires_poly_comms[0], dtype=np.uint64))
-        return (proof, hint, ch) if want_challenges else (proof, hint)
-
+        p = _table_proof(pk, wires, pub_inputs, blinders, "prove_with_link_hint", link=True, challenges=True)
+        _lib.check(ctx._lib.b200_plonk_prove(ctx._h, pk._h, p.src, _opt(p.pub), _ptr(p.bl), C.byref(p.proof), _ptr(p.link),
+                                             _ptr(p.challenges) if want_challenges else None))
+        return (p.proof, p.hint(), p.challenges) if want_challenges else (p.proof, p.hint())
 
     @staticmethod
     def prove_batch(ctx: Context, pk: ProvingKey, wires_list, pub_inputs_list, blinders_list, link_hints: bool = False,
@@ -661,13 +645,12 @@ class PlonkKzgSnark:
         arguments; statuses[i] is 0, or -7 (B200_ERR_UNSATISFIED) for a witness that does not satisfy the circuit, whose
         proof is zeroed and whose hint is None (hints is None without link_hints).  Argument errors raise ValueError before
         any device work; other failures raise B200Error."""
-        items, keep = _prove_items(pk, wires_list, pub_inputs_list, blinders_list, link_hints, want_challenges)
-        k = len(keep)
-        statuses = (C.c_int * max(1, k))()
-        rc = ctx._lib.b200_plonk_prove_batch(ctx._h, pk._h, items, k, statuses)
+        items, ps = _prove_items(pk, wires_list, pub_inputs_list, blinders_list, link_hints, want_challenges, "prove_batch")
+        statuses = (C.c_int * max(1, len(ps)))()
+        rc = ctx._lib.b200_plonk_prove_batch(ctx._h, pk._h, items, len(ps), statuses)
         if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
             _lib.check(rc)
-        return _batch_results(keep, statuses, link_hints, want_challenges)
+        return _batch_results(ps, statuses, link_hints, want_challenges)
 
     @staticmethod
     def prove_settlement(ctx: Context, srs: Bases, pk: ProvingKey, wires, pub_inputs, blinders, links):
@@ -678,123 +661,191 @@ class PlonkKzgSnark:
         `prove_with_link_hint`'s, link i equals `link_proofs(hint_i, settlement hint, layout_i)`; statuses[0] is the
         proof's, statuses[1 + i] link i's (0, or -7 = B200_ERR_UNSATISFIED: an unsatisfied witness zeroes everything, a
         stale hint zeroes its own link proof).  Argument errors raise ProverError before any library call."""
-        w, w_ptr = _wires_arg(pk.domain_size, wires, "prove_settlement")
-        pi, bl = _settlement_inputs(pk.num_inputs, pub_inputs, blinders, "prove_settlement")
-        arr, held, out = _settlement_links(links, len(srs), pk.domain_size, "prove_settlement")
-        proof = B200Proof()
-        st = (C.c_int * (len(out) + 1))()
-        rc = ctx._lib.b200_plonk_prove_settlement(ctx._h, srs._h, pk._h, w_ptr, _ptr(pi) if pi.size else None, _ptr(bl),
-                                                  C.byref(proof), None, arr, len(out), st)
-        if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
-            _lib.check(rc)
-        return proof, out, list(st)
+        (e, arr, n_links, st), finish, _ = _settlement_job(pk._h, pk, len(srs), links, _table_proof, wires, pub_inputs,
+                                                           blinders, where="prove_settlement")
+        e = e.contents
+        rc = ctx._lib.b200_plonk_prove_settlement(ctx._h, srs._h, pk._h, e.wires, e.pub_inputs, e.blinders, e.proof,
+                                                  e.link_poly, arr, n_links, st)
+        return finish(rc)
 
     @staticmethod
     def prove_settlement_witness(ctx: Context, srs: Bases, pk: ProvingKey, witness, blinders, links):
         """`prove_settlement` from the settlement's witness vector (`b200_plonk_prove_settlement_witness`) of a key made by
         `preprocess_wiring`: witness as `prove_witness` takes it.  Returns (proof, link_proofs, statuses, pub_inputs)."""
-        if pk.num_vars == 0:
-            raise ProverError(_lib.B200_ERR_INVALID, "prove_settlement_witness: the key holds no wiring (made by preprocess)")
-        try:
-            wit, wit_ptr = _witness_arg(pk, witness, "prove_settlement_witness")
-        except ValueError as e:
-            raise ProverError(_lib.B200_ERR_INVALID, str(e))
-        _, bl = _settlement_inputs(0, (), blinders, "prove_settlement_witness")
-        arr, held, out = _settlement_links(links, len(srs), pk.domain_size, "prove_settlement_witness")
-        proof = B200Proof()
-        pub = np.zeros((pk.num_inputs, 4), dtype=np.uint64)
-        st = (C.c_int * (len(out) + 1))()
-        rc = ctx._lib.b200_plonk_prove_settlement_witness(ctx._h, srs._h, pk._h, wit_ptr, _ptr(bl), C.byref(proof), None,
-                                                          _ptr(pub) if pub.size else None, arr, len(out), st)
-        if rc not in (_lib.B200_OK, _lib.B200_ERR_UNSATISFIED):
-            _lib.check(rc)
-        return proof, out, list(st), pub
+        (e, arr, n_links, st), finish, _ = _settlement_job(pk._h, pk, len(srs), links, _witness_proof, witness, blinders,
+                                                           where="prove_settlement_witness")
+        e = e.contents
+        rc = ctx._lib.b200_plonk_prove_settlement_witness(ctx._h, srs._h, pk._h, e.witness, e.blinders, e.proof,
+                                                          e.link_poly, e.pub_inputs_out, arr, n_links, st)
+        return finish(rc)
 
 
 B200ProveItem = _lib.STRUCTS["b200_prove_item"]  # one witness of a batch
 B200WitnessItem = _lib.STRUCTS["b200_witness_item"]  # one witness vector of a batch
 
 
-def _witness_arg(pk: ProvingKey, witness, where: str):
-    """A witness vector as (array kept alive or None, pointer): an array of the key's num_vars elements, or an address."""
+# ---- proof and link inputs -----------------------------------------------------------------------------------------
+# Every entry point that takes a proof or a link builds it with `_table_proof`, `_witness_proof` or `_link_item`.  They
+# check the input against the key's shape (`domain_size`, `num_inputs`, `num_vars` of a ProvingKey or a box key) and raise
+# ValueError before any library call, since the library reads fixed-size arrays through the pointers it is given.  A
+# message names the entry point, then the item, proof or link, then the field and the numbers.  Entry points that
+# refuse with ProverError convert in `_prover_errors`.
+
+def _opt(a):
+    """Pointer to an array, or NULL for no array or an empty one."""
+    return _ptr(a) if a is not None and a.size else None
+
+
+def _prover_errors(build):
+    """`build` with its argument errors (ValueError) raised as ProverError(B200_ERR_INVALID)."""
+    @functools.wraps(build)
+    def checked(*args, **kwargs):
+        try:
+            return build(*args, **kwargs)
+        except ValueError as e:
+            raise ProverError(_lib.B200_ERR_INVALID, str(e)) from None
+    return checked
+
+
+class _Proof(NamedTuple):
+    """One proof's checked inputs and the buffers the prover writes: `proof`, and the (n + 2, 4) `link` polynomial and
+    (6, 4) `challenges` when asked for (else None).  `held` is the wire table or witness array (None for an address),
+    `src` the pointer to it.  `pub` is a wire-table proof's public inputs, or the array a witness proof's public inputs
+    are written to."""
+    held: object
+    pub: np.ndarray
+    bl: np.ndarray
+    proof: B200Proof
+    link: object
+    challenges: object
+    src: object
+    witness: bool
+
+    def _proof_ptr(self):
+        return C.cast(C.pointer(self.proof), C.c_void_p)
+
+    def item(self):
+        """The proof as an item of a context batch: b200_witness_item or b200_prove_item."""
+        if self.witness:
+            return B200WitnessItem(self.src, _ptr(self.bl), self._proof_ptr(), _opt(self.link), _opt(self.challenges),
+                                   _opt(self.pub))
+        return B200ProveItem(self.src, _opt(self.pub), _ptr(self.bl), self._proof_ptr(), _opt(self.link),
+                             _opt(self.challenges))
+
+    def entry(self, pk):
+        """The proof as an entry of a pool job, key handle `pk`: b200_bundle_witness or b200_bundle_proof."""
+        if self.witness:
+            return BundleWitness(pk, self.src, _ptr(self.bl), self._proof_ptr(), _opt(self.link), _opt(self.pub))
+        return BundleProof(pk, self.src, _opt(self.pub), self.pub.shape[0], _ptr(self.bl), self._proof_ptr(),
+                           _opt(self.link))
+
+    def hint(self):
+        return LinkingHint(linking_wire_poly=self.link, linking_wire_comm=np.array(self.proof.wires_poly_comms[0],
+                                                                                   dtype=np.uint64))
+
+
+def _proof(shape, witness: bool, src, held, pub, blinders, link: bool, challenges: bool, where: str) -> _Proof:
+    """A `_Proof` with its blinders checked and its output buffers made."""
+    bl = np.ascontiguousarray(blinders, dtype=np.uint64)
+    if bl.size != 17 * 4:
+        raise ValueError(f"{where} has {bl.size // 4} blinders, the prover draws 17: blinders must be 17 Fr elements")
+    return _Proof(held, pub, bl, B200Proof(),
+                  np.zeros((shape.domain_size + 2, 4), dtype=np.uint64) if link else None,
+                  np.zeros((6, 4), dtype=np.uint64) if challenges else None, src, witness)
+
+
+def _table_proof(shape, wires, pub_inputs, blinders, where: str, link: bool = False, challenges: bool = False) -> _Proof:
+    """A proof of a 5 x n wire table, given as an array or as the address of one in device or pinned host memory."""
+    if isinstance(wires, (int, np.integer)):
+        w, src = None, C.c_void_p(int(wires))
+    else:
+        w = np.ascontiguousarray(wires, dtype=np.uint64)
+        if w.size != 5 * shape.domain_size * 4:
+            raise ValueError(f"{where}: the wire table has {w.size // 4} elements, the key needs 5 x {shape.domain_size}")
+        src = _ptr(w)
+    pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64)
+    if pi.size != 4 * shape.num_inputs:
+        raise ValueError(f"{where} has {pi.size // 4} public inputs for a key with {shape.num_inputs}: public inputs / "
+                         "blinders do not match the key")
+    return _proof(shape, False, src, w, pi.reshape(-1, 4), blinders, link, challenges, where)
+
+
+def _witness_proof(shape, witness, blinders, where: str, link: bool = False, challenges: bool = False) -> _Proof:
+    """A proof of a witness vector of a key made by `preprocess_wiring`, given as an array of the key's num_vars elements or
+    as the address of one in device or pinned host memory.  A key without wiring is ProverError, as the library says."""
+    if shape.num_vars == 0:
+        raise ProverError(_lib.B200_ERR_INVALID, f"{where} holds no wiring: its key was made by preprocess")
     if isinstance(witness, (int, np.integer)):
-        return None, C.c_void_p(int(witness))
-    wit = np.ascontiguousarray(witness, dtype=np.uint64)
-    if wit.size != 4 * pk.num_vars:
-        raise ValueError(f"{where}: the witness has {wit.size // 4} elements, the key takes {pk.num_vars}")
-    return wit, _ptr(wit)
+        wit, src = None, C.c_void_p(int(witness))
+    else:
+        wit = np.ascontiguousarray(witness, dtype=np.uint64)
+        if wit.size != 4 * shape.num_vars:
+            raise ValueError(f"{where}: the witness has {wit.size // 4} elements, the key takes {shape.num_vars}")
+        src = _ptr(wit)
+    pub = np.zeros((shape.num_inputs, 4), dtype=np.uint64)
+    return _proof(shape, True, src, wit, pub, blinders, link, challenges, where)
 
 
-def _witness_items(pk: ProvingKey, witness_list, blinders_list, link_hints: bool, want_challenges: bool, where: str):
-    """Checks a witness batch's arguments (ValueError) and builds its b200_witness_item array.  Returns (items, keep,
-    pub_inputs): keep[i] as `_prove_items` gives it, pub_inputs[i] the array item i's public inputs are written to."""
+def _witness_items(pk, witness_list, blinders_list, link_hints: bool, want_challenges: bool, where: str):
+    """A witness batch: (its b200_witness_item array, the `_Proof` of each item)."""
     witness_list, blinders_list = list(witness_list), list(blinders_list)
     if len(witness_list) != len(blinders_list):
         raise ValueError(f"{where}: {len(witness_list)} witness vectors and {len(blinders_list)} blinder vectors")
-    k, n = len(witness_list), pk.domain_size
-    items = (B200WitnessItem * max(1, k))()
-    keep, pubs = [], []
-    for i, (witness, blinders) in enumerate(zip(witness_list, blinders_list)):
-        wit, wit_ptr = _witness_arg(pk, witness, f"{where}: item {i}")
-        bl = np.ascontiguousarray(blinders, dtype=np.uint64)
-        if bl.size != 17 * 4:
-            raise ValueError(f"{where}: item {i} has {bl.size // 4} blinders, the prover draws 17")
-        proof = B200Proof()
-        link = np.zeros((n + 2, 4), dtype=np.uint64) if link_hints else None
-        ch = np.zeros((6, 4), dtype=np.uint64) if want_challenges else None
-        pub = np.zeros((pk.num_inputs, 4), dtype=np.uint64)
-        items[i] = B200WitnessItem(wit_ptr, _ptr(bl), C.cast(C.pointer(proof), C.c_void_p),
-                                   _ptr(link) if link is not None else None, _ptr(ch) if ch is not None else None,
-                                   _ptr(pub) if pub.size else None)
-        keep.append((wit, None, bl, proof, link, ch))
-        pubs.append(pub)
-    return items, keep, pubs
+    ps = [_witness_proof(pk, w, b, f"{where}: item {i}", link_hints, want_challenges)
+          for i, (w, b) in enumerate(zip(witness_list, blinders_list))]
+    return (B200WitnessItem * max(1, len(ps)))(*(p.item() for p in ps)), ps
 
 
-def _prove_items(pk: ProvingKey, wires_list, pub_inputs_list, blinders_list, link_hints: bool, want_challenges: bool):
-    """Checks a batch's arguments (ValueError) and builds its b200_prove_item array.  Returns (items, keep): keep[i] holds
-    the arrays item i points into, and its outputs (proof, link polynomial, challenges)."""
+def _prove_items(pk, wires_list, pub_inputs_list, blinders_list, link_hints: bool, want_challenges: bool,
+                 where: str = "prove_batch"):
+    """A batch of wire tables: (its b200_prove_item array, the `_Proof` of each item)."""
     wires_list, pub_inputs_list, blinders_list = list(wires_list), list(pub_inputs_list), list(blinders_list)
     k = len(wires_list)
     if len(pub_inputs_list) != k or len(blinders_list) != k:
-        raise ValueError(f"prove_batch: {k} wire tables, {len(pub_inputs_list)} public-input vectors and "
+        raise ValueError(f"{where}: {k} wire tables, {len(pub_inputs_list)} public-input vectors and "
                          f"{len(blinders_list)} blinder vectors: one of each per witness")
-    n = pk.domain_size
-    items = (B200ProveItem * max(1, k))()
-    keep = []
-    for i, (wires, pub_inputs, blinders) in enumerate(zip(wires_list, pub_inputs_list, blinders_list)):
-        if isinstance(wires, (int, np.integer)):
-            w, w_ptr = None, C.c_void_p(int(wires))
-        else:
-            w = np.ascontiguousarray(wires, dtype=np.uint64)
-            if w.size != 5 * n * 4:
-                raise ValueError(f"prove_batch: wire table {i} has {w.size // 4} elements, the key needs 5 x {n}")
-            w_ptr = _ptr(w)
-        pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64).reshape(-1, 4)
-        if pi.shape[0] != pk.num_inputs:
-            raise ValueError(f"prove_batch: item {i} has {pi.shape[0]} public inputs, the key takes {pk.num_inputs}")
-        bl = np.ascontiguousarray(blinders, dtype=np.uint64)
-        if bl.size != 17 * 4:
-            raise ValueError(f"prove_batch: item {i} has {bl.size // 4} blinders, the prover draws 17")
-        proof = B200Proof()
-        link = np.zeros((n + 2, 4), dtype=np.uint64) if link_hints else None
-        ch = np.zeros((6, 4), dtype=np.uint64) if want_challenges else None
-        items[i] = B200ProveItem(w_ptr, _ptr(pi) if pi.size else None, _ptr(bl), C.cast(C.pointer(proof), C.c_void_p),
-                                 _ptr(link) if link is not None else None, _ptr(ch) if ch is not None else None)
-        keep.append((w, pi, bl, proof, link, ch))
-    return items, keep
+    ps = [_table_proof(pk, w, pi, b, f"{where}: item {i}", link_hints, want_challenges)
+          for i, (w, pi, b) in enumerate(zip(wires_list, pub_inputs_list, blinders_list))]
+    return (B200ProveItem * max(1, k))(*(p.item() for p in ps)), ps
 
 
-def _batch_results(keep, statuses, link_hints: bool, want_challenges: bool):
-    proofs = [x[3] for x in keep]
-    st = [int(statuses[i]) for i in range(len(keep))]
-    hints = None
-    if link_hints:
-        hints = [LinkingHint(linking_wire_poly=x[4], linking_wire_comm=np.array(x[3].wires_poly_comms[0], dtype=np.uint64))
-                 if s == _lib.B200_OK else None for x, s in zip(keep, st)]
+def _batch_results(ps, statuses, link_hints: bool, want_challenges: bool):
+    st = [int(statuses[i]) for i in range(len(ps))]
+    hints = [p.hint() if s == _lib.B200_OK else None for p, s in zip(ps, st)] if link_hints else None
     if want_challenges:
-        return proofs, hints, st, [x[5] for x in keep]
-    return proofs, hints, st
+        return [p.proof for p in ps], hints, st, [p.challenges for p in ps]
+    return [p.proof for p in ps], hints, st
+
+
+def _link_hint(hint, where: str, name: str):
+    """(pointer, length, array or None, commitment) of `where`'s hint `name`: its polynomial is an array of (len, 4) limbs,
+    or (address, len) of one in device or pinned host memory; its commitment is 8 limbs (x || y)."""
+    poly = hint.linking_wire_poly
+    if isinstance(poly, tuple):
+        addr, n = poly
+        p, n, a = C.c_void_p(int(addr)), int(n), None
+    else:
+        a = np.ascontiguousarray(poly, dtype=np.uint64)
+        if a.size % 4:
+            raise ValueError(f"{where}'s {name} is not a vector of field elements (4 limbs each)")
+        a = a.reshape(-1, 4)
+        p, n = _ptr(a), a.shape[0]
+    c = np.ascontiguousarray(hint.linking_wire_comm, dtype=np.uint64).reshape(-1)
+    if c.size != 8:
+        raise ValueError(f"{where}'s {name} commitment must be 8 limbs (x || y), not {c.size}")
+    return p, n, a, c
+
+
+def _check_layout(lay: "GroupLayout", length: int, srs_len, where: str):
+    """`where`'s link group on polynomials of `length` coefficients, against an SRS of `srs_len` powers (None: not known
+    here)."""
+    if not 0 < lay.size < length:
+        raise ValueError(f"{where}'s group of {lay.size} roots does not fit polynomials of {length} coefficients "
+                         "(0 < size < length)")
+    if not 0 <= lay.alignment <= 28 or lay.offset < 0:
+        raise ValueError(f"{where} has alignment {lay.alignment} and offset {lay.offset} (0 <= alignment <= 28, offset >= 0)")
+    if srs_len is not None and length > srs_len:
+        raise ValueError(f"{where} has {length} coefficients, the SRS {srs_len} powers")
 
 
 def keccak256(data: bytes) -> bytes:
@@ -812,12 +863,9 @@ def plonk_last_timings(ctx: Context) -> dict:
 
 def prove_raw(ctx: Context, pk: ProvingKey, wires_ptr: int, pub_inputs: np.ndarray, blinders: np.ndarray) -> B200Proof:
     """prove with the wire table given by address (pinned host or device memory)."""
-    proof = B200Proof()
-    pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64)
-    bl = np.ascontiguousarray(blinders, dtype=np.uint64)
-    _lib.check(ctx._lib.b200_plonk_prove(ctx._h, pk._h, C.c_void_p(wires_ptr), _ptr(pi) if pi.size else None, _ptr(bl),
-                                         C.byref(proof), None, None))
-    return proof
+    p = _table_proof(pk, wires_ptr, pub_inputs, blinders, "prove_raw")
+    _lib.check(ctx._lib.b200_plonk_prove(ctx._h, pk._h, p.src, _opt(p.pub), _ptr(p.bl), C.byref(p.proof), None, None))
+    return p.proof
 
 
 class B200LinkProof(_lib.STRUCTS["b200_link_proof"]):
@@ -839,66 +887,36 @@ class GroupLayout:
 def link_proofs(ctx: Context, srs: Bases, hint_a: LinkingHint, hint_b: LinkingHint, layout: GroupLayout):
     """`PlonkKzgSnark::link_proofs::<SolidityTranscript>` (proof_linking/intent_only.rs:42-47).
     Returns (B200LinkProof, eta)."""
-    a1 = np.ascontiguousarray(hint_a.linking_wire_poly, dtype=np.uint64).reshape(-1, 4)
-    a2 = np.ascontiguousarray(hint_b.linking_wire_poly, dtype=np.uint64).reshape(-1, 4)
-    c1 = np.ascontiguousarray(hint_a.linking_wire_comm, dtype=np.uint64)
-    c2 = np.ascontiguousarray(hint_b.linking_wire_comm, dtype=np.uint64)
-    proof = B200LinkProof()
-    eta = np.zeros(4, dtype=np.uint64)
-    _lib.check(ctx._lib.b200_plonk_link(ctx._h, srs._h, _ptr(a1), a1.shape[0], _ptr(a2), a2.shape[0], _ptr(c1), _ptr(c2),
-                                        layout.alignment, layout.offset, layout.size, C.byref(proof), _ptr(eta)))
-    return proof, eta
+    it, keep = _link_item(hint_a, hint_b, layout, len(srs), "link_proofs: the link")
+    _lib.check(ctx._lib.b200_plonk_link(ctx._h, srs._h, it.a1, it.len1, it.a2, it.len2, it.comm1, it.comm2, it.alignment,
+                                        it.offset, it.size, it.proof, it.eta))
+    return keep[4], keep[5]
 
 
 B200LinkItem = _lib.STRUCTS["b200_link_item"]  # one link proof of a batch
 
 
-def _link_poly(poly, where: str):
-    """(pointer, length, array or None) of a hint's polynomial: an array of (len, 4) limbs, or (address, len) of one in
-    device or pinned host memory"""
-    if isinstance(poly, tuple):
-        addr, n = poly
-        return C.c_void_p(int(addr)), int(n), None
-    a = np.ascontiguousarray(poly, dtype=np.uint64)
-    if a.ndim != 2 or a.shape[1] != 4:
-        a = a.reshape(-1, 4) if a.size % 4 == 0 else None
-    if a is None:
-        raise ValueError(f"link_proofs_batch: {where} is not a vector of field elements (4 limbs each)")
-    return _ptr(a), a.shape[0], a
+def _link_item(hint_a, hint_b, lay, srs_len: int, where: str):
+    """One link proof of hint_a to hint_b on `lay`, checked: (its b200_link_item, (a1, a2, c1, c2, proof, eta)): the
+    arrays the item points into, then the buffers it writes."""
+    p1, n1, a1, c1 = _link_hint(hint_a, where, "hint_a")
+    p2, n2, a2, c2 = _link_hint(hint_b, where, "hint_b")
+    _check_layout(lay, max(n1, n2), srs_len, where)
+    proof, eta = B200LinkProof(), np.zeros(4, dtype=np.uint64)
+    item = B200LinkItem(p1, n1, p2, n2, _ptr(c1), _ptr(c2), lay.alignment, lay.offset, lay.size,
+                        C.cast(C.pointer(proof), C.c_void_p), _ptr(eta))
+    return item, (a1, a2, c1, c2, proof, eta)
 
 
-def _link_items(srs: Bases, triples):
-    """Checks a link batch's arguments (ValueError) and builds its b200_link_item array.  Returns (items, keep): keep[i]
-    holds the arrays item i points into, and its outputs (proof, eta)."""
-    triples = list(triples)
-    srs_len = len(srs)
-    items = (B200LinkItem * max(1, len(triples)))()
-    keep = []
+def _link_items(srs: Bases, triples, where: str = "link_proofs_batch"):
+    """A link batch: (its b200_link_item array, each item's arrays and buffers as `_link_item` gives them)."""
+    triples, srs_len = list(triples), len(srs)
+    built = []
     for i, t in enumerate(triples):
         if len(t) != 3:
-            raise ValueError(f"link_proofs_batch: item {i} is not a (hint_a, hint_b, layout) triple")
-        hint_a, hint_b, lay = t
-        p1, n1, a1 = _link_poly(hint_a.linking_wire_poly, f"item {i}'s first polynomial")
-        p2, n2, a2 = _link_poly(hint_b.linking_wire_poly, f"item {i}'s second polynomial")
-        c1 = np.ascontiguousarray(hint_a.linking_wire_comm, dtype=np.uint64).reshape(-1)
-        c2 = np.ascontiguousarray(hint_b.linking_wire_comm, dtype=np.uint64).reshape(-1)
-        if c1.size != 8 or c2.size != 8:
-            raise ValueError(f"link_proofs_batch: item {i}'s commitments must be 8 limbs (x || y) each")
-        n = max(n1, n2)
-        if not 0 < lay.size < n:
-            raise ValueError(f"link_proofs_batch: item {i}'s group of {lay.size} roots does not fit polynomials of {n} "
-                             "coefficients (0 < size < max(len1, len2))")
-        if not 0 <= lay.alignment <= 28 or lay.offset < 0:
-            raise ValueError(f"link_proofs_batch: item {i} has alignment {lay.alignment} and offset {lay.offset} "
-                             "(0 <= alignment <= 28, offset >= 0)")
-        if n > srs_len:
-            raise ValueError(f"link_proofs_batch: item {i} has {n} coefficients, the SRS {srs_len} powers")
-        proof = B200LinkProof()
-        eta = np.zeros(4, dtype=np.uint64)
-        items[i] = B200LinkItem(p1, n1, p2, n2, _ptr(c1), _ptr(c2), lay.alignment, lay.offset, lay.size,
-                                C.cast(C.pointer(proof), C.c_void_p), _ptr(eta))
-        keep.append((a1, a2, c1, c2, proof, eta))
-    return items, keep
+            raise ValueError(f"{where}: item {i} is not a (hint_a, hint_b, layout) triple")
+        built.append(_link_item(*t, srs_len, f"{where}: item {i}"))
+    return (B200LinkItem * max(1, len(built)))(*(it for it, _ in built)), [keep for _, keep in built]
 
 
 def _link_batch_results(keep, statuses):
@@ -912,7 +930,7 @@ def link_proofs_batch(ctx: Context, srs: Bases, triples):
     (proofs, etas, statuses): item i's proof and eta equal `link_proofs` of the same triple; statuses[i] is 0, or -7
     (B200_ERR_UNSATISFIED) when the two polynomials differ on the group, in which case the proof is zeroed and the eta is
     None.  Argument errors raise ValueError before any device work; other failures raise B200Error."""
-    items, keep = _link_items(srs, triples)
+    items, keep = _link_items(srs, triples, "link_proofs_batch")
     k = len(keep)
     statuses = (C.c_int * max(1, k))()
     rc = ctx._lib.b200_plonk_link_batch(ctx._h, srs._h, items, k, statuses)
@@ -922,61 +940,6 @@ def link_proofs_batch(ctx: Context, srs: Bases, triples):
 
 
 SettlementLink = _lib.STRUCTS["b200_settlement_link"]  # one stored hint of a settlement and its group
-
-
-def _wires_arg(n: int, wires, where: str):
-    """A 5 x n wire table as (array kept alive or None, pointer): an array, or an address."""
-    if isinstance(wires, (int, np.integer)):
-        return None, C.c_void_p(int(wires))
-    w = np.ascontiguousarray(wires, dtype=np.uint64)
-    if w.size != 5 * n * 4:
-        raise ProverError(_lib.B200_ERR_INVALID, f"{where}: the wire table has {w.size // 4} elements, the key needs 5 x {n}")
-    return w, _ptr(w)
-
-
-def _settlement_inputs(num_inputs: int, pub_inputs, blinders, where: str):
-    """The public inputs and the 17 blinders of a settlement, checked (ProverError)."""
-    pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64).reshape(-1, 4)
-    if pi.shape[0] != num_inputs:
-        raise ProverError(_lib.B200_ERR_INVALID, f"{where}: {pi.shape[0]} public inputs for a key with {num_inputs}")
-    bl = np.ascontiguousarray(blinders, dtype=np.uint64)
-    if bl.size != 17 * 4:
-        raise ProverError(_lib.B200_ERR_INVALID, f"{where}: {bl.size // 4} blinders, the prover draws 17")
-    return pi, bl
-
-
-def _settlement_links(links, srs_len, n: int, where: str):
-    """Checks a settlement's links = [(LinkingHint, GroupLayout)] against a key of domain size n (ProverError naming the
-    link; srs_len None skips the SRS length check) and builds their b200_settlement_link array.  Returns (array, arrays
-    to keep alive, link proofs)."""
-    links = list(links)
-    arr = (SettlementLink * max(1, len(links)))()
-    held, out = [], []
-    for i, t in enumerate(links):
-        if len(t) != 2:
-            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: link {i} is not a (hint, layout) pair")
-        hint, lay = t
-        try:
-            p, ln, a = _link_poly(hint.linking_wire_poly, f"link {i}'s hint")
-        except ValueError as e:
-            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: {e}")
-        c = np.ascontiguousarray(hint.linking_wire_comm, dtype=np.uint64).reshape(-1)
-        if c.size != 8:
-            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: link {i}'s hint commitment must be 8 limbs (x || y)")
-        m = max(ln, n + 2)
-        if not 0 < lay.size < m:
-            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: link {i}'s group of {lay.size} roots does not fit "
-                                                     f"polynomials of {m} coefficients")
-        if not 0 <= lay.alignment <= 28 or lay.offset < 0:
-            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: link {i} has alignment {lay.alignment} and offset "
-                                                     f"{lay.offset} (0 <= alignment <= 28, offset >= 0)")
-        if srs_len is not None and m > srs_len:
-            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: link {i} has {m} coefficients, the SRS {srs_len} powers")
-        lp = B200LinkProof()
-        arr[i] = SettlementLink(p, ln, _ptr(c), lay.alignment, lay.offset, lay.size, C.cast(C.pointer(lp), C.c_void_p), None)
-        held += [a, c, hint]
-        out.append(lp)
-    return arr, held, out
 
 
 def compute_poseidon_hash_batch(ctx: Context, values: np.ndarray) -> np.ndarray:
@@ -1035,12 +998,12 @@ BundleWitness = _lib.STRUCTS["b200_bundle_witness"]
 
 def _bundle_links(links, n_proofs: int, where: str):
     """The b200_bundle_link array of a bundle and the link proofs it writes into; a link naming a proof outside the
-    bundle raises ProverError before any device call."""
+    bundle raises ValueError before any device call."""
     arr_l = (BundleLink * max(len(links), 1))()
     out_links = []
     for i, (a, b, lay) in enumerate(links):
         if not (0 <= a < n_proofs and 0 <= b < n_proofs):
-            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: link {i} names proof ({a}, {b}) of a bundle of {n_proofs}")
+            raise ValueError(f"{where}: link {i} names proof ({a}, {b}) of a bundle of {n_proofs}")
         lp = B200LinkProof()
         arr_l[i].a, arr_l[i].b, arr_l[i].alignment, arr_l[i].offset, arr_l[i].size = a, b, lay.alignment, lay.offset, lay.size
         arr_l[i].proof = C.cast(C.pointer(lp), C.c_void_p)
@@ -1048,69 +1011,28 @@ def _bundle_links(links, n_proofs: int, where: str):
     return arr_l, out_links
 
 
-def _bundle_witness_arrays(proofs, links, resolve, where: str):
-    """Arrays of a witness bundle: `proofs` = [(key, witness, blinders)], resolve(key) -> (C handle, the key's shape:
-    domain_size, num_inputs, num_vars).  Blinder lengths, keys without wiring, witness lengths and link indices are
-    checked here (ProverError) before any device call.  Returns (b200_bundle_witness array, link array, objects to keep
-    alive, (proofs, link polys, link proofs, pub_inputs) the jobs write into)."""
-    arr_p = (BundleWitness * max(len(proofs), 1))()
-    keep, out_proofs, out_polys, out_pubs = [], [], [], []
-    for i, (key, witness, blinders) in enumerate(proofs):
+@_prover_errors
+def _bundle_job(proofs, links, resolve, build, struct, where: str):
+    """A bundle: `proofs` = [(key, *inputs)], each proof made by build(key's shape, *inputs) (`_table_proof` or
+    `_witness_proof`) into a `struct` entry; resolve(key) -> (C handle, shape).  Returns (entry array, link array, what the
+    job reads, what `wait` returns: ([proofs], [link polys], [link proofs]), and [pub_inputs] for witnesses)."""
+    ps, entries = [], []
+    for i, (key, *inputs) in enumerate(proofs):
         h, shape = resolve(key)
-        if shape.num_vars == 0:
-            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: the key of proof {i} holds no wiring (made by preprocess)")
-        try:
-            wit, wit_ptr = _witness_arg(shape, witness, f"{where}: proof {i}")
-        except ValueError as e:
-            raise ProverError(_lib.B200_ERR_INVALID, str(e))
-        bl = np.ascontiguousarray(blinders, dtype=np.uint64)
-        if bl.size != 4 * 17:
-            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: proof {i} has {bl.size // 4} blinders, the prover draws 17")
-        proof = B200Proof()
-        poly = np.zeros((shape.domain_size + 2, 4), dtype=np.uint64)
-        pub = np.zeros((shape.num_inputs, 4), dtype=np.uint64)
-        arr_p[i].pk, arr_p[i].witness, arr_p[i].blinders = h, wit_ptr, _ptr(bl)
-        arr_p[i].proof, arr_p[i].link_poly = C.cast(C.pointer(proof), C.c_void_p), _ptr(poly)
-        arr_p[i].pub_inputs_out = _ptr(pub) if pub.size else None
-        keep += [wit, bl, key]
-        out_proofs.append(proof)
-        out_polys.append(poly)
-        out_pubs.append(pub)
-    arr_l, out_links = _bundle_links(links, len(proofs), where)
-    return arr_p, arr_l, keep, (out_proofs, out_polys, out_links, out_pubs)
-
-
-def _bundle_table_arrays(proofs, links, resolve, where: str):
-    """`_bundle_witness_arrays` for a bundle of wire tables: `proofs` = [(key, wires_ptr, pub_inputs, blinders)].
-    Returns (b200_bundle_proof array, link array, objects to keep alive, (proofs, link polys, link proofs))."""
-    arr_p = (BundleProof * max(len(proofs), 1))()
-    keep, out_proofs, out_polys = [], [], []
-    for i, (key, wires_ptr, pub_inputs, blinders) in enumerate(proofs):
-        h, shape = resolve(key)
-        pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64)
-        bl = np.ascontiguousarray(blinders, dtype=np.uint64)
-        if pi.size != 4 * shape.num_inputs or bl.size != 4 * 17:
-            raise ProverError(_lib.B200_ERR_INVALID, f"{where}: public inputs / blinders do not match the key")
-        proof = B200Proof()
-        poly = np.zeros((shape.domain_size + 2, 4), dtype=np.uint64)
-        arr_p[i].pk, arr_p[i].wires = h, C.c_void_p(wires_ptr)
-        arr_p[i].pub_inputs = pi.ctypes.data_as(C.c_void_p) if pi.size else None
-        arr_p[i].num_inputs, arr_p[i].blinders = pi.size // 4, bl.ctypes.data_as(C.c_void_p)
-        arr_p[i].proof, arr_p[i].link_poly = C.cast(C.pointer(proof), C.c_void_p), poly.ctypes.data_as(C.c_void_p)
-        keep += [pi, bl, key]
-        out_proofs.append(proof)
-        out_polys.append(poly)
-    arr_l, out_links = _bundle_links(links, len(proofs), where)
-    return arr_p, arr_l, keep, (out_proofs, out_polys, out_links)
-
-
+        ps.append(build(shape, *inputs, f"{where}: proof {i}", link=True))
+        entries.append(ps[-1].entry(h))
+    arr_l, out_links = _bundle_links(links, len(ps), where)
+    out = ([p.proof for p in ps], [p.link for p in ps], out_links)
+    if struct is BundleWitness:
+        out += ([p.pub for p in ps],)
+    return (struct * max(1, len(ps)))(*entries), arr_l, (ps, [p[0] for p in proofs]), out
 
 
 # ---- queued jobs of a pool or a box --------------------------------------------------------------------------------
 # Each builder checks one job kind's arguments (ProverError or ValueError, before any library call) and returns
 # (args, finish, held): the C arguments after the pool or box handle and, where the entry takes them, the SRS and the key
-# handle; finish(rc), which turns the job's status into what `wait` returns; and the objects the job reads until then.  A
-# pool and a box submit the same job through their own entry point.
+# handle (a single proof's args start at its key handle); finish(rc), which turns the job's status into what `wait`
+# returns; and the objects the job reads until then.  A pool and a box submit the same job through their own entry point.
 
 def _finish(results, batch: bool = False):
     """finish(rc) of a job: raises for a failed job, else returns results().  A batch job (`batch`) reports an unsatisfied
@@ -1122,67 +1044,44 @@ def _finish(results, batch: bool = False):
     return finish
 
 
-def _prove_job(shape, wires_ptr: int, pub_inputs, blinders, with_link_poly: bool, where: str):
-    """One proof of a wire table at `wires_ptr`; `wait` returns the proof, or (proof, link_poly) with `with_link_poly`."""
-    pi = np.ascontiguousarray(pub_inputs, dtype=np.uint64)
-    bl = np.ascontiguousarray(blinders, dtype=np.uint64)
-    if pi.size != 4 * shape.num_inputs:
-        raise ProverError(_lib.B200_ERR_INVALID, f"{where}: {pi.size // 4} public inputs for a key with {shape.num_inputs}")
-    if bl.size != 4 * 17:
-        raise ProverError(_lib.B200_ERR_INVALID, f"{where}: blinders must be 17 Fr elements")
-    proof = B200Proof()
-    link = np.zeros((shape.domain_size + 2, 4), dtype=np.uint64) if with_link_poly else None
-    args = (C.c_void_p(wires_ptr), _ptr(pi) if pi.size else None, pi.size // 4, _ptr(bl), C.byref(proof),
-            _ptr(link) if link is not None else None)
-    return args, _finish(lambda: proof if link is None else (proof, link)), ()
+@_prover_errors
+def _prove_job(h, shape, build, *inputs, with_link_poly: bool, where: str):
+    """One proof, made by build(shape, *inputs) (`_table_proof` or `_witness_proof`).  args are its pool entry's fields, key
+    handle `h` first: the arguments of the single-proof submits.  `wait` returns the proof, or (proof, link_poly) with
+    `with_link_poly`, with a witness proof's pub_inputs after them."""
+    p = build(shape, *inputs, where, link=with_link_poly)
+    e = p.entry(h)
+    out = (p.proof,) + ((p.link,) if with_link_poly else ()) + ((p.pub,) if p.witness else ())
+    return tuple(getattr(e, f) for f, _ in e._fields_), _finish(lambda: out if len(out) > 1 else out[0]), p
 
 
-def _prove_witness_job(shape, witness, blinders, with_link_poly: bool, where: str):
-    """One proof of a witness vector; `wait` returns (proof, pub_inputs), or (proof, link_poly, pub_inputs) with
-    `with_link_poly`."""
-    try:
-        wit, wit_ptr = _witness_arg(shape, witness, where)
-    except ValueError as e:
-        raise ProverError(_lib.B200_ERR_INVALID, str(e))
-    bl = np.ascontiguousarray(blinders, dtype=np.uint64)
-    if bl.size != 4 * 17:
-        raise ProverError(_lib.B200_ERR_INVALID, f"{where}: blinders must be 17 Fr elements")
-    proof = B200Proof()
-    pub = np.zeros((shape.num_inputs, 4), dtype=np.uint64)
-    link = np.zeros((shape.domain_size + 2, 4), dtype=np.uint64) if with_link_poly else None
-    args = (wit_ptr, _ptr(bl), C.byref(proof), _ptr(link) if link is not None else None, _ptr(pub) if pub.size else None)
-    return args, _finish(lambda: (proof, pub) if link is None else (proof, link, pub)), wit
+SettlementLink = _lib.STRUCTS["b200_settlement_link"]  # one stored hint of a settlement and its group
 
 
-def _settlement_job(h, shape, srs_len, wires, pub_inputs, blinders, links, where: str):
-    """A settlement of a wire table, the key's handle `h` in its proof entry; args start at the proof entry.  `wait`
-    returns (proof, link_proofs, statuses) like `PlonkKzgSnark.prove_settlement`."""
-    w, w_ptr = _wires_arg(shape.domain_size, wires, where)
-    pi, bl = _settlement_inputs(shape.num_inputs, pub_inputs, blinders, where)
-    arr, held, out = _settlement_links(links, srs_len, shape.domain_size, where)
-    proof = B200Proof()
-    item = BundleProof(h, w_ptr, _ptr(pi) if pi.size else None, pi.shape[0], _ptr(bl), C.cast(C.pointer(proof), C.c_void_p),
-                       None)
+@_prover_errors
+def _settlement_job(h, shape, srs_len, links, build, *inputs, where: str):
+    """A settlement: the statement's proof made by build(shape, *inputs) (`_table_proof` or `_witness_proof`) in its pool
+    entry, key handle `h`, and links = [(LinkingHint, GroupLayout)] from stored hints to the statement's own (srs_len None:
+    the SRS length is not known here).  args start at a pointer to the entry.  `wait` returns (proof, link_proofs,
+    statuses), with a witness settlement's pub_inputs after them, like `PlonkKzgSnark.prove_settlement[_witness]`."""
+    p = build(shape, *inputs, where)
+    links = list(links)
+    arr = (SettlementLink * max(1, len(links)))()
+    held, out = [], []
+    for i, t in enumerate(links):
+        if len(t) != 2:
+            raise ValueError(f"{where}: link {i} is not a (hint, layout) pair")
+        hint, lay = t
+        ptr, n, a, c = _link_hint(hint, f"{where}: link {i}", "hint")
+        _check_layout(lay, max(n, shape.domain_size + 2), srs_len, f"{where}: link {i}")
+        lp = B200LinkProof()
+        arr[i] = SettlementLink(ptr, n, _ptr(c), lay.alignment, lay.offset, lay.size, C.cast(C.pointer(lp), C.c_void_p), None)
+        held += [a, c, hint]
+        out.append(lp)
     st = (C.c_int * (len(out) + 1))()
-    return (C.byref(item), arr, len(out), st), _finish(lambda: (proof, out, list(st)), batch=True), (w, held)
-
-
-def _settlement_witness_job(h, shape, srs_len, witness, blinders, links, where: str):
-    """`_settlement_job` from the settlement's witness vector; `wait` returns (proof, link_proofs, statuses,
-    pub_inputs) like `PlonkKzgSnark.prove_settlement_witness`."""
-    if shape.num_vars == 0:
-        raise ProverError(_lib.B200_ERR_INVALID, f"{where}: the key holds no wiring (made by preprocess)")
-    try:
-        wit, wit_ptr = _witness_arg(shape, witness, where)
-    except ValueError as e:
-        raise ProverError(_lib.B200_ERR_INVALID, str(e))
-    _, bl = _settlement_inputs(0, (), blinders, where)
-    arr, held, out = _settlement_links(links, srs_len, shape.domain_size, where)
-    proof = B200Proof()
-    pub = np.zeros((shape.num_inputs, 4), dtype=np.uint64)
-    item = BundleWitness(h, wit_ptr, _ptr(bl), C.cast(C.pointer(proof), C.c_void_p), None, _ptr(pub) if pub.size else None)
-    st = (C.c_int * (len(out) + 1))()
-    return (C.byref(item), arr, len(out), st), _finish(lambda: (proof, out, list(st), pub), batch=True), (wit, held)
+    pub = (p.pub,) if p.witness else ()
+    finish = _finish(lambda: (p.proof, out, list(st)) + pub, batch=True)
+    return (C.pointer(p.entry(h)), arr, len(out), st), finish, (p, held)
 
 
 def _verify_job(vks, pub_inputs, proofs, links, combined: bool, g2):
@@ -1315,43 +1214,40 @@ class ProverPool(_Tickets):
         """Queue one proof; returns the ticket.  `wires_ptr`: address of the 5 x n wire table (pinned host
         or device memory), which the caller keeps valid until `wait(ticket)` returns (pass the owning
         object as `keep` to let the pool hold a reference)."""
-        args, finish, held = _prove_job(pk, wires_ptr, pub_inputs, blinders, with_link_poly, "submit_prove")
-        return self._submit(self._lib.b200_pool_submit_prove, (pk._h, *args), finish, (held, keep, pk))
+        args, finish, p = _prove_job(pk._h, pk, _table_proof, wires_ptr, pub_inputs, blinders,
+                                     with_link_poly=with_link_poly, where="submit_prove")
+        return self._submit(self._lib.b200_pool_submit_prove, args, finish, (p, keep, pk))
 
     def submit_prove_witness(self, pk: "ProvingKey", witness, blinders: np.ndarray, with_link_poly: bool = False,
                              keep=None) -> int:
         """Queue one proof from a witness vector (array, or address in pinned host or device memory kept valid until
         `wait(ticket)` returns) of a key made by `preprocess_wiring`; returns the ticket.  `wait(ticket)` returns
         (proof, pub_inputs), or (proof, link_poly, pub_inputs) with `with_link_poly`."""
-        args, finish, held = _prove_witness_job(pk, witness, blinders, with_link_poly, "submit_prove_witness")
-        return self._submit(self._lib.b200_pool_submit_prove_witness, (pk._h, *args), finish, (held, keep, pk))
+        args, finish, p = _prove_job(pk._h, pk, _witness_proof, witness, blinders, with_link_poly=with_link_poly,
+                                     where="submit_prove_witness")
+        return self._submit(self._lib.b200_pool_submit_prove_witness, args, finish, (p, keep, pk))
 
     def submit_prove_batch(self, pk: "ProvingKey", wires_list, pub_inputs_list, blinders_list, link_hints: bool = False,
                            keep=None) -> int:
         """Queue one `b200_plonk_prove_batch` as a single job on one worker; returns the ticket.  Arguments as for
         `PlonkKzgSnark.prove_batch`; wire tables given by address stay owned by the caller until `wait(ticket)` returns
         (pass their owners as `keep`).  `wait(ticket)` returns (proofs, hints, statuses) like `prove_batch`."""
-        items, held = _prove_items(pk, wires_list, pub_inputs_list, blinders_list, link_hints, False)
-        statuses = (C.c_int * max(1, len(held)))()
-        finish = _finish(lambda: _batch_results(held, statuses, link_hints, False), batch=True)
-        return self._submit(self._lib.b200_pool_submit_prove_batch, (pk._h, items, len(held), statuses), finish,
-                            (held, keep, pk))
+        items, ps = _prove_items(pk, wires_list, pub_inputs_list, blinders_list, link_hints, False, "submit_prove_batch")
+        statuses = (C.c_int * max(1, len(ps)))()
+        finish = _finish(lambda: _batch_results(ps, statuses, link_hints, False), batch=True)
+        return self._submit(self._lib.b200_pool_submit_prove_batch, (pk._h, items, len(ps), statuses), finish,
+                            (ps, keep, pk))
 
     def submit_link(self, srs: "Bases", hint_a: "LinkingHint", hint_b: "LinkingHint", layout: "GroupLayout") -> int:
-        a1 = np.ascontiguousarray(hint_a.linking_wire_poly, dtype=np.uint64).reshape(-1, 4)
-        a2 = np.ascontiguousarray(hint_b.linking_wire_poly, dtype=np.uint64).reshape(-1, 4)
-        c1 = np.ascontiguousarray(hint_a.linking_wire_comm, dtype=np.uint64)
-        c2 = np.ascontiguousarray(hint_b.linking_wire_comm, dtype=np.uint64)
-        proof = B200LinkProof()
-        args = (srs._h, _ptr(a1), a1.shape[0], _ptr(a2), a2.shape[0], _ptr(c1), _ptr(c2), layout.alignment, layout.offset,
-                layout.size, C.byref(proof))
-        return self._submit(self._lib.b200_pool_submit_link, args, _finish(lambda: proof), (a1, a2, srs))
+        it, keep = _link_item(hint_a, hint_b, layout, len(srs), "submit_link: the link")
+        args = (srs._h, it.a1, it.len1, it.a2, it.len2, it.comm1, it.comm2, it.alignment, it.offset, it.size, it.proof)
+        return self._submit(self._lib.b200_pool_submit_link, args, _finish(lambda: keep[4]), (keep, srs))
 
     def submit_link_batch(self, srs: "Bases", triples, keep=None) -> int:
         """Queue one `b200_plonk_link_batch` as a single job on one worker; returns the ticket.  Arguments as for
         `link_proofs_batch`; polynomials given by address stay owned by the caller until `wait(ticket)` returns (pass
         their owners as `keep`).  `wait(ticket)` returns (proofs, etas, statuses) like `link_proofs_batch`."""
-        items, held = _link_items(srs, triples)
+        items, held = _link_items(srs, triples, "submit_link_batch")
         statuses = (C.c_int * max(1, len(held)))()
         finish = _finish(lambda: _link_batch_results(held, statuses), batch=True)
         return self._submit(self._lib.b200_pool_submit_link_batch, (srs._h, items, len(held), statuses), finish,
@@ -1362,7 +1258,7 @@ class ProverPool(_Tickets):
         blinders)], `links` = [(a, b, GroupLayout)] — link proof between the hints of proofs a and b, forked inside the
         pool once every proof is in (native_proof_manager.rs:526-584, 726-782).  `wait(ticket)` returns
         ([B200Proof], [link polys], [B200LinkProof])."""
-        arr_p, arr_l, keep, out = _bundle_table_arrays(proofs, links, self._resolve, "submit_bundle")
+        arr_p, arr_l, keep, out = _bundle_job(proofs, links, self._resolve, _table_proof, BundleProof, "submit_bundle")
         return self._submit(self._lib.b200_pool_submit_bundle, (srs._h, arr_p, len(proofs), arr_l, len(links)),
                             _finish(lambda: out), (keep, srs))
 
@@ -1371,7 +1267,8 @@ class ProverPool(_Tickets):
         [(pk, witness, blinders)], pk a key made by `preprocess_wiring`, witness an array or an address (pinned host or
         device memory, kept valid until `wait(ticket)` returns) as `submit_prove_witness` takes.  `wait(ticket)` returns
         ([B200Proof], [link polys], [B200LinkProof], [pub_inputs])."""
-        arr_p, arr_l, keep, out = _bundle_witness_arrays(proofs, links, self._resolve, "submit_bundle_witness")
+        arr_p, arr_l, keep, out = _bundle_job(proofs, links, self._resolve, _witness_proof, BundleWitness,
+                                              "submit_bundle_witness")
         args = (srs._h if srs is not None else None, arr_p, len(proofs), arr_l, len(links))
         return self._submit(self._lib.b200_pool_submit_bundle_witness, args, _finish(lambda: out), (keep, srs))
 
@@ -1381,30 +1278,28 @@ class ProverPool(_Tickets):
         for `PlonkKzgSnark.prove_witness_batch`; witnesses given by address stay owned by the caller until `wait(ticket)`
         returns (pass their owners as `keep`).  `wait(ticket)` returns (proofs, hints, statuses, pub_inputs) like
         `prove_witness_batch`."""
-        if pk.num_vars == 0:
-            raise ProverError(_lib.B200_ERR_INVALID, "submit_prove_witness_batch: the key holds no wiring (made by preprocess)")
-        try:
-            items, held, pubs = _witness_items(pk, witnesses, blinders_list, link_hints, False, "submit_prove_witness_batch")
-        except ValueError as e:
-            raise ProverError(_lib.B200_ERR_INVALID, str(e))
-        statuses = (C.c_int * max(1, len(held)))()
-        finish = _finish(lambda: _batch_results(held, statuses, link_hints, False) + (pubs,), batch=True)
-        return self._submit(self._lib.b200_pool_submit_prove_witness_batch, (pk._h, items, len(held), statuses), finish,
-                            (held, keep, pk))
+        items, ps = _prover_errors(_witness_items)(pk, witnesses, blinders_list, link_hints, False,
+                                                   "submit_prove_witness_batch")
+        statuses = (C.c_int * max(1, len(ps)))()
+        finish = _finish(lambda: _batch_results(ps, statuses, link_hints, False) + ([p.pub for p in ps],), batch=True)
+        return self._submit(self._lib.b200_pool_submit_prove_witness_batch, (pk._h, items, len(ps), statuses), finish,
+                            (ps, keep, pk))
 
     def submit_settlement(self, srs: "Bases", pk: "ProvingKey", wires, pub_inputs, blinders, links, keep=None) -> int:
         """Queue one `PlonkKzgSnark.prove_settlement` as ONE job on one worker (`b200_pool_submit_settlement`); returns the
         ticket.  Arguments as `prove_settlement` takes them; a wire table or hint given by address stays owned by the
         caller until `wait(ticket)` returns (pass its owner as `keep`).  `wait(ticket)` returns (proof, link_proofs,
         statuses) like `prove_settlement`."""
-        args, finish, held = _settlement_job(pk._h, pk, len(srs), wires, pub_inputs, blinders, links, "submit_settlement")
+        args, finish, held = _settlement_job(pk._h, pk, len(srs), links, _table_proof, wires, pub_inputs, blinders,
+                                             where="submit_settlement")
         return self._submit(self._lib.b200_pool_submit_settlement, (srs._h, *args), finish, (held, keep, pk, srs))
 
     def submit_settlement_witness(self, srs: "Bases", pk: "ProvingKey", witness, blinders, links, keep=None) -> int:
         """`submit_settlement` from the settlement's witness vector (`b200_pool_submit_settlement_witness`), arguments as
         `PlonkKzgSnark.prove_settlement_witness` takes them.  `wait(ticket)` returns (proof, link_proofs, statuses,
         pub_inputs)."""
-        args, finish, held = _settlement_witness_job(pk._h, pk, len(srs), witness, blinders, links, "submit_settlement_witness")
+        args, finish, held = _settlement_job(pk._h, pk, len(srs), links, _witness_proof, witness, blinders,
+                                             where="submit_settlement_witness")
         return self._submit(self._lib.b200_pool_submit_settlement_witness, (srs._h, *args), finish, (held, keep, pk, srs))
 
     def submit_verify(self, vks, pub_inputs, proofs, links=(), combined: bool = False, g2=None) -> int:
@@ -1525,21 +1420,23 @@ class ProverBox(_Tickets):
         """`ProverPool.submit_prove` on the least-loaded device (`b200_box_submit_prove`).  `wait(ticket)` returns the
         proof, or (proof, link_poly) with `with_link_poly`."""
         h, shape = self._resolve(pk)
-        args, finish, held = _prove_job(shape, wires_ptr, pub_inputs, blinders, with_link_poly, "box.submit_prove")
-        return self._submit(self._lib.b200_box_submit_prove, (h, *args), finish, (held, keep))
+        args, finish, p = _prove_job(h, shape, _table_proof, wires_ptr, pub_inputs, blinders,
+                                     with_link_poly=with_link_poly, where="box.submit_prove")
+        return self._submit(self._lib.b200_box_submit_prove, args, finish, (p, keep))
 
     def submit_prove_witness(self, pk, witness, blinders: np.ndarray, with_link_poly: bool = False, keep=None) -> int:
         """`ProverPool.submit_prove_witness` on the box (`b200_box_submit_prove_witness`): a witness in device memory runs
         on its own device, any other on the least-loaded one.  `wait(ticket)` returns (proof, pub_inputs), or (proof,
         link_poly, pub_inputs) with `with_link_poly`."""
         h, shape = self._resolve(pk)
-        args, finish, held = _prove_witness_job(shape, witness, blinders, with_link_poly, "box.submit_prove_witness")
-        return self._submit(self._lib.b200_box_submit_prove_witness, (h, *args), finish, (held, keep))
+        args, finish, p = _prove_job(h, shape, _witness_proof, witness, blinders, with_link_poly=with_link_poly,
+                                     where="box.submit_prove_witness")
+        return self._submit(self._lib.b200_box_submit_prove_witness, args, finish, (p, keep))
 
     def submit_bundle(self, srs, proofs, links) -> int:
         """`ProverPool.submit_bundle` on the least-loaded device (`b200_box_submit_bundle`): `proofs` = [(box key,
         wires_ptr, pub_inputs, blinders)].  `wait(ticket)` returns ([B200Proof], [link polys], [B200LinkProof])."""
-        arr_p, arr_l, keep, out = _bundle_table_arrays(proofs, links, self._resolve, "box.submit_bundle")
+        arr_p, arr_l, keep, out = _bundle_job(proofs, links, self._resolve, _table_proof, BundleProof, "box.submit_bundle")
         pks = (C.c_void_p * max(len(proofs), 1))(*[p[0] for p in proofs])
         return self._submit(self._lib.b200_box_submit_bundle, (srs, pks, arr_p, len(proofs), arr_l, len(links)),
                             _finish(lambda: out), keep)
@@ -1548,7 +1445,8 @@ class ProverBox(_Tickets):
         """`ProverPool.submit_bundle_witness` on one device of the box (`b200_box_submit_bundle_witness`): `proofs` = [(box
         key, witness, blinders)]; device-memory witnesses pin the bundle to their device (all on one).  `wait(ticket)`
         returns ([B200Proof], [link polys], [B200LinkProof], [pub_inputs])."""
-        arr_p, arr_l, keep, out = _bundle_witness_arrays(proofs, links, self._resolve, "box.submit_bundle_witness")
+        arr_p, arr_l, keep, out = _bundle_job(proofs, links, self._resolve, _witness_proof, BundleWitness,
+                                              "box.submit_bundle_witness")
         pks = (C.c_void_p * max(len(proofs), 1))(*[p[0] for p in proofs])
         return self._submit(self._lib.b200_box_submit_bundle_witness, (srs, pks, arr_p, len(proofs), arr_l, len(links)),
                             _finish(lambda: out), keep)
@@ -1558,14 +1456,16 @@ class ProverBox(_Tickets):
         SRS.  A wire table or hint polynomial in device memory pins the job to its device (all of them on one); otherwise
         the job goes to the least-loaded device.  `wait(ticket)` returns (proof, link_proofs, statuses)."""
         h, shape = self._resolve(pk)
-        args, finish, held = _settlement_job(h, shape, None, wires, pub_inputs, blinders, links, "box.submit_settlement")
+        args, finish, held = _settlement_job(h, shape, None, links, _table_proof, wires, pub_inputs, blinders,
+                                             where="box.submit_settlement")
         return self._submit(self._lib.b200_box_submit_settlement, (srs, h, *args), finish, (held, keep))
 
     def submit_settlement_witness(self, srs, pk, witness, blinders, links, keep=None) -> int:
         """`submit_settlement` from a witness vector (`b200_box_submit_settlement_witness`); the witness counts among the
         job's device pointers.  `wait(ticket)` returns (proof, link_proofs, statuses, pub_inputs)."""
         h, shape = self._resolve(pk)
-        args, finish, held = _settlement_witness_job(h, shape, None, witness, blinders, links, "box.submit_settlement_witness")
+        args, finish, held = _settlement_job(h, shape, None, links, _witness_proof, witness, blinders,
+                                             where="box.submit_settlement_witness")
         return self._submit(self._lib.b200_box_submit_settlement_witness, (srs, h, *args), finish, (held, keep))
 
     def submit_verify(self, vks, pub_inputs, proofs, links=(), combined: bool = False, g2=None) -> int:

@@ -411,7 +411,8 @@ int b200_plonk_batch_verify(b200_ctx* ctx, const b200_verifying_key* vks, size_t
                             const uint64_t g2_tau_h[16], int* all_accepted, uint8_t* verdicts);
 /* verdicts[i] (n_proofs + n_links bytes, proofs first) = b200_plonk_verify / b200_plonk_verify_link's answer for item i,
  * each item checked on its own, e(A_i, [tau]_2) == e(B_i, [1]_2), with no random combination and no bisection: the cost
- * does not depend on how many items fail.  The pairings run on the device, one thread per item.  Arguments, errors and
+ * does not depend on how many items fail.  The pairings run on the device, as b200_pairing_check_many runs them (one
+ * 16-lane group per item up to one wave of the device, one thread per item past it).  Arguments, errors and
  * rejections of malformed items exactly as b200_plonk_batch_verify; verdicts may be NULL only when there are no items. */
 int b200_plonk_verify_each(b200_ctx* ctx, const b200_verifying_key* vks, size_t n_vks, const b200_batch_proof* proofs,
                            size_t n_proofs, const b200_batch_link* links, size_t n_links, const uint64_t g2_h[16],
@@ -422,7 +423,9 @@ int b200_plonk_verify_each(b200_ctx* ctx, const b200_verifying_key* vks, size_t 
  * the curve, a coordinate >= q), the call fails with the same code and b200_last_error() names the first such check
  * (an off-curve G2 point fails every check: the message names the point).  At most 8 pairs per check (m <= 8, else
  * B200_ERR_INVALID); m = 0 makes every check 1.  The G2 points are validated and their Miller-loop lines computed on
- * the host; the G1 checks, the Miller loops and the final exponentiations run on the device, one thread per check.
+ * the host; the G1 checks, the Miller loops and the final exponentiations run on the device: while the checks fit in
+ * one wave of 24 per SM (3168 on a 132-SM H100) each check's Fq12 arithmetic is spread over a group of 16 lanes, for
+ * latency; past that each check runs on one thread, for throughput.  The answers do not depend on the path.
  * NULL pointers: B200_ERR_INVALID (g1_points / is_one may be NULL when there are no checks). */
 int b200_pairing_check_many(b200_ctx* ctx, const uint64_t* g2_points, size_t m, const uint64_t* g1_points,
                             size_t n_checks, uint8_t* is_one);

@@ -163,6 +163,13 @@ class Context:
         _lib.check(self._lib.b200_selftest_field(self._h, seed, iters, C.byref(bad)))
         return bad.value
 
+    def selftest_pairing(self, seed: int, iters: int) -> int:
+        """Mismatches between the 16-lane pairing arithmetic and the one-thread pairing functions over `iters` seeded
+        operands of every operation (`b200_selftest_pairing`); 0 expected."""
+        bad = C.c_uint64(0)
+        _lib.check(self._lib.b200_selftest_pairing(self._h, seed, iters, C.byref(bad)))
+        return bad.value
+
     def field_op(self, field: int, op: int, a: np.ndarray, b: np.ndarray) -> np.ndarray:
         a = np.ascontiguousarray(a, dtype=np.uint64).reshape(-1, 4)
         b = np.ascontiguousarray(b, dtype=np.uint64).reshape(-1, 4)

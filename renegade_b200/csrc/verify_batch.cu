@@ -25,9 +25,9 @@
 // An item with an off-curve point or a field element outside [0, p) is rejected and left out of the combination.
 //
 // b200_plonk_verify_each runs steps 1 and 2 (Batch::stage), then k_scalars with rho = 1, k_item_points (A_i and -B_i of
-// each item) and the device pairing (k_pairing_many over the lines of [tau]_2 and [1]_2 prepared on the host,
-// pairing.cuh): every item is checked on its own, so the cost does not depend on how many fail.  b200_pairing_check_many
-// exposes the pairing kernel itself.
+// each item) and the device pairing (pairing_many_enqueue over the lines of [tau]_2 and [1]_2 prepared on the host:
+// k_pairing_warp for a few items, k_pairing_many for many): every item is checked on its own, so the cost does not
+// depend on how many fail.  b200_pairing_check_many exposes the pairing kernels themselves.
 #include <cstring>
 #include <mutex>
 #include <string>
@@ -36,6 +36,7 @@
 #include "b200prover.h"
 #include "device_ctx.h"
 #include "pairing.cuh"
+#include "pairing_warp.cuh"
 #include "transcript.h"
 #include "verify_terms.h"
 
@@ -312,6 +313,37 @@ __global__ void __launch_bounds__(kPairThreads) k_pairing_many(const G2Prepared*
     is_one[c] = fq12_is_one(final_exponentiation(miller_loop_prepared(q, p, m), pc)) ? 1 : 0;
 }
 
+// The same checks with a 16-lane group per check (pairing_warp.cuh), two per warp: lane j < m loads and checks G1 point
+// j, the group's ballot decides, and the Fq12 arithmetic is spread over the group.  Every group reads the same
+// prepared lines, as above.
+constexpr int kPairWarpThreads = 128;  // 8 checks per block
+constexpr int kPairWarpBlocksPerSm = 3;  // 168 registers, no spills (-Xptxas -v)
+constexpr size_t kPairWarpChecksPerSm = (size_t)kPairWarpBlocksPerSm * kPairWarpThreads / pw::kGroup;
+__global__ void __launch_bounds__(kPairWarpThreads, kPairWarpBlocksPerSm)
+    k_pairing_warp(const G2Prepared* __restrict__ q, int m, const g1_affine* __restrict__ g1, size_t n, PairingConsts pc,
+                   uint8_t* __restrict__ is_one) {
+    __shared__ pw::Consts kc;
+    if (threadIdx.x == 0) pw::consts_init(&kc, pc);
+    __syncthreads();
+    const size_t c = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / pw::kGroup;
+    if (c >= n) return;  // the whole group
+    const pw::Lanes g = pw::lanes();
+    g1_affine p;
+    p.x = p.y = fe_zero();
+    if (g.lane < m) p = g1[c * m + g.lane];
+    const bool bad = g.lane < m && !g1_affine_on_curve(p);
+    const bool inf = g.lane < m && g1_affine_is_inf(p);
+    const unsigned shift = threadIdx.x & 16;
+    if ((__ballot_sync(g.mask, bad) & g.mask) != 0) {
+        if (g.lane == 0) is_one[c] = 2;
+        return;
+    }
+    const unsigned skip = (__ballot_sync(g.mask, inf) & g.mask) >> shift;
+    const fe f = pw::final_exp(pw::miller(q, m, p.x, p.y, skip, &kc), &kc);
+    const bool one = pw::is_one(f, &kc);
+    if (g.lane == 0) is_one[c] = one ? 1 : 0;
+}
+
 // verdict_i = ok_i && the item's pairing check holds
 __global__ void k_verdicts(const ItemState* __restrict__ st, const uint8_t* __restrict__ is_one, size_t k,
                            uint8_t* __restrict__ verdicts) {
@@ -321,8 +353,25 @@ __global__ void k_verdicts(const ItemState* __restrict__ st, const uint8_t* __re
 
 inline unsigned grid_of(size_t n, unsigned bs) { return (unsigned)((n + bs - 1) / bs); }
 
+// The checks one wave of k_pairing_warp holds on this device: kPairWarpChecksPerSm on every SM
+size_t pairing_warp_wave() {
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+        return 0;
+    return (size_t)sms * kPairWarpChecksPerSm;
+}
+
+// The group kernel while its grid fits in one wave (3168 checks on a 132-SM H100): every check then costs one group
+// pairing's latency.  Past one wave the one-thread kernel, whose throughput was built for many checks.  Measured
+// (tools/verify_latency_bench.py, H100 80GB HBM3 at 700 W, m = 2): the group kernel takes 4.4 ms up to n = 512 and 5.7 ms
+// at 2048, the one-thread kernel 32.1 ms at n = 1 to 32.7 ms at 4096; the switch sits at one wave because the group
+// kernel has not been measured past it.
 void pairing_many_enqueue(const G2Prepared* q, int m, const g1_affine* g1, size_t n, uint8_t* is_one, cudaStream_t st) {
-    B200_LAUNCH(k_pairing_many, grid_of(n, kPairThreads), kPairThreads, 0, st)(q, m, g1, n, pairing_consts(), is_one);
+    if (n <= pairing_warp_wave())
+        B200_LAUNCH(k_pairing_warp, grid_of(n * pw::kGroup, kPairWarpThreads), kPairWarpThreads, 0, st)(q, m, g1, n,
+                                                                                                    pairing_consts(), is_one);
+    else
+        B200_LAUNCH(k_pairing_many, grid_of(n, kPairThreads), kPairThreads, 0, st)(q, m, g1, n, pairing_consts(), is_one);
 }
 
 template <class T>

@@ -29,6 +29,7 @@ pub mod ffi_settlement;
 pub mod ffi_verifyjobs;
 pub mod ffi_express;
 pub mod ffi_reserved;
+pub mod ffi_selftest;
 
 use ark_bn254::{Bn254, Fq, Fr, G1Affine};
 use ark_ff::{BigInt, UniformRand};

@@ -308,7 +308,8 @@ typedef struct {
  * intent_and_balance.rs:66-72).  a1 / a2: the two `LinkingHint.linking_wire_poly` coefficient
  * vectors (Montgomery, host or device pointers; lengths may differ), comm1 / comm2 their
  * `linking_wire_comm`; (alignment, offset, size) = mpc-relation `GroupLayout`: the group sits on
- * the roots g^(offset + i), i < size, g the generator of the 2^alignment-th roots of unity.
+ * the roots g^(offset + i), i < size, g the generator of the 2^alignment-th roots of unity, so
+ * 1 <= size <= 2^alignment (the roots are distinct) and alignment <= 28.
  * eta (may be NULL) receives the Fiat–Shamir challenge.  Fails with B200_ERR_UNSATISFIED when a1 and a2
  * do not agree on the group (no link proof exists: wrong layout or mismatched witnesses); *proof is zeroed then and
  * eta is not written. */
@@ -335,7 +336,7 @@ typedef struct {
  * was proved, B200_ERR_UNSATISFIED when any was not.  An argument error fails the whole call before any device work with
  * B200_ERR_INVALID, and b200_last_error() names the item: a NULL ctx / srs, a NULL items pointer with k > 0, an item
  * with a NULL a1 / a2 / comm1 / comm2 / proof pointer, or one that b200_plonk_link refuses (size 0, size >= max(len1,
- * len2), alignment > 28, max(len1, len2) above the SRS length, or a transform above 2^28).  A CUDA or memory error fails
+ * len2), alignment > 28, size > 2^alignment, max(len1, len2) above the SRS length, or a transform above 2^28).  A CUDA or memory error fails
  * the whole call too.  k = 0 is accepted.
  * The batch runs in chunks of as many items as half the free device memory holds (at most 64); the results do not
  * depend on the chunk size.  It runs eagerly (no CUDA graphs) in the context's batch buffers, the ones
@@ -357,7 +358,8 @@ int b200_plonk_verify(unsigned log_n, size_t num_inputs, const uint64_t* k, cons
                       const uint64_t* sigma_comms, const uint64_t* pub_inputs, const b200_proof* proof,
                       const uint64_t g2_h[16], const uint64_t g2_tau_h[16], int* accepted);
 /* Replaces `PlonkKzgSnark::verify_link_proof::<SolidityTranscript>(&comm_a, &comm_b, &link_proof,
- * &group_layout, &open_key)` (proof_linking/intent_only.rs:77-84, `validate_*_link`). */
+ * &group_layout, &open_key)` (proof_linking/intent_only.rs:77-84, `validate_*_link`).  B200_ERR_INVALID for a layout
+ * b200_plonk_link refuses whatever the lengths: alignment > 28, size 0 or size > 2^alignment. */
 int b200_plonk_verify_link(const uint64_t* comm1, const uint64_t* comm2, unsigned alignment, size_t offset,
                            size_t size, const b200_link_proof* proof, const uint64_t g2_h[16],
                            const uint64_t g2_tau_h[16], int* accepted);
@@ -404,7 +406,7 @@ typedef struct {
  * combined check.  An item with an off-curve G1 point or a field element outside [0, p) is rejected (verdict 0) and
  * left out of the combination.
  * Errors: B200_ERR_NOT_ON_CURVE for an off-curve G2 point (a coordinate >= q included); B200_ERR_INVALID for a vk
- * index out of range, log_n > 28, a link with alignment > 28 or size == 0, or a NULL pointer.  Zero items are
+ * index out of range, log_n > 28, a link with alignment > 28, size == 0 or size > 2^alignment, or a NULL pointer.  Zero items are
  * accepted. */
 int b200_plonk_batch_verify(b200_ctx* ctx, const b200_verifying_key* vks, size_t n_vks, const b200_batch_proof* proofs,
                             size_t n_proofs, const b200_batch_link* links, size_t n_links, const uint64_t g2_h[16],

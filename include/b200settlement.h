@@ -43,8 +43,8 @@ typedef struct {
  * which links did.  Argument errors return B200_ERR_INVALID before any device work (no kernel launched, no output
  * written) and the message names the link: everything b200_plonk_prove refuses, a NULL srs, a NULL links pointer with
  * n_links > 0, a link with a NULL hint_poly / hint_comm / proof, or one b200_plonk_link would refuse with len1 = hint_len
- * and len2 = n + 2 (size 0, size >= max length, alignment > 28, a polynomial longer than the SRS).  n_links = 0 is a
- * plain proof. */
+ * and len2 = n + 2 (size 0, size >= max length, alignment > 28, size > 2^alignment, a polynomial longer than the SRS).
+ * n_links = 0 is a plain proof. */
 int b200_plonk_prove_settlement(b200_ctx* ctx, const b200_bases* srs, const b200_pk* pk, const uint64_t* wires,
                                 const uint64_t* pub_inputs, const uint64_t* blinders, b200_proof* proof, uint64_t* link_poly,
                                 const b200_settlement_link* links, size_t n_links, int* statuses);

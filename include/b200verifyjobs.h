@@ -34,8 +34,8 @@ extern "C" {
  *   B200_ERR_INVALID      a NULL pool / ticket / G2 record; a NULL vks / proofs / links array with a nonzero count;
  *                         NULL verdicts when there are items; a mode other than 0 or 1; a key with log_n > 28 or a NULL
  *                         k / selector / sigma pointer; a proof with a vk index out of range, a NULL proof or NULL public
- *                         inputs for a key with inputs; a link with a NULL comm1 / comm2 / proof, alignment > 28 or
- *                         size 0;
+ *                         inputs for a key with inputs; a link with a NULL comm1 / comm2 / proof, alignment > 28,
+ *                         size 0 or size > 2^alignment;
  *   B200_ERR_NOT_ON_CURVE a G2 record off the twist (a coordinate >= q included). */
 int b200_pool_submit_verify(b200_pool* pool, int mode, const b200_verifying_key* vks, size_t n_vks,
                             const b200_batch_proof* proofs, size_t n_proofs, const b200_batch_link* links, size_t n_links,

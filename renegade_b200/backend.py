@@ -476,9 +476,10 @@ def verify_link_proof(comm_a: np.ndarray, comm_b: np.ndarray, proof: "B200LinkPr
 class _VerifyBatch:
     """The Python argument checks and the C structs of `batch_verify` and `verify_each`: the distinct verifying keys, the
     proofs whose public-input count matches their key (the others are False verdicts without a device call), the
-    links and the one G2 pair.  `args` are the C call's arguments from ctx on, up to the outputs."""
+    links and the one G2 pair.  `args` are the C call's arguments from ctx on, up to the outputs; `where`, the entry point,
+    starts the message of a refused link."""
 
-    def __init__(self, vks, pub_inputs, proofs, links, g2):
+    def __init__(self, vks, pub_inputs, proofs, links, g2, where: str = "verify"):
         vks, pub_inputs, proofs, links = list(vks), list(pub_inputs), list(proofs), list(links)
         if not (len(vks) == len(pub_inputs) == len(proofs)):
             raise ValueError("one verifying key and one public-input vector per proof")
@@ -515,7 +516,8 @@ class _VerifyBatch:
             c_proofs.append(B200BatchProof(vk_index[key], _ptr(p) if p.size else None, C.cast(C.pointer(proof), C.c_void_p)))
             self.proof_pos.append(i)
         c_links = []
-        for comm_a, comm_b, lproof, layout in links:
+        for i, (comm_a, comm_b, lproof, layout) in enumerate(links):
+            _check_group_size(layout, f"{where}: link {i}")
             a, b = _u64(comm_a), _u64(comm_b)
             self.keep.append((a, b))
             c_links.append(B200BatchLink(_ptr(a), _ptr(b), layout.alignment, layout.offset, layout.size,
@@ -563,7 +565,7 @@ class PlonkKzgSnark:
         ValueError); `g2 = (g2_h, g2_tau_h)` supplies it when there are only links.  Returns (all_ok, verdicts) with
         verdicts[i] the single verifier's answer for item i, proofs first, then links.  A wrong public-input count is
         a False verdict, as in `verify`."""
-        b = _VerifyBatch(vks, pub_inputs, proofs, links, g2)
+        b = _VerifyBatch(vks, pub_inputs, proofs, links, g2, "batch_verify")
         if b.n_items == 0:
             return True, []
         verdicts = (C.c_uint8 * max(1, b.n_c))()
@@ -576,7 +578,7 @@ class PlonkKzgSnark:
         """The verdicts of `batch_verify`, each item checked on its own with its own pairing on `ctx`'s device
         (`b200_plonk_verify_each`): no bisection, so the cost does not depend on how many items fail.  Same arguments
         and argument errors as `batch_verify`; returns the list of verdicts, proofs first, then links."""
-        b = _VerifyBatch(vks, pub_inputs, proofs, links, g2)
+        b = _VerifyBatch(vks, pub_inputs, proofs, links, g2, "verify_each")
         if b.n_items == 0:
             return []
         verdicts = (C.c_uint8 * max(1, b.n_c))()
@@ -843,6 +845,14 @@ def _link_hint(hint, where: str, name: str):
     return p, n, a, c
 
 
+def _check_group_size(lay: "GroupLayout", where: str):
+    """`where`'s link group holds distinct roots: at most the 2^alignment of its subgroup (an alignment outside [0, 28] is
+    left to the caller's other checks)."""
+    if 0 <= lay.alignment <= 28 and lay.size > 1 << lay.alignment:
+        raise ValueError(f"{where}'s group of {lay.size} roots does not fit the 2^{lay.alignment} roots of unity of its "
+                         "alignment (size <= 2^alignment)")
+
+
 def _check_layout(lay: "GroupLayout", length: int, srs_len, where: str):
     """`where`'s link group on polynomials of `length` coefficients, against an SRS of `srs_len` powers (None: not known
     here)."""
@@ -851,6 +861,7 @@ def _check_layout(lay: "GroupLayout", length: int, srs_len, where: str):
                          "(0 < size < length)")
     if not 0 <= lay.alignment <= 28 or lay.offset < 0:
         raise ValueError(f"{where} has alignment {lay.alignment} and offset {lay.offset} (0 <= alignment <= 28, offset >= 0)")
+    _check_group_size(lay, where)
     if srs_len is not None and length > srs_len:
         raise ValueError(f"{where} has {length} coefficients, the SRS {srs_len} powers")
 
@@ -1091,10 +1102,10 @@ def _settlement_job(h, shape, srs_len, links, build, *inputs, where: str):
     return (C.pointer(p.entry(h)), arr, len(out), st), finish, (p, held)
 
 
-def _verify_job(vks, pub_inputs, proofs, links, combined: bool, g2):
+def _verify_job(vks, pub_inputs, proofs, links, combined: bool, g2, where: str):
     """One verification job.  The C call copies every input, so only the outputs have to live until the wait, which
     returns what `verify_each` (a verdict list) or, `combined`, `batch_verify` ((all_ok, verdicts)) returns."""
-    b = _VerifyBatch(vks, pub_inputs, proofs, links, g2)
+    b = _VerifyBatch(vks, pub_inputs, proofs, links, g2, where)
     if not hasattr(b, "args"):  # no items and no G2 pair: a job still checks its G2 records
         raise ValueError("a verification job without items needs g2=(g2_h, g2_tau_h)")
     verdicts = (C.c_uint8 * max(1, b.n_c))()
@@ -1314,7 +1325,7 @@ class ProverPool(_Tickets):
         `PlonkKzgSnark.verify_each` / `.batch_verify` take them; every input is copied at submit.  `wait(ticket)` returns
         what `verify_each` returns (the verdict list), or with `combined` what `batch_verify` returns ((all_ok,
         verdicts): one combined pairing, the failing items found by bisection inside the job)."""
-        job = _verify_job(vks, pub_inputs, proofs, links, combined, g2)
+        job = _verify_job(vks, pub_inputs, proofs, links, combined, g2, "submit_verify")
         return self._submit(self._lib.b200_pool_submit_verify, *job)
 
     def wait(self, ticket: int):
@@ -1478,7 +1489,7 @@ class ProverBox(_Tickets):
     def submit_verify(self, vks, pub_inputs, proofs, links=(), combined: bool = False, g2=None) -> int:
         """`ProverPool.submit_verify` on the least-loaded device (`b200_box_submit_verify`).  `wait(ticket)` returns the
         verdict list, or (all_ok, verdicts) with `combined`."""
-        job = _verify_job(vks, pub_inputs, proofs, links, combined, g2)
+        job = _verify_job(vks, pub_inputs, proofs, links, combined, g2, "box.submit_verify")
         return self._submit(self._lib.b200_box_submit_verify, *job)
 
     def verifying_key(self, pk):

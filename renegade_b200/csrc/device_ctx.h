@@ -336,7 +336,7 @@ int settlement_check(const b200_bases* srs, const b200_bundle_witness& proof, co
 
 // The item checks of b200_plonk_batch_verify / b200_plonk_verify_each (verify_batch.cu), which a pool also makes at submit:
 // B200_OK; B200_ERR_INVALID for a key with log_n > 28 or a NULL pointer, a proof with a vk index out of range or a NULL
-// proof / public inputs, a link with a NULL pointer, alignment > 28 or size 0; B200_ERR_NOT_ON_CURVE for a G2 record off
+// proof / public inputs, a link with a NULL pointer, alignment > 28, size 0 or size > 2^alignment; B200_ERR_NOT_ON_CURVE for a G2 record off
 // the twist.  The message starts with `who` and names the entry.  The arrays must be non-NULL where their count is not 0.
 int verify_check(const char* who, const b200_verifying_key* vks, size_t n_vks, const b200_batch_proof* proofs, size_t n_proofs,
                  const b200_batch_link* links, size_t n_links, const uint64_t g2_h[16], const uint64_t g2_tau_h[16]);

@@ -20,27 +20,51 @@ FF_D uint64_t splitmix(uint64_t seed, uint64_t j) {
     z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
     return z ^ (z >> 31);
 }
+// Uniform on [0, q): 254-bit draws (q > 2^253, so about 3 in 4 are accepted), the next draw while one is not below q
 FF_D fe random_fe(uint64_t seed, uint64_t i) {
     fe v;
+    for (uint64_t t = 0;; ++t) {
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const uint64_t x = splitmix(seed, 4 * i + k);
-        v.l[2 * k] = (uint32_t)x;
-        v.l[2 * k + 1] = (uint32_t)(x >> 32);
+        for (int k = 0; k < 4; ++k) {
+            const uint64_t x = splitmix(seed + t * 0x632BE59BD9B4E019ULL, 4 * i + k);
+            v.l[2 * k] = (uint32_t)x;
+            v.l[2 * k + 1] = (uint32_t)(x >> 32);
+        }
+        v.l[7] &= 0x3fffffffu;
+        if (fe_is_canonical<FqCfg>(v)) return v;
     }
-    v.l[7] &= 0x0fffffffu;  // < 2^252 < q
+}
+// The values at the top and the middle of Fq and at the powers of two a reduction meets: q - 1, (q - 1) / 2,
+// R mod q (the Montgomery one) and 2^252
+FF_D fe edge_fe(int e) {
+    fe v = fe_zero();
+    if (e == 0 || e == 1) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) v.l[k] = FqCfg::mod(k);
+        v.l[0] -= 1;  // q is odd
+        if (e == 1)
+#pragma unroll
+            for (int k = 0; k < 8; ++k) v.l[k] = (v.l[k] >> 1) | (k < 7 ? v.l[k + 1] << 31 : 0u);
+    } else if (e == 2) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) v.l[k] = FqCfg::one(k);
+    } else {
+        v.l[7] = 1u << 28;
+    }
     return v;
 }
 // Operand o of iteration i.  The shapes cycle so that every operation meets dense values, values with about half their
-// coefficients zero, the value 1, elements of Fq2 = Fq + Fq w^6 (the inversion's last step) and 0.
+// coefficients zero, the value 1, elements of Fq2 = Fq + Fq w^6 (the inversion's last step), 0, values made only of the
+// edge values of edge_fe, and dense values with about half their coefficients edge values.
 FF_D fq12 random_fq12(uint64_t seed, uint64_t i, int o) {
-    const int shape = (int)((i + o) % 6);
+    const int shape = (int)((i + o) % 8);
     const uint64_t zeros = splitmix(seed ^ 0x2e705ULL, 2 * i + o);
     fq12 a;
 #pragma unroll
     for (int k = 0; k < 12; ++k) {
         a.c[k] = random_fe(seed, (2 * i + o) * 12 + k);
         if ((shape == 2 && ((zeros >> k) & 1)) || (shape == 4 && k % 6) || shape == 5) a.c[k] = fe_zero();
+        if (shape == 6 || (shape == 7 && ((zeros >> k) & 1))) a.c[k] = edge_fe((int)((zeros >> (16 + 2 * k)) & 3));
     }
     return shape == 3 ? fq12_one() : a;
 }

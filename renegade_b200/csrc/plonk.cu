@@ -1652,7 +1652,7 @@ struct LinkItem {
 // B200_ERR_INVALID, with a message that starts with `where`, when no link proof is made for them.
 static int link_item(const Bases* srs, const b200_link_item& x, const std::string& where, LinkItem* it) {
     const size_t len = std::max(x.len1, x.len2);
-    if (x.size == 0 || x.size >= len || x.alignment > 28 || len > srs->n) {
+    if (x.size == 0 || x.size >= len || x.alignment > 28 || x.size > ((size_t)1 << x.alignment) || len > srs->n) {
         set_error(where + ": bad group layout or polynomial length");
         return B200_ERR_INVALID;
     }

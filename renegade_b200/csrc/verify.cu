@@ -318,7 +318,10 @@ int b200_plonk_verify(unsigned log_n, size_t num_inputs, const uint64_t* k, cons
 int b200_plonk_verify_link(const uint64_t* comm1, const uint64_t* comm2, unsigned alignment, size_t offset, size_t size,
                            const b200_link_proof* proof, const uint64_t g2_h[16], const uint64_t g2_tau_h[16], int* accepted) {
     B200_TRY
-    if (!comm1 || !comm2 || !proof || !g2_h || !g2_tau_h || !accepted || alignment > 28 || size == 0) return B200_ERR_INVALID;
+    // a group of more roots than the 2^alignment-th roots of unity holds has no layout (and Z_D would take `size` products)
+    if (!comm1 || !comm2 || !proof || !g2_h || !g2_tau_h || !accepted || alignment > 28 || size == 0 ||
+        size > ((size_t)1 << alignment))
+        return B200_ERR_INVALID;
     *accepted = 0;
     g1_affine points[vt::kLinkPoints];
     points[vt::kLinkC1] = g1_load(comm1);

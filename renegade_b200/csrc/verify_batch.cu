@@ -575,8 +575,10 @@ int verify_check(const char* who, const b200_verifying_key* vks, size_t n_vks, c
             return B200_ERR_INVALID;
         }
     for (size_t l = 0; l < n_links; ++l)
-        if (!links[l].comm1 || !links[l].comm2 || !links[l].proof || links[l].alignment > kMaxAlign || links[l].size == 0) {
-            set_error(w + ": bad link entry " + std::to_string(l) + " (alignment above 28, size 0 or a NULL pointer)");
+        if (!links[l].comm1 || !links[l].comm2 || !links[l].proof || links[l].alignment > kMaxAlign || links[l].size == 0 ||
+            links[l].size > ((uint64_t)1 << links[l].alignment)) {
+            set_error(w + ": bad link entry " + std::to_string(l) +
+                      " (alignment above 28, size 0 or above 2^alignment, or a NULL pointer)");
             return B200_ERR_INVALID;
         }
     if (!g2_records_on_curve(g2_tau_h, g2_h)) {

@@ -1,7 +1,8 @@
 """Test infrastructure: link-proof inputs built from their algebra instead of from two synthesised circuits.
 
 A link proof shows that two wire polynomials a1, a2 agree on the link group D = {g^(offset + i) : i < size}, g the
-generator of the 2^alignment-th roots of unity: q = (a1 - a2) / Z_D with Z_D = prod_{i < size} (X - g^(offset + i)).
+generator of the 2^alignment-th roots of unity (1 <= size <= 2^alignment, so the roots are distinct; an offset of 2^alignment
+or more names the roots of offset mod 2^alignment): q = (a1 - a2) / Z_D with Z_D = prod_{i < size} (X - g^(offset + i)).
 `pair` draws the shorter polynomial at random and sets the longer one to it plus Z_D * q for a random q of len - size
 coefficients, so that len1 and len2 take exactly the wanted values in either order.  `mismatch` adds c * Z_D / (X - root_j),
 which vanishes on every root of the group but the j-th.
@@ -41,7 +42,7 @@ class Case:
     @property
     def wraps(self) -> bool:
         """the roots pass g^0 = 1 (still distinct: size <= 2^alignment)"""
-        return self.offset + self.size > 1 << self.alignment
+        return self.offset % (1 << self.alignment) + self.size > 1 << self.alignment
 
 
 CASES = [
@@ -56,6 +57,11 @@ CASES = [
     Case("len1_just_above_len2", 7, 100, 20, 129, 128, N=256, q_len=109),  # 129 = N/2 + 1: the most slack
     Case("identical", 5, 20, 6, 40, 40, N=64, q_len=34, identical=True),
     Case("largest_srs", 10, 1000, 3, (1 << 17) + 2, (1 << 17) - 7, N=1 << 18, q_len=(1 << 17) - 1),
+    Case("offset_past_group", 5, (1 << 5) + 3, 6, 20, 14, N=32, q_len=14),    # the roots of offset 3
+    Case("offset_2_63", 6, (1 << 63) + 5, 7, 24, 30, N=32, q_len=23),         # the roots of offset 5
+    Case("whole_group_shifted", 3, 5, 8, 12, 9, N=16, q_len=4),               # Z_D = X^8 - 1, from g^5 round to g^4
+    Case("alignment_zero", 0, 7, 1, 9, 6, N=16, q_len=8),                     # g = 1: the group {1}
+    Case("alignment_28", 28, 12345, 4, 32, 25, N=32, q_len=28),               # 2^28-th roots, a 2^5 domain
 ]
 BY_NAME = {c.name: c for c in CASES}
 

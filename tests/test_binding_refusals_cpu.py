@@ -170,6 +170,23 @@ def _rows():
                      lambda call=call: call(x.hint, GroupLayout(4, 2, 0))))
         rows.append((name, "alignment 29", exc, rf"{where} has alignment 29 and offset 2 \(0 <= alignment <= 28",
                      lambda call=call: call(x.hint, GroupLayout(29, 2, 3))))
+        rows.append((name, "size 2^a + 1", exc, rf"{where}'s group of 17 roots does not fit the 2\^4 roots of unity",
+                     lambda call=call: call(x.hint, GroupLayout(4, 2, 17))))
+    # the verifiers take a link as (comm_a, comm_b, proof, layout): link 1, after a valid link 0
+    h, tau_h = _u64(16, 10).reshape(-1), _u64(16, 11).reshape(-1)
+    verifiers = {
+        "verify_each": lambda links: PlonkKzgSnark.verify_each(_objects(_NoLibrary())[0], [], [], [], links, g2=(h, tau_h)),
+        "batch_verify": lambda links: PlonkKzgSnark.batch_verify(_objects(_NoLibrary())[0], [], [], [], links, g2=(h, tau_h)),
+        "submit_verify": lambda links: _objects(_NoLibrary())[1].submit_verify([], [], [], links, g2=(h, tau_h)),
+        "box.submit_verify": lambda links: _objects(_NoLibrary())[2].submit_verify([], [], [], links, combined=True,
+                                                                                  g2=(h, tau_h)),
+    }
+    for name, call in verifiers.items():
+        link = lambda lay: (x.hint.linking_wire_comm, x.hint2.linking_wire_comm, B200LinkProof(), lay)  # noqa: E731
+        for a, size in ((4, 17), (0, 2), (28, (1 << 28) + 1), (4, 1 << 63)):
+            rows.append((name, f"size {size} at alignment {a}", ValueError,
+                         rf"{name}: link 1's group of {size} roots does not fit the 2\^{a} roots of unity",
+                         lambda call=call, a=a, size=size: call([link(x.lay), link(GroupLayout(a, 5, size))])))
     _, pool, box = _objects(_NoLibrary())
     two = lambda k, ptr: [(k, ptr, x.pub, x.bl)] * 2  # noqa: E731
     outside = [(0, 1, x.lay), (1, 2, x.lay)]

@@ -305,8 +305,8 @@ def test_real_private_match(ctx, srs_2_16, srs_2_16_g2):
         ct.clear_key_cache()
 
 
-@pytest.mark.parametrize("bad", ["size_zero", "size_is_len", "alignment", "longer_than_srs", "null_a1", "null_a2",
-                                 "null_comm1", "null_comm2", "null_proof"])
+@pytest.mark.parametrize("bad", ["size_zero", "size_is_len", "size_above_group", "alignment", "longer_than_srs", "null_a1",
+                                 "null_a2", "null_comm1", "null_comm2", "null_proof"])
 def test_argument_errors_fail_the_call_before_any_work(env, bad):
     e = env
     triples = [triple(e, WRAPS, seed=0x400 + i) for i in range(3)]
@@ -318,6 +318,8 @@ def test_argument_errors_fail_the_call_before_any_work(env, bad):
             it.size = 0
         elif bad == "size_is_len":
             it.size = max(it.len1, it.len2)
+        elif bad == "size_above_group":  # 2^3 + 1 roots at alignment 3, below the length 20
+            it.size = (1 << it.alignment) + 1
         elif bad == "alignment":
             it.alignment = 29
         elif bad == "longer_than_srs":

@@ -3,7 +3,8 @@ successive synthetic divisions: the device divides pointwise by Z_D on a coset o
 quotient's degree over coefficients [q_len, N).  The inputs are built from the algebra (`link_layouts.py`, whose shapes
 `test_link_layouts_cpu.py` pins): size 1, q_len 1, the whole subgroup (Z_D = X^(2^a) - 1), roots wrapping past g^0,
 an alignment above log2 N, len = N, len1 < len2 and len1 > len2 at several ratios, equal polynomials (identity quotient
-and opening commitments) and the largest SRS.  Each link proof and eta are byte-equal to the oracle's and accepted by the
+and opening commitments), the largest SRS, offsets of 2^a and more, the whole subgroup from g^5, alignment 0 and
+alignment 28.  Each link proof and eta are byte-equal to the oracle's and accepted by the
 oracle's and the product's link verifiers and by one batch verification; a difference on exactly one root is refused
 and the context keeps proving; a replayed graph gives the oracle's proof for new polynomials."""
 import numpy as np

@@ -36,7 +36,10 @@ def test_case_has_the_shape_it_claims(oracle, name):
     assert len(set(rts)) == c.size
     g = ll.generator(oracle, c.alignment)
     assert pow(g, 1 << c.alignment, ll.R) == 1 and (c.alignment == 0 or pow(g, 1 << (c.alignment - 1), ll.R) != 1)
-    assert c.wraps == (name in ("wraps",)) and (1 in rts) == (c.wraps or c.offset == 0)
+    assert c.wraps == (name in ("wraps", "whole_group_shifted"))
+    assert (1 in rts) == (c.wraps or c.offset % (1 << c.alignment) == 0)
+    same = ll.roots(oracle, ll.Case("", c.alignment, c.offset % (1 << c.alignment), c.size, c.len1, c.len2, c.N, c.q_len))
+    assert rts == same  # an offset names its roots modulo 2^alignment
     assert c.identical == (name == "identical")
     log_n = c.N.bit_length() - 1
     claims = {
@@ -52,6 +55,12 @@ def test_case_has_the_shape_it_claims(oracle, name):
         "len1_just_above_len2": c.len1 == c.len2 + 1 == c.N // 2 + 1,
         "identical": c.len1 == c.len2,
         "largest_srs": c.len == (1 << 17) + 2 and c.N == 1 << 18,
+        "offset_past_group": c.offset == (1 << c.alignment) + 3,
+        "offset_2_63": c.offset == (1 << 63) + 5 and c.offset < 1 << 64,
+        "whole_group_shifted": c.offset == 5 and c.size == 1 << c.alignment
+                               and ll.vanishing(rts) == [ll.R - 1] + [0] * (c.size - 1) + [1],
+        "alignment_zero": c.alignment == 0 and c.size == 1 and rts == [1],
+        "alignment_28": c.alignment == 28 and c.N == 32,
     }
     assert claims[name]
 

@@ -1144,6 +1144,25 @@ class _Tickets:
         result = self._wait(c_wait_info, ticket, info)
         return result, int(info[0]), int(info[1])
 
+    def _cancel(self, c_name: str, ticket: int) -> int:
+        # the ticket keeps its buffers: a running job may write them until it reaches an abort point, so they live
+        # until its wait
+        ticket = _ticket(ticket, "cancel")
+        dropped = C.c_size_t()
+        _lib.check(getattr(self._lib, c_name)(self._h, ticket, C.byref(dropped)))
+        return dropped.value
+
+    def _cancel_all(self, c_cancel_all) -> int:
+        dropped = C.c_size_t()
+        _lib.check(c_cancel_all(self._h, C.byref(dropped)))
+        return dropped.value
+
+
+def _ticket(ticket, who: str) -> int:
+    if isinstance(ticket, bool) or not isinstance(ticket, int) or not 0 < ticket < 1 << 64:
+        raise ValueError(f"{who}: a ticket is an int in [1, 2^64), not {ticket!r}")
+    return ticket
+
 
 def _express_count(express, who: str) -> int:
     if isinstance(express, bool) or not isinstance(express, int) or express < 0:
@@ -1345,6 +1364,18 @@ class ProverPool(_Tickets):
         ones)."""
         return self._wait_info(self._lib.b200_pool_wait_info, ticket)
 
+    def cancel(self, ticket: int) -> int:
+        """Cancel the ticket's job (`b200_pool_cancel`, b200cancel.h); returns how many of its queued jobs were dropped.
+        Dropped jobs never run; a running one stops at its next abort point (a host round trip of the prover or the
+        verifier).  `wait(ticket)` then raises B200Error with code B200_ERR_CANCELLED, or returns the job's result if it
+        finished first.  A finished or already cancelled ticket drops 0."""
+        return self._cancel("b200_pool_cancel", ticket)
+
+    def cancel_all(self) -> int:
+        """`cancel` for every job the pool holds (`b200_pool_cancel_all`); returns how many queued jobs were dropped.  Jobs
+        submitted afterwards run as usual.  `cancel_all()` then `close()` stops the pool without draining its queue."""
+        return self._cancel_all(self._lib.b200_pool_cancel_all)
+
     def wait_all(self) -> None:
         rc = self._lib.b200_pool_wait_all(self._h)
         self._jobs.clear()
@@ -1507,6 +1538,14 @@ class ProverBox(_Tickets):
     def wait_info(self, ticket: int):
         """`ProverPool.wait_info` on the pool of the ticket's device (`b200_box_wait_info`)."""
         return self._wait_info(self._lib.b200_box_wait_info, ticket)
+
+    def cancel(self, ticket: int) -> int:
+        """`ProverPool.cancel` on the pool of the ticket's device (`b200_box_cancel`)."""
+        return self._cancel("b200_box_cancel", ticket)
+
+    def cancel_all(self) -> int:
+        """`ProverPool.cancel_all` on every device (`b200_box_cancel_all`); returns the total dropped."""
+        return self._cancel_all(self._lib.b200_box_cancel_all)
 
     def ticket_device(self, ticket: int) -> int:
         return self._lib.b200_box_ticket_device(self._h, ticket)

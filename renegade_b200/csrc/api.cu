@@ -20,8 +20,16 @@ std::atomic<uint64_t> g_launch_host_ns{0};
 std::atomic<uint64_t> g_graph_launches{0};
 std::atomic<uint64_t> g_object_ids{1};
 thread_local uint64_t t_kernel_launches = 0;
+thread_local const std::atomic<bool>* t_cancel = nullptr;
 
 void set_error(const std::string& msg) { g_last_error = msg; }
+
+int cancelled(Context* c) {
+    for (cudaStream_t s : {c->stream, c->stream2, c->heavy})
+        if (s) cudaStreamSynchronize(s);
+    set_error("cancelled (B200_ERR_CANCELLED): the job was cancelled before it finished");
+    return B200_ERR_CANCELLED;
+}
 
 int cuda_fail(cudaError_t e, const char* what) {
     g_last_error = std::string(what) + ": " + cudaGetErrorString(e);

@@ -18,6 +18,7 @@
 
 #include "b200prover.h"  // error codes
 #include "b200settlement.h"  // settlement_check
+#include "b200cancel.h"      // B200_ERR_CANCELLED
 
 namespace b200 {
 
@@ -217,10 +218,19 @@ struct ProofGraphSet {
     bool timing = false;  // captured with the MSM's timing events as graph nodes
     cudaGraphExec_t exec[kProofSegs] = {};
     uint64_t kernels[kProofSegs] = {};
-    ~ProofGraphSet() {
-        for (auto& e : exec)
-            if (e) cudaGraphExecDestroy(e);
+    bool complete(int segs) const {  // every one of the first `segs` segments captured
+        for (int i = 0; i < segs; ++i)
+            if (!exec[i]) return false;
+        return true;
     }
+    void drop() {  // the next use captures every segment again
+        for (auto& e : exec)
+            if (e) {
+                cudaGraphExecDestroy(e);
+                e = nullptr;
+            }
+    }
+    ~ProofGraphSet() { drop(); }
 };
 
 // ---- context --------------------------------------------------------------------------------
@@ -267,6 +277,15 @@ struct Context {
 };
 
 int get_domain(Context* c, unsigned log_n, Domain** out);
+
+// Cancellation of pool jobs (b200cancel.h).  A pool worker points t_cancel at the flag of the job it runs for the length
+// of the call; every other thread leaves it null, so the single-context entry points never abort.  The prover, the link
+// prover and the verifiers test it only where the host already waits for the device (their abort points).
+extern thread_local const std::atomic<bool>* t_cancel;
+inline bool cancel_requested() { return t_cancel && t_cancel->load(std::memory_order_relaxed); }
+// At an abort point: waits for everything the context's streams still run (nothing may write into a buffer the next
+// call uses), records the message and returns B200_ERR_CANCELLED (api.cu).
+int cancelled(Context* c);
 
 // One group of a device's SMs that contexts can be bound to: the descriptor each bound context's green context is made
 // from, and the group's SM count as the split rounded it (api.cu).

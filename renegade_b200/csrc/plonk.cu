@@ -985,11 +985,7 @@ static ProofGraphSet* graph_set_for(Context* c, uint64_t key, const uint64_t* su
     if (gs->buffers != buffers || gs->timing != c->msm.timing) {  // a buffer moved since the capture (a larger key grew
                                                                   // it), or the MSM timing events were switched
         gs->timing = c->msm.timing;
-        for (auto& e : gs->exec)
-            if (e) {
-                cudaGraphExecDestroy(e);
-                e = nullptr;
-            }
+        gs->drop();
         gs->buffers = buffers;
     }
     return gs;
@@ -1191,6 +1187,14 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
     // graphs: only once a proof of this key has run eagerly on this context (every buffer has its final size then)
     ProofGraphSet* gset = single ? graph_set_for(c, pk->id) : nullptr;
     ProofGraphSet* gs = gset && gset->proofs_seen > 0 ? gset : nullptr;
+    // Abort points of a cancelled pool job (b200cancel.h): on entry and after each of the first four round trips.  A proof
+    // that captures its key's graphs drops the partial set, so that the next proof of the key captures all of them again.
+    const bool capturing = gs && !gs->complete(kProofSegs);
+    auto abort_job = [&]() {
+        if (capturing) gs->drop();
+        return cancelled(c);
+    };
+    if (cancel_requested()) return abort_job();
     ProofParams* hp = reinterpret_cast<ProofParams*>(bf.h_params->p);  // pinned staging copy, one block per proof
     ProofParams* dp = reinterpret_cast<ProofParams*>(bf.d_params->p);  // what the kernels read
     static_assert(sizeof(ProofParams) % sizeof(fe) == 0, "ProofParams is an array of field elements");
@@ -1330,6 +1334,7 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
         for (int i = 0; i < NW; ++i) trs[p].append_commitment(proof->wires_poly_comms[i]);
     }
     mark();  // [0] round 1
+    if (cancel_requested()) return abort_job();
 
     // ---- round 2 ------------------------------------------------------------------------------------
     std::vector<fe> beta(k), gamma(k), alpha(k), zeta(k), zeta_w(k), v(k);
@@ -1363,6 +1368,7 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
         trs[p].append_commitment(comms[p]);
     }
     mark();  // [1] round 2
+    if (cancel_requested()) return abort_job();
 
     // ---- round 3 ------------------------------------------------------------------------------------
     for (unsigned p = 0; p < k; ++p) {
@@ -1430,6 +1436,7 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
         for (int i = 0; i < NW; ++i) trs[p].append_commitment(proof->split_quot_poly_comms[i]);
     }
     mark();  // [3] round 3: quotient and its 5 commitments
+    if (cancel_requested()) return abort_job();
 
     // ---- round 4 ------------------------------------------------------------------------------------
     for (unsigned p = 0; p < k; ++p) {
@@ -1475,6 +1482,7 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
         trs[p].append_field_elem(proof->perm_next_eval);
     }
     mark();  // [4] round 4
+    if (cancel_requested()) return abort_job();
 
     // ---- round 5 ------------------------------------------------------------------------------------
     // pointers and lengths (proof 0's, and the stride to proof p's): launch arguments; scalars: ProofParams
@@ -1758,6 +1766,13 @@ static int link_chunk(Context* c, const ProverBufs& bf, const Bases* srs, LinkIt
                              (uint64_t)i0.size};
     ProofGraphSet* gset = single ? graph_set_for(c, ~(uint64_t)0, sub) : nullptr;
     ProofGraphSet* gs = gset && gset->proofs_seen > 0 ? gset : nullptr;
+    // abort points of a cancelled pool job: between the transform-size groups of an eager call and between the two
+    // segments; a call that captures drops the partial set
+    const bool capturing = gs && !gs->complete(2);
+    auto abort_job = [&]() {
+        if (capturing) gs->drop();
+        return cancelled(c);
+    };
     MsmPending pending;  // the commitments between commit_enqueue and commit_collect
 
     size_t at = 0;
@@ -1792,6 +1807,7 @@ static int link_chunk(Context* c, const ProverBufs& bf, const Bases* srs, LinkIt
         }
         B200_LAUNCH(k_link_roots, dim3(grid_for(max_size, 128), k), 128, 0, st)(d_desc, d_roots);
         for (size_t g = 0; g + 1 < grp.size(); ++g) {
+            if (!gs && g && cancel_requested()) return abort_job();
             const unsigned y0 = grp[g], kg = grp[g + 1] - y0;
             const Domain* dN = doms[g];
             const size_t N = (size_t)1 << dN->log_n, kN = (size_t)kg * N;
@@ -1819,6 +1835,7 @@ static int link_chunk(Context* c, const ProverBufs& bf, const Bases* srs, LinkIt
     if (rc != B200_OK) return rc;
     std::vector<g1_affine> comms(k);
     if ((rc = commit_collect(msm, pending, comms.data())) != B200_OK) return rc;
+    if (cancel_requested()) return abort_job();
     unsigned proved = 0;
     for (unsigned y = 0; y < k; ++y) {  // the flags were copied before the commitments' window sums on the same stream
         LinkItem& it = *items[y];
@@ -1902,6 +1919,7 @@ static int link_batch_run(Context* c, const Bases* srs, std::vector<LinkItem>& i
     std::stable_sort(order.begin(), order.end(), [](const LinkItem* a, const LinkItem* b) { return a->log_N < b->log_N; });
     const size_t chunk = link_batch_chunk(c, srs, its);
     for (size_t off = 0; off < k; off += chunk) {
+        if (cancel_requested()) return cancelled(c);  // an abort point: before each chunk
         const int rc = link_chunk(c, batch_bufs(c), srs, order.data() + off, (unsigned)std::min(chunk, k - off), /*single=*/false);
         if (rc != B200_OK) return rc;
     }
@@ -2249,6 +2267,7 @@ static int prove_batch_items(b200_ctx* ctx, const ProvingKey* key, std::vector<P
     B200_ENTER(ctx->c);
     const size_t chunk = prove_batch_chunk(&ctx->c, key, k);
     for (size_t off = 0; off < k; off += chunk) {
+        if (off && cancel_requested()) return cancelled(&ctx->c);  // an abort point: between chunks (prove() checks on entry)
         const unsigned cnt = (unsigned)std::min(chunk, k - off);
         const int rc = prove(&ctx->c, batch_bufs(&ctx->c), key, its.data() + off, cnt, /*single=*/false);
         if (rc != B200_OK && rc != B200_ERR_UNSATISFIED) return rc;  // B200_ERR_UNSATISFIED: every item of the chunk, see statuses

@@ -10,6 +10,8 @@
 // express workers whose contexts' streams outrank the normal workers' (and by normal workers when it backs up).
 // Reserved SMs (b200reserved.h): the same pool with the express workers' contexts bound to a group of SMs of their own
 // and the normal workers' to the rest, through green contexts (api.cu).
+// Cancellation (b200cancel.h): a ticket's queued jobs are dropped from both queues; its running ones see their job's
+// flag through b200::t_cancel, which the worker sets for the length of the call, and stop at their next abort point.
 //
 // Host-only code (std::thread) above the same C ABI the single-context entry points use.
 #include <algorithm>
@@ -22,6 +24,7 @@
 #include <thread>
 #include <vector>
 
+#include "b200cancel.h"
 #include "b200express.h"
 #include "b200prover.h"
 #include "b200reserved.h"
@@ -78,6 +81,7 @@ struct Job {
     std::shared_ptr<Bundle> bundle;  // set for the sub-jobs of a bundle (the bundle holds their ticket)
     Held held;
     std::function<int(b200_ctx*)> call;
+    std::atomic<bool> cancel{false};  // set by a cancel while the job runs; the call reads it at its abort points
 };
 
 std::unique_ptr<Job> proof_job(const b200_bundle_proof& in) {
@@ -113,8 +117,16 @@ struct Done {
     int status = B200_OK;
     std::string message;
     uint64_t completed = 0;  // the pool's completed count right after the ticket's last job
-    unsigned worker = 0;     // the worker that ran that job (express workers after the normal ones)
+    unsigned worker = 0;     // the worker that ran that job (express workers after the normal ones); kNoWorker: dropped
 };
+constexpr unsigned kNoWorker = ~0u;
+
+Done cancelled_done() {
+    Done d;
+    d.status = B200_ERR_CANCELLED;
+    d.message = "pool: the job was cancelled (B200_ERR_CANCELLED)";
+    return d;
+}
 
 // A bundle: proofs first, then — once all of them are in — the link proofs between their wire-0 polynomials; one
 // ticket for the whole thing.  Its links name proofs of the same bundle only; a settlement linked against hints kept from
@@ -135,7 +147,8 @@ struct Bundle {
     size_t pending = 0;     // sub-jobs of the current phase still queued or running
     bool linking = false;   // false: proof phase, true: link phase
     bool expedited = false; // its link jobs are forked onto the express queue
-    Done result;            // first failure wins
+    bool cancelled = false; // forks no link jobs; finishes with B200_ERR_CANCELLED once its running sub-jobs are out
+    Done result;            // first failure wins (a cancel overrides it)
 };
 
 }  // namespace
@@ -151,6 +164,7 @@ struct b200_pool {
     std::mutex mu;
     std::condition_variable cv_job, cv_express, cv_done;  // cv_job: normal workers, cv_express: express workers
     std::deque<std::unique_ptr<Job>> queue, express;
+    std::vector<Job*> running;       // per worker: the job it runs, or nullptr
     unsigned idle_express = 0;       // express workers running no job (and not yet gone at shutdown)
     std::map<uint64_t, Done> done;   // finished, not yet waited for
     std::set<uint64_t> inflight;     // queued or running
@@ -176,6 +190,51 @@ struct b200_pool {
         if (w >= n_normal) return express.empty() ? nullptr : &express;
         if (express.size() > idle_express) return &express;
         return queue.empty() ? nullptr : &queue;
+    }
+
+    // A bundle whose last sub-job is out (finished with `last`, or dropped): its ticket is done.  Caller holds mu.
+    void finish_bundle(Bundle& b, const Done& last) {
+        b.result.completed = last.completed;
+        b.result.worker = last.worker;
+        bundles.erase(b.ticket);
+        inflight.erase(b.ticket);
+        done.emplace(b.ticket, b.result);
+    }
+
+    // Cancels the jobs of `ticket`, or of every ticket with `all`: drops the queued ones (each counts as completed and
+    // failed) and flags the running ones.  Caller holds mu.  Returns how many it dropped.
+    size_t cancel(uint64_t ticket, bool all) {
+        auto hit = [&](const Job& j) { return all || j.ticket == ticket; };
+        for (auto& kv : bundles)
+            if (all || kv.first == ticket) {
+                kv.second->cancelled = true;  // no link jobs from now on, and the ticket's status is the cancel
+                kv.second->result = cancelled_done();
+            }
+        for (Job* j : running)
+            if (j && hit(*j)) j->cancel = true;
+        std::vector<std::unique_ptr<Job>> gone;
+        for (std::deque<std::unique_ptr<Job>>* q : {&queue, &express}) {
+            std::deque<std::unique_ptr<Job>> rest;
+            for (std::unique_ptr<Job>& j : *q) {
+                if (hit(*j)) gone.push_back(std::move(j));
+                else rest.push_back(std::move(j));
+            }
+            q->swap(rest);
+        }
+        for (std::unique_ptr<Job>& j : gone) {
+            ++n_completed;
+            ++n_failed;
+            Done d = cancelled_done();
+            d.completed = n_completed;
+            d.worker = kNoWorker;
+            if (!j->bundle) {
+                inflight.erase(j->ticket);
+                done.emplace(j->ticket, std::move(d));
+            } else if (--j->bundle->pending == 0) {
+                finish_bundle(*j->bundle, d);
+            }
+        }
+        return gone.size();
     }
 
     void notify_jobs(bool to_express) {
@@ -204,13 +263,17 @@ struct b200_pool {
                 q->pop_front();
                 ++n_running;
                 if (is_express) --idle_express;
+                running[w] = job.get();
             }
             Done d;
+            b200::t_cancel = &job->cancel;
             d.status = job->call(ctxs[w]);
+            b200::t_cancel = nullptr;
             if (d.status != B200_OK) d.message = b200_last_error();  // this worker's thread-local message
             bool new_jobs = false, new_express = false;
             {
                 std::lock_guard<std::mutex> lk(mu);
+                running[w] = nullptr;
                 --n_running;
                 if (is_express) ++idle_express;
                 ++n_completed;
@@ -233,11 +296,7 @@ struct b200_pool {
                             new_jobs = true;
                             new_express = b.expedited;
                         } else {
-                            b.result.completed = d.completed;
-                            b.result.worker = d.worker;
-                            bundles.erase(b.ticket);
-                            inflight.erase(b.ticket);
-                            done.emplace(b.ticket, b.result);
+                            finish_bundle(b, d);
                         }
                     }
                 }
@@ -324,6 +383,7 @@ static int pool_create(int device, unsigned n_workers, unsigned n_express, const
     }
     p->n_normal = n_workers;
     p->idle_express = n_express;
+    p->running.assign(p->ctxs.size(), nullptr);
     if (groups) {
         p->sms[0] = groups[1].sms;
         p->sms[1] = groups[0].sms;
@@ -640,6 +700,42 @@ int b200_pool_expedite(b200_pool* pool, uint64_t ticket, size_t* moved) {
     *moved = n;
     if (n) pool->notify_jobs(true);
     return B200_OK;
+    B200_CATCH
+}
+
+// b200_pool_cancel and b200_pool_cancel_all (all = true, ticket unused)
+static int pool_cancel(b200_pool* pool, uint64_t ticket, bool all, size_t* dropped, const char* who) {
+    if (!pool || !dropped || (!all && ticket == 0)) {
+        b200::set_error(std::string(who) + ": null pool or dropped, or ticket 0");
+        return B200_ERR_INVALID;
+    }
+    size_t n = 0;
+    {
+        std::lock_guard<std::mutex> lk(pool->mu);
+        if (!all && ticket >= pool->next_ticket) {
+            b200::set_error(std::string(who) + ": unknown ticket");
+            return B200_ERR_INVALID;
+        }
+        if (!all && !pool->inflight.count(ticket) && !pool->done.count(ticket)) {
+            b200::set_error(std::string(who) + ": ticket already waited for");
+            return B200_ERR_INVALID;
+        }
+        n = pool->cancel(ticket, all);
+    }
+    *dropped = n;
+    if (n) pool->cv_done.notify_all();  // waits on the dropped tickets, and b200_pool_wait_all
+    return B200_OK;
+}
+
+int b200_pool_cancel(b200_pool* pool, uint64_t ticket, size_t* dropped) {
+    B200_TRY
+    return pool_cancel(pool, ticket, false, dropped, "pool_cancel");
+    B200_CATCH
+}
+
+int b200_pool_cancel_all(b200_pool* pool, size_t* dropped) {
+    B200_TRY
+    return pool_cancel(pool, 0, true, dropped, "pool_cancel_all");
     B200_CATCH
 }
 
@@ -1134,6 +1230,32 @@ int b200_box_expedite(b200_box* box, uint64_t ticket, size_t* moved) {
     uint64_t t = 0;
     b200_pool* p = box_ticket_pool(box, ticket, "box_expedite", &t);
     return p ? b200_pool_expedite(p, t, moved) : B200_ERR_INVALID;
+    B200_CATCH
+}
+
+int b200_box_cancel(b200_box* box, uint64_t ticket, size_t* dropped) {
+    B200_TRY
+    uint64_t t = 0;
+    b200_pool* p = box_ticket_pool(box, ticket, "box_cancel", &t);
+    return p ? b200_pool_cancel(p, t, dropped) : B200_ERR_INVALID;
+    B200_CATCH
+}
+
+int b200_box_cancel_all(b200_box* box, size_t* dropped) {
+    B200_TRY
+    if (!box || !dropped) {
+        b200::set_error("box_cancel_all: null box or dropped");
+        return B200_ERR_INVALID;
+    }
+    size_t total = 0;
+    for (b200_pool* p : box->pools) {
+        size_t n = 0;
+        const int rc = b200_pool_cancel_all(p, &n);
+        if (rc != B200_OK) return rc;
+        total += n;
+    }
+    *dropped = total;
+    return B200_OK;
     B200_CATCH
 }
 

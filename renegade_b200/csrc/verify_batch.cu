@@ -412,6 +412,7 @@ struct Batch {
 
     // verdicts of the items listed in `idx` (all valid), whose combined check is known to fail
     int bisect(const std::vector<uint32_t>& idx, const uint64_t g2_tau_h[16], const uint64_t g2_h[16], uint8_t* verdicts) {
+        if (cancel_requested()) return cancelled(c);  // an abort point of a cancelled pool job: each bisection step
         if (idx.size() == 1) {
             verdicts[idx[0]] = 0;
             return B200_OK;
@@ -611,6 +612,8 @@ extern "C" int b200_plonk_batch_verify(b200_ctx* ctx, const b200_verifying_key* 
     cudaStream_t st = ctx->c.stream;
     Batch bt;
     bt.c = &ctx->c;
+    // abort points of a cancelled pool job: on entry, after the item digests are read back, before each combined check
+    if (cancel_requested()) return cancelled(&ctx->c);
     if ((rc = bt.stage(vks, n_vks, proofs, n_proofs, links, n_links)) != B200_OK) return rc;
     B200_LAUNCH(k_gather_bases, grid_of(k, 128), 128, 0, st)((const ItemDev*)bt.items.p, k, (const vt::ProofIn*)bt.proofs.p,
                                                             (const LinkDev*)bt.links.p, (g1_affine*)bt.bases_pts.p);
@@ -621,6 +624,7 @@ extern "C" int b200_plonk_batch_verify(b200_ctx* ctx, const b200_verifying_key* 
     B200_CUDA(cudaMemcpyAsync(hdig.data(), bt.digest.p, k * 32, cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaMemcpyAsync(hst.data(), bt.state.p, k * sizeof(ItemState), cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaStreamSynchronize(st));
+    if (cancel_requested()) return cancelled(&ctx->c);
     Seed seed;
     {
         static const char tag[] = "b200 batch verify v1";
@@ -646,6 +650,7 @@ extern "C" int b200_plonk_batch_verify(b200_ctx* ctx, const b200_verifying_key* 
         if (mask[i]) valid.push_back((uint32_t)i);
     }
     bool ok = true;
+    if (cancel_requested()) return cancelled(&ctx->c);
     if (!valid.empty() && (rc = bt.check(mask, g2_tau_h, g2_h, &ok)) != B200_OK) return rc;
     *all_accepted = ok && valid.size() == k ? 1 : 0;
     if (verdicts) {
@@ -674,7 +679,10 @@ extern "C" int b200_plonk_verify_each(b200_ctx* ctx, const b200_verifying_key* v
     cudaStream_t st = ctx->c.stream;
     Batch bt;
     bt.c = &ctx->c;
+    // abort points of a cancelled pool job: on entry and between the staging and the per-item checks
+    if (cancel_requested()) return cancelled(&ctx->c);
     if ((rc = bt.stage(vks, n_vks, proofs, n_proofs, links, n_links)) != B200_OK) return rc;
+    if (cancel_requested()) return cancelled(&ctx->c);
     DevBuf d_q, d_ab, d_one, d_verdicts;
     if ((rc = upload(&d_q, q, st)) || (rc = d_ab.reserve(2 * k * sizeof(g1_affine))) || (rc = d_one.reserve(k)) ||
         (rc = d_verdicts.reserve(k)))

@@ -206,6 +206,28 @@ class ProverService:
         self.expedite_settlements = expedite_settlements
         self.stats = {"requests": 0, "proofs": 0, "link_proofs": 0, "errors": 0}
         self._lock = threading.Lock()
+        self._idle = threading.Condition(self._lock)  # notified when the last request in flight is answered
+        self._in_flight = 0
+        self._stopping = False
+
+    def shutdown(self, server=None) -> None:
+        """Stop now, the way the reference's proof manager stops on its cancel channel: no request is accepted any more
+        (503), `server` (what `make_server` returned) stops serving, every job on the pool is cancelled
+        (`ProverPool.cancel_all`), so the requests still in flight are answered with a 500 at once instead of after their
+        proofs, and once they all are, the pool is closed.  Without a pool the requests in flight run to their end."""
+        with self._lock:
+            self._stopping = True
+        if server is not None:
+            server.shutdown()
+        with self._idle:
+            while self._in_flight:
+                if self.pool is not None:  # also the jobs a request submitted just after an earlier cancel_all
+                    self.pool.cancel_all()
+                self._idle.wait(0.05)
+        if self.pool is not None:
+            self.pool.close()
+        if server is not None:
+            server.server_close()
 
     # -- proving ------------------------------------------------------------------------------------------------
     def handle(self, path: str, body: Dict[str, Any]) -> Dict[str, Any]:
@@ -299,6 +321,18 @@ class ProverService:
             def do_POST(self):
                 with service._lock:
                     service.stats["requests"] += 1
+                    if service._stopping:
+                        self.close_connection = True
+                        return self._send(503, {"error": "the prover service is shutting down"})
+                    service._in_flight += 1
+                try:
+                    self._post()
+                finally:
+                    with service._lock:
+                        service._in_flight -= 1
+                        service._idle.notify_all()
+
+            def _post(self):
                 try:
                     n = int(self.headers.get("Content-Length", "0"))
                 except ValueError:
@@ -324,6 +358,10 @@ class ProverService:
                     with service._lock:
                         service.stats["errors"] += 1
                     return self._send(500, {"error": f"ProverError::{e}"})
+                except _lib.B200Error as e:  # a job cancelled at shutdown on a path that does not wrap library errors
+                    with service._lock:
+                        service.stats["errors"] += 1
+                    return self._send(500, {"error": f"ProverError::Plonk({e})"})
                 self._send(200, resp)
 
         return ThreadingHTTPServer((host, port), Handler)

@@ -13,6 +13,7 @@
 //! | `native_proof_manager.rs:514-660` | a settlement arm: `singleprover_prove_with_hint`, then `link_proofs` against each stored hint | [`GpuProver::prove_settlement`], [`GpuProver::prove_settlement_from_witness`] |
 //! | `gossip-server/src/orderbook.rs:180-229` | the order check: two proofs and one link proof per order (`todo!` upstream) | [`GpuProver::submit_verify`], [`GpuProver::submit_verify_combined`] |
 //! | `primitives/srs.rs:63-71` | `parse_ptau_file` + `powers_of_g` | [`GpuProver::load_srs`] |
+//! | `native_proof_manager.rs:167-178` | the cancel channel: `ProofManagerError::Cancelled` at once | [`GpuProver::cancel_all`], [`GpuProver::shutdown_now`] |
 //!
 //! Marshalling rules (SURVEY.md §7 "Rust ABI hazards"): `Fr`/`Fq` are `Fp(BigInt<4>, PhantomData)` holding the
 //! Montgomery limbs — reading `.0 .0` is the value the C ABI wants; `G1Affine` is `repr(Rust)` {x, y, infinity} and is
@@ -30,6 +31,7 @@ pub mod ffi_verifyjobs;
 pub mod ffi_express;
 pub mod ffi_reserved;
 pub mod ffi_selftest;
+pub mod ffi_cancel;
 
 use ark_bn254::{Bn254, Fq, Fr, G1Affine};
 use ark_ff::{BigInt, UniformRand};
@@ -69,7 +71,7 @@ fn check(rc: c_int) -> Result<(), PlonkError> {
     let msg = unsafe { CStr::from_ptr(ffi::b200_last_error()) }.to_string_lossy().into_owned();
     Err(match rc {
         ffi::B200_ERR_UNSATISFIED => PlonkError::WrongQuotientPolyDegree(0, 0),
-        _ => PlonkError::InvalidParameters(msg),
+        _ => PlonkError::InvalidParameters(msg),  // B200_ERR_CANCELLED too: its message names the code
     })
 }
 
@@ -480,6 +482,43 @@ impl GpuProver {
         })?;
         Ok(report)
     }
+
+    /// Cancels a pool job by ticket (`b200_pool_cancel`): its queued jobs are dropped and never run, a running one stops
+    /// at its next abort point (a host round trip; no kernel is interrupted).  Returns how many queued jobs were dropped.
+    /// Its wait then fails with `B200_ERR_CANCELLED` (or returns its real status if it finished first); the job's outputs
+    /// must not be read.  A finished or already cancelled ticket is `Ok(0)`.
+    pub fn cancel(&self, ticket: u64) -> Result<usize, PlonkError> {
+        let mut dropped = 0usize;
+        check(unsafe { ffi_cancel::b200_pool_cancel(self.pool, ticket, &mut dropped) })?;
+        Ok(dropped)
+    }
+
+    /// `cancel` for every job the pool holds (`b200_pool_cancel_all`).  Jobs submitted afterwards run as usual.
+    pub fn cancel_all(&self) -> Result<usize, PlonkError> {
+        let mut dropped = 0usize;
+        check(unsafe { ffi_cancel::b200_pool_cancel_all(self.pool, &mut dropped) })?;
+        Ok(dropped)
+    }
+
+    /// Stops now: cancels every job, then destroys the pool (dropping `self`), which waits at most for each worker's
+    /// next abort point instead of draining the queue.  The shape of the reference's cancel channel
+    /// (native_proof_manager.rs:167-178): on the signal the coordinator returns `ProofManagerError::Cancelled`; the
+    /// threads still blocked in a wait see `B200_ERR_CANCELLED` once `cancel_all` runs, so their tickets are gone
+    /// before this is called:
+    ///
+    /// ```ignore
+    /// if cancel_channel.has_changed()? {
+    ///     prover.cancel_all()?;                 // every waiting job thread returns its error now
+    ///     pool_threads.join();                  // the borrows of `prover` end
+    ///     Arc::try_unwrap(prover).ok().unwrap().shutdown_now()?;
+    ///     return Err(ProofManagerError::Cancelled("received cancel signal".to_string()));
+    /// }
+    /// ```
+    pub fn shutdown_now(self) -> Result<(), PlonkError> {
+        let r = self.cancel_all().map(|_| ());
+        drop(self);  // b200_pool_destroy: nothing is left queued
+        r
+    }
 }
 
 /// replaces `read_ptau_section3` (srs.rs:147-157): `(h, beta_h)`, the two G2 records of the ptau's section 3 in the
@@ -527,6 +566,13 @@ pub struct VerifyTicket<'a> {
     _prover: std::marker::PhantomData<&'a GpuProver>,
 }
 unsafe impl Send for VerifyTicket<'_> {}
+
+impl VerifyTicket<'_> {
+    /// The pool ticket, for [`GpuProver::cancel`].
+    pub fn id(&self) -> u64 {
+        self.ticket
+    }
+}
 
 impl Drop for VerifyTicket<'_> {
     fn drop(&mut self) {

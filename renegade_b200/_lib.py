@@ -1,9 +1,10 @@
 """ctypes binding of libb200prover.so, derived from its C ABI, include/b200prover.h, include/b200settlement.h,
-include/b200verifyjobs.h, include/b200express.h, include/b200reserved.h, include/b200selftest.h and include/b200cancel.h.
+include/b200verifyjobs.h, include/b200express.h, include/b200reserved.h, include/b200selftest.h, include/b200cancel.h and
+include/b200compact.h.
 
 The headers are parsed once, at import, and are the only description of the ABI here: `EXPORTS` lists the core
 header's entry points in header order, `SETTLEMENT_EXPORTS` those of the settlement header, `VERIFY_JOB_EXPORTS` those of
-the verification-job header, `EXPRESS_EXPORTS` those of the express-lane header, `RESERVED_EXPORTS` those of the reserved-SM header, `SELFTEST_EXPORTS` those of the self-test header, `CANCEL_EXPORTS` those of the cancellation header, `B200_OK` / `B200_ERR_*` are the `#define`s of the core header and of the cancellation header (B200_ERR_CANCELLED), `STRUCTS` holds one ctypes
+the verification-job header, `EXPRESS_EXPORTS` those of the express-lane header, `RESERVED_EXPORTS` those of the reserved-SM header, `SELFTEST_EXPORTS` those of the self-test header, `CANCEL_EXPORTS` those of the cancellation header, `COMPACT_EXPORTS` those of the compact-key header (and `FOOTPRINT_PARTS` its one macro), `B200_OK` / `B200_ERR_*` are the `#define`s of the core header and of the cancellation header (B200_ERR_CANCELLED), `STRUCTS` holds one ctypes
 class per struct of any header (by C name), and `load()` gives every entry point the argtypes / restype of its
 declaration.  tools/gen_rust_ffi.py writes the Rust shim's ffi*.rs modules from the same parse, and tests/test_abi_cpu.py checks the parse, the struct layouts and the scalar types
 against a C compiler.
@@ -26,6 +27,7 @@ EXPRESS_HEADER = os.path.join(os.path.dirname(_HERE), "include", "b200express.h"
 RESERVED_HEADER = os.path.join(os.path.dirname(_HERE), "include", "b200reserved.h")
 SELFTEST_HEADER = os.path.join(os.path.dirname(_HERE), "include", "b200selftest.h")
 CANCEL_HEADER = os.path.join(os.path.dirname(_HERE), "include", "b200cancel.h")
+COMPACT_HEADER = os.path.join(os.path.dirname(_HERE), "include", "b200compact.h")
 # B200_LIB_PATH: developer knob to load an alternative build of the same library (tuning experiments)
 LIB_PATH = os.environ.get("B200_LIB_PATH") or os.path.join(_HERE, "libb200prover.so")
 
@@ -98,7 +100,8 @@ def _struct(name: str, fields) -> type:
     return type(name, (C.Structure,), {"_fields_": members})
 
 
-for _h in (HEADER, SETTLEMENT_HEADER, VERIFY_JOB_HEADER, EXPRESS_HEADER, RESERVED_HEADER, SELFTEST_HEADER, CANCEL_HEADER):
+for _h in (HEADER, SETTLEMENT_HEADER, VERIFY_JOB_HEADER, EXPRESS_HEADER, RESERVED_HEADER, SELFTEST_HEADER, CANCEL_HEADER,
+           COMPACT_HEADER):
     if not os.path.exists(_h):
         raise ImportError(f"{_h} is missing: the binding of libb200prover is derived from it")
 _, _structs, _funcs, _codes = parse_header()
@@ -108,6 +111,8 @@ _, _e_structs, _e_funcs, _ = parse_header(EXPRESS_HEADER)
 _, _r_structs, _r_funcs, _ = parse_header(RESERVED_HEADER)
 _, _t_structs, _t_funcs, _ = parse_header(SELFTEST_HEADER)
 _, _c_structs, _c_funcs, _c_codes = parse_header(CANCEL_HEADER)
+_, _k_structs, _k_funcs, _k_macros = parse_header(COMPACT_HEADER)
+FOOTPRINT_PARTS = _k_macros["B200_FOOTPRINT_PARTS"]  # entries of b200_plonk_footprint's out[]
 _codes = {**_codes, **_c_codes}  # the code table: the core header's, then B200_ERR_CANCELLED
 globals().update(_codes)  # B200_OK, B200_ERR_INVALID, ..., B200_ERR_UNSATISFIED, B200_ERR_CANCELLED
 EXPORTS = [name for name, _, _ in _funcs]
@@ -117,10 +122,11 @@ EXPRESS_EXPORTS = [name for name, _, _ in _e_funcs]
 RESERVED_EXPORTS = [name for name, _, _ in _r_funcs]
 SELFTEST_EXPORTS = [name for name, _, _ in _t_funcs]
 CANCEL_EXPORTS = [name for name, _, _ in _c_funcs]
+COMPACT_EXPORTS = [name for name, _, _ in _k_funcs]
 STRUCTS = {name: _struct(name, fields) for name, fields in {**_structs, **_s_structs, **_v_structs, **_e_structs,
-                                                        **_r_structs, **_t_structs, **_c_structs}.items()}
+                                                        **_r_structs, **_t_structs, **_c_structs, **_k_structs}.items()}
 _SIGNATURES = {name: ([_ctype(t) for _, t in args], _ctype(ret, ret=True))
-               for name, ret, args in _funcs + _s_funcs + _v_funcs + _e_funcs + _r_funcs + _t_funcs + _c_funcs}
+               for name, ret, args in _funcs + _s_funcs + _v_funcs + _e_funcs + _r_funcs + _t_funcs + _c_funcs + _k_funcs}
 
 
 class B200Error(RuntimeError):

@@ -388,6 +388,11 @@ class ProvingKey:
         """Length of the witness vector a proof of this key takes; 0 for a key without wiring (`preprocess`)."""
         return int(self._ctx._lib.b200_pk_num_vars(self._h))
 
+    @property
+    def compact(self) -> bool:
+        """True for a key made with compact=True (b200compact.h): no coset tables, round 3 one coset at a time."""
+        return bool(self._ctx._lib.b200_pk_is_compact(self._h))
+
     def free(self):
         if self._h:
             self._ctx._lib.b200_pk_free(self._ctx._h, self._h)
@@ -587,28 +592,41 @@ class PlonkKzgSnark:
 
     @staticmethod
     def preprocess(ctx: Context, srs: Bases, log_n: int, num_inputs: int, selectors: np.ndarray,
-                   perm: np.ndarray, k: np.ndarray) -> ProvingKey:
+                   perm: np.ndarray, k: np.ndarray, compact: bool = False) -> ProvingKey:
+        """compact=True: a compact key (b200_plonk_preprocess_compact), the same verifying key and proofs from a fraction
+        of the device memory (`footprint`), at the cost of round-3 time."""
         sel = np.ascontiguousarray(selectors, dtype=np.uint64).reshape(13, 1 << log_n, 4)
         pm = np.ascontiguousarray(perm, dtype=np.uint64).reshape(5 << log_n)
         kk = np.ascontiguousarray(k, dtype=np.uint64).reshape(5, 4)
         h = C.c_void_p()
-        _lib.check(ctx._lib.b200_plonk_preprocess(ctx._h, srs._h, log_n, num_inputs, _ptr(sel), _ptr(pm), _ptr(kk),
-                                                  C.byref(h)))
+        fn = ctx._lib.b200_plonk_preprocess_compact if compact else ctx._lib.b200_plonk_preprocess
+        _lib.check(fn(ctx._h, srs._h, log_n, num_inputs, _ptr(sel), _ptr(pm), _ptr(kk), C.byref(h)))
         return ProvingKey(ctx, h, log_n, num_inputs, kk)
 
     @staticmethod
     def preprocess_wiring(ctx: Context, srs: Bases, log_n: int, num_inputs: int, selectors: np.ndarray,
-                          wire_vars: np.ndarray, num_vars: int, k: np.ndarray) -> ProvingKey:
+                          wire_vars: np.ndarray, num_vars: int, k: np.ndarray, compact: bool = False) -> ProvingKey:
         """`preprocess` from the circuit's wiring (b200_plonk_preprocess_wiring): wire_vars[i, j] = the variable on wire i of
         row j (5 x n, < num_vars).  The copy permutation is derived on the device and the key keeps the wiring, so its
-        proofs are made from witness vectors (`prove_witness`)."""
+        proofs are made from witness vectors (`prove_witness`).  compact=True as for `preprocess`."""
         sel = np.ascontiguousarray(selectors, dtype=np.uint64).reshape(13, 1 << log_n, 4)
         wv = np.ascontiguousarray(wire_vars, dtype=np.uint32).reshape(5 << log_n)
         kk = np.ascontiguousarray(k, dtype=np.uint64).reshape(5, 4)
         h = C.c_void_p()
-        _lib.check(ctx._lib.b200_plonk_preprocess_wiring(ctx._h, srs._h, log_n, num_inputs, _ptr(sel), wv.ctypes.data_as(C.c_void_p), num_vars,
-                                                         _ptr(kk), C.byref(h)))
+        fn = ctx._lib.b200_plonk_preprocess_wiring_compact if compact else ctx._lib.b200_plonk_preprocess_wiring
+        _lib.check(fn(ctx._h, srs._h, log_n, num_inputs, _ptr(sel), wv.ctypes.data_as(C.c_void_p), num_vars, _ptr(kk), C.byref(h)))
         return ProvingKey(ctx, h, log_n, num_inputs, kk)
+
+    FOOTPRINT_PARTS = ("key", "ntt_scratch", "domain", "srs", "msm_scratch", "runtime", "workspace", "ntt_scratch2",
+                       "batch_workspace", "batch_ntt_scratch", "batch_ntt_scratch2", "batch_msm_scratch")
+
+    @staticmethod
+    def footprint(log_n: int, k: int = 1, compact: bool = False) -> dict:
+        """b200_plonk_footprint: the device bytes of one context with one key of domain 2^log_n and a call of k proofs,
+        {part: bytes} in the header's order.  Needs no device."""
+        out = (C.c_uint64 * _lib.FOOTPRINT_PARTS)()
+        _lib.check(_lib.load().b200_plonk_footprint(log_n, k, int(compact), out))
+        return dict(zip(PlonkKzgSnark.FOOTPRINT_PARTS, (int(v) for v in out)))
 
     @staticmethod
     def prove_witness(ctx: Context, pk: ProvingKey, witness, blinders: np.ndarray, want_challenges: bool = False):

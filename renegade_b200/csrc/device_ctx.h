@@ -198,6 +198,11 @@ int msm_launch_batch(const Bases* b, size_t base_off, const fe* d_scalars, size_
                      int montgomery, MsmEpilogue e, MsmScratch* s, cudaStream_t st, MsmPending* pending,
                      g1_xyzz* d_point = nullptr);
 int msm_finish_batch(MsmScratch* s, const MsmPending& p, g1_affine* out, int* out_inf);
+// Bytes an MsmScratch grows to for one launch of `batch` MSMs of `points` points under plan `pl`, rounded up: the
+// histogram, offsets and cursor, one entry per digit, the buckets, the segment index, sums and order, the heavy-bucket
+// list, the reduction tree (a serial level of fan-in >= 2 plus the row and column sums) and the window and bit sums.
+// For planning (b200_plonk_footprint); msm_launch_batch makes the allocations.
+size_t msm_scratch_estimate(const MsmPlan& pl, size_t points, size_t batch);
 // the identity as the device point of an MSM without points, in one launch
 int msm_identity_point(g1_xyzz* d_point, cudaStream_t st);
 void msm_collect_timing(MsmScratch* s, size_t n, unsigned batch);

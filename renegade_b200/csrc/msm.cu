@@ -1174,6 +1174,18 @@ static size_t sm_count(const MsmScratch* s) {
     return (size_t)sms;
 }
 
+size_t msm_scratch_estimate(const MsmPlan& pl, size_t points, size_t batch) {
+    const size_t n_buckets = (size_t)pl.n_phys * ((size_t)1 << (pl.c - 1)) * batch;
+    const size_t n_windows = (size_t)pl.n_phys * batch;
+    const size_t entries = points * (size_t)pl.n_digits * batch;
+    const size_t segs = entries / kSegLen + n_buckets;
+    const size_t heavy = segs / (kCombineSeq + 1) + 2;
+    const int l_log = pl.c / 2;
+    const size_t tree = (n_buckets >> 1) + n_windows * (((size_t)1 << l_log) + ((size_t)1 << (pl.c - 1 - l_log))) + 1;
+    return 4 * (5 * n_buckets + 2) + 4 * entries + (sizeof(g1_xyzz) + 8) * segs + 4 * segs + 4 * heavy +
+           sizeof(g1_xyzz) * (tree + 65 * n_windows) + 4096;
+}
+
 int msm_launch_batch(const Bases* b, size_t base_off, const fe* d_scalars, size_t n, size_t stride, unsigned batch,
                      int montgomery, MsmEpilogue epilogue, MsmScratch* s, cudaStream_t st, MsmPending* pending,
                      g1_xyzz* d_point) {

@@ -19,6 +19,7 @@
 #include <cstring>
 #include <vector>
 
+#include "b200compact.h"
 #include "b200prover.h"
 #include "b200settlement.h"
 #include "device_ctx.h"
@@ -386,6 +387,65 @@ __global__ void __launch_bounds__(128) k_quotient(QuotArgs a) {
     fe_store(a.out + pr * m + i, acc);
 }
 
+// k_quotient on one coset, for compact keys (b200compact.h): every input holds coset `j` only (n points, s_j w_n^h), so
+// z(w x) is the next point mod n and 1 / Z_H = 1 / (c_j - 1) is one value.  Same products in the same order as
+// k_quotient, hence the same values.  blockIdx.y: proof.
+struct QuotCosetArgs {
+    const fe* sel;     // NS x n: the key's selectors on coset j
+    const fe* sig;     // NW x n
+    const fe* ext;     // per proof NW x n: wires 0..4
+    const fe* pi;      // per proof n: public-input polynomial
+    const fe* zext;    // per proof n: z
+    const fe* pts;     // nc x n: the key's evaluation points (row j read)
+    const fe* l1_inv;  // nc x n
+    fe* out;           // proof p's coset j at out + p * ostride + j * n
+    size_t ostride;
+    unsigned log_n;
+    KArr k;
+    const fe* chal;    // device: beta, gamma, alpha, alpha^2
+    size_t dstride;
+    fe zh_inv;         // 1 / (c_j - 1)
+};
+__global__ void __launch_bounds__(128) k_quotient_coset(QuotCosetArgs a, int j) {
+    const size_t n = (size_t)1 << a.log_n;
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const size_t pr = blockIdx.y, at = (size_t)j * n + i;
+    const fe* ext = a.ext + pr * NW * n;
+    const fe* zext = a.zext + pr * n;
+    const fe* chal = a.chal + pr * a.dstride;
+    const fe beta = fe_load_ro(chal), gamma = fe_load_ro(chal + 1);
+    fe w[NW];
+#pragma unroll
+    for (int q = 0; q < NW; ++q) w[q] = fe_load_ro(ext + q * n + i);
+    fe acc = FADD(fe_load_ro(a.sel + 11 * n + i), fe_load_ro(a.pi + pr * n + i));
+#pragma unroll 1
+    for (int q = 0; q < 4; ++q) {
+        acc = FADD(acc, FMUL(fe_load_ro(a.sel + q * n + i), w[q]));
+        const fe w2 = fe_sqr<Fr>(w[q]);
+        acc = FADD(acc, FMUL(fe_load_ro(a.sel + (6 + q) * n + i), FMUL(fe_sqr<Fr>(w2), w[q])));
+    }
+    const fe w01 = FMUL(w[0], w[1]), w23 = FMUL(w[2], w[3]);
+    acc = FADD(acc, FMUL(fe_load_ro(a.sel + 4 * n + i), w01));
+    acc = FADD(acc, FMUL(fe_load_ro(a.sel + 5 * n + i), w23));
+    acc = FADD(acc, FMUL(fe_load_ro(a.sel + 12 * n + i), FMUL(FMUL(w01, w23), w[4])));
+    acc = FSUB(acc, FMUL(fe_load_ro(a.sel + 10 * n + i), w[4]));
+    const fe zx = fe_load_ro(zext + i);
+    const fe zxw = fe_load_ro(zext + ((i + 1) & (n - 1)));
+    const fe bx = FMUL(beta, fe_load_ro(a.pts + at));
+    fe p1 = zx, p2 = zxw;
+#pragma unroll 1
+    for (int q = 0; q < NW; ++q) {
+        const fe t = FADD(w[q], gamma);
+        p1 = FMUL(p1, FADD(t, FMUL(a.k.v[q], bx)));
+        p2 = FMUL(p2, FADD(t, FMUL(beta, fe_load_ro(a.sig + q * n + i))));
+    }
+    acc = FADD(acc, FMUL(fe_load_ro(chal + 2), FSUB(p1, p2)));
+    acc = FMUL(acc, a.zh_inv);
+    acc = FADD(acc, FMUL(FMUL(fe_load_ro(chal + 3), FSUB(zx, fe_one<Fr>())), fe_load_ro(a.l1_inv + at)));
+    fe_store(a.out + pr * a.ostride + at, acc);
+}
+
 // flag bit 0: a coefficient above `deg` is non-zero; bit 1: coefficient `deg` is zero; blockIdx.y: proof (its m
 // coefficients and its own flag)
 __global__ void k_check_degree(const fe* __restrict__ q, size_t deg, size_t m, uint32_t* flag) {
@@ -563,6 +623,8 @@ struct ProvingKey {
     uint32_t* wire_vars = nullptr;
     size_t num_vars = 0;
     std::vector<uint32_t> pub_vars;
+    // compact keys (b200compact.h) hold no ce_sel / ce_sig: round 3 evaluates the key one coset at a time
+    bool compact = false;
     ~ProvingKey() {
         for (fe* p : {sel_coeffs, sig_coeffs, sig_evals, ce_sel, ce_sig, dom, coset_pts, l1_inv, cscale, cscale_inv})
             if (p) cudaFree(p);
@@ -741,6 +803,7 @@ static void eval_batch(const fe* const* polys, const size_t* lens, const fe* poi
 // input) for the commitments.  With k = 1 this is the single prover's layout.
 struct Workspace {
     fe *wires_ev, *wpoly, *pi_poly, *zpoly, *num, *den, *tmp, *scan, *ext, *zext, *quot, *split, *lin, *sdiv, *hscr, *escr, *evals;
+    fe* kev = nullptr;  // compact keys: the key's NS + NW polynomials on the current coset, directly before `ext`
     uint32_t* flag;  // one per proof
     size_t S;  // stride of the (n + 3)-coefficient polynomials
 };
@@ -751,7 +814,16 @@ static size_t workspace_elems(size_t n, unsigned k) {
                 4 * (S / CH + 4 * CH + 64) + kMaxEval * (S / CH + S / CH / CH + 2 * CH + 16) + kEvalSlots) +
            (k + 7) / 8 + 8;
 }
-static Workspace carve(fe* base, size_t n, unsigned k) {
+// Compact keys: round 3 transforms, per coset, one batch of the key's NS + NW polynomials and each proof's NW wires, public
+// input and z (n elements each), in place of the default key's 7 coset tables per proof (ext and zext, 7 x 8n).
+static size_t coset_batch(unsigned k) { return NS + NW + (size_t)(NW + 2) * k; }
+static size_t compact_workspace_elems(size_t n, unsigned k) { return workspace_elems(n, k) - (size_t)k * 7 * 8 * n + coset_batch(k) * n; }
+// NTT scratch of a compact key's prover call: the per-coset batch, the round-1 batch of (NW + 1) k polynomials of n + 4,
+// and the k staged witness vectors
+static size_t compact_nscr_elems(size_t n, unsigned k, size_t num_vars) {
+    return std::max({coset_batch(k) * n, (size_t)k * (NW + 1) * (n + 4), (size_t)k * num_vars});
+}
+static Workspace carve(fe* base, size_t n, unsigned k, bool compact = false) {
     Workspace w;
     const size_t S = n + 4, m = 8 * n;
     w.S = S;
@@ -764,8 +836,15 @@ static Workspace carve(fe* base, size_t n, unsigned k) {
     w.den = p; p += k * n;
     w.tmp = p; p += k * n;
     w.scan = p; p += k * (2 * (n / CH) + 4 * CH + 64);  // all levels of the product scan: n / CH * (1 + 1/CH + ...)
-    w.ext = p; p += k * (NW + 1) * m;
-    w.zext = p; p += k * m;
+    if (compact) {  // [key NS + NW][wires k NW][public inputs k][z k], n each: one batch of transforms per coset
+        w.kev = p;
+        w.ext = p + (NS + NW) * n;
+        w.zext = w.ext + k * (NW + 1) * n;
+        p += coset_batch(k) * n;
+    } else {
+        w.ext = p; p += k * (NW + 1) * m;
+        w.zext = p; p += k * m;
+    }
     w.quot = p; p += k * m;
     w.split = p; p += k * NW * S;
     w.lin = p; p += k * S;
@@ -808,10 +887,60 @@ static int coset_evals(const ProvingKey* pk, const Domain* dn, const fe* src, si
     return ntt_device(dn, dst, scratch, /*inverse=*/0, /*coset=*/0, count * (unsigned)pk->nc, n, st);
 }
 
+// Round 3 of a compact key, for the k proofs of a call: per coset j, the key's NS + NW polynomials and each proof's wires,
+// public input and z are folded onto coset j and transformed in one batch (w.kev .. w.zext), and k_quotient_coset fills
+// quotient rows j of every proof.  Then the inverse transforms (scratch: the per-coset buffers, free by then) and the
+// coset combination, as for a default key.  quot ends up as the default key's.
+static int compact_quotient(const ProvingKey* pk, const Domain* dn, const Workspace& w, unsigned k, const fe* chal, size_t dstride,
+                            fe* nscr, cudaStream_t st) {
+    const size_t n = pk->n, m = pk->m, S = w.S;
+    const unsigned grid = grid_for(n, 256);
+    for (int j = 0; j < pk->nc; ++j) {
+        CosetConsts cc{};
+        cc.cn[0] = pk->cc.cn[j];
+        const fe* cs = pk->cscale + (size_t)j * n;
+        B200_LAUNCH(k_coset_fold, dim3(grid, 1, NS), 256, 0, st)(pk->sel_coeffs, n, n, n, 1, cc, cs, w.kev);
+        B200_LAUNCH(k_coset_fold, dim3(grid, 1, NW), 256, 0, st)(pk->sig_coeffs, n, n, n, 1, cc, cs, w.kev + NS * n);
+        B200_LAUNCH(k_coset_fold, dim3(grid, 1, (NW + 1) * k), 256, 0, st)(w.wpoly, S, n + 2, n, 1, cc, cs, w.ext);
+        B200_LAUNCH(k_coset_fold, dim3(grid, 1, k), 256, 0, st)(w.zpoly, S, n + 3, n, 1, cc, cs, w.zext);
+        int r = ntt_device(dn, w.kev, nscr, /*inverse=*/0, /*coset=*/0, (unsigned)coset_batch(k), n, st);
+        if (r != B200_OK) return r;
+        QuotCosetArgs q;
+        q.sel = w.kev;
+        q.sig = w.kev + NS * n;
+        q.ext = w.ext;
+        q.pi = w.ext + (size_t)k * NW * n;
+        q.zext = w.zext;
+        q.pts = pk->coset_pts;
+        q.l1_inv = pk->l1_inv;
+        q.out = w.quot;
+        q.ostride = m;
+        q.log_n = pk->log_n;
+        q.k = pk->k;
+        q.chal = chal;
+        q.dstride = dstride;
+        q.zh_inv = pk->zh_inv[j];
+        B200_LAUNCH(k_quotient_coset, dim3(grid_for(n, 128), k), 128, 0, st)(q, j);
+    }
+    // nc inverse transforms per proof, as many proofs at a time as the per-coset buffers hold as scratch
+    const unsigned per = (unsigned)std::max<size_t>(1, std::min<size_t>(k, coset_batch(k) / (size_t)pk->nc));
+    for (unsigned p0 = 0; p0 < k; p0 += per) {
+        const unsigned cnt = std::min(per, k - p0);
+        const int r = ntt_device(dn, w.quot + (size_t)p0 * m, w.kev, 1, 0, (unsigned)pk->nc * cnt, n, st);
+        if (r != B200_OK) return r;
+    }
+    if (pk->nc == 6) B200_LAUNCH(k_coset_combine<6>, dim3(grid_for(n, 128), k), 128, 0, st)(w.quot, n, pk->cscale_inv, pk->comb);
+    else B200_LAUNCH(k_coset_combine<8>, dim3(grid_for(n, 128), k), 128, 0, st)(w.quot, n, pk->cscale_inv, pk->comb);
+    return B200_OK;
+}
+
 // The copy permutation comes from the caller (h_perm) or, with h_perm null, is derived on the device from the wiring
 // (h_wire_vars, num_vars), which the key then keeps.
+// compact: a key without the coset tables ce_sel / ce_sig (b200compact.h); its preprocessing transforms and commits in
+// batches no larger than a proof's, so that neither its NTT nor its MSM scratch outgrows what its proofs use.
 static int preprocess(Context* c, const Bases* srs, unsigned log_n, size_t num_inputs, const fe* h_selectors,
-                      const uint64_t* h_perm, const uint32_t* h_wire_vars, size_t num_vars, const fe* h_k, ProvingKey** out) {
+                      const uint64_t* h_perm, const uint32_t* h_wire_vars, size_t num_vars, const fe* h_k, ProvingKey** out,
+                      bool compact = false) {
     const size_t n = (size_t)1 << log_n;
     // 6 cosets (6n > 5n + 7 points) from n = 16 on; all 8 for the tiny domains, where 6n would not exceed
     // the quotient's degree by enough to keep the degree check meaningful.  Six cosets determine t for a satisfied
@@ -836,6 +965,7 @@ static int preprocess(Context* c, const Bases* srs, unsigned log_n, size_t num_i
     pk->nc = nc;
     pk->num_inputs = num_inputs;
     pk->srs = srs;
+    pk->compact = compact;
     for (int i = 0; i < NW; ++i) pk->k.v[i] = h_k[i];
     int rc;
     Domain* dn = nullptr;
@@ -851,12 +981,14 @@ static int preprocess(Context* c, const Bases* srs, unsigned log_n, size_t num_i
         return code;
     };
     if ((rc = alloc_fe(&pk->sel_coeffs, NS * n)) || (rc = alloc_fe(&pk->sig_coeffs, NW * n)) ||
-        (rc = alloc_fe(&pk->sig_evals, NW * n)) || (rc = alloc_fe(&pk->ce_sel, NS * m)) ||
-        (rc = alloc_fe(&pk->ce_sig, NW * m)) || (rc = alloc_fe(&pk->dom, n)) || (rc = alloc_fe(&pk->coset_pts, m)) ||
+        (rc = alloc_fe(&pk->sig_evals, NW * n)) || (!compact && (rc = alloc_fe(&pk->ce_sel, NS * m))) ||
+        (!compact && (rc = alloc_fe(&pk->ce_sig, NW * m))) || (rc = alloc_fe(&pk->dom, n)) || (rc = alloc_fe(&pk->coset_pts, m)) ||
         (rc = alloc_fe(&pk->l1_inv, m)) || (rc = alloc_fe(&pk->cscale, m)) || (rc = alloc_fe(&pk->cscale_inv, m)))
         return fail(rc);
     if (cudaMalloc(&d_perm, NW * n * 8) != cudaSuccess) return fail(B200_ERR_CUDA);
-    if ((rc = c->ntt_scratch.reserve((size_t)NS * m * sizeof(fe))) != B200_OK) return fail(rc);
+    // compact: the NS selector transforms of size n need NS n elements
+    if ((rc = compact ? c->ntt_scratch.reserve((size_t)NS * n * sizeof(fe)) : c->ntt_scratch.reserve((size_t)NS * m * sizeof(fe))) != B200_OK)
+        return fail(rc);
     fe* scratch = reinterpret_cast<fe*>(c->ntt_scratch.p);
 
     const fe one = fe_one<Fr>();
@@ -889,7 +1021,9 @@ static int preprocess(Context* c, const Bases* srs, unsigned log_n, size_t num_i
         }
     }
     B200_LAUNCH(k_l1_denominators, grid_for(m, 256), 256, 0, st)(pk->coset_pts, m, host_from_u64(n), pk->l1_inv);
-    batch_inverse_enqueue(nullptr, pk->l1_inv, pk->ce_sel /*scratch, overwritten below*/, m, st);
+    if (!compact) batch_inverse_enqueue(nullptr, pk->l1_inv, pk->ce_sel /*scratch, overwritten below*/, m, st);
+    else  // one coset at a time, in the NTT scratch (the inverses are exact: the split does not change them)
+        for (int j = 0; j < nc; ++j) batch_inverse_enqueue(nullptr, pk->l1_inv + (size_t)j * n, scratch, n, st);
 
     // selectors: evaluations -> coefficients -> commitments
     cudaMemcpyAsync(pk->sel_coeffs, h_selectors, NS * n * sizeof(fe), cudaMemcpyHostToDevice, st);
@@ -907,14 +1041,22 @@ static int preprocess(Context* c, const Bases* srs, unsigned log_n, size_t num_i
     B200_LAUNCH(k_sigma_evals, grid_for(NW * n, 256), 256, 0, st)(d_perm, pk->dom, n, pk->k, pk->sig_evals);
     cudaMemcpyAsync(pk->sig_coeffs, pk->sig_evals, NW * n * sizeof(fe), cudaMemcpyDeviceToDevice, st);
     if ((rc = ntt_device(dn, pk->sig_coeffs, scratch, 1, 0, NW, n, st)) != B200_OK) return fail(rc);
-    // resident evaluations of the 18 fixed polynomials on the quotient domain
-    if ((rc = coset_evals(pk, dn, pk->sel_coeffs, n, n, NS, pk->ce_sel, scratch, st)) != B200_OK) return fail(rc);
-    if ((rc = coset_evals(pk, dn, pk->sig_coeffs, n, n, NW, pk->ce_sig, scratch, st)) != B200_OK) return fail(rc);
+    // resident evaluations of the 18 fixed polynomials on the quotient domain (a compact key's round 3 makes them per coset)
+    if (!compact) {
+        if ((rc = coset_evals(pk, dn, pk->sel_coeffs, n, n, NS, pk->ce_sel, scratch, st)) != B200_OK) return fail(rc);
+        if ((rc = coset_evals(pk, dn, pk->sig_coeffs, n, n, NW, pk->ce_sig, scratch, st)) != B200_OK) return fail(rc);
+    }
     if (cudaStreamSynchronize(st) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "preprocess"));
     cudaFree(d_perm);
     d_perm = nullptr;
-    // the 18 commitments of the verifying key
-    if ((rc = commit_batch(c, pk, pk->sel_coeffs, n, n, NS, pk->sel_comms)) != B200_OK) return fail(rc);
+    // the 18 commitments of the verifying key; a compact key's selectors in batches of at most NW, a proof's largest
+    if (!compact) {
+        if ((rc = commit_batch(c, pk, pk->sel_coeffs, n, n, NS, pk->sel_comms)) != B200_OK) return fail(rc);
+    } else {
+        for (unsigned s0 = 0; s0 < (unsigned)NS; s0 += NW)
+            if ((rc = commit_batch(c, pk, pk->sel_coeffs + (size_t)s0 * n, n, n, std::min<unsigned>(NW, NS - s0), pk->sel_comms + s0)) != B200_OK)
+                return fail(rc);
+    }
     if ((rc = commit_batch(c, pk, pk->sig_coeffs, n, n, NW, pk->sig_comms)) != B200_OK) return fail(rc);
     *out = pk;
     return B200_OK;
@@ -1164,11 +1306,18 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
     int rc;
     // h_small: the k degree flags, then k x 2 NW evaluations, then the k batched polynomials' values at zeta
     const size_t flags_bytes = ((size_t)k * 4 + 63) / 64 * 64;
-    if ((rc = bf.ws->reserve(workspace_elems(n, k) * sizeof(fe))) != B200_OK) return rc;
+    const bool compact = pk->compact;
+    if ((rc = compact ? bf.ws->reserve(compact_workspace_elems(n, k) * sizeof(fe)) : bf.ws->reserve(workspace_elems(n, k) * sizeof(fe))) !=
+        B200_OK)
+        return rc;
     const bool from_witness = items[0].witness != nullptr;  // every item of a call has the same kind of input
     // the NTT scratch doubles as the staging area of the witness vectors: the gather has read them before round 1 uses it
-    if ((rc = bf.nscr->reserve((size_t)k * std::max(7 * m, from_witness ? pk->num_vars : 0) * sizeof(fe))) != B200_OK) return rc;
-    if ((rc = bf.nscr2->reserve((size_t)k * 6 * m * sizeof(fe))) != B200_OK) return rc;
+    if (compact) {  // no side-stream coset evaluations: no second NTT scratch
+        if ((rc = bf.nscr->reserve(compact_nscr_elems(n, k, from_witness ? pk->num_vars : 0) * sizeof(fe))) != B200_OK) return rc;
+    } else {
+        if ((rc = bf.nscr->reserve((size_t)k * std::max(7 * m, from_witness ? pk->num_vars : 0) * sizeof(fe))) != B200_OK) return rc;
+        if ((rc = bf.nscr2->reserve((size_t)k * 6 * m * sizeof(fe))) != B200_OK) return rc;
+    }
     if ((rc = bf.h_small->reserve(std::max<size_t>(4096, flags_bytes + (size_t)k * (2 * NW + 1) * sizeof(fe)))) != B200_OK) return rc;
     if ((rc = bf.h_params->reserve(k * sizeof(ProofParams))) != B200_OK) return rc;
     if ((rc = bf.d_params->reserve(k * sizeof(ProofParams))) != B200_OK) return rc;
@@ -1177,7 +1326,7 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
         B200_CUDA(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
         B200_CUDA(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
     }
-    Workspace w = carve(reinterpret_cast<fe*>(bf.ws->p), n, k);
+    Workspace w = carve(reinterpret_cast<fe*>(bf.ws->p), n, k, compact);
     fe* nscr = reinterpret_cast<fe*>(bf.nscr->p);
     const size_t S = w.S;
     Domain* dn = nullptr;
@@ -1189,7 +1338,12 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
     ProofGraphSet* gs = gset && gset->proofs_seen > 0 ? gset : nullptr;
     // Abort points of a cancelled pool job (b200cancel.h): on entry and after each of the first four round trips.  A proof
     // that captures its key's graphs drops the partial set, so that the next proof of the key captures all of them again.
-    const bool capturing = gs && !gs->complete(kProofSegs);
+    auto all_captured = [&]() {  // every segment the key's proofs run: a compact key's have no side-stream segment 1
+        for (int i = 0; i < kProofSegs; ++i)
+            if (!gs->exec[i] && !(compact && i == 1)) return false;
+        return true;
+    };
+    const bool capturing = gs && !all_captured();
     auto abort_job = [&]() {
         if (capturing) gs->drop();
         return cancelled(c);
@@ -1312,7 +1466,7 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
             if (pending) cudaStreamSynchronize(c->stream2);  // error paths: never leave the side stream running
         }
     } side{c};
-    {
+    if (!compact) {  // a compact key evaluates them per coset in round 3
         cudaStream_t s2 = c->stream2;
         B200_CUDA(cudaEventRecord(c->ev_fork, st));
         B200_CUDA(cudaStreamWaitEvent(s2, c->ev_fork, 0));
@@ -1377,7 +1531,7 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
         hp[p].chal[3] = fe_sqr<Fr>(alpha[p]);
         for (int i = 0; i < 4; ++i) hp[p].blind_q[i] = items[p].blinders[13 + i];
     }
-    B200_CUDA(cudaStreamWaitEvent(st, c->ev_join, 0));  // join: wire / PI coset evaluations are ready
+    if (!compact) B200_CUDA(cudaStreamWaitEvent(st, c->ev_join, 0));  // join: wire / PI coset evaluations are ready
     side.pending = false;
     const size_t deg = NW * (n + 1) + 2;
     uint32_t* h_flag = reinterpret_cast<uint32_t*>(bf.h_small->p);  // pinned; read after the commitments below are in
@@ -1386,11 +1540,14 @@ static int prove(Context* c, const ProverBufs& bf, const ProvingKey* pk, ProveIt
     rc = commit_enqueue(4, w.split, n + 3, S, NW * k, [&]() -> int {
         int r = push_params();
         if (r != B200_OK) return r;
-        {
+        if (compact) {
             HeavyScope hv(c, st);
-            if ((r = coset_evals(pk, dn, w.zpoly, S, n + 3, k, w.zext, nscr, hv.run)) != B200_OK) return r;
-        }
-        {
+            if ((r = compact_quotient(pk, dn, w, k, &dp->chal[0], D, nscr, hv.run)) != B200_OK) return r;
+        } else {
+            {
+                HeavyScope hv(c, st);
+                if ((r = coset_evals(pk, dn, w.zpoly, S, n + 3, k, w.zext, nscr, hv.run)) != B200_OK) return r;
+            }
             QuotArgs q;
             q.sel = pk->ce_sel;
             q.sig = pk->ce_sig;
@@ -1617,7 +1774,9 @@ static size_t prove_batch_chunk(Context* c, const ProvingKey* pk, size_t k) {
     const MsmPlan& pl = pk->srs->plan;
     const size_t msm_per_commit = n * (size_t)pl.n_digits * 4 * 2 + ((size_t)pl.n_phys << (pl.c - 1)) * sizeof(g1_xyzz) * 4;
     // (a witness vector is staged in the first NTT scratch, 7m elements unless the vector is longer)
-    const size_t per_proof = (workspace_elems(n, 1) + 6 * m + std::max(7 * m, pk->num_vars)) * sizeof(fe) + NW * msm_per_commit;
+    const size_t per_proof = (pk->compact ? compact_workspace_elems(n, 1) + compact_nscr_elems(n, 1, pk->num_vars)
+                                          : workspace_elems(n, 1) + 6 * m + std::max(7 * m, pk->num_vars)) * sizeof(fe) +
+                             NW * msm_per_commit;
     size_t free_b = 0, total_b = 0;
     if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) free_b = 0;
     const Context::BatchBufs& b = c->batch;
@@ -2049,7 +2208,7 @@ static int prove_settlement(b200_ctx* ctx, const Bases* srs, const ProvingKey* p
         return rc;
     }
     if (rc != B200_OK) return rc;
-    const fe* d_p = carve(reinterpret_cast<fe*>(ctx->c.plonk_ws.p), pk->n, 1).wpoly;
+    const fe* d_p = carve(reinterpret_cast<fe*>(ctx->c.plonk_ws.p), pk->n, 1, pk->compact).wpoly;
     for (LinkItem& it : its) {
         it.a2 = d_p;
         it.comm2 = item->proof->wires_poly_comms[0];
@@ -2074,26 +2233,25 @@ static int prove_settlement(b200_ctx* ctx, const Bases* srs, const ProvingKey* p
 
 }  // namespace b200
 
-extern "C" {
+namespace b200 {
 
-int b200_plonk_preprocess(b200_ctx* ctx, const b200_bases* srs, unsigned log_n, size_t num_inputs,
-                          const uint64_t* selectors_evals, const uint64_t* perm, const uint64_t* k, b200_pk** out) {
+static int preprocess_perm(b200_ctx* ctx, const b200_bases* srs, unsigned log_n, size_t num_inputs, const uint64_t* selectors_evals,
+                           const uint64_t* perm, const uint64_t* k, b200_pk** out, bool compact) {
     B200_TRY
     if (!ctx || !srs || !selectors_evals || !perm || !k || !out) return B200_ERR_INVALID;
     std::lock_guard<std::mutex> lk(ctx->c.mu);
     B200_ENTER(ctx->c);
     ProvingKey* pk = nullptr;
     int rc = preprocess(&ctx->c, srs->b, log_n, num_inputs, reinterpret_cast<const fe*>(selectors_evals), perm, nullptr, 0,
-                        reinterpret_cast<const fe*>(k), &pk);
+                        reinterpret_cast<const fe*>(k), &pk, compact);
     if (rc != B200_OK) return rc;
     *out = new b200_pk{pk};
     return B200_OK;
     B200_CATCH
 }
 
-int b200_plonk_preprocess_wiring(b200_ctx* ctx, const b200_bases* srs, unsigned log_n, size_t num_inputs,
-                                 const uint64_t* selectors_evals, const unsigned* wire_vars, size_t num_vars, const uint64_t* k,
-                                 b200_pk** out) {
+static int preprocess_wiring(b200_ctx* ctx, const b200_bases* srs, unsigned log_n, size_t num_inputs, const uint64_t* selectors_evals,
+                             const unsigned* wire_vars, size_t num_vars, const uint64_t* k, b200_pk** out, bool compact) {
     static_assert(sizeof(unsigned) == sizeof(uint32_t), "wire_vars holds 32-bit indices");
     B200_TRY
     if (!ctx || !srs || !selectors_evals || !wire_vars || !k || !out) return B200_ERR_INVALID;
@@ -2105,11 +2263,68 @@ int b200_plonk_preprocess_wiring(b200_ctx* ctx, const b200_bases* srs, unsigned 
     B200_ENTER(ctx->c);
     ProvingKey* pk = nullptr;
     int rc = preprocess(&ctx->c, srs->b, log_n, num_inputs, reinterpret_cast<const fe*>(selectors_evals), nullptr,
-                        reinterpret_cast<const uint32_t*>(wire_vars), num_vars, reinterpret_cast<const fe*>(k), &pk);
+                        reinterpret_cast<const uint32_t*>(wire_vars), num_vars, reinterpret_cast<const fe*>(k), &pk, compact);
     if (rc != B200_OK) return rc;
     *out = new b200_pk{pk};
     return B200_OK;
     B200_CATCH
+}
+
+// b200_plonk_footprint's parts (b200compact.h), from the allocation rules of preprocess(), prove() and msm_launch_batch
+static void footprint(unsigned log_n, unsigned k, bool compact, uint64_t out[B200_FOOTPRINT_PARTS]) {
+    const size_t n = (size_t)1 << log_n, nc = log_n >= 4 ? 6 : 8, m = nc * n, fb = sizeof(fe);
+    const MsmPlan pl = msm_choose_plan(n + 3, 0, ~(size_t)0);  // the SRS's plan with every window table
+    const size_t sel_msm = msm_scratch_estimate(pl, n, compact ? NW : NS), wire_msm = msm_scratch_estimate(pl, n + 3, NW);
+    for (int i = 0; i < B200_FOOTPRINT_PARTS; ++i) out[i] = 0;
+    out[0] = ((NS + 2 * NW + 1) * n + (compact ? 4 : NS + NW + 4) * m) * fb + NW * n * 4;
+    out[1] = (compact ? std::max((size_t)NS * n, k == 1 ? compact_nscr_elems(n, 1, 0) : 0) : NS * m) * fb;
+    out[2] = 3 * n * fb;
+    out[3] = (size_t)pl.n_tables * (n + 3) * sizeof(g1_affine);
+    out[4] = std::max(sel_msm, wire_msm);
+    out[5] = (uint64_t)1 << 30;
+    if (k == 1) {
+        out[6] = (compact ? compact_workspace_elems(n, 1) : workspace_elems(n, 1)) * fb;
+        out[7] = compact ? 0 : 6 * m * fb;
+    } else {
+        out[8] = (compact ? compact_workspace_elems(n, k) : workspace_elems(n, k)) * fb;
+        out[9] = (compact ? compact_nscr_elems(n, k, 0) : (size_t)k * 7 * m) * fb;
+        out[10] = compact ? 0 : (size_t)k * 6 * m * fb;
+        out[11] = msm_scratch_estimate(pl, n + 3, (size_t)k * NW);
+    }
+}
+
+}  // namespace b200
+
+extern "C" {
+
+int b200_plonk_preprocess(b200_ctx* ctx, const b200_bases* srs, unsigned log_n, size_t num_inputs,
+                          const uint64_t* selectors_evals, const uint64_t* perm, const uint64_t* k, b200_pk** out) {
+    return preprocess_perm(ctx, srs, log_n, num_inputs, selectors_evals, perm, k, out, false);
+}
+
+int b200_plonk_preprocess_wiring(b200_ctx* ctx, const b200_bases* srs, unsigned log_n, size_t num_inputs,
+                                 const uint64_t* selectors_evals, const unsigned* wire_vars, size_t num_vars, const uint64_t* k,
+                                 b200_pk** out) {
+    return preprocess_wiring(ctx, srs, log_n, num_inputs, selectors_evals, wire_vars, num_vars, k, out, false);
+}
+
+int b200_plonk_preprocess_compact(b200_ctx* ctx, const b200_bases* srs, unsigned log_n, size_t num_inputs,
+                                  const uint64_t* selectors_evals, const uint64_t* perm, const uint64_t* k, b200_pk** out) {
+    return preprocess_perm(ctx, srs, log_n, num_inputs, selectors_evals, perm, k, out, true);
+}
+
+int b200_plonk_preprocess_wiring_compact(b200_ctx* ctx, const b200_bases* srs, unsigned log_n, size_t num_inputs,
+                                         const uint64_t* selectors_evals, const unsigned* wire_vars, size_t num_vars,
+                                         const uint64_t* k, b200_pk** out) {
+    return preprocess_wiring(ctx, srs, log_n, num_inputs, selectors_evals, wire_vars, num_vars, k, out, true);
+}
+
+int b200_pk_is_compact(const b200_pk* pk) { return pk && pk->pk->compact ? 1 : 0; }
+
+int b200_plonk_footprint(unsigned log_n, size_t k, int compact, uint64_t out[12]) {
+    if (!out || log_n < 2 || log_n > 25 || k < 1 || k > kMaxBatchChunk) return refuse("plonk_footprint: log_n outside [2, 25], k outside [1, 64] or a NULL out");
+    footprint(log_n, (unsigned)k, compact != 0, out);
+    return B200_OK;
 }
 
 int b200_pk_verifying_key(const b200_pk* pk, uint64_t* selector_comms, uint64_t* sigma_comms) {

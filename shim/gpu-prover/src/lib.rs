@@ -14,6 +14,7 @@
 //! | `gossip-server/src/orderbook.rs:180-229` | the order check: two proofs and one link proof per order (`todo!` upstream) | [`GpuProver::submit_verify`], [`GpuProver::submit_verify_combined`] |
 //! | `primitives/srs.rs:63-71` | `parse_ptau_file` + `powers_of_g` | [`GpuProver::load_srs`] |
 //! | `native_proof_manager.rs:167-178` | the cancel channel: `ProofManagerError::Cancelled` at once | [`GpuProver::cancel_all`], [`GpuProver::shutdown_now`] |
+//! | `circuit-types/src/traits.rs:850`  | the same, for domains up to 2^23: round 3 one coset at a time | [`GpuProver::preprocess_wiring_compact`] |
 //!
 //! Marshalling rules (SURVEY.md §7 "Rust ABI hazards"): `Fr`/`Fq` are `Fp(BigInt<4>, PhantomData)` holding the
 //! Montgomery limbs — reading `.0 .0` is the value the C ABI wants; `G1Affine` is `repr(Rust)` {x, y, infinity} and is
@@ -32,6 +33,7 @@ pub mod ffi_express;
 pub mod ffi_reserved;
 pub mod ffi_selftest;
 pub mod ffi_cancel;
+pub mod ffi_compact;
 
 use ark_bn254::{Bn254, Fq, Fr, G1Affine};
 use ark_ff::{BigInt, UniformRand};
@@ -165,6 +167,24 @@ impl GpuProver {
         check(unsafe {
             ffi::b200_plonk_preprocess_wiring(ctx, self.srs, n.trailing_zeros(), cs.num_inputs(), selectors.as_ptr(),
                                               wire_vars.as_ptr(), cs.num_vars(), k.as_ptr(), &mut pk)
+        })?;
+        Ok(GpuProvingKey { raw: pk, num_inputs: cs.num_inputs(), log_n: n.trailing_zeros() })
+    }
+
+    /// `preprocess_wiring` making a compact key (b200compact.h): no coset tables in the key, round 3 one coset at a
+    /// time, so that 2^23 domains fit one 80 GB GPU.  Same verifying key, same proofs; every prove method takes it.
+    /// `b200_plonk_footprint` gives the device bytes of either kind before anything is allocated.
+    pub fn preprocess_wiring_compact(&self, cs: &PlonkCircuit<Fr>) -> Result<GpuProvingKey, PlonkError> {
+        let n = cs.eval_domain_size()?;
+        let selectors: Vec<u64> = cs.selector_evals().iter().flat_map(|col| col.iter().flat_map(fr_limbs)).collect(); // 13 x n
+        let wire_vars: Vec<c_uint> = cs.wire_variables().iter().flat_map(|col| col.iter().map(|v| *v as c_uint)).collect(); // 5 x n
+        let k: Vec<u64> = cs.coset_representatives().iter().flat_map(fr_limbs).collect();
+        let ctx = unsafe { ffi::b200_pool_ctx(self.pool, 0) };
+        let mut pk = std::ptr::null_mut();
+        check(unsafe {
+            ffi_compact::b200_plonk_preprocess_wiring_compact(ctx, self.srs, n.trailing_zeros(), cs.num_inputs(),
+                                                              selectors.as_ptr(), wire_vars.as_ptr(), cs.num_vars(), k.as_ptr(),
+                                                              &mut pk)
         })?;
         Ok(GpuProvingKey { raw: pk, num_inputs: cs.num_inputs(), log_n: n.trailing_zeros() })
     }
